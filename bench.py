@@ -2,7 +2,7 @@
 """bench.py -- images/sec (forward + backward) of the hot path
 ERFNet -> activation/mask -> weighted least squares -> backprojection loss.
 
-    python bench.py --gpus N --steps K --warmup W            # our arm (sm_100a kernels via the C ABI)
+    python bench.py --gpus N --steps K --warmup W            # our arm (sm_90a kernels via the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own modules on the host cores, rank 0 only
 
 Workload (BASELINE.json configs[1]): egolane 2-lane, order 2, batch 32 per GPU, 256x512, fp32 I/O,
@@ -12,6 +12,8 @@ Multi-GPU = weak scaling: 32 images per GPU, per-replica BN statistics, one flat
 
 One JSON line on stdout (rank 0).  `value`: inputs resident in HBM.  `e2e`: through the public modules
 with HOST (pinned) inputs copied in every step and the loss read back every step.
+--dump-outputs DIR: after the timed steps, DIR/<name>.npy holds what the last timed step computed (the loss and every
+parameter gradient, rank 0); inputs and initial weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -31,37 +33,23 @@ CONFIGS = {
     3: dict(name="tusimple_4lane_b64_256x512", nclasses=4, order=3, mask=0.2, resize=256, batch=64),
     4: dict(name="tusimple_4lane_b32pergpu_320x640", nclasses=4, order=3, mask=0.2, resize=320, batch=32),
 }
-MODE_DTYPE = {"tf32x3": "fp32 (storage fp32; products 3xTF32 on tcgen05 = fp32-grade; fp32 accumulate)",
-              "tf32": "tf32 (storage fp32; single-pass TF32 products on tcgen05; fp32 accumulate)",
+MODE_DTYPE = {"tf32x3": "fp32 (storage fp32; products 3xTF32 on tensor cores = fp32-grade; fp32 accumulate)",
+              "tf32": "tf32 (storage fp32; single-pass TF32 products on tensor cores; fp32 accumulate)",
               "fp32": "fp32 (CUDA-core FFMA)"}
-MODE_TEXT = {"tf32x3": "3xTF32 on tcgen05 (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, TMEM fp32 accumulators) for every convolution but the "
-                       "3->13 stem and the 16->L output ConvTranspose2d (fp32 FFMA): 3-tap convs conv_tc_x3.cu (C=16 as 4-pixel "
-                       "super-pixels), stride-2 layers conv_tcg.cu, weight gradients wgrad_tc_x3.cu / wgrad_tcg.cu",
-             "tf32": "single-pass TF32 on tcgen05 for the same layers (what cuDNN's default does for the reference's fp32 convs)",
+MODE_TEXT = {"tf32x3": "3xTF32 (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 register accumulators) for every convolution but the "
+                       "3->13 stem and the 16->L output ConvTranspose2d (fp32 FFMA): 3-tap convs on wgmma conv_tc.cu (C=16 as "
+                       "4-pixel super-pixels), stride-2 layers on wgmma conv_tcg.cu, weight gradients on mma.sync wgrad_tcg.cu",
+             "tf32": "single-pass TF32 on the same kernels (what cuDNN's default does for the reference's fp32 convs)",
              "fp32": "every convolution on the CUDA-core FFMA kernels (conv_f32.cu, wgrad_f32.cu)"}
 MODE_ACCURACY = {"tf32x3": "meets the reference-fp32 gates: on the reference's golden inputs |ours - fp64| <= 4 |reference fp32 - fp64| + "
-                           "1e-4 for every block output, beta and the loss (tests/test_net_gpu.py, __graft_entry__.smoke(); measured "
-                           "numbers in profiles/r02/accuracy_*.json)",
-                 "tf32": "beta 1.1e-3 (2 lanes, order 2) / 2.1e-3 (4 lanes, order 3) norm-wise from fp64 on the golden inputs -- OUTSIDE "
-                         "the 1e-4 gate; labelled extra only (profiles/r01/tf32_accuracy_*.json)",
+                           "1e-4 for every block output, beta and the loss (tests/test_net_gpu.py, __graft_entry__.smoke())",
+                 "tf32": "beta ~1e-3 norm-wise from fp64 on the golden inputs -- OUTSIDE the 1e-4 gate; labelled extra only "
+                         "(tests/test_net_gpu.py::test_full_path_tf32_mode_accuracy)",
                  "fp32": "meets the same gates as tf32x3 (tests/test_net_gpu.py)"}
 FWD_GFLOP_PER_IMG = {(2, 256): 13.231, (4, 256): 13.239, (4, 320): 20.686, (2, 320): 20.673}   # SURVEY.md 8d
 FWD_GFLOP_PER_IMG_CLAS = {(4, 256): 15.497}        # + the two Classification heads
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
-
-
-def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            d = json.load(open(p))
-            d["_source"] = "measured"
-            return d
-        except Exception:
-            pass
-    d = dict(FALLBACK_PEAKS)
-    d["_source"] = "fallback"
-    return d
+# NVIDIA H100 SXM data sheet (700 W board), dense: HBM3 bandwidth, BF16 and TF32 tensor rates -- not measured here
+PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "tf32_tflops": 495.0, "_source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -133,9 +121,9 @@ def host_batch(cfg, seed, pinned):
 
 
 # ----------------------------------------------------------------------------------------------
-# reference arm / cpu_baseline: the reference's OWN modules (unmodified; /root/reference in the build container,
-# the verbatim copy under baseline/_ref/ on the GPU box -- oracle/reference_import.py) on the host cores, kind
-# "reference"; only if neither is present, the oracle's CPU restatement (kind "port").
+# reference arm / cpu_baseline: the reference's OWN modules (unmodified; the upstream checkout or the copy build() made
+# under oracle/_ref/ -- oracle/reference_import.py) on the host cores, kind "reference"; only if neither is present, the
+# oracle's CPU restatement (kind "port").
 # ----------------------------------------------------------------------------------------------
 def _pick_threads(one_step_probe, cores):
     """ "all the host threads it can use": the thread count that is actually fastest on this host (128 threads on
@@ -223,7 +211,7 @@ def cpu_reference_run(cfg, steps, warmup, sample_images):
 
 def gpu_stock_reference_run(cfg, steps, warmup, allow_tf32):
     """Labelled extra (BASELINE.md section 2, "library-kernel comparison point"): the reference's OWN modules, unmodified, on
-    the same B200 through stock PyTorch (cuDNN / cuBLAS / torch.inverse), `cudnn.benchmark = True` as BP/main.py:62 sets it,
+    the same GPU through stock PyTorch (cuDNN / cuBLAS / torch.inverse), `cudnn.benchmark = True` as BP/main.py:62 sets it,
     with torch's default TF32 convolutions (allow_tf32 True: 1e-3-accurate) or strict fp32 (False).  Eager launches, the
     way the reference runs.  None of this repo's kernels is on that path."""
     import contextlib
@@ -366,6 +354,16 @@ def _arm_watchdog(seconds):
     faulthandler.dump_traceback_later(seconds + 15, exit=True, file=sys.stderr)
 
 
+def dump_outputs(outdir, loss, model):
+    """The last timed step's results as DIR/<name>.npy: the loss (float64) and every parameter gradient (float32)."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    np.save(os.path.join(outdir, "loss.npy"), np.asarray(loss.detach().double().cpu().numpy(), dtype=np.float64))
+    for name, p in model.named_parameters():
+        if p.grad is not None:
+            np.save(os.path.join(outdir, "grad.%s.npy" % name), p.grad.detach().float().cpu().numpy())
+
+
 def run_ours(a, cfg):
     import torch
     import torch.distributed as dist
@@ -482,11 +480,13 @@ def run_ours(a, cfg):
             gstep = None
             a.graph = False
 
+    last_loss = [None]
+
     def dev_step():
         if gstep is not None:
             gstep()
         else:
-            step(dx, dxgt, dvalid)
+            last_loss[0] = step(dx, dxgt, dvalid)
 
     if gstep is not None:
         gstep.prefetch(hx, hxgt, hvalid)          # batch 0 of the e2e loop
@@ -508,6 +508,8 @@ def run_ours(a, cfg):
 
     sampler = ClockSampler(local) if rank == 0 else None
     ms_dev = timed(dev_step, a.steps)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, gstep.loss if gstep is not None else last_loss[0], model)
     for _ in range(2):
         e2e_step()
     ms_e2e = timed(e2e_step, a.steps)
@@ -577,7 +579,7 @@ def run_ours(a, cfg):
 
     # one traced step: CUDA events around every C-ABI launch on the launching stream
     table, roofline, roofline_lsq, roofline_kernels = None, None, None, None
-    peaks = load_peaks()
+    peaks = PEAKS
     # every rank runs the step (it contains the gradient all-reduce); only rank 0 records the events
     if rank == 0:
         _capi.TRACE = []
@@ -596,9 +598,8 @@ def run_ours(a, cfg):
         table = {k: dict(v, share=v["ms"] / tot if tot else 0.0) for k, v in sorted(agg.items(), key=lambda kv: -kv[1]["ms"])}
         dom = next(iter(table))
         d = table[dom]
-        hbm_peak = peaks.get("hbm_gbs", FALLBACK_PEAKS["hbm_gbs"])
-        bf16_peak = peaks.get("bf16_tflops_sustained", FALLBACK_PEAKS["bf16_tflops_sustained"])
-        tf32_peak = bf16_peak / 2.0     # MEASURED_PEAKS.json has no TF32 entry: dense TF32 = half the dense bf16 rate
+        hbm_peak = peaks["hbm_gbs"]
+        tf32_peak = peaks["tf32_tflops"]
         TENSOR_KERNELS = {"lf_conv1d_tc_x3": 3, "lf_conv1d_tc": 1, "lf_wgrad3_tc_x3": 3, "lf_wgrad3_tc": 1, "lf_conv_tcg": None,
                           "lf_wgrad_tcg": None}
 
@@ -616,7 +617,7 @@ def run_ours(a, cfg):
             if name in TENSOR_KERNELS and tens is not None:
                 passes = TENSOR_KERNELS[name] or (3 if a.conv_mode == "tf32x3" else 1)
                 return dict(base, **tens, other_roof=hbm,
-                            peak_source=peaks["_source"] + ": 1/2 of the sustained dense bf16 rate (no TF32 entry in MEASURED_PEAKS.json)",
+                            peak_source=peaks["_source"] + ": dense TF32",
                             algorithmic="2 * pixels * taps * Cin * Cout FLOPs per launch (one multiply-add per product)",
                             tensor_passes_per_product=passes,
                             tensor_pipe_work_frac=passes * tens["frac"])
@@ -626,17 +627,6 @@ def run_ours(a, cfg):
             return None
 
         roofline = kernel_roofline(dom, d)
-        # DRAM traffic per launch of the dominant kernel: a STATIC figure from the committed `ncu --set full` capture of this
-        # kernel (profiles/r02), taken on this workload's shapes -- not measured in this run; null for other workloads
-        if roofline is not None:
-            roofline["traffic"], roofline["traffic_source"] = None, None
-            try:
-                cap = json.load(open(os.path.join(ROOT, "profiles", "r02", "ncu_%s.json" % dom)))
-                if cap.get("workload") == cfg["name"] and cap.get("batch") == B:
-                    roofline["traffic"] = cap["mean_traffic_bytes_per_launch"]
-                    roofline["traffic_source"] = "static: profiles/r02/ncu_%s.json (%s)" % (dom, cap.get("how", ""))
-            except (OSError, ValueError, KeyError):
-                pass
         roofline_kernels = [r for r in (kernel_roofline(k, v) for k, v in list(table.items())[:10]) if r is not None]
         for k in ("lf_lsq_fwd", "lf_lsq_bwd"):
             if k in table:
@@ -647,9 +637,8 @@ def run_ours(a, cfg):
                                    "frac": ach / hbm_peak, "avg_launch_ms": dd["ms"] / dd["launches"],
                                    "note": "algorithmic bytes (SURVEY.md 8d: no credit for the masked rows the kernel skips); "
                                            "launch-latency regime at this size; see tools/bench_lsq.py for the stress config"}
-        outdir = os.path.join(ROOT, "gpurun_out")
-        if os.path.isdir(outdir):
-            json.dump(table, open(os.path.join(outdir, "kernel_table_%s_n%d.json" % (a.conv_mode, world)), "w"), indent=1)
+        if a.dump_outputs:
+            json.dump(table, open(os.path.join(a.dump_outputs, "kernel_table_%s_n%d.json" % (a.conv_mode, world)), "w"), indent=1)
 
     cpu = None
     if rank == 0 and world == 1 and not a.no_cpu_baseline:
@@ -667,7 +656,7 @@ def run_ours(a, cfg):
                 "config": {"workload": cfg["name"], "per_gpu_batch": B, "global_batch": world * B,
                            "resolution": "%dx%d" % (cfg["resize"], 2 * cfg["resize"]), "nclasses": L,
                            "order": cfg["order"], "parallelism": "dp%d" % world,
-                           "l2": "no flush needed: ~6 GB of activations per step >> 126 MB L2",
+                           "l2": "no flush needed: ~6 GB of activations per step >> 50 MB L2",
                            "conv_mode": a.conv_mode + ": " + MODE_TEXT[a.conv_mode],
                            "init": "kaiming, torch.manual_seed(0)",
                            "launch": "one CUDA graph replay per step" if a.graph else "eager launches"},
@@ -713,8 +702,10 @@ def main():
                     help="skip the two labelled extra timings (fp32 FFMA mode, single-pass TF32 mode) reported next to the headline")
     ap.add_argument("--conv-mode", dest="conv_mode", default=os.environ.get("LANEFIT_CONV_MODE", "tf32x3"),
                     choices=["fp32", "tf32", "tf32x3"],
-                    help="tf32x3 = tcgen05 with 3xTF32 operand splits (fp32-grade, default); tf32 = single-pass TF32 on tcgen05 "
-                         "(labelled extra, 1e-3 accuracy); fp32 = CUDA-core FFMA kernels")
+                    help="tf32x3 = tensor cores with 3xTF32 operand splits (fp32-grade, default); tf32 = single-pass TF32 on "
+                         "tensor cores (labelled extra, 1e-3 accuracy); fp32 = CUDA-core FFMA kernels")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss and parameter gradients to DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--max-seconds", dest="max_seconds", type=int, default=int(os.environ.get("LANEFIT_BENCH_MAX_SECONDS", "900")),
                     help="wall-clock watchdog: abort (exit 3, stacks on stderr) instead of hanging the box")
     a = ap.parse_args()

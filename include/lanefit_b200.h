@@ -1,5 +1,5 @@
 /*
- * lanefit_b200.h -- C ABI of the B200-native (sm_100a) hot path of
+ * lanefit_b200.h -- C ABI of the H100-native (sm_90a) hot path of
  * wvangansbeke/LaneDetection_End2End.
  *
  * The reference is pure Python/PyTorch and has NO FFI of its own (SURVEY.md 8b);
@@ -139,7 +139,7 @@ typedef struct LfConvArgs {
 } LfConvArgs;
 int lf_conv_f32(const LfConvArgs* args, lf_stream_t stream);
 
-/* tcgen05 (TF32 in, fp32 accumulate) implementation of the factorised 3-tap convolutions of
+/* Tensor-core (wgmma; TF32 in, fp32 accumulate) implementation of the factorised 3-tap convolutions of
  * non_bottleneck_1d (BP/Networks/ERFNet.py:29-37) and their input gradients, for dense NHWC fp32
  * tensors with C in {64,128} channels in and out:
  *   out[n,y,x,co] = epi( sum_{t<3} sum_ci in[n, y+dy[t], x+dx[t], ci] * wpack[co*3*C + t*C + ci] )
@@ -172,35 +172,29 @@ typedef struct LfConvTcArgs {
 } LfConvTcArgs;
 /* 0 = unsupported shape, else the number of CTA rows of colsum_partial */
 int lf_conv1d_tc_supported(int N, int H, int W, int C);
-/* 3xTF32 variant (csrc/conv_tc_x3.cu): same arguments and epilogue, but `wpack` is the pre-split operand
+/* 3xTF32 variant (csrc/conv_tc.cu): same arguments and epilogue, but `wpack` is the pre-split operand
  * [2][C][3*C] (TF32 hi parts, then lo parts: LF_PACK_TF32_HI / _LO) and every product is formed as
  * a_hi*w_hi + (a_hi*w_lo + a_lo*w_hi) with fp32 accumulation -- results agree with lf_conv_f32 to fp32 round-off
- * (the arithmetic the reference's fp32 Conv2d performs, BP/Networks/ERFNet.py:29-37) while running on tcgen05.
+ * (the arithmetic the reference's fp32 Conv2d performs, BP/Networks/ERFNet.py:29-37) while running on tensor cores.
  * lf_conv1d_tc_x3_rows: 0 if a call with taps {-dil,0,+dil} along y (vertical) or x is not served, else the number of
  * rows of colsum_partial / stats_partial.  Unsupported shapes return LF_ERR_UNSUPPORTED (no fallback inside). */
 int lf_conv1d_tc_x3_rows(int N, int H, int W, int C, int vertical, int dil);
 int lf_conv1d_tc_x3(const LfConvTcArgs* args, lf_stream_t stream);
-/* timing experiments only (tools/x3_ablate.py): bit0 skips the epilogue body, bit2 the in-place a_lo rewrite, bit3 the
- * lo MMAs; outputs are meaningless while bits are set.  0 = normal operation. */
-void lf_conv1d_tc_x3_set_debug(int bits);
 int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream);
 /* 2 (default) = halo-slab kernel (one TMA slab per 32-channel chunk shared by the three taps);
  * 1 = first version (one TMA box per tap).  Same results; process-wide switch for A/B measurements. */
 void lf_conv1d_tc_set_variant(int variant);
-/* timing experiments only (tools/tc_ablate.py): bit0 skips the epilogue body, bit1 skips the TMA loads;
- * outputs are meaningless while bits are set.  0 = normal operation. */
-void lf_conv1d_tc_set_debug(int bits);
 /* 1 if a call with taps {-dil,0,+dil} along y (vertical) or x runs on the slab kernel, i.e. may ask for stats_partial */
 int lf_conv1d_tc_slab_ok(int N, int H, int W, int C, int vertical, int dil);
 
-/* tcgen05 weight gradient of the same 3-tap convolutions:
+/* Tensor-core weight gradient of the same 3-tap convolutions:
  *   partial[cta][t][ci][co] = sum over this CTA's pixel range of x[n,y+dy[t],x+dx[t],ci] * dy[n,y,x,co]
  * nctas = lf_wgrad3_tc_ctas(...) (0 = unsupported shape); finish with
  * lf_wgrad_reduce(partial, nctas, 3, C, C, C, C, dst, st, sp, sq). */
 int lf_wgrad3_tc_ctas(int N, int H, int W, int C);
 int lf_wgrad3_tc(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
                  float* partial, int nctas, lf_stream_t stream);
-/* 3xTF32 variant (csrc/wgrad_tc_x3.cu): same arguments and partial layout; both operands are split into TF32 hi / lo
+/* 3xTF32 variant (csrc/wgrad_tcg.cu): same arguments and partial layout; both operands are split into TF32 hi / lo
  * parts on the fly and every product is x_hi*g_hi + (x_hi*g_lo + x_lo*g_hi), fp32 accumulate -- results agree with
  * lf_wgrad_f32 to fp32 round-off (the weight gradient the reference's autograd forms in fp32). */
 int lf_wgrad3_tc_x3_ctas(int N, int H, int W, int C);
@@ -311,7 +305,7 @@ int lf_outconv_bwd_weight(const float* x, const float* d_out, int N, int H, int 
 
 /* NCHW fp32 image [N,C,H,W] -> NHWC padded to Cpad channels (zeros), the stem's input layout */
 int lf_nchw_to_nhwc_pad(const float* in, int N, int C, int H, int W, int Cpad, float* out, lf_stream_t stream);
-/* tcgen05 gather-GEMM convolution for the resolution-changing layers (csrc/conv_tcg.cu): the 3x3 stride-2
+/* wgmma gather-GEMM convolution for the resolution-changing layers (csrc/conv_tcg.cu): the 3x3 stride-2
  * Conv2d of DownsamplerBlock (BP/Networks/ERFNet.py:15,19-22), the 3x3 stride-2 ConvTranspose2d of UpsamplerBlock
  * (:66-73) and their input gradients, TF32 multiply / fp32 accumulate:
  *   out[n*osn + (oy*oy_mul + oy0)*osy + ox*osx + c] =
@@ -342,7 +336,7 @@ typedef struct LfConvTcgArgs {
 int lf_conv_tcg_supported(int N, int Hs, int Ws, int Kc, int Ng);
 int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream);
 
-/* Weight gradients of the same layers on tcgen05 (csrc/wgrad_tcg.cu), over the same views:
+/* Weight gradients of the same layers on tensor cores (csrc/wgrad_tcg.cu), over the same views:
  *   D[blk*32 + c][n] = sum_{img,y,x} A_{map[blk]}(img, y+dy[blk], x+dx[blk], cblk[blk]*32 + c) * B(img, y, x, n)
  * for blk < nblocks (<= LF_WGRAD_TCG_MAX_BLOCKS), c < 32, n < Nn (multiple of 32, <= 128; ceil(nblocks/4)*Nn <= 512).
  * partial: [nctas][nblocks*32][Nn] per-CTA partial sums (nctas from lf_wgrad_tcg_ctas); reduce with lf_wgrad_reduce

@@ -2,7 +2,7 @@
 same class names, constructor arguments, sub-module / parameter names (so ``state_dict``s
 and ``define_init_weights`` work unchanged) and forward signatures.  The ``nn.Conv2d`` /
 ``nn.BatchNorm2d`` / ``nn.ConvTranspose2d`` children are PARAMETER CONTAINERS only -- their
-own forward is never called; every block runs as one autograd Function over the sm_100a
+own forward is never called; every block runs as one autograd Function over the sm_90a
 kernels (ops_net.py).  Feature maps travel between blocks as NHWC memory viewed with the
 reference's NCHW shape (channels_last), so chaining blocks costs no layout change.
 """

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's ``Networks/LSQ_layer.py`` (BP variant; the BEV
 variant is ``LSQ_layer_bev.py``): same public names, constructor arguments, forward
 signatures, return arities/dtypes and error behaviour, with the device work done by
-the fused sm_100a kernels in csrc/lsq.cu through the C ABI.
+the fused sm_90a kernels in csrc/lsq.cu through the C ABI.
 
   activation_layer        BP/Networks/LSQ_layer.py:27-47
   ProjectiveGridGenerator :50-68
@@ -126,7 +126,7 @@ class Weighted_least_squares(nn.Module):
 class Classification(nn.Module):
     """Line-type / horizon heads on the encoder output (BP/Networks/LSQ_layer.py:157-207; SURVEY.md 8f rank 2).
     The torch modules below only hold the parameters / buffers under the reference's names (``--clas 1`` checkpoints
-    round-trip); ``forward`` runs every stage on the library's kernels through ``ops_heads`` (tcgen05 gather-GEMM
+    round-trip); ``forward`` runs every stage on the library's kernels through ``ops_heads`` (tensor-core gather-GEMM
     convolutions, the ERFNet BatchNorm kernels with eps 1e-5, max / row-mean pooling, HBM-bound fully connected
     layers) -- forward and backward, no torch operator on a feature map."""
 

@@ -1,4 +1,4 @@
-"""lanedetection_end2end_b200 -- B200-native (sm_100a) hot path of
+"""lanedetection_end2end_b200 -- H100-native (sm_90a) hot path of
 wvangansbeke/LaneDetection_End2End: ERFNet encoder/decoder -> per-lane weight maps ->
 differentiable weighted least-squares layer -> loss on the curve coefficients.
 

@@ -117,9 +117,7 @@ _NET_PROTOS = {
     "lf_conv1d_tc_supported": (_i, [_i, _i, _i, _i]),
     "lf_conv1d_tc_x3": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
     "lf_conv1d_tc_x3_rows": (_i, [_i, _i, _i, _i, _i, _i]),
-    "lf_conv1d_tc_x3_set_debug": (None, [_i]),
     "lf_conv1d_tc_set_variant": (None, [_i]),
-    "lf_conv1d_tc_set_debug": (None, [_i]),
     "lf_conv1d_tc_slab_ok": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad3_tc_ctas": (_i, [_i, _i, _i, _i]),
     "lf_wgrad3_tc": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
@@ -246,5 +244,5 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise LanefitError(
-                "lanedetection_end2end_b200 runs on CUDA (sm_100a) only; got a %s tensor. "
+                "lanedetection_end2end_b200 runs on CUDA (sm_90a) only; got a %s tensor. "
                 "There is no CPU fallback by design." % t.device)

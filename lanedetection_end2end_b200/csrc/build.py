@@ -1,4 +1,4 @@
-"""Build liblanefit_b200.so in-tree with nvcc for sm_100a (no torch headers involved).
+"""Build liblanefit_b200.so in-tree with nvcc for sm_90a (H100) (no torch headers involved).
 
     python -m lanedetection_end2end_b200.csrc.build [--force] [--verbose]
 """
@@ -11,7 +11,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(os.path.dirname(HERE), "liblanefit_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -42,7 +42,7 @@ def build(force=False, verbose=False):
         res = list(ex.map(compile_one, srcs))
     objs = [o for o, _ in res]
     if force or any(c for _, c in res) or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -1,5 +1,5 @@
 // Generic NHWC fp32 implicit-GEMM convolution on CUDA cores ("parity mode": fp32-exact,
-// used for every layer shape; the tcgen05 kernels in conv_tc.cu take over the dense
+// used for every layer shape; the tensor-core kernels in conv_tc.cu take over the dense
 // 1-D convolutions in fast mode).
 //
 // One launch computes, for an output sub-grid ("phase") enumerated as (n, j < Hs, i < Ws):

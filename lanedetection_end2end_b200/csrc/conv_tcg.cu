@@ -1,6 +1,6 @@
-// tcgen05 "gather-GEMM" convolution for ERFNet's resolution-changing layers: the 3x3 stride-2 Conv2d of
+// Hopper (sm_90a) wgmma "gather-GEMM" convolution for ERFNet's resolution-changing layers: the 3x3 stride-2 Conv2d of
 // DownsamplerBlock (BP/Networks/ERFNet.py:15,19-22), the 3x3 stride-2 ConvTranspose2d of UpsamplerBlock
-// (:66-73) and the input gradients of both.  TF32 multiply / fp32 accumulate, fp32 NHWC storage.
+// (:66-73) and the input gradients of both.  fp32 NHWC storage, fp32 accumulate.
 //
 //   out[n, oy*oy_mul + oy0, ox, c] = bias[c] + sum_{t<ntaps} sum_{k<Kc} A_{map[t]}[n, oy+dy[t], ox+dx[t], k] * Wg[c][t*Kc + k]
 //
@@ -12,15 +12,13 @@
 //     Kc = 2*Cin, weights zero where a (pair offset, half) combination is not a kernel column;
 //   * stride-2 transposed conv (Up forward, Down input-gradient): one launch per output row parity
 //     (2 or 4 taps over the un-strided input), Ng = 2*Cout = both output columns of the pair.
-// Structure = conv_tc_v1.cu (one TMA box [128 px x 32 ch] per tap and 32-channel chunk, OOB zero fill = conv
-// padding, mbarrier ring, warp-specialised, accumulators double-buffered in TMEM) except that the weight
-// chunk [Ng x 32] streams through the ring next to its activation box (the weight matrices of these
-// layers, up to 393 KB, do not fit in shared memory) and Ng is a run-time multiple of 16 (<= 128).
-//
-// precision 1 (3xTF32, template X3; see conv_tc_x3.cu for the arithmetic): the weight chunk is the pre-split pair
-// [W_hi rows | W_lo rows] (one TMA box of 2*Ng rows = ONE UMMA operand of N = 2*Ng), pass 1 = A_hi * [W_hi | W_lo]^T
-// into TMEM columns [0,Ng) | [Ng,2Ng); when it has completed two split warps rewrite the activation box in place with
-// A_lo, and pass 2 = A_lo * W_hi^T accumulates into [Ng,2Ng) one stage later.  The epilogue adds the two ranges.
+// One TMA box [128 px x 32 ch] per tap and 32-channel chunk (OOB zero fill = conv padding) and the weight chunk
+// [Ng x 32] next to it stream through an mbarrier ring (the weight matrices of these layers, up to 393 KB, do not fit in
+// shared memory); Ng is a run-time multiple of 16 (<= 128), covered by wgmma m64n16k8 column blocks.
+// Two consumer warpgroups own 64 pixel rows each (A fragments loaded from the swizzled box into registers, B through a
+// shared-memory descriptor), accumulate in registers and store the tile with bias / ReLU; warp 8 is the TMA producer.
+// precision 1 (3xTF32, template X3; arithmetic in tc_ptx.cuh): the weight chunk is the pre-split pair [W_hi rows | W_lo
+// rows] (one TMA box of 2*Ng rows); a_hi*w_hi accumulates apart from a_hi*w_lo + a_lo*w_hi and the two are added at the end.
 #include <cuda.h>
 
 #include "lf_common.cuh"
@@ -28,13 +26,13 @@
 
 namespace lf {
 
-constexpr int TG_THREADS = 192;       // producer, MMA issuer, 4 epilogue warps
-constexpr int TG_THREADS_X3 = 256;    // + 2 split warps (warps 2, 3)
+constexpr int TG_THREADS = 288;
 constexpr int TG_BM = 128;
 constexpr int TG_A_BYTES = TG_BM * 128;  // 16 KB
 constexpr int TG_MAX_STAGES = 8;
 constexpr int TG_MAXT = LF_TCG_MAX_TAPS;
-constexpr int TG_SMEM_LIMIT = 226 * 1024;
+constexpr int TG_SMEM_LIMIT = 227 * 1024;
+constexpr int TG_NB = 8;                 // column blocks of 16 (Ng <= 128)
 
 struct TgArgs {
     float* out;
@@ -47,37 +45,18 @@ struct TgArgs {
     int kchunks, Ng, ntaps;
     int map[TG_MAXT], dy[TG_MAXT], dx[TG_MAXT];
     int stages, stage_bytes;
-    uint32_t idesc;       // pass 1: N = Ng (TF32) or 2*Ng (3xTF32)
-    uint32_t idesc_lo;    // 3xTF32 pass 2: N = Ng
     int total_tiles;
 };
 
-__device__ __forceinline__ uint64_t tg_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ __forceinline__ float tg_lo(float a) {   // tf32(a - trunc_tf32(a)), see conv_tc_x3.cu
-    const float r = a - __uint_as_float(__float_as_uint(a) & 0xffffe000u);
-    return __uint_as_float((__float_as_uint(r) + 0x1000u) & 0xffffe000u);
-}
-
 template <bool X3>
-__global__ void __launch_bounds__(X3 ? TG_THREADS_X3 : TG_THREADS, 1)
+__global__ void __launch_bounds__(TG_THREADS, 1)
 conv_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB, const TgArgs a) {
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)a.stages * a.stage_bytes);
-    uint64_t* full = bars;                       // [TG_MAX_STAGES]
-    uint64_t* empty = bars + TG_MAX_STAGES;      // [TG_MAX_STAGES]
-    uint64_t* tfull = bars + 2 * TG_MAX_STAGES;  // [2]
-    uint64_t* tempty = tfull + 2;                // [2]
-    uint64_t* hdone = tempty + 2;                // [TG_MAX_STAGES] X3: pass 1 done, the A box may be rewritten
-    uint64_t* lordy = hdone + TG_MAX_STAGES;     // [TG_MAX_STAGES] X3: A_lo written
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(lordy + TG_MAX_STAGES);
-    constexpr int EPI_W0 = X3 ? 4 : 2;           // first epilogue warp
-    constexpr int BUF_COLS = X3 ? 256 : 128;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)a.stages * a.stage_bytes);
+    uint64_t* empty = full + TG_MAX_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_x = a.Ws / a.bx, tiles_y = a.Hs / a.by;
@@ -88,24 +67,14 @@ conv_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < a.stages; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-            mbar_init(&hdone[s], 1);
-            mbar_init(&lordy[s], 2);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&tfull[b], 1);
-            mbar_init(&tempty[b], 4);  // one arrive per epilogue warp
+            mbar_init(&empty[s], 8);   // one arrive per consumer warp
         }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 2 * BUF_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();   // everything above overlapped the previous kernel's tail; global memory is touched only from here on
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer (converged warp, elected lane issues) =================
         const bool leader = elect_one();
         int stage = 0;
@@ -132,142 +101,107 @@ conv_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer (converged warp, elected lane issues) =================
-        const bool leader = elect_one();
-        const int ksteps = a.ntaps * a.kchunks;
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        // X3: pass 2 (A_lo * W_hi) of the previous stage, issued one stage late
-        bool p_valid = false, p_last = false;
-        int p_stage = 0, p_buf = 0;
-        uint32_t p_phase = 0, p_dtmem = 0;
-        auto pass2 = [&]() {
-            mbar_wait(&lordy[p_stage], p_phase);
-            tc_fence_after();
-            const uint32_t st = smem_u32(smem + (size_t)p_stage * a.stage_bytes);
-            const uint64_t adesc = tg_desc_sw128(st);
-            const uint64_t bdesc = tg_desc_sw128(st + TG_A_BYTES);
+        return;
+    }
+
+    // ================= consumers: warpgroup wg owns pixel rows [64 wg, 64 wg + 64) =================
+    const int wg = warp >> 2, wl = warp & 3;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int ra = 64 * wg + 16 * wl + g;   // fragment rows ra, ra + 8
+    const int nblk = a.Ng >> 4;
+    const int ksteps = a.ntaps * a.kchunks;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int mt = blockIdx.x; mt < a.total_tiles; mt += gridDim.x) {
+        float acc[TG_NB][8], acs[TG_NB][8];
 #pragma unroll
-            for (int k8 = 0; k8 < 4; ++k8)
-                if (leader) umma_tf32(p_dtmem + a.Ng, adesc + 2 * k8, bdesc + 2 * k8, a.idesc_lo, 1u);
-            if (leader) {
-                umma_commit(&empty[p_stage]);
-                if (p_last) umma_commit(&tfull[p_buf]);
-            }
-        };
-        for (int mt = blockIdx.x; mt < a.total_tiles; mt += gridDim.x, ++it) {
-            const int buf = it & 1;
-            const uint32_t use_parity = (it >> 1) & 1;
-            mbar_wait(&tempty[buf], use_parity ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + buf * BUF_COLS;
-            for (int ks = 0; ks < ksteps; ++ks) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint32_t st = smem_u32(smem + (size_t)stage * a.stage_bytes);
-                const uint64_t adesc = tg_desc_sw128(st);
-                const uint64_t bdesc = tg_desc_sw128(st + TG_A_BYTES);
+        for (int j = 0; j < TG_NB; ++j)
 #pragma unroll
-                for (int k8 = 0; k8 < 4; ++k8)  // 8 tf32 = 32 bytes per MMA
-                    if (leader) umma_tf32(d_tmem, adesc + 2 * k8, bdesc + 2 * k8, a.idesc, (ks | k8) != 0 ? 1u : 0u);
-                if (X3) {
-                    if (leader) umma_commit(&hdone[stage]);
-                    if (p_valid) pass2();
-                    p_valid = true;
-                    p_stage = stage; p_phase = phase; p_buf = buf; p_dtmem = d_tmem;
-                    p_last = (ks == ksteps - 1);
-                } else {
-                    if (leader) umma_commit(&empty[stage]);
-                }
-                if (++stage == a.stages) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            if (!X3 && leader) umma_commit(&tfull[buf]);
-        }
-        if (X3 && p_valid) pass2();
-    } else if (X3 && warp < EPI_W0) {
-        // ================= split warps (X3): A box <- A_lo in place once pass 1 has read it =================
-        const int tid = threadIdx.x - 64;
-        const int ksteps = a.ntaps * a.kchunks;
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int mt = blockIdx.x; mt < a.total_tiles; mt += gridDim.x) {
-            for (int ks = 0; ks < ksteps; ++ks) {
-                mbar_wait(&full[stage], phase);
-                mbar_wait(&hdone[stage], phase);
-                float4* p = reinterpret_cast<float4*>(smem + (size_t)stage * a.stage_bytes);
-#pragma unroll 4
-                for (int i = tid; i < TG_A_BYTES / 16; i += 64) {
-                    float4 v = p[i];
-                    v.x = tg_lo(v.x); v.y = tg_lo(v.y); v.z = tg_lo(v.z); v.w = tg_lo(v.w);
-                    p[i] = v;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&lordy[stage]);
-                if (++stage == a.stages) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-        }
-    } else {
-        // ================= epilogue (warps 2..5): thread = pixel row of the tile =================
-        const int lane_base = (warp & 3) * 32;
-        const int m = lane_base + lane;
-        const int yy = m / a.bx, xx = m - yy * a.bx;
-        int it = 0;
-        for (int mt = blockIdx.x; mt < a.total_tiles; mt += gridDim.x, ++it) {
-            const int buf = it & 1;
-            const uint32_t use_parity = (it >> 1) & 1;
-            const int tx = mt % tiles_x;
-            const int ty = (mt / tiles_x) % tiles_y;
-            const int n = mt / (tiles_x * tiles_y);
-            float* orow = a.out + (size_t)n * a.osn + (size_t)((ty * a.by + yy) * a.oy_mul + a.oy0) * a.osy +
-                          (size_t)(tx * a.bx + xx) * a.osx;
-            mbar_wait(&tfull[buf], use_parity);
-            tc_fence_after();
-            for (int c0 = 0; c0 < a.Ng; c0 += 16) {
-                uint32_t v[16];
-                const uint32_t taddr = tmem_base + ((uint32_t)lane_base << 16) + buf * BUF_COLS + c0;
-                tmem_ld16(taddr, v);
-                if (X3) {
-                    uint32_t sm[16];
-                    tmem_ld16(taddr + a.Ng, sm);
-                    tmem_ld_wait();
+            for (int i = 0; i < 8; ++i) acc[j][i] = acs[j][i] = 0.f;
+        for (int ks = 0; ks < ksteps; ++ks) {
+            mbar_wait(&full[stage], phase);
+            const uint8_t* st = smem + (size_t)stage * a.stage_bytes;
+            uint32_t ah[4][4], al[4][4];
 #pragma unroll
-                    for (int q = 0; q < 16; ++q) v[q] = __float_as_uint(__uint_as_float(sm[q]) + __uint_as_float(v[q]));
-                } else {
-                    tmem_ld_wait();
-                }
+            for (int k8 = 0; k8 < 4; ++k8) {
+                const int c = 8 * k8 + t4;
+                const float v[4] = {*reinterpret_cast<const float*>(st + sw128_off(ra, c)),
+                                    *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c)),
+                                    *reinterpret_cast<const float*>(st + sw128_off(ra, c + 4)),
+                                    *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c + 4))};
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
-                    float4 o = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]),
-                                           __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3]));
-                    if (a.bias) {
-                        const float4 b = __ldg(reinterpret_cast<const float4*>(a.bias + c0 + 4 * q));
-                        o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
+                    if (X3) {
+                        tf32_split(v[q], ah[k8][q], al[k8][q]);
+                    } else {
+                        ah[k8][q] = tf32_rna(v[q]);
                     }
-                    if (a.relu) {
-                        o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-                    }
-                    *reinterpret_cast<float4*>(orow + c0 + 4 * q) = o;
                 }
             }
-            tc_fence_before();
+            const uint64_t bd = wgmma_desc_sw128(smem_u32(st + TG_A_BYTES));
+            const uint64_t lo_rows = (uint64_t)(a.Ng * 128) >> 4;   // W_lo rows follow the Ng W_hi rows
+            // One column block at a time: its 32 products are summed by the tensor core from zero and added to the running
+            // fp32 sum with a rounded FADD (the tensor core's own accumulation does not round like IEEE adds, see conv_tc.cu).
+#pragma unroll
+            for (int j = 0; j < TG_NB; ++j) {
+                if (j < nblk) {
+                    const uint64_t bj = bd + (uint64_t)((j * 16 * 128) >> 4);
+                    float part[8];
+                    wgmma_fence();
+#pragma unroll
+                    for (int k8 = 0; k8 < 4; ++k8) {
+                        wgmma_m64n16k8_tf32(part, ah[k8], bj + 2 * k8, k8);   // k8 = 0: part = product
+                        if (X3) {
+                            wgmma_m64n16k8_tf32(acs[j], ah[k8], bj + lo_rows + 2 * k8, 1);   // a_hi * w_lo
+                            wgmma_m64n16k8_tf32(acs[j], al[k8], bj + 2 * k8, 1);             // a_lo * w_hi
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait0();
+                    reg_fence(part);
+                    if (X3) reg_fence(acs[j]);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) acc[j][i] += part[i];
+                }
+            }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[buf]);
+            if (lane == 0) mbar_arrive(&empty[stage]);
+            if (++stage == a.stages) {
+                stage = 0;
+                phase ^= 1;
+            }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 2 * BUF_COLS);
+        // epilogue: this thread holds rows ra, ra + 8 and columns 16 j + 8 h + 2 t4 (+1)
+        const int tx = mt % tiles_x;
+        const int ty = (mt / tiles_x) % tiles_y;
+        const int n = mt / (tiles_x * tiles_y);
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+            const int m = ra + 8 * rh;
+            const int yy = m / a.bx, xx = m - yy * a.bx;
+            float* orow = a.out + (size_t)n * a.osn + (size_t)((ty * a.by + yy) * a.oy_mul + a.oy0) * a.osy +
+                          (size_t)(tx * a.bx + xx) * a.osx;
+#pragma unroll
+            for (int j = 0; j < TG_NB; ++j) {
+                if (j < nblk) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i = 4 * h + 2 * rh;
+                        const int c = 16 * j + 8 * h + 2 * t4;
+                        float2 o = X3 ? make_float2(acs[j][i] + acc[j][i], acs[j][i + 1] + acc[j][i + 1])
+                                      : make_float2(acc[j][i], acc[j][i + 1]);
+                        if (a.bias) {
+                            const float2 b = __ldg(reinterpret_cast<const float2*>(a.bias + c));
+                            o.x += b.x; o.y += b.y;
+                        }
+                        if (a.relu) {
+                            o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f);
+                        }
+                        *reinterpret_cast<float2*>(orow + c) = o;
+                    }
+                }
+            }
+        }
     }
 }
 
@@ -330,11 +264,9 @@ extern "C" int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream_) {
     const bool x3 = p.precision == 1;
     const int nb = x3 ? 2 * p.Ng : p.Ng;   // rows of the weight chunk: W, or W_hi | W_lo
     a.stage_bytes = TG_A_BYTES + nb * 128;
-    int stages = (TG_SMEM_LIMIT - 1024 - 512) / a.stage_bytes;
+    int stages = (TG_SMEM_LIMIT - 1024 - 256) / a.stage_bytes;
     if (stages > TG_MAX_STAGES) stages = TG_MAX_STAGES;
     a.stages = stages;
-    a.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(nb >> 3) << 17) | ((uint32_t)(TG_BM >> 4) << 24);
-    a.idesc_lo = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.Ng >> 3) << 17) | ((uint32_t)(TG_BM >> 4) << 24);
     a.total_tiles = p.N * (p.Hs / a.by) * (p.Ws / a.bx);
 
     CUtensorMap tmA0, tmA1, tmB;
@@ -352,15 +284,13 @@ extern "C" int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream_) {
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-    const int smem_bytes = 1024 + a.stages * a.stage_bytes + 512;
+    const int smem_bytes = 1024 + a.stages * a.stage_bytes + 256;
     cudaError_t e = x3 ? cudaFuncSetAttribute(conv_tcg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM_LIMIT)
                        : cudaFuncSetAttribute(conv_tcg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM_LIMIT);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
-    if (x3) lf_launch(conv_tcg_kernel<true>, grid, TG_THREADS_X3, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    if (x3) lf_launch(conv_tcg_kernel<true>, grid, TG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
     else lf_launch(conv_tcg_kernel<false>, grid, TG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
     return check_launch();
 }

@@ -75,7 +75,8 @@ extern "C" int lf_frame_preprocess(const unsigned char* frames, int N, int Hin, 
     LF_REQUIRE(frames && xb && xk && yb && yk && out && N >= 1 && Ho >= 1 && Wo >= 1 && kx >= 1 && ky >= 1);
     LF_REQUIRE(crop_y0 >= 0 && crop_rows >= 1 && crop_y0 + crop_rows <= Hin && (layout == 0 || layout == 1));
     const long long total = (long long)N * Ho * Wo;
-    const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const long long cap = (long long)device_sms() * 16;
+    const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
     lf_launch(frame_preprocess_kernel, grid, 256, 0, stream, (const uint8_t*)frames, N, Hin, Win, crop_y0, xb, xk, kx, yb, yk, ky, Ho, Wo,
               (const uint8_t*)flip, layout, out);
     return check_launch();

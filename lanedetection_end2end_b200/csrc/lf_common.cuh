@@ -1,4 +1,4 @@
-// Shared helpers for the lanefit_b200 kernels (sm_100a only).
+// Shared helpers for the lanefit_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -23,13 +23,12 @@ inline int check_launch() {
 
 // ---------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  Every kernel of the library is launched through lf_launch(); with the switch on
-// (lf_set_pdl(1) / LANEFIT_PDL=1; DEFAULT OFF -- measured on the B200, session 8: 16.707 ms per step with it, 16.740 ms
-// without, inside the run-to-run noise: the whole step already replays as one CUDA graph, and a tcgen05 kernel's CTA
-// (200+ KB of shared memory) cannot become resident next to its predecessor's, so there is no prologue to overlap; the
-// mechanism stays because it is free when off and validated when on: full GPU suite + compute-sanitizer with it on)
+// (lf_set_pdl(1) / LANEFIT_PDL=1; DEFAULT OFF: the whole step already replays as one CUDA graph, and a tensor-core kernel's CTA (up to 227 KB of shared
+// memory) cannot become resident next to its predecessor's, so there is little prologue to overlap; the gain with it on
+// is not measured on the H100)
 // the launch carries cudaLaunchAttributeProgrammaticStreamSerialization, so the
 // grid may be scheduled while its predecessor in the stream is still draining: its launch latency and on-chip prologue
-// (barrier init, TMEM allocation, descriptor prefetch) overlap the predecessor's tail instead of following it.  The
+// (barrier init, descriptor prefetch) overlap the predecessor's tail instead of following it.  The
 // contract every kernel keeps: pdl_trigger() first (dependents may be scheduled once ALL CTAs of this grid are
 // resident -- so a waiting dependent can never starve CTAs of this grid that have not started), and pdl_wait() before
 // the first global-memory access (reads of the predecessor's results AND writes: the allocator may hand a buffer the
@@ -39,6 +38,18 @@ inline int check_launch() {
 // kernel otherwise (CUDA graph replay included).
 // ---------------------------------------------------------------------------------
 bool pdl_enabled();
+
+// SMs of the current device; launch sizes follow it (132 on an H100 SXM).  The fallback serves host-side sizing queries
+// on a machine without a device, where nothing is launched.
+inline int device_sms() {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0) {
+        cudaGetLastError();
+        return 132;
+    }
+    return sms;
+}
 
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -78,8 +89,7 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
-// Packed fp32 pairs (sm_100: FMUL2 / FADD2 / FFMA2 process two IEEE fp32 lanes per instruction; each lane is rounded
-// exactly like the scalar op).  Used where a bandwidth kernel is issue-bound on per-element fp32 math (lsq.cu).
+// Packed fp32 pairs: two IEEE fp32 lanes in one 64-bit value, each lane rounded exactly like the scalar op (lsq.cu).
 typedef unsigned long long f32x2_t;
 __device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) {
     f32x2_t r;
@@ -88,19 +98,23 @@ __device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) {
 }
 __device__ __forceinline__ void f2_unpack(f32x2_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 __device__ __forceinline__ f32x2_t f2_mul(f32x2_t a, f32x2_t b) {
-    f32x2_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2_t f2_add(f32x2_t a, f32x2_t b) {
-    f32x2_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2_t f2_fma(f32x2_t a, f32x2_t b, f32x2_t c) {
-    f32x2_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    f2_unpack(c, c0, c1);
+    return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 // streaming 128-bit load (read once, do not pollute L1)

@@ -287,7 +287,8 @@ extern "C" int lf_rowmean_bwd(const float* dout, int B, int H, int W, int C, flo
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     LF_REQUIRE(dout && dx && B >= 1 && H >= 1 && W >= 1 && C >= 1);
     const long long total = (long long)B * H * W * C;
-    const int grid = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+    const long long cap = (long long)device_sms() * 8;
+    const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
     lf_launch(rowmean_bwd_kernel, grid, 256, 0, stream, dout, H, W, C, total, dx);
     return check_launch();
 }

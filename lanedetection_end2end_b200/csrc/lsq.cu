@@ -1,4 +1,4 @@
-// Fused weighted least-squares layer for sm_100a:  activation -> row mask ->
+// Fused weighted least-squares layer for sm_90a:  activation -> row mask ->
 // moments of (m*a(o))^2 over the BEV meshgrid -> (order+1)x(order+1) solve, and its
 // closed-form backward.  Replaces BP/Networks/LSQ_layer.py:19-20,27-47,85-154,237-238,
 // 295,301 and BP/Networks/gels.py:9-25 of the reference (see include/lanefit_b200.h).
@@ -374,7 +374,7 @@ __device__ __forceinline__ int packed_holder(int i) {
 // Forward, row-separable fast path.  grid = (nchunks, B, ceil(L/4)), 256 threads.
 // ---------------------------------------------------------------------------------
 // NL = lanes per CTA (compile time, so the loads of all lanes and column steps of a row are in flight
-// together: the kernel is latency-bound otherwise -- ncu: long_scoreboard stalls, profiles/r01).
+// together: the kernel is latency-bound otherwise -- long-scoreboard stalls).
 template <int ACT_T, bool BF16, int NL>
 __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_kernel(const LsqArgs a) {
     pdl_entry();
@@ -440,9 +440,8 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
                     float o[V];
                     load_mapv<BF16>(a.o, off, o);
                     float sa = 0.f, sb = 0.f;
-                    // (packed fp32 pairs -- FMUL2 / FADD2 / FFMA2 -- were tried here in round 2: fewer instructions but more live
-                    // registers; the forward got SLOWER at 128 registers / thread (bf16 L=4: 0.36 -> 0.31 of the copy bandwidth,
-                    // profiles/r02/lsq_stress_s10.jsonl).  The backward kernel keeps them: bit-identical there, +15 % on bf16.)
+                    // (the backward kernel writes its math with the f2_* pair helpers of lf_common.cuh; on sm_90a they are
+                    // two scalar ops each, rounded identically)
 #pragma unroll
                     for (int e = 0; e < V; ++e) {
                         o[e] = act_fn<ACT_T>(o[e], a.act);
@@ -666,9 +665,7 @@ __global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_kernel(const LsqA
 // per SM (the tail wave of a 1.7-wave grid cost 15 % in round 1), at least one row per warp and chunk, and few enough
 // chunks that the per-CTA tail (block reduction, fence, ticket) stays small.
 static int pick_nchunks(int B, int groups, int H, int mask_rows, int ctas_per_sm) {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     const long long slots = (long long)sms * ctas_per_sm, units = (long long)B * groups;
     const int ha = H - mask_rows > 0 ? H - mask_rows : 1;
     const int n_max = ha / LSQ_WARPS > 1 ? ha / LSQ_WARPS : 1;          // >= 8 unmasked rows per chunk

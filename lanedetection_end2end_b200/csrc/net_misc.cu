@@ -1,4 +1,4 @@
-// Bandwidth-bound ERFNet pieces for sm_100a: BatchNorm2d (training statistics, apply,
+// Bandwidth-bound ERFNet pieces for sm_90a: BatchNorm2d (training statistics, apply,
 // backward), 2x2 max pooling into a channel slice, the 16->L output ConvTranspose2d and the
 // module-boundary layout changes.  All NHWC fp32, 128-bit accesses, deterministic two-stage
 // reductions (fp64 partials, fixed summation order).
@@ -9,7 +9,7 @@
 namespace lf {
 
 constexpr int BN_THREADS = 256;
-constexpr int BN_MAX_BLOCKS = 148 * 4;
+static inline int bn_max_blocks() { return device_sms() * 4; }
 constexpr int BN_MIN_PIX_PER_BLOCK = 128;
 
 __device__ __forceinline__ float gate(float v, float m) { return m > 0.f ? v : 0.f; }
@@ -469,7 +469,8 @@ __global__ void batched_transpose_kernel(const float* __restrict__ in, int R, in
     }
 }
 
-static inline int grid_for(long long n, int threads, int maxblocks = 148 * 16) {
+static inline int grid_for(long long n, int threads, int maxblocks = 0) {
+    if (maxblocks <= 0) maxblocks = device_sms() * 16;
     long long b = (n + threads - 1) / threads;
     if (b > maxblocks) b = maxblocks;
     if (b < 1) b = 1;
@@ -484,7 +485,7 @@ using namespace lf;
 extern "C" int lf_bn_blocks(long long npix, int C) {
     (void)C;
     long long b = (npix + BN_MIN_PIX_PER_BLOCK - 1) / BN_MIN_PIX_PER_BLOCK;
-    if (b > BN_MAX_BLOCKS) b = BN_MAX_BLOCKS;
+    if (b > bn_max_blocks()) b = bn_max_blocks();
     return (int)(b < 1 ? 1 : b);
 }
 
@@ -678,7 +679,7 @@ __global__ void __launch_bounds__(256) pack_gather_kernel(const PackJob* __restr
         const int i = __ldg(j.idx + k);
         float v = i >= 0 ? __ldg(j.src + (i & LF_PACK_INDEX_MASK)) : 0.f;
         if (i >= 0 && (i & (LF_PACK_TF32_HI | LF_PACK_TF32_LO))) {
-            // 3xTF32 operand split (conv_tc_x3.cu): hi = TF32 round-to-nearest of v, lo = TF32 rounding of v - hi; both
+            // 3xTF32 operand split (conv_tc.cu): hi = TF32 round-to-nearest of v, lo = TF32 rounding of v - hi; both
             // have their 13 low mantissa bits cleared, so the tensor core's own fp32 -> TF32 conversion is the identity
             const float hi = __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u);
             v = (i & LF_PACK_TF32_HI) ? hi : __uint_as_float((__float_as_uint(v - hi) + 0x1000u) & 0xffffe000u);

@@ -117,7 +117,8 @@ __global__ void ce2d_finalize_kernel(const double* __restrict__ partial, int nbl
 
 static int seg_blocks(long long total) {
     const long long b = (total + SEG_THREADS - 1) / SEG_THREADS;
-    return (int)(b < 148 * 8 ? (b < 1 ? 1 : b) : 148 * 8);
+    const long long cap = (long long)device_sms() * 8;
+    return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
 }  // namespace lf

@@ -1,4 +1,5 @@
-// Shared tcgen05 / TMA / mbarrier PTX wrappers and tensor-map helpers (sm_100a).
+// Shared Hopper (sm_90a) tensor-core PTX wrappers: TMA, mbarrier, wgmma, mma.sync, TF32 operand splitting and the
+// tensor-map helpers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -31,22 +32,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "r"(addr), "r"(parity)
             : "memory");
         if (done) break;
-        if (++spins > TC_SPIN_LIMIT) __trap();  // never hang the GPU on a protocol bug
+        if (++spins > TC_SPIN_LIMIT) __trap();  // a protocol bug ends the kernel with an error instead of hanging the GPU
     }
 }
-// One lane of a CONVERGED warp (elect.sync).  The tcgen05 / TMA issuing warps run their loops with all 32 lanes so
-// that descriptors, coordinates and barrier addresses are warp-uniform values (uniform registers); only the issuing
-// instruction itself is predicated on the elected lane.  Running the whole loop under `if (lane == 0)` instead makes
-// every UTCHMMA / UTMALDG operand a per-thread value that the compiler moves into uniform registers with an
-// ELECT + 5x R2UR + branch "waterfall" per instruction (~17 extra instructions per MMA).
+// One lane of a converged warp: the TMA issuing warp runs its loop with all 32 lanes so that coordinates and barrier
+// addresses stay warp-uniform; only the issuing instruction is predicated on the elected lane.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, uint64_t* bar, void* dst, int c0, int c1) {
     asm volatile(
@@ -66,40 +62,82 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* tm, uint64_t* bar
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------------------------------
+// TF32 operands.  Every product the tensor core forms here takes operands that are exact TF32 values (low 13 mantissa
+// bits zero), so the result does not depend on how the hardware would round an fp32 bit pattern.
+// 3xTF32: a = hi + lo with hi = tf32_rna(a) and lo = tf32_rna(a - hi) (a - hi is exact); a*w = hi*w_hi + (hi*w_lo +
+// lo*w_hi) up to O(2^-22 |a||w|), below the fp32 rounding of the sum.
+// ------------------------------------------------------------------------------------------
+// round-to-nearest (ties away) to TF32 with the dropped bits cleared
+__device__ __forceinline__ uint32_t tf32_rna(float a) { return (__float_as_uint(a) + 0x1000u) & 0xffffe000u; }
+__device__ __forceinline__ void tf32_split(float a, uint32_t& hi, uint32_t& lo) {
+    hi = tf32_rna(a);
+    lo = tf32_rna(a - __uint_as_float(hi));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, TF32 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "[%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
+// Element (row r, column c < 32) of a [rows x 32] fp32 tile that TMA wrote with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128
+// bytes, the 16-byte chunk index XORed with r & 7.  Byte offset from the tile base.
+__device__ __forceinline__ uint32_t sw128_off(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 2) ^ r) & 7) << 4) + ((c & 3) << 2)); }
+
+// ------------------------------------------------------------------------------------------
+// wgmma (warpgroup MMA).  B operand: K-major, 128B-swizzled tile in shared memory (rows of 32 fp32 = 128 bytes, 8-row
+// groups 1024 bytes apart) = exactly what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B.  Descriptor: start >> 4 (bits 0-13),
+// LBO >> 4 (16-29; unused for swizzled K-major), SBO >> 4 (32-45), layout 1 = SWIZZLE_128B (bits 62-63).  The tile base
+// must be 1024-byte aligned; the k-th group of 8 TF32 along K starts 32*k bytes later (+2 in the start field).
+// A operand: registers, the m64k8 TF32 fragment of this thread:
+//   a[0] = A[16w + g][t], a[1] = A[16w + g + 8][t], a[2] = A[16w + g][t + 4], a[3] = A[16w + g + 8][t + 4]
+// (w = warp within the warpgroup, g = lane / 4, t = lane % 4).  Accumulator fragment of m64nN, register i:
+//   row 16w + g + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2t + (i & 1).
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from touching accumulator registers across an asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 64] (+)= A[64 x 8] * B[64 x 8]^T, TF32 in, fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 16] (+)= A[64 x 8] * B[16 x 8]^T
+__device__ __forceinline__ void wgmma_m64n16k8_tf32(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+
+// mma.sync m16n8k8 TF32 (warp-level): a as for wgmma within one warp's 16 rows; b[0] = B[k = t][n = g], b[1] = B[t + 4][g];
+// d[i]: row g + 8 * (i >> 1), column 2t + (i & 1).
+__device__ __forceinline__ void mma_m16n8k8_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
 
 // ------------------------------------------------------------------------------------------
 // host: cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link)
@@ -122,17 +160,18 @@ inline TcEncodeTiledFn tc_get_encode_fn() {
     return fn;
 }
 
-// dense NHWC fp32 activations [N,H,W,C] viewed as (ci:32, cblk:C/32, x:W, y:H, n:N); one box =
+// Strided fp32 view (element strides sx, sy, sn; channels contiguous) as (ci:32, cblk:C/32, x:W, y:H, n:N); one box =
 // [bx*by pixels] x [32 channels] = rows of 128 bytes, 128B-swizzled; out-of-bounds -> zeros
-inline bool tc_encode_nhwc_map(TcEncodeTiledFn enc, CUtensorMap* tm, const float* base, int N, int H, int W, int C, int bx,
-                               int by, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+inline bool tc_encode_view(TcEncodeTiledFn enc, CUtensorMap* tm, const float* base, int N, int H, int W, int C, long long sx,
+                           long long sy, long long sn, int bx, int by) {
     cuuint64_t dims[5] = {32, (cuuint64_t)(C / 32), (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t strides[4] = {128, (cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
+    cuuint64_t strides[4] = {128, (cuuint64_t)sx * 4, (cuuint64_t)sy * 4, (cuuint64_t)sn * 4};
     cuuint32_t box[5] = {32, 1, (cuuint32_t)bx, (cuuint32_t)by, 1};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+
 
 }  // namespace lf

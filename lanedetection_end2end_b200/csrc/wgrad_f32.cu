@@ -507,7 +507,7 @@ __global__ void vec_reduce_kernel(const float* __restrict__ partial, int nsplit,
 }
 
 constexpr int COLSUM_THREADS = 256;
-constexpr int COLSUM_MAX_BLOCKS = 148 * 4;
+static inline int colsum_max_blocks() { return device_sms() * 4; }
 constexpr int COLSUM_MIN_PIX = 128;
 
 // partial[blk][c] = sum over the block's pixel range of src[p*cstride + coff + c].
@@ -590,9 +590,7 @@ extern "C" int lf_wgrad_f32_nsplit(const LfWgradArgs* args) {
     if (!args) return 0;
     WsPlan wsp;
     if (!ws_make_plan(*args, &wsp)) return 0;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     const long long M = (long long)args->N * args->Hs * args->Ws;
     long long n = 2LL * sms;
     const long long max_split = (M + 4LL * wsp.PXS - 1) / (4LL * wsp.PXS);   // at least 4 steps per CTA
@@ -640,7 +638,7 @@ extern "C" int lf_vec_reduce(const float* partial, int nsplit, int C, int Cpad, 
 
 extern "C" int lf_colsum_blocks(long long npix) {
     long long b = (npix + COLSUM_MIN_PIX - 1) / COLSUM_MIN_PIX;
-    if (b > COLSUM_MAX_BLOCKS) b = COLSUM_MAX_BLOCKS;
+    if (b > colsum_max_blocks()) b = colsum_max_blocks();
     return (int)(b < 1 ? 1 : b);
 }
 

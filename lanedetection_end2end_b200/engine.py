@@ -15,7 +15,7 @@ import os
 import torch
 
 # lf_backproj_loss: one launch for the loss of all lanes + its gradient instead of ~40 tiny float64 torch launches.
-# GPU-validated (tests/test_net_gpu.py::test_fused_backprojection_loss_kernel, profiles/r02): on by default;
+# GPU-validated (tests/test_net_gpu.py::test_fused_backprojection_loss_kernel): on by default;
 # LANEFIT_FUSED_LOSS=0 falls back to the torch ops of Loss_crit.backprojection_loss.forward_lanes.
 FUSED_LOSS = os.environ.get("LANEFIT_FUSED_LOSS", "1") != "0"
 

@@ -13,7 +13,7 @@ convolution that feeds it (w' = w * scale[co], b' = b * scale + shift) and every
 
 The folded, GEMM-layout (and TF32 hi/lo split) operands are built once per set of parameter / running-statistics versions
 and cached on the module -- parameter-sized torch ops, nothing per step.  Only taken for inference (no autograd graph) on
-shapes the tcgen05 kernels serve; everything else keeps the unfused eval path of ops_net (same results to fp32 rounding,
+shapes the tensor-core kernels serve; everything else keeps the unfused eval path of ops_net (same results to fp32 rounding,
 tests/test_net_gpu.py::test_eval_fused_matches_unfused)."""
 import torch
 

@@ -2,7 +2,7 @@
 on the library's kernels: each head is four conv -> BatchNorm2d(eps 1e-5) -> ReLU stages on the shared encoder output
 ([B,128,32,64]), a pooling step and one or two fully connected layers.
 
-  conv 1x1 / 3x3 (stride 1)   lf_conv_tcg, the run-time-tap gather-GEMM on tcgen05 (1 or 9 taps over one NHWC view; 3xTF32 in
+  conv 1x1 / 3x3 (stride 1)   lf_conv_tcg, the run-time-tap gather-GEMM on tensor cores (1 or 9 taps over one NHWC view; 3xTF32 in
                               the default mode), input gradient = the same kernel with mirrored taps and transposed weights,
                               weight gradient = lf_wgrad_tcg over the same taps; in fp32 mode (or for shapes the tensor-core
                               kernels do not tile) the CUDA-core implicit GEMM lf_conv_f32 / lf_wgrad_f32.

@@ -23,10 +23,10 @@ LfConvArgs, LfWgradArgs, LfConvTcArgs = _capi.LfConvArgs, _capi.LfWgradArgs, _ca
 
 # Convolution arithmetic for the dense 3-tap convolutions of non_bottleneck_1d (C in {64,128}):
 #   "fp32": CUDA-core FFMA implicit GEMM (parity mode, fp32-exact)
-#   "tf32x3": tcgen05 tensor cores, every product formed from TF32 hi/lo splits of both operands
+#   "tf32x3": tensor cores, every product formed from TF32 hi/lo splits of both operands
 #           (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 accumulate): fp32-grade results at tensor-core speed -- the
-#           default, and the mode bench.py times (csrc/conv_tc_x3.cu);
-#   "tf32": tcgen05 tensor cores, single-pass TF32 multiply / fp32 accumulate (what cuDNN does for the reference's
+#           default, and the mode bench.py times (csrc/conv_tc.cu);
+#   "tf32": tensor cores, single-pass TF32 multiply / fp32 accumulate (what cuDNN does for the reference's
 #           fp32 convs on Ampere+ GPUs; 1e-3 from fp32 on the curve coefficients -- a labelled extra);
 #   shapes a tensor-core kernel does not take stay on the fp32 kernel in every mode.
 CONV_MODES = ("fp32", "tf32", "tf32x3")
@@ -41,7 +41,7 @@ def set_conv_mode(mode):
 
 
 def tc_mode():
-    """True when the dense convolutions run on tcgen05 (either TF32 flavour)."""
+    """True when the dense convolutions run on tensor cores (either TF32 flavour)."""
     return CONV_MODE in ("tf32", "tf32x3")
 
 
@@ -270,7 +270,7 @@ def _wgrad_tcg_ctas(*args):
 
 
 def _wgrad_tcg_taps_per_launch(N, Hs, Ws, C, Nn):
-    """6, 3 or 2 taps per launch (TMEM columns, block table and shared-memory stages permitting), 0 = unsupported."""
+    """6, 3 or 2 taps per launch (block table and shared-memory stages permitting), 0 = unsupported."""
     per_tap = (2 * C) // 32
     for tpl in (6, 3, 2):
         nb = tpl * per_tap
@@ -471,7 +471,7 @@ def pack_tc_dgrad(w):
 # super-channels).  A 3-tap convolution of the original is a 3-tap convolution of the super-pixel grid
 # with 64x64 weight blocks built from the 16x16 ones: block-diagonal for the vertical (3x1) conv, banded
 # for the horizontal (1x3) conv whose x-1 / x+1 taps cross into the neighbouring super-pixel.  3/4 of the
-# MMA work multiplies zeros, but the tcgen05 kernels are ~3x faster than the CUDA-core kernels on these
+# MMA work multiplies zeros, but the tensor-core kernels are faster than the CUDA-core kernels on these
 # bandwidth-bound layers and nothing new runs on the device.
 # ----------------------------------------------------------------------------------------
 SUPER = 4
@@ -548,7 +548,7 @@ def super_ok(x, dil):
 
 
 def tc_rows(x, vertical=None, dil=1, stats=False):
-    """0 if the active tcgen05 kernel does not take this call, else the row count of its colsum / stats partials.
+    """0 if the active tensor-core kernel does not take this call, else the row count of its colsum / stats partials.
     tf32: any 3-tap pattern on a supported shape (the per-tap variant is the in-library fallback; `stats` needs the
     slab kernel); tf32x3: per (axis, dilation) -- vertical=None asks for d=1 along both axes."""
     N, H, W, C = x.shape
@@ -577,7 +577,7 @@ def _taps_axis(taps):
 
 def run_conv_tc(taps, x, wpack, out, bias=None, relu=False, mask_src=None, add_src=None, add_mask=None, colsum=None,
                 mask_affine=None, stats_partial=None):
-    """3-tap convolution on tcgen05.  taps: [(dy, dx)] * 3 in weight-slot order.  colsum: optional [C]
+    """3-tap convolution on tensor cores.  taps: [(dy, dx)] * 3 in weight-slot order.  colsum: optional [C]
     tensor receiving the column sums of `out` (bias gradient), accumulated in the kernel's epilogue."""
     N, H, W, C = x.shape
     a = LfConvTcArgs()
@@ -640,7 +640,7 @@ def _super_conv_launch(taps, xs, w, vertical, transposed, out, N, H, W, C, cs, e
 
 def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, **epi):
     """One factorised 3-tap convolution of non_bottleneck_1d (or its input gradient when
-    ``transposed``): dispatches to the tcgen05 kernel in tf32 mode, else to the fp32 kernel.
+    ``transposed``): dispatches to the tensor-core kernel in tf32 mode, else to the fp32 kernel.
     ``colsum`` ([C] tensor): also produce the per-channel sums of the result.
     ``wp``: the already packed tensor-core operand (ops_eval's BatchNorm-folded weights) -- tensor-core routes only."""
     N, H, W, C = x.shape
@@ -689,7 +689,7 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
     """Weight + bias gradient of one factorised 3-tap convolution -> (dw [Co,Ci,kh,kw], db [Co] or None).
     bias_grad: "compute" (column sums of d_out), or "skip" (the caller gets it elsewhere)."""
     N, H, W, C = x_in.shape
-    sfx = "_x3" if wgrad_x3() else ""          # which tcgen05 weight-gradient kernel
+    sfx = "_x3" if wgrad_x3() else ""          # which tensor-core weight-gradient kernel
     if super_ok(x_in, dil) and d_out.is_contiguous():
         Cs, Ws = SUPER * C, W // SUPER
         nctas = getattr(_lib(), "lf_wgrad3_tc%s_ctas" % sfx)(N, H, Ws, Cs)
@@ -730,8 +730,15 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
     return dw, db
 
 
+def _sm_count():
+    import torch
+    if not torch.cuda.is_available():
+        return 132      # host-side planning without a device (nothing is launched)
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
 def _nsplit_for(tiles, M):
-    target = 148 * 6
+    target = _sm_count() * 6
     ns = max(1, min((target + tiles - 1) // tiles, max(1, M // 256)))
     return int(ns)
 
@@ -827,7 +834,7 @@ def bn_forward_stats(x, gamma, beta, running_mean, running_var, training, eps=BN
 
 
 def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running_var, training):
-    """conv (forward) followed by the BatchNorm statistics of its output -> (out, BNState).  On the tcgen05 slab
+    """conv (forward) followed by the BatchNorm statistics of its output -> (out, BNState).  On the tensor-core slab
     kernel the per-channel sums are accumulated in the conv epilogue, saving a full pass over `out`."""
     N, H, W, C = x.shape
     rows = tc_rows(x, vertical, dil, stats=True) if training else 0
@@ -915,7 +922,7 @@ def dgrad_relu_bn_fused(d_out, w, vertical, dil, x, s, gamma):
 
 def _require_training_for_backward(training):
     if not training:
-        raise RuntimeError("backward through eval-mode BatchNorm is not implemented on the B200 path "
+        raise RuntimeError("backward through eval-mode BatchNorm is not implemented on the H100 path "
                            "(the reference only back-propagates in train mode, BP/main.py:232,338)")
 
 

@@ -1,8 +1,9 @@
-"""Import the UNMODIFIED reference from /root/reference (TEST INFRASTRUCTURE).
+"""Import the UNMODIFIED reference project (TEST INFRASTRUCTURE).
 
-/root/reference exists in the build container only; on the GPU box the verbatim copy under baseline/_ref/ (written
-by ``install()``, git-ignored) is used instead.  Nothing under ``-m gpu`` or ``smoke()`` calls this; ``bench.py`` uses it
-for the reference arm / cpu_baseline only (kind "reference").
+The reference is an upstream checkout: $LANEFIT_REFERENCE_DIR, else ../reference next to this repository.  ``install()``
+(called by ``__graft_entry__.build()``) copies its hot-path modules into oracle/_ref/ (git-ignored), which is used when
+the checkout itself is not reachable.  No test and neither ``smoke()`` nor ``bench.py``'s timed path needs it;
+``bench.py`` uses it for the reference arm / cpu_baseline only (kind "reference"; without it, the oracle port is timed).
 Recipe = SURVEY.md Appendix A: the reference modules use top-level
 ``import Networks`` and need ``matplotlib`` at import time
 (Backprojection_Loss/Networks/utils.py:17-21), which this image lacks -> stub it.
@@ -11,12 +12,10 @@ import os
 import sys
 import types
 
-# /root/reference exists in the build container only.  ``install()`` (called by __graft_entry__.build() there) copies the
-# few Python files of the hot path, unmodified, into baseline/_ref/ -- git-ignored, but shipped to the GPU box with the
-# snapshot -- so that ``bench.py --impl reference`` / ``cpu_baseline`` can time the REAL reference modules there.
 _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INSTALLED_ROOT = os.path.join(_REPO, "baseline", "_ref")
-_CANDIDATES = ["/root/reference", INSTALLED_ROOT]
+SOURCE_ROOT = os.environ.get("LANEFIT_REFERENCE_DIR") or os.path.join(os.path.dirname(_REPO), "reference")
+INSTALLED_ROOT = os.path.join(_REPO, "oracle", "_ref")
+_CANDIDATES = [SOURCE_ROOT, INSTALLED_ROOT]
 _HOT_PATH_FILES = ["Networks/__init__.py", "Networks/ERFNet.py", "Networks/LSQ_layer.py", "Networks/gels.py",
                    "Networks/utils.py", "Loss_crit.py"]
 
@@ -28,18 +27,18 @@ def _root():
     return None
 
 
-REFERENCE_ROOT = _root() or "/root/reference"
+REFERENCE_ROOT = _root() or SOURCE_ROOT
 
 
 def available():
     return _root() is not None
 
 
-def install(src="/root/reference", dst=INSTALLED_ROOT):
-    """Copy the reference's hot-path modules (both variants) verbatim from `src` to baseline/_ref.  No-op (False) when
-    `src` is absent (the GPU box: it uses what the snapshot brought)."""
+def install(src=SOURCE_ROOT, dst=INSTALLED_ROOT):
+    """Copy the reference's hot-path modules (both variants) verbatim from `src` to oracle/_ref.  No-op (False) when
+    `src` is absent or unreadable."""
     import shutil
-    if not os.path.isdir(os.path.join(src, "Backprojection_Loss", "Networks")):
+    if not os.access(os.path.join(src, "Backprojection_Loss", "Networks"), os.R_OK | os.X_OK):
         return False
     for variant in ("Backprojection_Loss", "Birds_Eye_View_Loss"):
         for rel in _HOT_PATH_FILES:

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 (TF32) 3-tap convolution kernel (csrc/conv_tc.cu) against the fp32 CUDA-core
+"""GPU tests of the tensor-core (TF32) 3-tap convolution kernel (csrc/conv_tc.cu) against the fp32 CUDA-core
 kernel (csrc/conv_f32.cu) and against torch-CPU fp64.
 
 Two kinds of checks:
@@ -343,13 +343,13 @@ def test_tcg_weight_gradients(kind, C, O, tot, H, W, N, mode):
 
 
 # ------------------------------------------------------------------------------------------------------
-# 3xTF32 mode (csrc/conv_tc_x3.cu): fp32-grade products on tcgen05 -- GENERIC operands, fp32-level gates
+# 3xTF32 mode (csrc/conv_tc.cu): fp32-grade products on tensor cores -- GENERIC operands, fp32-level gates
 # ------------------------------------------------------------------------------------------------------
 X3_CASES = CASES + [
     (2, 128, 32, 64, True, 8),      # tall tile (32 x 4): halo 2d / TA
     (2, 128, 32, 64, False, 8),
     (1, 128, 40, 80, False, 16),    # 320x640 geometry, 48 KB slab: two pipeline stages
-    (9, 128, 32, 64, True, 1),      # 9 tiles per CTA pair: three groups of TMEM buffers, weight slots refilled
+    (9, 128, 32, 64, True, 1),      # 9 tiles per CTA pair: several tiles per persistent CTA
     (1, 64, 128, 64, False, 1),     # the super-pixel view of a C=16 decoder layer
 ]
 
@@ -472,7 +472,7 @@ def test_x3_weight_gradient_generic_operands(N, C, H, W, vertical, dil):
     e_x3 = float((res["tf32x3"].double().cpu() - wd.grad).abs().max()) / scale
     e_f32 = float((res["fp32"].double().cpu() - wd.grad).abs().max()) / scale
     print("wgrad x3 err %.2e  fp32-kernel err %.2e" % (e_x3, e_f32))
-    # the sum runs over up to 65 536 pixels; the TMEM accumulator adds 8 products per instruction in fp32 (measured
+    # the sum runs over up to 65 536 pixels; the tensor-core accumulator adds 8 products per instruction in fp32 (measured
     # 3.8e-6 at N=32, the split-K FFMA kernel's hierarchical sum 5.7e-7) -- an fp32 dot product of that length
     assert e_x3 <= 1e-5, (e_x3, e_f32)
 

@@ -2,7 +2,7 @@
 and backward) through the reference-mirroring modules, against the torch-CPU oracle and the
 committed golden outputs of the reference itself.
 
-Both fp32-accurate modes (3xTF32 on tcgen05 = default; CUDA-core FFMA): block-level gate 1e-4 norm-wise (typically 1e-6).
+Both fp32-accurate modes (3xTF32 on tensor cores = default; CUDA-core FFMA): block-level gate 1e-4 norm-wise (typically 1e-6).
 Whole-path gate vs the reference (SURVEY.md 7.2 #1): |ours - fp64| <= |ref32 - fp64| * 4 + 1e-4.
 """
 import json
@@ -21,7 +21,7 @@ TOL = 1e-4
 
 @pytest.fixture(autouse=True, params=["tf32x3", "fp32"])
 def conv_mode(request):
-    """Every parity test of this module runs in both fp32-accurate arithmetic modes: 3xTF32 on tcgen05 (the library
+    """Every parity test of this module runs in both fp32-accurate arithmetic modes: 3xTF32 on tensor cores (the library
     default and the mode bench.py times) and the CUDA-core FFMA kernels.  Same gates for both."""
     from lanedetection_end2end_b200 import ops_net
     ops_net.set_conv_mode(request.param)
@@ -88,8 +88,7 @@ def check_grads(block, oracle_P, prefix, tol=TOL, flips=0):
     flips > 0 (rel_up_to_relu_flips found ReLU-mask flips against the fp64 oracle in this run -- a pre-activation within
     fp32 round-off of zero landing on the other side): ONE flipped bit adds / removes a single (pixel, channel) product
     in the weight gradients that consume it -- up to max|activation| * max|gradient| on the ~3 C entries of that output
-    channel, 2.3 % of the largest entry in the measured case (profiles/r02/diag_block_s8.jsonl: conv3x1_2.weight, C = 128,
-    d = 16, one flip; the same block has 0 flips and 1e-6 errors in the other arithmetic mode) -- and shifts everything
+    channel, a few % of the largest entry) -- and shifts everything
     behind the next BatchNorm by ~1/pixels through the batch statistics.  A wrong tap, stride or operand corrupts MOST
     entries by O(1) instead.  So the gate becomes robust: at most 5 % of the entries beyond 1e-2 of the scale (measured
     with one flip: 0.2-0.5 % on every entry behind the BatchNorm, 1.1 % / 2.3 % on the two gradients that consume the flipped
@@ -332,7 +331,7 @@ def test_error_conventions():
 
 @pytest.mark.parametrize("name", ["net_l2_d2", "net_l4_d3"])
 def test_full_path_tf32_mode_accuracy(name):
-    """The fast mode (tcgen05 TF32 convolutions in the 15 non_bottleneck_1d blocks with C=64/128) is NOT
+    """The fast mode (tensor-core TF32 convolutions in the 15 non_bottleneck_1d blocks with C=64/128) is NOT
     expected to meet the 1e-4 fp32 gate -- TF32 keeps 10 mantissa bits, exactly like cuDNN's default for the
     reference's fp32 convs on GPU.  This test pins how far it is from the fp64 truth on the golden inputs and
     writes the numbers next to the bench output."""
@@ -375,7 +374,7 @@ def test_full_path_tf32_mode_accuracy(name):
         with open(os.path.join(outdir, "tf32_accuracy_%s.json" % name), "w") as f:
             json.dump(rec, f)
     print(rec)
-    # measured (profiles/r01/tf32_accuracy_*.json): beta 5e-4 (order 2) / 2e-3 (order 3) norm-wise; individual
+    # measured (tests/golden/tf32_accuracy_*.json, H100): beta ~7e-4 norm-wise; individual
     # decoder outputs of this random-weight, batch-2 network move by up to 17 % of the max (ReLU/BN chaos),
     # which the weighted fit averages out
     # gate = about 2x the measured error (ADVICE r1): an accuracy regression of the TF32 kernels must not pass

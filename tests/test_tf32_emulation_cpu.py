@@ -1,8 +1,8 @@
 """What does TF32 do to the REFERENCE?  On Ampere-and-later GPUs PyTorch runs the reference's fp32 convolutions through
 cuDNN with `torch.backends.cudnn.allow_tf32 = True` (the default), i.e. with operands rounded to TF32 (10 mantissa bits)
-and fp32 accumulation -- the arithmetic of our tcgen05 fast mode.  This test re-runs the oracle's fp32 restatement of
+and fp32 accumulation -- the arithmetic of our tensor-core fast mode.  This test re-runs the oracle's fp32 restatement of
 the reference with every convolution's operands rounded to TF32 and measures how far the curve coefficients move from
-the fp64 golden: the same 5e-4 .. 2e-3 our fast mode shows on the GPU (profiles/r01/tf32_accuracy_*.json), two orders
+the fp64 golden: the same 5e-4 .. 2e-3 our fast mode shows on the H100 (tests/golden/tf32_accuracy_*.json), two orders
 above the fp32-vs-fp64 noise.  I.e. the fast mode is as close to the fp64 truth as the reference itself is when it runs
 on a GPU with its default settings; the 1e-4 gates are met by the fp32 parity mode."""
 import json
@@ -69,15 +69,12 @@ def test_reference_with_tf32_convolutions_moves_as_much_as_our_fast_mode(name, m
     err_fp32_ref = normwise(g["beta_f32"], g["beta_f64"])
     rec = {"case": name, "beta_normwise_err_reference_with_tf32_convs": err_tf32_ref,
            "beta_normwise_err_reference_fp32": err_fp32_ref}
-    ours_path = os.path.join(ROOT, "profiles", "r01", "tf32_accuracy_%s.json" % name)
-    if os.path.exists(ours_path):
-        ours = json.load(open(ours_path))["beta_normwise_err_tf32"]
-        rec["beta_normwise_err_ours_tf32_mode_on_b200"] = ours
-        # same order of magnitude: neither is more than 8x the other
-        assert ours <= 8 * err_tf32_ref and err_tf32_ref <= 8 * ours, rec
-    out = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(out):
-        json.dump(rec, open(os.path.join(out, "tf32_reference_emulation_%s.json" % name), "w"))
+    # our single-pass TF32 mode's beta error on the same golden inputs, measured on the H100
+    # (tests/test_net_gpu.py::test_full_path_tf32_mode_accuracy)
+    ours = json.load(open(os.path.join(ROOT, "tests", "golden", "tf32_accuracy_%s.json" % name)))["beta_normwise_err_tf32"]
+    rec["beta_normwise_err_ours_tf32_mode_h100"] = ours
+    # same order of magnitude: neither is more than 8x the other
+    assert ours <= 8 * err_tf32_ref and err_tf32_ref <= 8 * ours, rec
     # TF32 rounding of the convolutions alone moves beta well beyond the fp32 noise and beyond 1e-4
     assert err_tf32_ref > 10 * err_fp32_ref, rec
     assert 1e-4 < err_tf32_ref < 2e-2, rec

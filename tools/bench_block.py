@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel timing of one non_bottleneck_1d block (forward + backward) at the bench shapes, in fp32 (CUDA-core)
-and tf32 (tcgen05) conv modes.  CUDA events around every C-ABI launch (the _capi.TRACE hook)."""
+and tf32 (tensor-core) conv modes.  CUDA events around every C-ABI launch (the _capi.TRACE hook)."""
 import argparse
 import json
 import os
@@ -20,7 +20,7 @@ def main():
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--modes", nargs="+", default=["fp32", "tf32"])
     ap.add_argument("--shapes", nargs="+", default=["128,32,64,2", "64,64,128,1"])   # C,H,W,dil
-    ap.add_argument("--variant", type=int, default=2, help="tcgen05 conv variant (2 = halo slab, 1 = per-tap boxes)")
+    ap.add_argument("--variant", type=int, default=2, help="tensor-core conv variant (2 = halo slab, 1 = per-tap boxes)")
     a = ap.parse_args()
     _capi.lib().lf_conv1d_tc_set_variant(a.variant)
     for shp in a.shapes:
