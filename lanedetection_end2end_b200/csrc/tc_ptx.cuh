@@ -1,5 +1,5 @@
-// Shared Hopper (sm_90a) tensor-core PTX wrappers: TMA, mbarrier, wgmma, mma.sync, TF32 operand splitting and the
-// tensor-map helpers.
+// Shared Hopper (sm_90a) tensor-core PTX wrappers: TMA, mbarrier, wgmma, shared-memory accesses, TF32 operand
+// splitting and the tensor-map helpers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -120,6 +120,28 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], const uint32
           "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+// D[64 x 48] (+)= A[64 x 8] * B[48 x 8]^T
+__device__ __forceinline__ void wgmma_m64n48k8_tf32(float (&d)[24], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+        "{%24, %25, %26, %27}, %28, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 32] (+)= A[64 x 8] * B[32 x 8]^T
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 // D[64 x 16] (+)= A[64 x 8] * B[16 x 8]^T
 __device__ __forceinline__ void wgmma_m64n16k8_tf32(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
     asm volatile(
@@ -129,15 +151,32 @@ __device__ __forceinline__ void wgmma_m64n16k8_tf32(float (&d)[8], const uint32_
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
-
-// mma.sync m16n8k8 TF32 (warp-level): a as for wgmma within one warp's 16 rows; b[0] = B[k = t][n = g], b[1] = B[t + 4][g];
-// d[i]: row g + 8 * (i >> 1), column 2t + (i & 1).
-__device__ __forceinline__ void mma_m16n8k8_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T for N in {16, 32, 48, 64}
+template <int N>
+__device__ __forceinline__ void wgmma_m64k8_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    static_assert(N == 16 || N == 32 || N == 48 || N == 64, "wgmma_m64k8_tf32: N");
+    if constexpr (N == 16) wgmma_m64n16k8_tf32(d, a, bdesc, accumulate);
+    else if constexpr (N == 32) wgmma_m64n32k8_tf32(d, a, bdesc, accumulate);
+    else if constexpr (N == 48) wgmma_m64n48k8_tf32(d, a, bdesc, accumulate);
+    else wgmma_m64n64k8_tf32(d, a, bdesc, accumulate);
 }
+
+// Shared-state-space accesses (addresses from smem_u32): LDS / STS without generic-address translation.
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ float4 lds_f32x4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// orders this thread's generic-proxy shared-memory stores before later async-proxy (wgmma, TMA) accesses
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
 // host: cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link)

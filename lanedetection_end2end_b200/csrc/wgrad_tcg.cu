@@ -1,23 +1,35 @@
-// Tensor-core weight gradients (Hopper, sm_90a), one kernel for every convolution of the network:
+// Tensor-core weight gradients (Hopper, sm_90a), one wgmma kernel for every convolution of the network:
 //
 //     D[blk*32 + c][n] = sum_{img,y,x} A_{map[blk]}(img, y + dy[blk], x + dx[blk], cblk[blk]*32 + c) * B(img, y, x, n)
 //
 // i.e. one 32-channel block of one tap per `blk` (up to 24 blocks), n < Nn (multiple of 32, <= 128), over strided NHWC
 // views.  Its callers:
 //  * lf_wgrad_tcg: the resolution-changing layers (3x3 stride-2 Conv2d of DownsamplerBlock, 3x3 stride-2 ConvTranspose2d
-//    of UpsamplerBlock; BP/Networks/ERFNet.py:15,101) on the pair-pixel / row-parity views of conv_tcg.cu;
+//    of UpsamplerBlock; BP/Networks/ERFNet.py:15,101) on the pair-pixel / row-parity views of conv_tcg.cu, and the
+//    Classification heads;
 //  * lf_wgrad3_tc / lf_wgrad3_tc_x3: the factorised 3-tap convolutions (C in {64,128}), dW[t][ci][co] = block t*C/32 + cb
 //    of X shifted by tap t against dY -- the partial layout [3][C][C] is the block layout above.
-// The K dimension of these GEMMs is the pixel index, so both operands lie MN-major in the NHWC boxes.  wgmma reads TF32
-// operands from shared memory only K-major, so the fragments are loaded by the threads from the swizzled TMA boxes and
-// multiplied with mma.sync m16n8k8.
+// The K dimension of these GEMMs is the pixel index, so both operands lie MN-major in the NHWC boxes TMA loads.  wgmma
+// takes A (rows = x-channels, k = pixels) from registers, which the threads load from the swizzled box like any other
+// fragment; it reads TF32 B only K-major from shared memory, so the dY boxes are transposed in shared memory first.
 //
-// One CTA = one pixel range (split K; blockIdx.x) x one group of four blocks (128 rows of D; blockIdx.y).  Stage =
-// [B boxes: Nn/32 x (32 px x 32 ch)][A boxes of the group], 128B-swizzled, TMA zero-fills out-of-image pixels (conv
-// padding); an mbarrier ring feeds 8 MMA warps (warp w: block w & 3, output columns half w >> 2), warp 8 is the TMA
-// producer.  Every CTA writes its slice [128 rows][Nn] of one partial; lf_wgrad_reduce sums the partials in fixed order.
-// precision 1 (3xTF32; tc_ptx.cuh): both operands split into hi / lo in registers, every product is
-// a_hi*b_hi + (a_hi*b_lo + a_lo*b_hi), the correction terms accumulated apart and added at the end.
+// One CTA = one pixel range (split K; blockIdx.x) x one pair of blocks (64 rows of D = one m64 tile; blockIdx.y), so
+// every block list, odd ones included, keeps all MMA warps busy.  Stage = [B boxes: Nn/32 x (32 px x 32 ch)][the two A
+// boxes of the pair], 128B-swizzled; TMA zero-fills out-of-image pixels (conv padding).  Warp 8 is the TMA producer;
+// warps 0-7 form two consumer warpgroups of NW = wgt_cols(Nn) output columns each.  Nn <= 64: both own all columns and
+// take alternate stages (one wgmma of N = Nn per k8 instead of two of Nn/2: the kernel is bound by wgmma issue, not by
+// tensor-core FLOPs), and warpgroup 1 hands its sums to warpgroup 0 at the end (fixed order).  Nn = 96 / 128: each owns
+// half the columns and takes every stage.  Per stage, a warpgroup
+//  * transposes its columns of the stage's dY boxes into a K-major, 128B-swizzled [NW x 32 px] tile (the layout TMA
+//    would write for K-major data; 3xTF32: a hi tile and a lo tile, every element split once per CTA), double-buffered
+//    so that one stage's stores never meet the previous stage's wgmma reads;
+//  * loads the m64k8 A fragments of the pair (the rows of warp w come from block w/2) and issues wgmma m64nNWk8.  Each
+//    stage's 32 pixels of the large term are summed by the tensor core from zero and added to the fp32 register sum
+//    with FADD (the tensor core's accumulation drifts further than an FFMA chain over 10^4+ pixels); 3xTF32
+//    (tc_ptx.cuh): every product is a_hi*b_hi + (a_hi*b_lo + a_lo*b_hi), the correction terms accumulated on the tensor
+//    core and added in the epilogue.
+// The next stage's fragments are not loaded while a stage's wgmma runs: ptxas then reuses the A registers the running
+// wgmma still reads.  Every CTA writes its slice [64 rows][Nn] of one partial; lf_wgrad_reduce sums them in fixed order.
 #include <cuda.h>
 
 #include "lf_common.cuh"
@@ -25,11 +37,11 @@
 
 namespace lf {
 
-constexpr int WG_THREADS = 288;
+constexpr int WG_THREADS = 288;              // two consumer warpgroups + the TMA warp
 constexpr int WG_KP = 32;                    // pixels per stage
 constexpr int WG_BOX = WG_KP * 128;          // one [32 px x 32 ch] box = 4 KB
 constexpr int WG_MAXB = LF_WGRAD_TCG_MAX_BLOCKS;
-constexpr int WG_MAX_STAGES = 6;
+constexpr int WG_MAX_STAGES = 8;
 constexpr int WG_SMEM_LIMIT = 227 * 1024;
 
 struct WgtArgs {
@@ -42,14 +54,25 @@ struct WgtArgs {
     int total_patches;
 };
 
-template <bool X3>
+// B columns per consumer warpgroup for Nn B columns: Nn itself (the warpgroups take alternate stages) up to 64; above,
+// three m64nNn accumulator sets would not fit the 168 registers a thread has here (each warpgroup takes half the columns)
+constexpr int wgt_cols(int nn) { return nn <= 64 ? nn : nn / 2; }
+// shared memory of the transposed B tiles: [2 warpgroups][2 buffers][hi (, lo)] x [cols x 32 px]
+constexpr int wgt_bt_bytes(int nn, bool x3) { return 2 * 2 * (x3 ? 2 : 1) * wgt_cols(nn) * 128; }
+
+template <int NN, bool X3>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmB, const WgtArgs a) {
+    constexpr int NW = wgt_cols(NN);                    // B columns per warpgroup = wgmma N
+    constexpr bool KSPLIT = NW == NN;                   // warpgroups split the stages, not the columns
+    constexpr int BT_TILE = NW * 128;                   // one K-major [NW x 32 px] tile (1024-byte multiple)
+    constexpr int BT_SET = (X3 ? 2 : 1) * BT_TILE;      // hi tile, then lo tile
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)a.stages * a.stage_bytes);
+    uint8_t* bt = smem + (size_t)a.stages * a.stage_bytes;
+    uint64_t* full = reinterpret_cast<uint64_t*>(bt + wgt_bt_bytes(NN, X3));
     uint64_t* empty = full + WG_MAX_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -57,8 +80,8 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     const int p_begin = blockIdx.x * per;
     const int p_end = min(a.total_patches, p_begin + per);
     const int tiles_x = a.Ws / a.bx, tiles_y = a.Hs / a.by;
-    const int blk0 = 4 * blockIdx.y;                  // first block of this CTA's group
-    const int na = min(4, a.nblocks - blk0);          // blocks in the group
+    const int blk0 = 2 * blockIdx.y;                  // first block of this CTA's pair
+    const int na = min(2, a.nblocks - blk0);          // blocks in the pair
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA0);
@@ -66,7 +89,7 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < a.stages; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 8);   // one arrive per MMA warp
+            mbar_init(&empty[s], KSPLIT ? 4 : 8);   // one arrive per MMA warp that reads the stage
         }
         fence_barrier_init();
     }
@@ -102,96 +125,118 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         return;
     }
 
-    // MMA warps: block bi of the group (32 rows = two m16 tiles), columns [nh * Nn/2, (nh + 1) * Nn/2) = nt n8 tiles
-    const int bi = warp & 3, nh = warp >> 2;
+    // consumer warpgroup wg, warp wl: D rows 16*wl + g (+8) = channel 16*(wl & 1) + g (+8) of block blk0 + (wl >> 1),
+    // columns [c0, c0 + NW); KSPLIT: warpgroup wg takes the stages p_begin + wg, p_begin + wg + 2, ...
+    const int wg = warp >> 2, wl = warp & 3;
     const int g = lane >> 2, t4 = lane & 3;
-    const int nt = a.Nn >> 4;
-    const int n_base = nh * (a.Nn >> 1);
-    const bool active = bi < na;
-    float acc[2][8][4], acs[2][8][4];
+    const bool rows_ok = (wl >> 1) < na;   // false: the second block of an odd list's last pair (A = 0, not stored)
+    const int arow = 16 * (wl & 1) + g;
+    const int c0 = KSPLIT ? 0 : wg * NW;
+    const uint32_t bt_wg = smem_u32(bt) + wg * 2 * BT_SET;
+    float acc[NW / 2], part[NW / 2], acs[NW / 2];   // running sum; one stage's large term; 3xTF32 correction terms
 #pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
+    for (int i = 0; i < NW / 2; ++i) acc[i] = part[i] = acs[i] = 0.f;
+    uint32_t buf = 0;
+    for (int p = p_begin + (KSPLIT ? wg : 0); p < p_end; p += (KSPLIT ? 2 : 1)) {
+        const int j = p - p_begin;
+        const int stage = j % a.stages;
+        mbar_wait(&full[stage], (j / a.stages) & 1);
+        const uint32_t st = smem_u32(smem) + stage * a.stage_bytes;
+        // A fragments (a[0..3] = A[arow][k0], A[arow + 8][k0], A[arow][k0 + 4], A[arow + 8][k0 + 4], A[c][k] = X[px k][ch c])
+        float av[WG_KP / 8][4];
+        const uint32_t abox = st + (a.nb_b + (wl >> 1)) * WG_BOX;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
+            const int k0 = 8 * k8 + t4;
+            av[k8][0] = rows_ok ? lds_f32(abox + sw128_off(k0, arow)) : 0.f;
+            av[k8][1] = rows_ok ? lds_f32(abox + sw128_off(k0, arow + 8)) : 0.f;
+            av[k8][2] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow)) : 0.f;
+            av[k8][3] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow + 8)) : 0.f;
+        }
+        // transpose: warp wl takes the 4-column chunks q = wl + 4i of this warpgroup's columns, lane = pixel.  Reads are
+        // one 16-byte chunk per lane, writes one column (32 pixels = one swizzled 128-byte row): both conflict-free.
+        const uint32_t bhi = bt_wg + buf * BT_SET;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) acc[mi][j][q] = acs[mi][j][q] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int p = p_begin; p < p_end; ++p) {
-        mbar_wait(&full[stage], phase);
-        const uint8_t* st = smem + (size_t)stage * a.stage_bytes;
-        if (active) {
-            const uint8_t* abox = st + (a.nb_b + bi) * WG_BOX;
+        for (int i = 0; i < NW / 16; ++i) {
+            const int q = wl + 4 * i;
+            const int n = c0 + 4 * q;   // first B column of the chunk
+            const float4 v4 = lds_f32x4(st + (n >> 5) * WG_BOX + sw128_off(lane, n & 31));
+            const float v[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
-            for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
-                const int k0 = 8 * k8 + t4;   // pixel rows k0, k0 + 4
-                uint32_t ah[2][4], al[2][4];
-#pragma unroll
-                for (int mi = 0; mi < 2; ++mi) {
-                    const int r = 16 * mi + g;
-                    const float v[4] = {*reinterpret_cast<const float*>(abox + sw128_off(k0, r)),
-                                        *reinterpret_cast<const float*>(abox + sw128_off(k0, r + 8)),
-                                        *reinterpret_cast<const float*>(abox + sw128_off(k0 + 4, r)),
-                                        *reinterpret_cast<const float*>(abox + sw128_off(k0 + 4, r + 8))};
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (X3) {
-                            tf32_split(v[q], ah[mi][q], al[mi][q]);
-                        } else {
-                            ah[mi][q] = tf32_rna(v[q]);
-                        }
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    if (j < nt) {
-                        const int nn = n_base + 8 * j + g;
-                        const uint8_t* bbox = st + (nn >> 5) * WG_BOX;
-                        const float w0 = *reinterpret_cast<const float*>(bbox + sw128_off(k0, nn & 31));
-                        const float w1 = *reinterpret_cast<const float*>(bbox + sw128_off(k0 + 4, nn & 31));
-                        uint32_t bh[2], bl[2];
-                        if (X3) {
-                            tf32_split(w0, bh[0], bl[0]);
-                            tf32_split(w1, bh[1], bl[1]);
-                        } else {
-                            bh[0] = tf32_rna(w0); bh[1] = tf32_rna(w1);
-                        }
-#pragma unroll
-                        for (int mi = 0; mi < 2; ++mi) {
-                            mma_m16n8k8_tf32(acc[mi][j], ah[mi], bh);
-                            if (X3) {
-                                mma_m16n8k8_tf32(acs[mi][j], ah[mi], bl);
-                                mma_m16n8k8_tf32(acs[mi][j], al[mi], bh);
-                            }
-                        }
-                    }
+            for (int e = 0; e < 4; ++e) {
+                const uint32_t off = sw128_off(4 * q + e, lane);
+                if (X3) {
+                    uint32_t hi, lo;
+                    tf32_split(v[e], hi, lo);
+                    sts_u32(bhi + off, hi);
+                    sts_u32(bhi + BT_TILE + off, lo);
+                } else {
+                    sts_u32(bhi + off, tf32_rna(v[e]));
                 }
             }
         }
+        uint32_t ah[WG_KP / 8][4], al[WG_KP / 8][4];
+#pragma unroll
+        for (int k8 = 0; k8 < WG_KP / 8; ++k8)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                if (X3) {
+                    tf32_split(av[k8][q], ah[k8][q], al[k8][q]);
+                } else {
+                    ah[k8][q] = tf32_rna(av[k8][q]);
+                }
+            }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + wg, 128);   // the warpgroup's B tiles are complete
+        const uint64_t bd = wgmma_desc_sw128(bhi);
+        wgmma_fence();
+#pragma unroll
+        for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
+            wgmma_m64k8_tf32<NW>(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous stage dropped)
+            if (X3) {
+                wgmma_m64k8_tf32<NW>(acs, ah[k8], bd + (BT_TILE >> 4) + 2 * k8, 1);   // a_hi * b_lo
+                wgmma_m64k8_tf32<NW>(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * b_hi
+            }
+        }
+        wgmma_commit();
+        // the stage's boxes have been read into registers and B tiles: hand them back to the producer
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[stage]);
-        if (++stage == a.stages) {
-            stage = 0;
-            phase ^= 1;
+        wgmma_wait0();
+        reg_fence(part);
+        if (X3) reg_fence(acs);
+#pragma unroll
+        for (int i = 0; i < NW / 2; ++i) acc[i] += part[i];
+        buf ^= 1;
+    }
+#pragma unroll
+    for (int i = 0; i < NW / 2; ++i)
+        if (X3) acc[i] = acs[i] + acc[i];   // small terms first
+    if (KSPLIT) {
+        // warpgroup 1 hands its sums to warpgroup 0 through its own (now idle) B buffers, same fragment order; the two
+        // halves are added in a fixed order
+        float* xfer = reinterpret_cast<float*>(bt + BT_SET * 2) + (threadIdx.x & 127) * (NW / 2);
+        if (wg == 1) {
+#pragma unroll
+            for (int i = 0; i < NW / 2; i += 2) *reinterpret_cast<float2*>(xfer + i) = make_float2(acc[i], acc[i + 1]);
+        }
+        named_bar_sync(3, 256);
+        if (wg == 1) return;
+#pragma unroll
+        for (int i = 0; i < NW / 2; i += 2) {
+            const float2 o = *reinterpret_cast<const float2*>(xfer + i);
+            acc[i] += o.x;
+            acc[i + 1] += o.y;
         }
     }
-    if (!active) return;
-    float* dst = a.partial + ((size_t)blockIdx.x * a.nblocks * 32 + (size_t)(blk0 + bi) * 32) * a.Nn;
+    if (!rows_ok) return;
+    float* dst = a.partial + ((size_t)blockIdx.x * a.nblocks * 32 + (size_t)blk0 * 32) * a.Nn + c0;
 #pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            if (j < nt) {
-                const int c = n_base + 8 * j + 2 * t4;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = 16 * mi + g + 8 * h;
-                    const float2 o = X3 ? make_float2(acs[mi][j][2 * h] + acc[mi][j][2 * h], acs[mi][j][2 * h + 1] + acc[mi][j][2 * h + 1])
-                                        : make_float2(acc[mi][j][2 * h], acc[mi][j][2 * h + 1]);
-                    *reinterpret_cast<float2*>(dst + (size_t)r * a.Nn + c) = o;
-                }
-            }
-        }
+    for (int i = 0; i < NW / 2; i += 2) {
+        const int r = 16 * wl + g + 8 * ((i >> 1) & 1);
+        const int c = 8 * (i >> 2) + 2 * t4;
+        *reinterpret_cast<float2*>(dst + (size_t)r * a.Nn + c) = make_float2(acc[i], acc[i + 1]);
+    }
 }
 
 static bool wgt_pick_patch(int Hs, int Ws, int* bx, int* by) {
@@ -210,11 +255,13 @@ static bool wgt_encode(TcEncodeTiledFn enc, CUtensorMap* tm, const LfTcgView& v,
     return tc_encode_view(enc, tm, v.ptr, N, v.H, v.W, C, v.sx, v.sy, v.sn, bx, by);
 }
 
-// split-K slices for `patches` pixel patches: at least `min_per` patches per slice, at most one slice per SM
-static int wgt_split(long long patches, int min_per) {
+// split-K slices for `patches` pixel patches and `nblocks` blocks: at least `min_per` patches per slice, and at most as
+// many slices as fill the SMs once with one CTA per (slice, pair of blocks)
+static int wgt_split(long long patches, int min_per, int nblocks) {
     long long s = patches / min_per;
-    const int sms = device_sms();
-    if (s > sms) s = sms;
+    long long cap = device_sms() / ((nblocks + 1) / 2);
+    if (cap < 1) cap = 1;
+    if (s > cap) s = cap;
     return (int)(s < 1 ? 1 : s);
 }
 
@@ -223,7 +270,26 @@ static int wgt_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) {
     if (N <= 0 || Ka % 32 != 0 || Ka < 32 || Nn % 32 != 0 || Nn < 32 || Nn > 128 || nblocks < 1 || nblocks > WG_MAXB) return 0;
     if (!wgt_pick_patch(Hs, Ws, &bx, &by)) return 0;
     if (!tc_get_encode_fn()) return 0;
-    return wgt_split((long long)N * (Hs / by) * (Ws / bx), 4);
+    return wgt_split((long long)N * (Hs / by) * (Ws / bx), 4, nblocks);
+}
+
+template <int NN, bool X3>
+static cudaError_t wgt_launch(dim3 grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
+                              const CUtensorMap& tmB, const WgtArgs& a) {
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tcg_kernel<NN, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    if (e != cudaSuccess) return e;
+    return lf_launch(wgrad_tcg_kernel<NN, X3>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
+}
+
+template <bool X3>
+static cudaError_t wgt_launch_nn(dim3 grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
+                                 const CUtensorMap& tmB, const WgtArgs& a) {
+    switch (a.Nn) {
+        case 32: return wgt_launch<32, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        case 64: return wgt_launch<64, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        case 96: return wgt_launch<96, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        default: return wgt_launch<128, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    }
 }
 
 // a: A views and their block table, b: the B view; the launch of the generic kernel
@@ -242,8 +308,9 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
         two = two || map[b] == 1;
     }
     LF_REQUIRE(!two || av[1].ptr);
-    a.stage_bytes = (a.nb_b + 4) * WG_BOX;
-    int stages = (WG_SMEM_LIMIT - 1024 - 256) / a.stage_bytes;
+    const int fixed = 1024 + wgt_bt_bytes(Nn, x3) + 256;   // alignment slack + transposed B tiles + barriers
+    a.stage_bytes = (a.nb_b + 2) * WG_BOX;
+    int stages = (WG_SMEM_LIMIT - fixed) / a.stage_bytes;
     if (stages > WG_MAX_STAGES) stages = WG_MAX_STAGES;
     a.stages = stages;
     a.total_patches = N * (Hs / a.by) * (Ws / a.bx);
@@ -252,13 +319,11 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
     if (!wgt_encode(enc, &tmA0, av[0], N, Ka, a.bx, a.by)) return LF_ERR_CUDA;
     if (!wgt_encode(enc, &tmA1, two ? av[1] : av[0], N, Ka, a.bx, a.by)) return LF_ERR_CUDA;
     if (!wgt_encode(enc, &tmB, bv, N, Nn, a.bx, a.by)) return LF_ERR_CUDA;
-    const int smem_bytes = 1024 + a.stages * a.stage_bytes + 256;
-    const dim3 grid(nsplit, (nblocks + 3) / 4);
-    cudaError_t e = x3 ? cudaFuncSetAttribute(wgrad_tcg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes)
-                       : cudaFuncSetAttribute(wgrad_tcg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    const int smem_bytes = fixed + a.stages * a.stage_bytes;
+    const dim3 grid(nsplit, (nblocks + 1) / 2);
+    const cudaError_t e = x3 ? wgt_launch_nn<true>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                             : wgt_launch_nn<false>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
-    if (x3) lf_launch(wgrad_tcg_kernel<true>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
-    else lf_launch(wgrad_tcg_kernel<false>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
     return check_launch();
 }
 
@@ -286,7 +351,7 @@ static int wgrad3_ctas(int N, int H, int W, int C, int min_per) {
     if (!(C == 64 || C == 128) || N <= 0) return 0;
     if (!wgt_pick_patch(H, W, &bx, &by)) return 0;
     if (!tc_get_encode_fn()) return 0;
-    return wgt_split((long long)N * (H / by) * (W / bx), min_per);
+    return wgt_split((long long)N * (H / by) * (W / bx), min_per, 3 * C / 32);
 }
 
 static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
@@ -316,3 +381,4 @@ extern "C" int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, in
                                float* partial, int nctas, lf_stream_t stream) {
     return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, true, stream);
 }
+
