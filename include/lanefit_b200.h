@@ -181,6 +181,11 @@ int lf_conv1d_tc_supported(int N, int H, int W, int C);
 int lf_conv1d_tc_x3_rows(int N, int H, int W, int C, int vertical, int dil);
 int lf_conv1d_tc_x3(const LfConvTcArgs* args, lf_stream_t stream);
 int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream);
+/* BF16 variant: same arguments and epilogue, but `wpack` points at a [C][3*C] bf16 operand (LfPackJob.dst_dtype =
+ * LF_BF16) and the activations are rounded to bf16 (nearest even) in the kernel; products are exact in fp32, fp32
+ * accumulate.  It serves exactly the shapes of lf_conv1d_tc and runs on the slab kernel exactly where lf_conv1d_tc does,
+ * so lf_conv1d_tc_supported and lf_conv1d_tc_slab_ok answer for it. */
+int lf_conv1d_tc_bf16(const LfConvTcArgs* args, lf_stream_t stream);
 /* 2 (default) = halo-slab kernel (one TMA slab per 32-channel chunk shared by the three taps);
  * 1 = first version (one TMA box per tap).  Same results; process-wide switch for A/B measurements. */
 void lf_conv1d_tc_set_variant(int variant);
@@ -200,6 +205,11 @@ int lf_wgrad3_tc(const float* x, const float* dy, int N, int H, int W, int C, co
 int lf_wgrad3_tc_x3_ctas(int N, int H, int W, int C);
 int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
                     float* partial, int nctas, lf_stream_t stream);
+/* BF16 variant: same arguments and partial layout; both operands rounded to bf16 (nearest even) in the kernel, fp32
+ * accumulate. */
+int lf_wgrad3_tc_bf16_ctas(int N, int H, int W, int C);
+int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
+                      float* partial, int nctas, lf_stream_t stream);
 
 /* Weight gradient as a split-K GEMM over pixels:
  *   partial[s][t][cp][cq] = sum_{(n,j,i) in split s} P[n, j*psy+pdy[t], i*psx+pdx[t], cp]
@@ -330,7 +340,8 @@ typedef struct LfConvTcgArgs {
     int Kc, Ng, ntaps;
     int map[LF_TCG_MAX_TAPS], dy[LF_TCG_MAX_TAPS], dx[LF_TCG_MAX_TAPS];
     int precision;          /* 0 = TF32 multiply; 1 = 3xTF32 (fp32-grade): wg is [2][Ng][ntaps*Kc], the TF32 hi parts then
-                               the lo parts (LF_PACK_TF32_HI / _LO), activations are split in shared memory */
+                               the lo parts (LF_PACK_TF32_HI / _LO), activations are split in shared memory;
+                               2 = BF16 multiply: wg is [Ng][ntaps*Kc] bf16, activations rounded to bf16 in the kernel */
     int relu;               /* ReLU on conv + bias (eval-mode layers with the BatchNorm folded into wg / bias) */
 } LfConvTcgArgs;
 int lf_conv_tcg_supported(int N, int Hs, int Ws, int Kc, int Ng);
@@ -350,10 +361,12 @@ typedef struct LfWgradTcgArgs {
     int Ka, Nn, nblocks;
     int map[LF_WGRAD_TCG_MAX_BLOCKS], dy[LF_WGRAD_TCG_MAX_BLOCKS], dx[LF_WGRAD_TCG_MAX_BLOCKS], cblk[LF_WGRAD_TCG_MAX_BLOCKS];
     int nctas;
-    int precision;          /* 0 = TF32 multiply; 1 = 3xTF32 (both operands split in shared memory, fp32-grade) */
+    int precision;          /* 0 = TF32 multiply; 1 = 3xTF32 (both operands split in shared memory, fp32-grade);
+                               2 = BF16 multiply (both operands rounded to bf16 in the kernel) */
 } LfWgradTcgArgs;
 int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);
-int lf_wgrad_tcg_ctas_x3(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);   /* same, for precision 1 */
+int lf_wgrad_tcg_ctas_x3(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);     /* same, for precision 1 */
+int lf_wgrad_tcg_ctas_bf16(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);   /* same, for precision 2 */
 int lf_wgrad_tcg(const LfWgradTcgArgs* args, lf_stream_t stream);
 
 /* Batched weight packing (host side: ops_net.WeightPackCache).  The reference keeps Conv2d / ConvTranspose2d
@@ -368,9 +381,13 @@ int lf_wgrad_tcg(const LfWgradTcgArgs* args, lf_stream_t stream);
 #define LF_PACK_TF32_LO 0x40000000
 typedef struct LfPackJob {
     const float* src;   /* parameter in the reference layout (device) */
-    float* dst;         /* packed operand (device) */
+    void* dst;          /* packed operand (device), of dtype dst_dtype */
     const int* idx;     /* n gather indices into src, -1 = zero (device) */
     long long n;
+    int dst_dtype;      /* LF_F32, or LF_BF16: every element rounded to bf16 (nearest even; = torch's .to(torch.bfloat16)),
+                           the weight operand of lf_conv1d_tc_bf16 / lf_conv_tcg (precision 2).  Not combined with the
+                           TF32 flags. */
+    int pad;
 } LfPackJob;
 int lf_pack_gather(const LfPackJob* jobs_dev, int njobs, int blocks_per_job, lf_stream_t stream);
 

@@ -106,6 +106,7 @@ class LfWgradTcgArgs(ctypes.Structure):
 _NET_PROTOS = {
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg_ctas_x3": (_i, [_i, _i, _i, _i, _i, _i]),
+    "lf_wgrad_tcg_ctas_bf16": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg": (_i, [ctypes.POINTER(LfWgradTcgArgs), _p]),
     "lf_reduce_multi": (_i, [ctypes.POINTER(LfReduceJob), _i, _p]),
     "lf_conv_tcg_supported": (_i, [_i, _i, _i, _i, _i]),
@@ -116,6 +117,7 @@ _NET_PROTOS = {
     "lf_conv1d_tc": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
     "lf_conv1d_tc_supported": (_i, [_i, _i, _i, _i]),
     "lf_conv1d_tc_x3": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
+    "lf_conv1d_tc_bf16": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
     "lf_conv1d_tc_x3_rows": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_conv1d_tc_set_variant": (None, [_i]),
     "lf_conv1d_tc_slab_ok": (_i, [_i, _i, _i, _i, _i, _i]),
@@ -123,6 +125,8 @@ _NET_PROTOS = {
     "lf_wgrad3_tc": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
     "lf_wgrad3_tc_x3_ctas": (_i, [_i, _i, _i, _i]),
     "lf_wgrad3_tc_x3": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
+    "lf_wgrad3_tc_bf16_ctas": (_i, [_i, _i, _i, _i]),
+    "lf_wgrad3_tc_bf16": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
     "lf_wgrad_reduce": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "lf_vec_reduce": (_i, [_p, _i, _i, _i, _p, _p]),
     "lf_colsum_blocks": (_i, [ctypes.c_longlong]),

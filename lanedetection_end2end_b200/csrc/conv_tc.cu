@@ -1,11 +1,14 @@
 // Hopper (sm_90a) wgmma implicit-GEMM kernel for ERFNet's factorised 3-tap convolutions
 // (non_bottleneck_1d: conv3x1 / conv1x3 with dilation, BP/Networks/ERFNet.py:29-37,44-53) and their input gradients,
-// C in {64, 128}, NHWC fp32 activations, fp32 accumulate.  Two precisions (template X3):
+// C in {64, 128}, NHWC fp32 activations, fp32 accumulate.  Three operand precisions (template P, tc_ptx.cuh TcPrec):
 //  * TF32 (lf_conv1d_tc): operands rounded to TF32 (the arithmetic cuDNN uses for the reference's fp32 convs on
 //    Ampere and later), one product per multiply;
 //  * 3xTF32 (lf_conv1d_tc_x3, the library default): every fp32 operand is split a = a_hi + a_lo (tc_ptx.cuh) and each
 //    product is a_hi*w_hi + (a_hi*w_lo + a_lo*w_hi) with fp32 accumulation -- as accurate as an fp32 FFMA chain.  The
 //    weights arrive pre-split from the packer ([2][Cout][3C]: hi rows, then lo rows; both exact TF32 values).
+//  * BF16 (lf_conv1d_tc_bf16): both operands rounded to bf16 (nearest even) -- the activations while their k16 fragments
+//    are formed (pairs of adjacent channels, one 8-byte load each), the weights by the packer ([Cout][3C] bf16, 64-byte
+//    rows, 64B-swizzled tiles of half the TF32 size: resident wherever the TF32 tiles are); products exact in fp32.
 //
 //   out[n,y,x,co] = epi( sum_{t<3} sum_{ci} in[n, (y,x) + o_t, ci] * Wp[co][t*C + ci] )
 //
@@ -45,6 +48,8 @@ constexpr int TC_STG_BYTES = 128 * TC_STG_LD * 4; // 18 KB per half
 constexpr int TC_ATOM = TC_BN * 128;              // one [64 out x 32 in] weight tile, 8 KB
 constexpr int TC_SMEM_LIMIT = 227 * 1024;
 constexpr int TC_FIXED_SMEM = 1024 + 2 * TC_STG_BYTES + 256;   // alignment slack + staging + barriers
+// bytes of one [64 out x 32 in] weight tile in precision P: TF32, TF32 hi + lo, or bf16 (64-byte rows, 64B-swizzled)
+constexpr int tc_w_atom(int P) { return P == TC_X3 ? 2 * TC_ATOM : P == TC_BF16 ? TC_ATOM / 2 : TC_ATOM; }
 
 static int g_tc_variant = 2;  // 2 = halo slab, 1 = one box per tap
 
@@ -70,12 +75,13 @@ struct TcArgs {
     int stages, stage_bytes, a_bytes;   // a stage = a_bytes of activations [+ the three weight tiles of its chunk]
 };
 
-template <int C, bool X3, bool RES>
+template <int C, int P, bool RES>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     pdl_trigger();
+    constexpr bool X3 = P == TC_X3;
     constexpr int NCB = C / TC_KCH;
-    constexpr int W_ATOM = X3 ? 2 * TC_ATOM : TC_ATOM;   // 3xTF32: hi tile, then lo tile
+    constexpr int W_ATOM = tc_w_atom(P);   // 3xTF32: hi tile, then lo tile; bf16: half-size tile
     constexpr int B_RES_BYTES = RES ? 3 * NCB * W_ATOM : 0;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -206,42 +212,68 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
             for (int t = 0; t < 3; ++t) {
                 const uint8_t* view = st + a.tap_row[t] * 128;   // 1024-byte aligned: the swizzle phase is the view's row
-                uint32_t ah[4][4], al[4][4];
+                if constexpr (P == TC_BF16) {
+                    // k16 fragments: two adjacent channels per register = one 8-byte load inside a 16-byte chunk
+                    uint32_t ab[2][4];
 #pragma unroll
-                for (int k8 = 0; k8 < 4; ++k8) {
-                    const int c = 8 * k8 + t4;
-                    const float v[4] = {*reinterpret_cast<const float*>(view + sw128_off(ra, c)),
-                                        *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c)),
-                                        *reinterpret_cast<const float*>(view + sw128_off(ra, c + 4)),
-                                        *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c + 4))};
+                    for (int kk = 0; kk < 2; ++kk) {
+                        const int c = 16 * kk + 2 * t4;
+                        const float2 v0 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c));
+                        const float2 v1 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c));
+                        const float2 v2 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c + 8));
+                        const float2 v3 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c + 8));
+                        ab[kk][0] = pack_bf16x2(v0.x, v0.y);
+                        ab[kk][1] = pack_bf16x2(v1.x, v1.y);
+                        ab[kk][2] = pack_bf16x2(v2.x, v2.y);
+                        ab[kk][3] = pack_bf16x2(v3.x, v3.y);
+                    }
+                    const uint64_t bd = wgmma_desc_sw64(wbase + t * W_TAP);
+                    wgmma_fence();
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (X3) {
-                            tf32_split(v[q], ah[k8][q], al[k8][q]);
-                        } else {
-                            ah[k8][q] = tf32_rna(v[q]);
+                    for (int kk = 0; kk < 2; ++kk) wgmma_m64n64k16_bf16(part, ab[kk], bd + 2 * kk, kk);
+                    wgmma_commit();
+                    wgmma_wait0();
+                    reg_fence(part);
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) acc[i] += part[i];
+                } else {
+                    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+                    for (int k8 = 0; k8 < 4; ++k8) {
+                        const int c = 8 * k8 + t4;
+                        const float v[4] = {*reinterpret_cast<const float*>(view + sw128_off(ra, c)),
+                                            *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c)),
+                                            *reinterpret_cast<const float*>(view + sw128_off(ra, c + 4)),
+                                            *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c + 4))};
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) {
+                            if (X3) {
+                                tf32_split(v[q], ah[k8][q], al[k8][q]);
+                            } else {
+                                ah[k8][q] = tf32_rna(v[q]);
+                            }
                         }
                     }
-                }
-                const uint64_t bd = wgmma_desc_sw128(wbase + t * W_TAP);
-                wgmma_fence();
+                    const uint64_t bd = wgmma_desc_sw128(wbase + t * W_TAP);
+                    wgmma_fence();
 #pragma unroll
-                for (int k8 = 0; k8 < 4; ++k8) {
-                    wgmma_m64n64k8_tf32(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous tap dropped)
-                    if (X3) {
-                        wgmma_m64n64k8_tf32(acs, ah[k8], bd + (TC_ATOM >> 4) + 2 * k8, 1);   // a_hi * w_lo
-                        wgmma_m64n64k8_tf32(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * w_hi
+                    for (int k8 = 0; k8 < 4; ++k8) {
+                        wgmma_m64n64k8_tf32(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous tap dropped)
+                        if (X3) {
+                            wgmma_m64n64k8_tf32(acs, ah[k8], bd + (TC_ATOM >> 4) + 2 * k8, 1);   // a_hi * w_lo
+                            wgmma_m64n64k8_tf32(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * w_hi
+                        }
                     }
-                }
-                wgmma_commit();
-                wgmma_wait0();
-                reg_fence(part);
-                if (X3) reg_fence(acs);
-                // The tensor core adds into its accumulator without IEEE rounding; a chain over all 3*C products drifts
-                // several times further from the exact sum than an fp32 FFMA chain does.  Each tap's 32 products are
-                // summed there from zero and added to the running sum here, rounded to nearest.
+                    wgmma_commit();
+                    wgmma_wait0();
+                    reg_fence(part);
+                    if (X3) reg_fence(acs);
+                    // The tensor core adds into its accumulator without IEEE rounding; a chain over all 3*C products drifts
+                    // several times further from the exact sum than an fp32 FFMA chain does.  Each tap's 32 products are
+                    // summed there from zero and added to the running sum here, rounded to nearest.
 #pragma unroll
-                for (int i = 0; i < 32; ++i) acc[i] += part[i];
+                    for (int i = 0; i < 32; ++i) acc[i] += part[i];
+                }
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[stage]);
@@ -346,8 +378,8 @@ static int tc_m_ctas(int N, int C, int tiles_per_image) {
 }
 
 // Shared memory: resident weights when they leave room for two stages, else streamed per stage.
-static bool tc_fit(int C, bool x3, TcPlan* p) {
-    const int w_atom = (x3 ? 2 : 1) * TC_ATOM;
+static bool tc_fit(int C, int prec, TcPlan* p) {
+    const int w_atom = tc_w_atom(prec);
     const int b_res = 3 * (C / TC_KCH) * w_atom;
     TcArgs& g = p->geo;
     g.a_bytes = g.nloads * g.load_rows * 128;
@@ -365,7 +397,7 @@ static bool tc_fit(int C, bool x3, TcPlan* p) {
 // Halo-slab plan: taps {-d, 0, +d} (forward) or {+d, 0, -d} (input gradient) along one axis.  TA x TB = 128 pixels with
 // TB a power of two such that the tap shift d*TB is a multiple of the 8-row swizzle period; the slab with the fewest
 // rows wins (tall tiles for the large dilations: halo 2d / TA).
-static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* dx, bool x3, TcPlan* p) {
+static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p) {
     if (!(C == 64 || C == 128) || N <= 0) return false;
     const bool vert = dy[0] != 0 || dy[2] != 0;
     const int* o = vert ? dy : dx;
@@ -396,13 +428,13 @@ static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* d
     g.load_a[0] = -dil;
     g.load_b[0] = 0;
     for (int t = 0; t < 3; ++t) g.tap_row[t] = (fwd_order ? t : 2 - t) * dil * g.TB;
-    if (!tc_fit(C, x3, p)) return false;
+    if (!tc_fit(C, prec, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
     return tc_get_encode_fn() != nullptr;
 }
 
 // Per-tap plan: any three taps; a bx x by = 128 pixel patch with bx | W, by | H (wide patches preferred).
-static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* dx, TcPlan* p) {
+static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p) {
     if (!(C == 64 || C == 128) || N <= 0) return false;
     TcArgs& g = p->geo;
     int sh = 7;
@@ -421,28 +453,40 @@ static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* d
         g.load_b[t] = dx ? dx[t] : 0;
         g.tap_row[t] = t * 128;
     }
-    if (!tc_fit(C, false, p)) return false;
+    if (!tc_fit(C, prec, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
     return tc_get_encode_fn() != nullptr;
 }
 
-template <int C, bool X3, bool RES>
+template <int C, int P, bool RES>
 static cudaError_t tc_launch(int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB,
                              const TcArgs& a) {
-    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel<C, X3, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT);
+    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel<C, P, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT);
     if (e != cudaSuccess) return e;
-    return lf_launch(conv1d_tc_kernel<C, X3, RES>, grid, TC_THREADS, smem_bytes, stream, tmA, tmB, a);
+    return lf_launch(conv1d_tc_kernel<C, P, RES>, grid, TC_THREADS, smem_bytes, stream, tmA, tmB, a);
 }
 
-static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, bool x3) {
+template <int P>
+static cudaError_t tc_launch_p(bool res, int C, int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
+                               const CUtensorMap& tmB, const TcArgs& a) {
+    if (C == 128) return res ? tc_launch<128, P, true>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<128, P, false>(grid, smem_bytes, stream, tmA, tmB, a);
+    return res ? tc_launch<64, P, true>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<64, P, false>(grid, smem_bytes, stream, tmA, tmB, a);
+}
+
+static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!args) return LF_ERR_INVALID_ARGUMENT;
     const LfConvTcArgs& p = *args;
     LF_REQUIRE(p.in && p.wpack && p.out);
     LF_REQUIRE(!p.mask_scale || (p.mask_shift && p.mask_src && p.stats_partial));
+    const bool x3 = prec == TC_X3;
     TcPlan pl{};
-    const bool slab = (x3 || g_tc_variant != 1) && tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, x3, &pl);
-    if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, &pl))) return LF_ERR_UNSUPPORTED;
+    // bf16 takes the slab exactly where TF32 does (its smaller weight tiles fit wherever the TF32 ones do), so that
+    // lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for both
+    const bool slab = (x3 || g_tc_variant != 1) &&
+                      (prec != TC_BF16 || tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, TC_TF32, &pl)) &&
+                      tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl);
+    if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl))) return LF_ERR_UNSUPPORTED;
     TcArgs a = pl.geo;
     a.out = p.out; a.bias = p.bias; a.mask_src = p.mask_src; a.add_src = p.add_src; a.add_mask = p.add_mask;
     a.colsum_partial = p.colsum_partial;
@@ -469,26 +513,26 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, bool x3) {
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
     {
-        // packed weights [Cout][3*C] (K contiguous); 3xTF32: [2][Cout][3*C] (hi, lo) as one [2*Cout][3*C] matrix
+        // packed weights [Cout][3*C] (K contiguous); 3xTF32: [2][Cout][3*C] (hi, lo) as one [2*Cout][3*C] matrix;
+        // bf16: [Cout][3*C] bf16, [64 x 32] boxes of 64-byte rows, 64B-swizzled
+        const bool bf = prec == TC_BF16;
+        const int esz = bf ? 2 : 4;
         cuuint64_t dims[2] = {(cuuint64_t)(3 * p.C), (cuuint64_t)((x3 ? 2 : 1) * p.C)};
-        cuuint64_t strides[1] = {(cuuint64_t)(3 * p.C) * 4};
+        cuuint64_t strides[1] = {(cuuint64_t)(3 * p.C) * esz};
         cuuint32_t box[2] = {32, TC_BN};
         cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(p.wpack), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+        CUresult r = enc(&tmB, bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                         const_cast<float*>(p.wpack), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         bf ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
     const int grid = pl.m_ctas * a.n_halves;
     const int s = pl.smem_bytes;
     cudaError_t e;
-    if (p.C == 128) {
-        if (x3) e = pl.res ? tc_launch<128, true, true>(grid, s, stream, tmA, tmB, a) : tc_launch<128, true, false>(grid, s, stream, tmA, tmB, a);
-        else e = pl.res ? tc_launch<128, false, true>(grid, s, stream, tmA, tmB, a) : tc_launch<128, false, false>(grid, s, stream, tmA, tmB, a);
-    } else {
-        if (x3) e = pl.res ? tc_launch<64, true, true>(grid, s, stream, tmA, tmB, a) : tc_launch<64, true, false>(grid, s, stream, tmA, tmB, a);
-        else e = pl.res ? tc_launch<64, false, true>(grid, s, stream, tmA, tmB, a) : tc_launch<64, false, false>(grid, s, stream, tmA, tmB, a);
-    }
+    if (prec == TC_X3) e = tc_launch_p<TC_X3>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
+    else if (prec == TC_BF16) e = tc_launch_p<TC_BF16>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
+    else e = tc_launch_p<TC_TF32>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
     return check_launch();
 }
@@ -500,19 +544,19 @@ using namespace lf;
 extern "C" void lf_conv1d_tc_set_variant(int v) { g_tc_variant = (v == 1) ? 1 : 2; }
 
 // 0 if the shape is unsupported, else the number of rows of the optional colsum_partial / stats_partial outputs.  Every
-// shape the slab plan takes is also taken by the per-tap plan (same number of CTAs), which serves the TF32 calls the slab
-// does not fit.
+// shape the slab plan takes is also taken by the per-tap plan (same number of CTAs), which serves the TF32 and bf16
+// calls the slab does not fit.  The bf16 entry serves exactly the shapes and slab cases of the TF32 one.
 extern "C" int lf_conv1d_tc_supported(int N, int H, int W, int C) {
     TcPlan pl{};
-    return tc_plan_taps(N, H, W, C, nullptr, nullptr, &pl) ? pl.m_ctas : 0;
+    return tc_plan_taps(N, H, W, C, nullptr, nullptr, TC_TF32, &pl) ? pl.m_ctas : 0;
 }
 
-// 1 if a TF32 call with these taps runs on the halo-slab path
+// 1 if a TF32 (or bf16) call with these taps runs on the halo-slab path
 extern "C" int lf_conv1d_tc_slab_ok(int N, int H, int W, int C, int vertical, int dil) {
     if (g_tc_variant == 1 || dil < 1) return 0;
     TcPlan pl{};
     const int zero[3] = {0, 0, 0}, off[3] = {-dil, 0, dil};
-    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, false, &pl) ? 1 : 0;
+    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_TF32, &pl) ? 1 : 0;
 }
 
 // rows of colsum_partial / stats_partial (= CTAs per 64-channel half), 0 if a 3xTF32 call with these taps is not served
@@ -520,8 +564,9 @@ extern "C" int lf_conv1d_tc_x3_rows(int N, int H, int W, int C, int vertical, in
     if (dil < 1) return 0;
     TcPlan pl{};
     const int zero[3] = {0, 0, 0}, off[3] = {-dil, 0, dil};
-    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, true, &pl) ? pl.m_ctas : 0;
+    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_X3, &pl) ? pl.m_ctas : 0;
 }
 
-extern "C" int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, false); }
-extern "C" int lf_conv1d_tc_x3(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, true); }
+extern "C" int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_TF32); }
+extern "C" int lf_conv1d_tc_x3(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_X3); }
+extern "C" int lf_conv1d_tc_bf16(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_BF16); }

@@ -17,8 +17,10 @@
 // shared memory); Ng is a run-time multiple of 16 (<= 128), covered by wgmma m64n16k8 column blocks.
 // Two consumer warpgroups own 64 pixel rows each (A fragments loaded from the swizzled box into registers, B through a
 // shared-memory descriptor), accumulate in registers and store the tile with bias / ReLU; warp 8 is the TMA producer.
-// precision 1 (3xTF32, template X3; arithmetic in tc_ptx.cuh): the weight chunk is the pre-split pair [W_hi rows | W_lo
-// rows] (one TMA box of 2*Ng rows); a_hi*w_hi accumulates apart from a_hi*w_lo + a_lo*w_hi and the two are added at the end.
+// precision 1 (3xTF32; arithmetic in tc_ptx.cuh): the weight chunk is the pre-split pair [W_hi rows | W_lo rows] (one
+// TMA box of 2*Ng rows); a_hi*w_hi accumulates apart from a_hi*w_lo + a_lo*w_hi and the two are added at the end.
+// precision 2 (bf16): the weight chunk is [Ng x 32] bf16 from the packer (64-byte rows, 64B-swizzled), the activations
+// are rounded to bf16 while their k16 fragments are formed; two wgmma m64n16k16 per column block and chunk.
 #include <cuda.h>
 
 #include "lf_common.cuh"
@@ -48,10 +50,11 @@ struct TgArgs {
     int total_tiles;
 };
 
-template <bool X3>
+template <int P>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 conv_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB, const TgArgs a) {
+    constexpr bool X3 = P == TC_X3;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -121,47 +124,81 @@ conv_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         for (int ks = 0; ks < ksteps; ++ks) {
             mbar_wait(&full[stage], phase);
             const uint8_t* st = smem + (size_t)stage * a.stage_bytes;
-            uint32_t ah[4][4], al[4][4];
+            if constexpr (P == TC_BF16) {
+                // k16 fragments (tc_ptx.cuh): two adjacent channels per register, one 8-byte load each; weight chunk
+                // [Ng x 32] bf16, 64B-swizzled, column block j = 16 rows = 1024 bytes
+                uint32_t ab[2][4];
 #pragma unroll
-            for (int k8 = 0; k8 < 4; ++k8) {
-                const int c = 8 * k8 + t4;
-                const float v[4] = {*reinterpret_cast<const float*>(st + sw128_off(ra, c)),
-                                    *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c)),
-                                    *reinterpret_cast<const float*>(st + sw128_off(ra, c + 4)),
-                                    *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c + 4))};
+                for (int kk = 0; kk < 2; ++kk) {
+                    const int c = 16 * kk + 2 * t4;
+                    const float2 v0 = *reinterpret_cast<const float2*>(st + sw128_off(ra, c));
+                    const float2 v1 = *reinterpret_cast<const float2*>(st + sw128_off(ra + 8, c));
+                    const float2 v2 = *reinterpret_cast<const float2*>(st + sw128_off(ra, c + 8));
+                    const float2 v3 = *reinterpret_cast<const float2*>(st + sw128_off(ra + 8, c + 8));
+                    ab[kk][0] = pack_bf16x2(v0.x, v0.y);
+                    ab[kk][1] = pack_bf16x2(v1.x, v1.y);
+                    ab[kk][2] = pack_bf16x2(v2.x, v2.y);
+                    ab[kk][3] = pack_bf16x2(v3.x, v3.y);
+                }
+                const uint64_t bd = wgmma_desc_sw64(smem_u32(st + TG_A_BYTES));
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    if (X3) {
-                        tf32_split(v[q], ah[k8][q], al[k8][q]);
-                    } else {
-                        ah[k8][q] = tf32_rna(v[q]);
+                for (int j = 0; j < TG_NB; ++j) {
+                    if (j < nblk) {
+                        const uint64_t bj = bd + (uint64_t)((j * 16 * 64) >> 4);
+                        float part[8];
+                        wgmma_fence();
+#pragma unroll
+                        for (int kk = 0; kk < 2; ++kk) wgmma_m64n16k16_bf16(part, ab[kk], bj + 2 * kk, kk);
+                        wgmma_commit();
+                        wgmma_wait0();
+                        reg_fence(part);
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) acc[j][i] += part[i];
                     }
                 }
-            }
-            const uint64_t bd = wgmma_desc_sw128(smem_u32(st + TG_A_BYTES));
-            const uint64_t lo_rows = (uint64_t)(a.Ng * 128) >> 4;   // W_lo rows follow the Ng W_hi rows
-            // One column block at a time: its 32 products are summed by the tensor core from zero and added to the running
-            // fp32 sum with a rounded FADD (the tensor core's own accumulation does not round like IEEE adds, see conv_tc.cu).
+            } else {
+                uint32_t ah[4][4], al[4][4];
 #pragma unroll
-            for (int j = 0; j < TG_NB; ++j) {
-                if (j < nblk) {
-                    const uint64_t bj = bd + (uint64_t)((j * 16 * 128) >> 4);
-                    float part[8];
-                    wgmma_fence();
+                for (int k8 = 0; k8 < 4; ++k8) {
+                    const int c = 8 * k8 + t4;
+                    const float v[4] = {*reinterpret_cast<const float*>(st + sw128_off(ra, c)),
+                                        *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c)),
+                                        *reinterpret_cast<const float*>(st + sw128_off(ra, c + 4)),
+                                        *reinterpret_cast<const float*>(st + sw128_off(ra + 8, c + 4))};
 #pragma unroll
-                    for (int k8 = 0; k8 < 4; ++k8) {
-                        wgmma_m64n16k8_tf32(part, ah[k8], bj + 2 * k8, k8);   // k8 = 0: part = product
+                    for (int q = 0; q < 4; ++q) {
                         if (X3) {
-                            wgmma_m64n16k8_tf32(acs[j], ah[k8], bj + lo_rows + 2 * k8, 1);   // a_hi * w_lo
-                            wgmma_m64n16k8_tf32(acs[j], al[k8], bj + 2 * k8, 1);             // a_lo * w_hi
+                            tf32_split(v[q], ah[k8][q], al[k8][q]);
+                        } else {
+                            ah[k8][q] = tf32_rna(v[q]);
                         }
                     }
-                    wgmma_commit();
-                    wgmma_wait0();
-                    reg_fence(part);
-                    if (X3) reg_fence(acs[j]);
+                }
+                const uint64_t bd = wgmma_desc_sw128(smem_u32(st + TG_A_BYTES));
+                const uint64_t lo_rows = (uint64_t)(a.Ng * 128) >> 4;   // W_lo rows follow the Ng W_hi rows
+                // One column block at a time: its 32 products are summed by the tensor core from zero and added to the running
+                // fp32 sum with a rounded FADD (the tensor core's own accumulation does not round like IEEE adds, see conv_tc.cu).
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) acc[j][i] += part[i];
+                for (int j = 0; j < TG_NB; ++j) {
+                    if (j < nblk) {
+                        const uint64_t bj = bd + (uint64_t)((j * 16 * 128) >> 4);
+                        float part[8];
+                        wgmma_fence();
+#pragma unroll
+                        for (int k8 = 0; k8 < 4; ++k8) {
+                            wgmma_m64n16k8_tf32(part, ah[k8], bj + 2 * k8, k8);   // k8 = 0: part = product
+                            if (X3) {
+                                wgmma_m64n16k8_tf32(acs[j], ah[k8], bj + lo_rows + 2 * k8, 1);   // a_hi * w_lo
+                                wgmma_m64n16k8_tf32(acs[j], al[k8], bj + 2 * k8, 1);             // a_lo * w_hi
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait0();
+                        reg_fence(part);
+                        if (X3) reg_fence(acs[j]);
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) acc[j][i] += part[i];
+                    }
                 }
             }
             __syncwarp();
@@ -228,6 +265,15 @@ static bool tg_encode_view(TcEncodeTiledFn enc, CUtensorMap* tm, const LfTcgView
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+template <int P>
+static cudaError_t tg_launch(int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
+                             const CUtensorMap& tmB, const TgArgs& a) {
+    cudaError_t e = cudaFuncSetAttribute(conv_tcg_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM_LIMIT);
+    if (e != cudaSuccess) return e;
+    lf_launch(conv_tcg_kernel<P>, grid, TG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    return cudaSuccess;
+}
+
 }  // namespace lf
 
 using namespace lf;
@@ -260,10 +306,10 @@ extern "C" int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream_) {
         two = two || p.map[t] == 1;
     }
     LF_REQUIRE(!two || p.a[1].ptr);
-    LF_REQUIRE(p.precision == 0 || p.precision == 1);
-    const bool x3 = p.precision == 1;
+    LF_REQUIRE(p.precision == TC_TF32 || p.precision == TC_X3 || p.precision == TC_BF16);
+    const bool x3 = p.precision == TC_X3, bf = p.precision == TC_BF16;
     const int nb = x3 ? 2 * p.Ng : p.Ng;   // rows of the weight chunk: W, or W_hi | W_lo
-    a.stage_bytes = TG_A_BYTES + nb * 128;
+    a.stage_bytes = TG_A_BYTES + nb * (bf ? 64 : 128);   // bf16 rows: 32 bf16 = 64 bytes (Ng * 64 is a 1024 multiple)
     int stages = (TG_SMEM_LIMIT - 1024 - 256) / a.stage_bytes;
     if (stages > TG_MAX_STAGES) stages = TG_MAX_STAGES;
     a.stages = stages;
@@ -273,24 +319,25 @@ extern "C" int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream_) {
     if (!tg_encode_view(enc, &tmA0, p.a[0], p.N, p.Kc, a.bx, a.by)) return LF_ERR_CUDA;
     if (!tg_encode_view(enc, &tmA1, two ? p.a[1] : p.a[0], p.N, p.Kc, a.bx, a.by)) return LF_ERR_CUDA;
     {
-        // weights [Ng][ntaps*Kc] (K contiguous); 3xTF32: [2][Ng][ntaps*Kc] = hi rows, then lo rows, one box of 2*Ng rows
+        // weights [Ng][ntaps*Kc] (K contiguous); 3xTF32: [2][Ng][ntaps*Kc] = hi rows, then lo rows, one box of 2*Ng rows;
+        // bf16: [Ng][ntaps*Kc] bf16, 64B-swizzled
         const int K = p.ntaps * p.Kc;
         cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)nb};
-        cuuint64_t strides[1] = {(cuuint64_t)K * 4};
+        cuuint64_t strides[1] = {(cuuint64_t)K * (bf ? 2 : 4)};
         cuuint32_t box[2] = {32, (cuuint32_t)nb};
         cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(p.wg), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+        CUresult r = enc(&tmB, bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                         const_cast<float*>(p.wg), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         bf ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
     const int sms = device_sms();
     const int grid = a.total_tiles < sms ? a.total_tiles : sms;
     const int smem_bytes = 1024 + a.stages * a.stage_bytes + 256;
-    cudaError_t e = x3 ? cudaFuncSetAttribute(conv_tcg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM_LIMIT)
-                       : cudaFuncSetAttribute(conv_tcg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM_LIMIT);
+    cudaError_t e = x3 ? tg_launch<TC_X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                    : bf ? tg_launch<TC_BF16>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                         : tg_launch<TC_TF32>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
-    if (x3) lf_launch(conv_tcg_kernel<true>, grid, TG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
-    else lf_launch(conv_tcg_kernel<false>, grid, TG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
     return check_launch();
 }

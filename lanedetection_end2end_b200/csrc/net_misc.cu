@@ -666,11 +666,13 @@ extern "C" int lf_outconv_bwd_weight(const float* x, const float* d_out, int N, 
 // ------------------------------------------------------------------------------------------
 struct PackJob {
     const float* src;
-    float* dst;
+    void* dst;
     const int* idx;
     long long n;
+    int dst_dtype;   // LF_F32, or LF_BF16: the operand of the bf16 convolution mode, rounded to nearest even
+    int pad;
 };
-static_assert(sizeof(PackJob) == 32, "LfPackJob layout");
+static_assert(sizeof(PackJob) == 40, "LfPackJob layout");
 
 __global__ void __launch_bounds__(256) pack_gather_kernel(const PackJob* __restrict__ jobs) {
     pdl_entry();
@@ -684,7 +686,8 @@ __global__ void __launch_bounds__(256) pack_gather_kernel(const PackJob* __restr
             const float hi = __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u);
             v = (i & LF_PACK_TF32_HI) ? hi : __uint_as_float((__float_as_uint(v - hi) + 0x1000u) & 0xffffe000u);
         }
-        j.dst[k] = v;
+        if (j.dst_dtype == LF_BF16) static_cast<__nv_bfloat16*>(j.dst)[k] = __float2bfloat16_rn(v);
+        else static_cast<float*>(j.dst)[k] = v;
     }
 }
 

@@ -1,5 +1,5 @@
-// Shared Hopper (sm_90a) tensor-core PTX wrappers: TMA, mbarrier, wgmma, shared-memory accesses, TF32 operand
-// splitting and the tensor-map helpers.
+// Shared Hopper (sm_90a) tensor-core PTX wrappers: TMA, mbarrier, wgmma (TF32 and BF16), shared-memory accesses, TF32
+// operand splitting, bf16 packing and the tensor-map helpers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -159,6 +159,89 @@ __device__ __forceinline__ void wgmma_m64k8_tf32(float (&d)[N / 2], const uint32
     else if constexpr (N == 32) wgmma_m64n32k8_tf32(d, a, bdesc, accumulate);
     else if constexpr (N == 48) wgmma_m64n48k8_tf32(d, a, bdesc, accumulate);
     else wgmma_m64n64k8_tf32(d, a, bdesc, accumulate);
+}
+
+// ------------------------------------------------------------------------------------------
+// BF16 operands (the "bf16" convolution mode): both operands rounded to bf16 (round to nearest even), products exact in
+// fp32, fp32 accumulate.  Operand precision of the tensor-core kernel templates (= the `precision` fields of the C ABI):
+// ------------------------------------------------------------------------------------------
+enum TcPrec : int { TC_TF32 = 0, TC_X3 = 1, TC_BF16 = 2 };
+
+// bf16x2 of (lo, hi), round to nearest even: `lo` in bits 0-15 (the lower K index of a fragment register)
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+
+// B operand: K-major, 64B-swizzled bf16 tile in shared memory (rows of 32 bf16 = 64 bytes, 8-row groups 512 bytes
+// apart) = what TMA writes for a [rows x 32] bf16 box with CU_TENSOR_MAP_SWIZZLE_64B: the 16-byte chunk index within a
+// row is XORed with (r >> 1) & 3.  Descriptor: layout 2 = SWIZZLE_64B, SBO = 512; the tile base must be 512-byte
+// aligned; the k-th group of 16 bf16 along K starts 32*k bytes later (+2 in the start field).
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
+}
+// Byte offset of bf16 element (row r, k < 32) of such a tile
+__device__ __forceinline__ uint32_t sw64_off(int r, int k) { return (uint32_t)(r * 64 + ((((k >> 3) ^ (r >> 1)) & 3) << 4) + ((k & 7) << 1)); }
+
+// A operand: registers, the m64k16 BF16 fragment of this thread (PTX ISA, "Register fragment for matrix A" of
+// wgmma .m64nNk16), two bf16 per register, the lower K index in the low half:
+//   a[0] = A[16w + g][2t, 2t+1],     a[1] = A[16w + g + 8][2t, 2t+1],
+//   a[2] = A[16w + g][2t+8, 2t+9],   a[3] = A[16w + g + 8][2t+8, 2t+9]
+// (w, g, t as for TF32).  The accumulator fragment is the one of the TF32 instructions.  B K-major: imm-trans-b = 0.
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, BF16 in, fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 48] (+)= A[64 x 16] * B[48 x 16]^T
+__device__ __forceinline__ void wgmma_m64n48k16_bf16(float (&d)[24], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+        "{%24, %25, %26, %27}, %28, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T
+__device__ __forceinline__ void wgmma_m64n32k16_bf16(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T
+__device__ __forceinline__ void wgmma_m64n16k16_bf16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T for N in {16, 32, 48, 64}
+template <int N>
+__device__ __forceinline__ void wgmma_m64k16_bf16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    static_assert(N == 16 || N == 32 || N == 48 || N == 64, "wgmma_m64k16_bf16: N");
+    if constexpr (N == 16) wgmma_m64n16k16_bf16(d, a, bdesc, accumulate);
+    else if constexpr (N == 32) wgmma_m64n32k16_bf16(d, a, bdesc, accumulate);
+    else if constexpr (N == 48) wgmma_m64n48k16_bf16(d, a, bdesc, accumulate);
+    else wgmma_m64n64k16_bf16(d, a, bdesc, accumulate);
 }
 
 // Shared-state-space accesses (addresses from smem_u32): LDS / STS without generic-address translation.

@@ -28,6 +28,11 @@
 //    with FADD (the tensor core's accumulation drifts further than an FFMA chain over 10^4+ pixels); 3xTF32
 //    (tc_ptx.cuh): every product is a_hi*b_hi + (a_hi*b_lo + a_lo*b_hi), the correction terms accumulated on the tensor
 //    core and added in the epilogue.
+// BF16 (precision 2): an m64k16 A register packs two pixels of one channel (two LDS from two box rows); the transposition
+// writes bf16 pixel pairs into a 64B-swizzled K-major [NW x 32 px] tile, one 32-bit store each after lane pairs swap half
+// their columns.  BF16 wgmma could read B MN-major (imm-trans-b = 1) and skip the transposition, but the K-major tile
+// keeps one B layout and descriptor (wgmma_desc_sw64) for all three tensor-core kernels; double-buffering and the proxy
+// fence are unchanged.  Two wgmma m64nNWk16 per stage.
 // The next stage's fragments are not loaded while a stage's wgmma runs: ptxas then reuses the A registers the running
 // wgmma still reads.  Every CTA writes its slice [64 rows][Nn] of one partial; lf_wgrad_reduce sums them in fixed order.
 #include <cuda.h>
@@ -57,22 +62,26 @@ struct WgtArgs {
 // B columns per consumer warpgroup for Nn B columns: Nn itself (the warpgroups take alternate stages) up to 64; above,
 // three m64nNn accumulator sets would not fit the 168 registers a thread has here (each warpgroup takes half the columns)
 constexpr int wgt_cols(int nn) { return nn <= 64 ? nn : nn / 2; }
-// shared memory of the transposed B tiles: [2 warpgroups][2 buffers][hi (, lo)] x [cols x 32 px]
-constexpr int wgt_bt_bytes(int nn, bool x3) { return 2 * 2 * (x3 ? 2 : 1) * wgt_cols(nn) * 128; }
+// shared memory of one warpgroup's transposed B tiles: [2 buffers][hi (, lo)] x [cols x 32 px].  bf16 tiles are half the
+// size, but the region keeps the TF32 size: warpgroup 1 hands its cols/2 fp32 sums per thread over through it at the end.
+constexpr int wgt_wg_bytes(int nn, int prec) { return 2 * (prec == TC_X3 ? 2 : 1) * wgt_cols(nn) * 128; }
+constexpr int wgt_bt_bytes(int nn, int prec) { return 2 * wgt_wg_bytes(nn, prec); }
 
-template <int NN, bool X3>
+template <int NN, int P>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmB, const WgtArgs a) {
+    constexpr bool X3 = P == TC_X3, BF = P == TC_BF16;
     constexpr int NW = wgt_cols(NN);                    // B columns per warpgroup = wgmma N
     constexpr bool KSPLIT = NW == NN;                   // warpgroups split the stages, not the columns
-    constexpr int BT_TILE = NW * 128;                   // one K-major [NW x 32 px] tile (1024-byte multiple)
+    constexpr int BT_TILE = NW * (BF ? 64 : 128);       // one K-major [NW x 32 px] tile (TF32: 1024-, bf16: 512-byte multiple)
     constexpr int BT_SET = (X3 ? 2 : 1) * BT_TILE;      // hi tile, then lo tile
+    constexpr int BT_WG = wgt_wg_bytes(NN, P);          // one warpgroup's region (two sets, or the final hand-over)
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* bt = smem + (size_t)a.stages * a.stage_bytes;
-    uint64_t* full = reinterpret_cast<uint64_t*>(bt + wgt_bt_bytes(NN, X3));
+    uint64_t* full = reinterpret_cast<uint64_t*>(bt + wgt_bt_bytes(NN, P));
     uint64_t* empty = full + WG_MAX_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -132,7 +141,7 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     const bool rows_ok = (wl >> 1) < na;   // false: the second block of an odd list's last pair (A = 0, not stored)
     const int arow = 16 * (wl & 1) + g;
     const int c0 = KSPLIT ? 0 : wg * NW;
-    const uint32_t bt_wg = smem_u32(bt) + wg * 2 * BT_SET;
+    const uint32_t bt_wg = smem_u32(bt) + wg * BT_WG;
     float acc[NW / 2], part[NW / 2], acs[NW / 2];   // running sum; one stage's large term; 3xTF32 correction terms
 #pragma unroll
     for (int i = 0; i < NW / 2; ++i) acc[i] = part[i] = acs[i] = 0.f;
@@ -143,15 +152,28 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         mbar_wait(&full[stage], (j / a.stages) & 1);
         const uint32_t st = smem_u32(smem) + stage * a.stage_bytes;
         // A fragments (a[0..3] = A[arow][k0], A[arow + 8][k0], A[arow][k0 + 4], A[arow + 8][k0 + 4], A[c][k] = X[px k][ch c])
+        // bf16 (m64k16): register q of step kk holds pixels k0, k0 + 1 (k0 = 16 kk + 2 t4, + 8 for q >= 2) of channel
+        // arow (+ 8 for odd q) = two LDS from two box rows; av[kk][q] / av[kk][4 + q] are the low / high halves
         float av[WG_KP / 8][4];
         const uint32_t abox = st + (a.nb_b + (wl >> 1)) * WG_BOX;
+        if constexpr (BF) {
 #pragma unroll
-        for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
-            const int k0 = 8 * k8 + t4;
-            av[k8][0] = rows_ok ? lds_f32(abox + sw128_off(k0, arow)) : 0.f;
-            av[k8][1] = rows_ok ? lds_f32(abox + sw128_off(k0, arow + 8)) : 0.f;
-            av[k8][2] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow)) : 0.f;
-            av[k8][3] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow + 8)) : 0.f;
+            for (int kk = 0; kk < WG_KP / 16; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int k0 = 16 * kk + 2 * t4 + 8 * (q >> 1), r = arow + 8 * (q & 1);
+                    av[2 * kk][q] = rows_ok ? lds_f32(abox + sw128_off(k0, r)) : 0.f;
+                    av[2 * kk + 1][q] = rows_ok ? lds_f32(abox + sw128_off(k0 + 1, r)) : 0.f;
+                }
+        } else {
+#pragma unroll
+            for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
+                const int k0 = 8 * k8 + t4;
+                av[k8][0] = rows_ok ? lds_f32(abox + sw128_off(k0, arow)) : 0.f;
+                av[k8][1] = rows_ok ? lds_f32(abox + sw128_off(k0, arow + 8)) : 0.f;
+                av[k8][2] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow)) : 0.f;
+                av[k8][3] = rows_ok ? lds_f32(abox + sw128_off(k0 + 4, arow + 8)) : 0.f;
+            }
         }
         // transpose: warp wl takes the 4-column chunks q = wl + 4i of this warpgroup's columns, lane = pixel.  Reads are
         // one 16-byte chunk per lane, writes one column (32 pixels = one swizzled 128-byte row): both conflict-free.
@@ -162,16 +184,27 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
             const int n = c0 + 4 * q;   // first B column of the chunk
             const float4 v4 = lds_f32x4(st + (n >> 5) * WG_BOX + sw128_off(lane, n & 31));
             const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+            if constexpr (BF) {
+                // a bf16 pair of pixels (2m, 2m + 1) per 32-bit store: lane pairs swap half their columns, the even lane
+                // then stores columns 0, 1 of the chunk and the odd lane columns 2, 3, at pixel pair m = lane / 2
+                const bool odd = lane & 1;
+                const float r0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 1);
+                const float r1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 1);
+                const int e0 = odd ? 2 : 0;
+                sts_u32(bhi + sw64_off(4 * q + e0, lane & ~1), odd ? pack_bf16x2(r0, v[2]) : pack_bf16x2(v[0], r0));
+                sts_u32(bhi + sw64_off(4 * q + e0 + 1, lane & ~1), odd ? pack_bf16x2(r1, v[3]) : pack_bf16x2(v[1], r1));
+            } else {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const uint32_t off = sw128_off(4 * q + e, lane);
-                if (X3) {
-                    uint32_t hi, lo;
-                    tf32_split(v[e], hi, lo);
-                    sts_u32(bhi + off, hi);
-                    sts_u32(bhi + BT_TILE + off, lo);
-                } else {
-                    sts_u32(bhi + off, tf32_rna(v[e]));
+                for (int e = 0; e < 4; ++e) {
+                    const uint32_t off = sw128_off(4 * q + e, lane);
+                    if (X3) {
+                        uint32_t hi, lo;
+                        tf32_split(v[e], hi, lo);
+                        sts_u32(bhi + off, hi);
+                        sts_u32(bhi + BT_TILE + off, lo);
+                    } else {
+                        sts_u32(bhi + off, tf32_rna(v[e]));
+                    }
                 }
             }
         }
@@ -180,7 +213,9 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         for (int k8 = 0; k8 < WG_KP / 8; ++k8)
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
-                if (X3) {
+                if (BF) {
+                    if (k8 < WG_KP / 16) ah[k8][q] = pack_bf16x2(av[2 * k8][q], av[2 * k8 + 1][q]);
+                } else if (X3) {
                     tf32_split(av[k8][q], ah[k8][q], al[k8][q]);
                 } else {
                     ah[k8][q] = tf32_rna(av[k8][q]);
@@ -188,14 +223,19 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
             }
         fence_proxy_async_smem();
         named_bar_sync(1 + wg, 128);   // the warpgroup's B tiles are complete
-        const uint64_t bd = wgmma_desc_sw128(bhi);
+        const uint64_t bd = BF ? wgmma_desc_sw64(bhi) : wgmma_desc_sw128(bhi);
         wgmma_fence();
+        if constexpr (BF) {
 #pragma unroll
-        for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
-            wgmma_m64k8_tf32<NW>(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous stage dropped)
-            if (X3) {
-                wgmma_m64k8_tf32<NW>(acs, ah[k8], bd + (BT_TILE >> 4) + 2 * k8, 1);   // a_hi * b_lo
-                wgmma_m64k8_tf32<NW>(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * b_hi
+            for (int kk = 0; kk < WG_KP / 16; ++kk) wgmma_m64k16_bf16<NW>(part, ah[kk], bd + 2 * kk, kk);
+        } else {
+#pragma unroll
+            for (int k8 = 0; k8 < WG_KP / 8; ++k8) {
+                wgmma_m64k8_tf32<NW>(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous stage dropped)
+                if (X3) {
+                    wgmma_m64k8_tf32<NW>(acs, ah[k8], bd + (BT_TILE >> 4) + 2 * k8, 1);   // a_hi * b_lo
+                    wgmma_m64k8_tf32<NW>(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * b_hi
+                }
             }
         }
         wgmma_commit();
@@ -215,7 +255,7 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     if (KSPLIT) {
         // warpgroup 1 hands its sums to warpgroup 0 through its own (now idle) B buffers, same fragment order; the two
         // halves are added in a fixed order
-        float* xfer = reinterpret_cast<float*>(bt + BT_SET * 2) + (threadIdx.x & 127) * (NW / 2);
+        float* xfer = reinterpret_cast<float*>(bt + BT_WG) + (threadIdx.x & 127) * (NW / 2);
         if (wg == 1) {
 #pragma unroll
             for (int i = 0; i < NW / 2; i += 2) *reinterpret_cast<float2*>(xfer + i) = make_float2(acc[i], acc[i + 1]);
@@ -273,28 +313,28 @@ static int wgt_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) {
     return wgt_split((long long)N * (Hs / by) * (Ws / bx), 4, nblocks);
 }
 
-template <int NN, bool X3>
+template <int NN, int P>
 static cudaError_t wgt_launch(dim3 grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
                               const CUtensorMap& tmB, const WgtArgs& a) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tcg_kernel<NN, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tcg_kernel<NN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return e;
-    return lf_launch(wgrad_tcg_kernel<NN, X3>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    return lf_launch(wgrad_tcg_kernel<NN, P>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
 }
 
-template <bool X3>
+template <int P>
 static cudaError_t wgt_launch_nn(dim3 grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
                                  const CUtensorMap& tmB, const WgtArgs& a) {
     switch (a.Nn) {
-        case 32: return wgt_launch<32, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
-        case 64: return wgt_launch<64, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
-        case 96: return wgt_launch<96, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
-        default: return wgt_launch<128, X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        case 32: return wgt_launch<32, P>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        case 64: return wgt_launch<64, P>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        case 96: return wgt_launch<96, P>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+        default: return wgt_launch<128, P>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
     }
 }
 
 // a: A views and their block table, b: the B view; the launch of the generic kernel
 static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int Ws, int Ka, int Nn, int nblocks, const int* map,
-                   const int* dy, const int* dx, const int* cblk, float* partial, int nsplit, bool x3, cudaStream_t stream) {
+                   const int* dy, const int* dx, const int* cblk, float* partial, int nsplit, int prec, cudaStream_t stream) {
     TcEncodeTiledFn enc = tc_get_encode_fn();
     if (!enc) return LF_ERR_UNSUPPORTED;
     WgtArgs a{};
@@ -308,7 +348,7 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
         two = two || map[b] == 1;
     }
     LF_REQUIRE(!two || av[1].ptr);
-    const int fixed = 1024 + wgt_bt_bytes(Nn, x3) + 256;   // alignment slack + transposed B tiles + barriers
+    const int fixed = 1024 + wgt_bt_bytes(Nn, prec) + 256;   // alignment slack + transposed B tiles + barriers
     a.stage_bytes = (a.nb_b + 2) * WG_BOX;
     int stages = (WG_SMEM_LIMIT - fixed) / a.stage_bytes;
     if (stages > WG_MAX_STAGES) stages = WG_MAX_STAGES;
@@ -321,8 +361,9 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
     if (!wgt_encode(enc, &tmB, bv, N, Nn, a.bx, a.by)) return LF_ERR_CUDA;
     const int smem_bytes = fixed + a.stages * a.stage_bytes;
     const dim3 grid(nsplit, (nblocks + 1) / 2);
-    const cudaError_t e = x3 ? wgt_launch_nn<true>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
-                             : wgt_launch_nn<false>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    const cudaError_t e = prec == TC_X3     ? wgt_launch_nn<TC_X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                          : prec == TC_BF16 ? wgt_launch_nn<TC_BF16>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                                            : wgt_launch_nn<TC_TF32>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
     return check_launch();
 }
@@ -334,14 +375,15 @@ using namespace lf;
 // number of split-K slices (= partials) lf_wgrad_tcg will use, 0 = unsupported
 extern "C" int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
 extern "C" int lf_wgrad_tcg_ctas_x3(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
+extern "C" int lf_wgrad_tcg_ctas_bf16(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
 
 extern "C" int lf_wgrad_tcg(const LfWgradTcgArgs* args, lf_stream_t stream_) {
     if (!args) return LF_ERR_INVALID_ARGUMENT;
     const LfWgradTcgArgs& p = *args;
     LF_REQUIRE(p.a[0].ptr && p.b.ptr && p.partial && p.nctas >= 1);
-    LF_REQUIRE(p.precision == 0 || p.precision == 1);
+    LF_REQUIRE(p.precision == TC_TF32 || p.precision == TC_X3 || p.precision == TC_BF16);
     if (!wgt_ctas(p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks)) return LF_ERR_UNSUPPORTED;
-    return wgt_run(p.a, p.b, p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks, p.map, p.dy, p.dx, p.cblk, p.partial, p.nctas, p.precision == 1,
+    return wgt_run(p.a, p.b, p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks, p.map, p.dy, p.dx, p.cblk, p.partial, p.nctas, p.precision,
                    reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -355,7 +397,7 @@ static int wgrad3_ctas(int N, int H, int W, int C, int min_per) {
 }
 
 static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                      float* partial, int nctas, bool x3, lf_stream_t stream_) {
+                      float* partial, int nctas, int prec, lf_stream_t stream_) {
     LF_REQUIRE(x && dy && partial && tap_dy && tap_dx && nctas >= 1);
     if (!(C == 64 || C == 128)) return LF_ERR_UNSUPPORTED;
     const LfTcgView xv{x, H, W, (long long)H * W * C, (long long)W * C, C};
@@ -368,17 +410,22 @@ static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int 
             const int b = t * cbs + cb;
             map[b] = 0; bdy[b] = tap_dy[t]; bdx[b] = tap_dx[t]; cblk[b] = cb;
         }
-    return wgt_run(av, gv, N, H, W, C, C, 3 * cbs, map, bdy, bdx, cblk, partial, nctas, x3, reinterpret_cast<cudaStream_t>(stream_));
+    return wgt_run(av, gv, N, H, W, C, C, 3 * cbs, map, bdy, bdx, cblk, partial, nctas, prec, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int lf_wgrad3_tc_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 4); }
 extern "C" int lf_wgrad3_tc_x3_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 8); }
+extern "C" int lf_wgrad3_tc_bf16_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 4); }
 extern "C" int lf_wgrad3_tc(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
                             float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, false, stream);
+    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_TF32, stream);
 }
 extern "C" int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
                                float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, true, stream);
+    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_X3, stream);
+}
+extern "C" int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
+                                 float* partial, int nctas, lf_stream_t stream) {
+    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_BF16, stream);
 }
 

@@ -63,7 +63,7 @@ def nb1d(x, mod):
             w = conv.weight.detach() * scale.view(-1, 1, 1, 1)
             b = conv.bias.detach() * scale + shift
             wp = o.pack_tc_super(w, False, False) if sup else o.pack_tc_fwd(w)
-            res.append(((o.split_tf32(wp) if o.x3_mode() else wp).contiguous(), b.contiguous()))
+            res.append((o.tc_operand(wp).contiguous(), b.contiguous()))
         return res
 
     (wp2, b2), (wp4, b4) = _cached(mod, [c2.weight, c2.bias, c4.weight, c4.bias] + _bn_tensors(mod.bn1) + _bn_tensors(mod.bn2), build)
@@ -86,7 +86,7 @@ def down(x, mod):
         wf = w.detach() * scale[:cc].view(-1, 1, 1, 1)
         b = mod.conv.bias.detach() * scale[:cc] + shift[:cc]
         wg = o.pack_tcg_s2conv(wf)
-        return (o.split_tf32(wg) if o.x3_mode() else wg).contiguous(), b.contiguous(), scale.contiguous(), shift.contiguous()
+        return o.tc_operand(wg).contiguous(), b.contiguous(), scale.contiguous(), shift.contiguous()
 
     wg, b, scale, shift = _cached(mod, [w, mod.conv.bias] + _bn_tensors(mod.bn), build)
     cat = torch.empty(N, H // 2, W // 2, cc + cin, dtype=torch.float32, device=x.device)
@@ -108,7 +108,7 @@ def up(x, mod):
         wf = w.detach() * scale.view(1, -1, 1, 1)
         b = (mod.conv.bias.detach() * scale + shift).repeat(2)
         wgs = tuple(o.pack_tcg_s2convT(wf, par, ci) for par in (0, 1))
-        return tuple((o.split_tf32(g) if o.x3_mode() else g).contiguous() for g in wgs), b.contiguous()
+        return tuple(o.tc_operand(g).contiguous() for g in wgs), b.contiguous()
 
     wgs, b2 = _cached(mod, [w, mod.conv.bias] + _bn_tensors(mod.bn), build)
     out = torch.empty(N, 2 * H, 2 * W, co, dtype=torch.float32, device=x.device)

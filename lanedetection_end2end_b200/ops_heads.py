@@ -44,7 +44,7 @@ def run_tcg_dense(x, wg, taps, Ng, out, bias=None):
     a.wg, a.bias, a.out = wg.data_ptr(), (bias.data_ptr() if bias is not None else None), out.data_ptr()
     a.osn, a.osy, a.osx, a.oy_mul, a.oy0 = H * W * cot, W * cot, cot, 1, 0
     a.N, a.Hs, a.Ws, a.Kc, a.Ng, a.ntaps = N, H, W, C, Ng, len(taps)
-    a.precision = int(wg.dim() == 3)
+    a.precision = o.tcg_precision(wg)
     for t, (dy, dx) in enumerate(taps):
         a.map[t], a.dy[t], a.dx[t] = 0, dy, dx
     _capi.call("lf_conv_tcg", ctypes.byref(a), o._stream(), flops=2 * N * H * W * len(taps) * C * Ng,
@@ -58,7 +58,7 @@ def conv_fwd(x, w, b):
     Co, _, kh, kw = w.shape
     out = torch.empty(N, H, W, Co, dtype=torch.float32, device=x.device)
     if dense_tcg_ok(x, Co):
-        return run_tcg_dense(x, o.packed(w, "tc_fwd", o.pack_tc_fwd, split=o.x3_mode()), _taps(kh, kw), Co, out, bias=b)
+        return run_tcg_dense(x, o.packed(w, "tc_fwd", o.pack_tc_fwd, split=o.pack_split()), _taps(kh, kw), Co, out, bias=b)
     phases, _ = plans.conv_fwd_plan(H, W, kh, kw, 1, (kh - 1) // 2, (kw - 1) // 2, 1, 1)
     return o.run_conv(phases, x, o.packed(w, "conv_fwd", o.pack_conv_fwd), Ci, out, Co, bias=b)
 
@@ -68,7 +68,7 @@ def conv_dgrad(dy, w):
     _, Ci, kh, kw = w.shape
     dx = torch.empty(N, H, W, Ci, dtype=torch.float32, device=dy.device)
     if dense_tcg_ok(dy, Ci):
-        return run_tcg_dense(dy, o.packed(w, "tc_dgrad", o.pack_tc_dgrad, split=o.x3_mode()), _taps(kh, kw, mirror=True), Ci, dx)
+        return run_tcg_dense(dy, o.packed(w, "tc_dgrad", o.pack_tc_dgrad, split=o.pack_split()), _taps(kh, kw, mirror=True), Ci, dx)
     phases, _ = plans.conv_dgrad_plan_s1(H, W, kh, kw, (kh - 1) // 2, (kw - 1) // 2, 1, 1)
     return o.run_conv(phases, dy, o.packed(w, "conv_dgrad", o.pack_conv_dgrad), Co, dx, Ci)
 
@@ -103,7 +103,7 @@ def _wgrad_tcg_dense(x, dy, taps):
         a.a[1] = a.a[0]
         a.b = o._tcg_view(dy, H, W, H * W * Co, W * Co, Co)
         a.partial, a.N, a.Hs, a.Ws, a.Ka, a.Nn, a.nblocks, a.nctas = partial.data_ptr(), N, H, W, Ci, Co, nblocks, nctas
-        a.precision = int(o.wgrad_x3())
+        a.precision = o.wgrad_precision()
         for i in range(nblocks):
             dyy, dxx = taps[t0 + i // per_tap]
             a.map[i], a.dy[i], a.dx[i], a.cblk[i] = 0, dyy, dxx, i % per_tap

@@ -28,8 +28,10 @@ LfConvArgs, LfWgradArgs, LfConvTcArgs = _capi.LfConvArgs, _capi.LfWgradArgs, _ca
 #           default, and the mode bench.py times (csrc/conv_tc.cu);
 #   "tf32": tensor cores, single-pass TF32 multiply / fp32 accumulate (what cuDNN does for the reference's
 #           fp32 convs on Ampere+ GPUs; 1e-3 from fp32 on the curve coefficients -- a labelled extra);
+#   "bf16": tensor cores, both operands rounded to bf16 (nearest even) inside the kernels, exact products, fp32
+#           accumulate; storage stays fp32 (a labelled fast mode, ~5e-3 from fp64 on the curve coefficients);
 #   shapes a tensor-core kernel does not take stay on the fp32 kernel in every mode.
-CONV_MODES = ("fp32", "tf32", "tf32x3")
+CONV_MODES = ("fp32", "tf32", "tf32x3", "bf16")
 CONV_MODE = os.environ.get("LANEFIT_CONV_MODE", "tf32x3")
 
 
@@ -41,12 +43,32 @@ def set_conv_mode(mode):
 
 
 def tc_mode():
-    """True when the dense convolutions run on tensor cores (either TF32 flavour)."""
-    return CONV_MODE in ("tf32", "tf32x3")
+    """True when the dense convolutions run on tensor cores (TF32, 3xTF32 or BF16)."""
+    return CONV_MODE in ("tf32", "tf32x3", "bf16")
 
 
 def x3_mode():
     return CONV_MODE == "tf32x3"
+
+
+def bf16_mode():
+    return CONV_MODE == "bf16"
+
+
+def pack_split():
+    """The operand form the active mode's tensor-core kernels read, as the ``split`` argument of packed():
+    True = the TF32 hi/lo pair (tf32x3), "bf16" = bf16 operand, False = the fp32 operand."""
+    return "bf16" if bf16_mode() else x3_mode()
+
+
+def tc_operand(t):
+    """A packed fp32 tensor-core operand in the active mode's form (what packed() serves for ``pack_split()``)."""
+    return split_tf32(t) if x3_mode() else t.to(torch.bfloat16) if bf16_mode() else t
+
+
+def tcg_precision(wg):
+    """LfConvTcgArgs.precision of a packed operand: 2 = bf16, 1 = [2, Ng, K] TF32 hi / lo pair, 0 = TF32."""
+    return 2 if wg.dtype == torch.bfloat16 else int(wg.dim() == 3)
 
 
 # Experiment switch (labelled extra in bench.py, never a default): in tf32x3 mode, run ONLY the weight-gradient kernels as
@@ -59,6 +81,11 @@ WGRAD_SINGLE_PASS = os.environ.get("LANEFIT_WGRAD_TF32", "0") == "1"
 
 def wgrad_x3():
     return x3_mode() and not WGRAD_SINGLE_PASS
+
+
+def wgrad_precision():
+    """LfWgradTcgArgs.precision of the active mode (0 = TF32, 1 = 3xTF32, 2 = BF16)."""
+    return 2 if bf16_mode() else int(wgrad_x3())
 
 
 def split_tf32(t):
@@ -193,7 +220,7 @@ def run_tcg_s2conv(x, wg, O, out, bias=None, relu=False):
     a.wg, a.bias, a.out = wg.data_ptr(), (bias.data_ptr() if bias is not None else None), out.data_ptr()
     a.osn, a.osy, a.osx, a.oy_mul, a.oy0 = Ho * Wo * cot, Wo * cot, cot, 1, 0
     a.N, a.Hs, a.Ws, a.Kc, a.Ng, a.ntaps = N, Ho, Wo, 2 * C, wg.shape[-2], 6
-    a.precision = int(wg.dim() == 3)       # [2, Ng, K]: the TF32 hi / lo pair of the 3xTF32 mode
+    a.precision = tcg_precision(wg)
     a.relu = int(relu)
     for t, (m, dy, dx) in enumerate(TCG_S2CONV_TAPS):
         a.map[t], a.dy[t], a.dx[t] = m, dy, dx
@@ -221,7 +248,7 @@ def run_tcg_s2convT(x, I, wgs, O, out, bias2=None, relu=False):
         a.wg, a.bias, a.out = wgs[par].data_ptr(), (bias2.data_ptr() if bias2 is not None else None), out.data_ptr()
         a.osn, a.osy, a.osx, a.oy_mul, a.oy0 = 4 * H * W * O, 2 * W * O, 2 * O, 2, par
         a.N, a.Hs, a.Ws, a.Kc, a.Ng, a.ntaps = N, H, W, kc, 2 * O, len(taps)
-        a.precision = int(wgs[par].dim() == 3)
+        a.precision = tcg_precision(wgs[par])
         a.relu = int(relu)
         for t, (dy, dx, _ky) in enumerate(taps):
             a.map[t], a.dy[t], a.dx[t] = 0, dy, dx
@@ -266,7 +293,8 @@ def wgrad_tcg_ok(a_t, C, b_t, Nn):
 
 
 def _wgrad_tcg_ctas(*args):
-    return int((_lib().lf_wgrad_tcg_ctas_x3 if wgrad_x3() else _lib().lf_wgrad_tcg_ctas)(*args))
+    return int((_lib().lf_wgrad_tcg_ctas_bf16 if bf16_mode() else _lib().lf_wgrad_tcg_ctas_x3 if wgrad_x3()
+                else _lib().lf_wgrad_tcg_ctas)(*args))
 
 
 def _wgrad_tcg_taps_per_launch(N, Hs, Ws, C, Nn):
@@ -299,7 +327,7 @@ def run_wgrad_tcg(a_t, C, b_t, Nn):
         a.a[1] = _tcg_view(a_t, Hs, Ws, H2 * W2 * C, 2 * W2 * C, 2 * C, W2 * C)
         a.b = _tcg_view(b_t, Hs, Ws, Hs * Ws * cb_tot, Ws * cb_tot, cb_tot)
         a.partial, a.N, a.Hs, a.Ws, a.Ka, a.Nn, a.nblocks, a.nctas = partial.data_ptr(), N, Hs, Ws, Ka, Nn, nblocks, nctas
-        a.precision = int(wgrad_x3())
+        a.precision = wgrad_precision()
         for i in range(nblocks):
             m, dy, dx = TCG_S2CONV_TAPS[t0 + i // per_tap]
             a.map[i], a.dy[i], a.dx[i], a.cblk[i] = m, dy, dx, i % per_tap
@@ -362,6 +390,8 @@ class WeightPackCache:
         self.by_ptr = {p.data_ptr(): p for m in mods for p in m.parameters() if p.is_cuda}
 
     def get(self, w, kind, fn, split=False):
+        """split: False (fp32 operand), True (TF32 hi/lo pair) or "bf16" -- part of the key, so a mode switch never
+        serves an operand of another form."""
         if not w.is_cuda:
             return None
         p = self.by_ptr.get(w.data_ptr())
@@ -373,11 +403,12 @@ class WeightPackCache:
             if torch.cuda.is_current_stream_capturing():
                 return None
             idx = pack_gather_table(fn, p.shape)
-            if split:       # [2, ...]: TF32 hi parts, then lo parts (structural zeros stay negative)
+            if split is True:       # [2, ...]: TF32 hi parts, then lo parts (structural zeros stay negative)
                 assert p.numel() <= _capi.PACK_INDEX_MASK
                 idx = torch.stack([torch.where(idx >= 0, idx | _capi.PACK_TF32_HI, idx),
                                    torch.where(idx >= 0, idx | _capi.PACK_TF32_LO, idx)])
-            self.entries[key] = [p, idx.to(w.device), torch.empty(idx.shape, dtype=torch.float32, device=w.device), -1]
+            dtype = torch.bfloat16 if split == "bf16" else torch.float32
+            self.entries[key] = [p, idx.to(w.device), torch.empty(idx.shape, dtype=dtype, device=w.device), -1]
             self.dirty = True
             return None
         if e[3] != p._version or e[0] is not p:
@@ -395,7 +426,9 @@ class WeightPackCache:
         if self.dirty:
             if torch.cuda.is_current_stream_capturing():
                 return                      # keep serving the operands that are already in the table
-            rows = [[e[0].data_ptr(), e[2].data_ptr(), e[1].data_ptr(), e[1].numel()] for e in self.entries.values()]
+            # LfPackJob rows: src, dst, idx, n, dst_dtype (the int64 holds the dtype and the zero pad field)
+            rows = [[e[0].data_ptr(), e[2].data_ptr(), e[1].data_ptr(), e[1].numel(), _capi.dtype_id(e[2])]
+                    for e in self.entries.values()]
             dev = next(iter(self.entries.values()))[2].device
             self.jobs = torch.tensor(rows, dtype=torch.int64).to(dev)
             self.job_entries = list(self.entries.values())
@@ -409,13 +442,15 @@ ACTIVE_PACKS = None
 
 
 def packed(w, kind, fn, split=False):
-    """The packed operand ``fn(w)`` (``split``: its TF32 hi/lo pair, see split_tf32): from the active WeightPackCache
-    when current, else computed now."""
+    """The packed operand ``fn(w)`` (``split``: True = its TF32 hi/lo pair, see split_tf32; "bf16" = rounded to bf16):
+    from the active WeightPackCache when current, else computed now."""
     c = ACTIVE_PACKS
     if c is not None:
         t = c.get(w, kind, fn, split)
         if t is not None:
             return t
+    if split == "bf16":
+        return fn(w).to(torch.bfloat16)
     return split_tf32(fn(w)) if split else fn(w)
 
 
@@ -600,7 +635,8 @@ def run_conv_tc(taps, x, wpack, out, bias=None, relu=False, mask_src=None, add_s
         a.dy[t], a.dx[t] = dy, dx
     a.relu = int(relu)
     n_operands = 2 + (mask_src is not None) + (add_src is not None) + (add_mask is not None)
-    _capi.call("lf_conv1d_tc_x3" if x3_mode() else "lf_conv1d_tc", ctypes.byref(a), _stream(), flops=2 * N * H * W * 3 * C * C,
+    entry = "lf_conv1d_tc_x3" if x3_mode() else "lf_conv1d_tc_bf16" if bf16_mode() else "lf_conv1d_tc"
+    _capi.call(entry, ctypes.byref(a), _stream(), flops=2 * N * H * W * 3 * C * C,
                nbytes=4 * n_operands * N * H * W * C)
     if part is not None:
         if _DEFERRED is not None:
@@ -634,7 +670,7 @@ def flush_deferred_reductions(jobs):
 
 def _super_conv_launch(taps, xs, w, vertical, transposed, out, N, H, W, C, cs, epi_s, wp=None):
     if wp is None:
-        wp = packed(w, "tc_super_%d%d" % (vertical, transposed), lambda t: pack_tc_super(t, vertical, transposed), split=x3_mode())
+        wp = packed(w, "tc_super_%d%d" % (vertical, transposed), lambda t: pack_tc_super(t, vertical, transposed), split=pack_split())
     run_conv_tc(taps, xs, wp, out.view(N, H, W // SUPER, SUPER * C), colsum=cs, **epi_s)
 
 
@@ -666,8 +702,8 @@ def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, **epi):
         sgn = -1 if transposed else 1
         taps = [((sgn * (k - 1) * dil, 0) if vertical else (0, sgn * (k - 1) * dil)) for k in range(3)]
         if wp is None:
-            wp = (packed(w, "tc_dgrad", pack_tc_dgrad, split=x3_mode()) if transposed
-                  else packed(w, "tc_fwd", pack_tc_fwd, split=x3_mode()))
+            wp = (packed(w, "tc_dgrad", pack_tc_dgrad, split=pack_split()) if transposed
+                  else packed(w, "tc_fwd", pack_tc_fwd, split=pack_split()))
         return run_conv_tc(taps, x, wp, out, colsum=colsum, **epi)
     if wp is not None:
         raise _capi.LanefitError("conv3: a pre-packed operand needs a tensor-core route")
@@ -689,7 +725,7 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
     """Weight + bias gradient of one factorised 3-tap convolution -> (dw [Co,Ci,kh,kw], db [Co] or None).
     bias_grad: "compute" (column sums of d_out), or "skip" (the caller gets it elsewhere)."""
     N, H, W, C = x_in.shape
-    sfx = "_x3" if wgrad_x3() else ""          # which tensor-core weight-gradient kernel
+    sfx = "_x3" if wgrad_x3() else "_bf16" if bf16_mode() else ""   # which tensor-core weight-gradient kernel
     if super_ok(x_in, dil) and d_out.is_contiguous():
         Cs, Ws = SUPER * C, W // SUPER
         nctas = getattr(_lib(), "lf_wgrad3_tc%s_ctas" % sfx)(N, H, Ws, Cs)
@@ -841,7 +877,7 @@ def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running
     if rows > 0:
         part = torch.empty(rows * 2 * C, dtype=torch.float64, device=x.device)
         taps = [(((k - 1) * dil, 0) if vertical else (0, (k - 1) * dil)) for k in range(3)]
-        out = run_conv_tc(taps, x, packed(w, "tc_fwd", pack_tc_fwd, split=x3_mode()), torch.empty_like(x), bias=bias,
+        out = run_conv_tc(taps, x, packed(w, "tc_fwd", pack_tc_fwd, split=pack_split()), torch.empty_like(x), bias=bias,
                           stats_partial=part)
         return out, bn_finalize(part, rows, N * H * W, C, gamma, beta, running_mean, running_var)
     out = conv3(x, w, vertical, dil, False, bias=bias)
@@ -906,7 +942,7 @@ def dgrad_relu_bn_fused(d_out, w, vertical, dil, x, s, gamma):
         return None
     part = torch.empty(rows * 2 * C, dtype=torch.float64, device=d_out.device)
     taps = [((-(k - 1) * dil, 0) if vertical else (0, -(k - 1) * dil)) for k in range(3)]
-    g = run_conv_tc(taps, d_out, packed(w, "tc_dgrad", pack_tc_dgrad, split=x3_mode()), torch.empty_like(d_out), mask_src=x,
+    g = run_conv_tc(taps, d_out, packed(w, "tc_dgrad", pack_tc_dgrad, split=pack_split()), torch.empty_like(d_out), mask_src=x,
                     stats_partial=part, mask_affine=(s.scale, s.shift))
     npix = N * H * W
     buf = torch.empty(4, C, dtype=torch.float32, device=d_out.device)
@@ -942,7 +978,7 @@ class DownFunction(torch.autograd.Function):
         phases, (Ho, Wo) = plans.conv_fwd_plan(H, W, 3, 3, 2, 1, 1, 1, 1)
         cat = _empty((N, Ho, Wo, cout), x)
         if cc % 16 == 0 and tcg_s2conv_ok(x, cin, cc):
-            run_tcg_s2conv(x, packed(w, "tcg_s2conv", pack_tcg_s2conv, split=x3_mode()), cc, cat, bias=b)
+            run_tcg_s2conv(x, packed(w, "tcg_s2conv", pack_tcg_s2conv, split=pack_split()), cc, cat, bias=b)
         else:
             wmat = packed(w, "conv_fwd_%d" % cin_gemm, lambda t: pack_conv_fwd(t, cin_gemm))
             run_conv(phases, x, wmat, cin_gemm, cat, cc, 0, bias=b)
@@ -982,7 +1018,7 @@ class DownFunction(torch.autograd.Function):
             dx = _empty((N, H, W, cx), x)
             if cx == cin and tcg_s2convT_ok(dcat, cc, cin):
                 kc = plans.pad_to(cc, 32)
-                wgs = tuple(packed(w, "tcg_s2convT%d_%d" % (par, kc), lambda t, par=par: pack_tcg_s2convT(t, par, kc), split=x3_mode())
+                wgs = tuple(packed(w, "tcg_s2convT%d_%d" % (par, kc), lambda t, par=par: pack_tcg_s2convT(t, par, kc), split=pack_split())
                             for par in (0, 1))
                 run_tcg_s2convT(dcat, cc, wgs, cin, dx)
             else:
@@ -1083,7 +1119,7 @@ class UpFunction(torch.autograd.Function):
         co = w.shape[1]
         phases, (Ho, Wo) = plans.transposed_gather_plan(H, W, 2 * H, 2 * W, 3, 1)
         if tcg_s2convT_ok(x, ci, co):
-            wgs = tuple(packed(w, "tcg_s2convT%d_%d" % (par, ci), lambda t, par=par: pack_tcg_s2convT(t, par, ci), split=x3_mode())
+            wgs = tuple(packed(w, "tcg_s2convT%d_%d" % (par, ci), lambda t, par=par: pack_tcg_s2convT(t, par, ci), split=pack_split())
                         for par in (0, 1))
             u = run_tcg_s2convT(x, ci, wgs, co, _empty((N, Ho, Wo, co), x), bias2=packed(b, "tile2", lambda t: t.repeat(2)))
         else:
@@ -1111,7 +1147,7 @@ class UpFunction(torch.autograd.Function):
             run_wgrad(plans.convT_wgrad_plan(H, W, 3, 1), x, ci, du, co, 0, N, dw, (1, co * 9, 9))
         run_colsum(du, co, 0, db)
         if ci % 16 == 0 and tcg_s2conv_ok(du, co, ci):
-            dx = run_tcg_s2conv(du, packed(w, "tcg_s2conv", pack_tcg_s2conv, split=x3_mode()), ci, torch.empty_like(x))
+            dx = run_tcg_s2conv(du, packed(w, "tcg_s2conv", pack_tcg_s2conv, split=pack_split()), ci, torch.empty_like(x))
         else:
             pd, _ = plans.convT_dgrad_plan(2 * H, 2 * W, H, W, 3, 1)
             dx = run_conv(pd, du, packed(w, "convT_dgrad", pack_convT_dgrad), co, torch.empty_like(x), ci)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-shape timing of the 3-tap convolution / input-gradient / weight-gradient kernels in every conv mode.
 
-    python tools/bench_ops.py [--batch 32] [--modes tf32x3 tf32] > gpurun_out/ops.jsonl
+    python tools/bench_ops.py [--batch 32] [--modes tf32x3 tf32 bf16] > ops.jsonl
 
 One JSON line per (mode, op, shape): mean launch time over `--iters` back-to-back launches on tensors larger than L2 in
 aggregate (each op cycles through `--rot` independent input sets), CUDA events on the launching stream."""
@@ -49,8 +49,7 @@ def main():
                 bb = b.repeat(4)
             else:
                 wf, wd, tf, td, view, bb = o.pack_tc_fwd(w), o.pack_tc_dgrad(w), taps(1), taps(-1), (lambda t: t), b
-            if mode == "tf32x3":
-                wf, wd = o.split_tf32(wf), o.split_tf32(wd)
+            wf, wd = o.tc_operand(wf), o.tc_operand(wd)   # tf32x3: the TF32 hi / lo pair; bf16: bf16 operands
             outs = [torch.empty_like(view(xs[0])) for _ in range(a.rot)]
             ops = {
                 "fwd_bias_relu": lambda i: o.run_conv_tc(tf, view(xs[i]), wf, outs[i], bias=bb, relu=True),
