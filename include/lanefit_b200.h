@@ -169,6 +169,11 @@ typedef struct LfConvTcArgs {
     int dy[3], dx[3];
     int relu;                /* bit 0: ReLU on conv + bias (before mask / add_src); bit 1: ReLU after add_src -- the closing
                                 relu(conv + x) of an eval-mode block whose BatchNorm is folded into the weights */
+    int in_dtype, out_dtype, mask_dtype; /* element types of `in`, `out` and `mask_src`: LF_F32 (0, every pointer above
+                                typed float), or LF_BF16 -- lf_conv1d_tc_bf16 only, else LF_ERR_UNSUPPORTED.  A bf16 `in`
+                                gives the same results as its fp32 copy (the kernel rounds fp32 activations to bf16 itself);
+                                a bf16 `out` is the fp32 result rounded to nearest even (colsum / stats are of the fp32
+                                values); a bf16 `mask_src` gates like its fp32 copy.  Same shapes and slab cases as fp32. */
 } LfConvTcArgs;
 /* 0 = unsupported shape, else the number of CTA rows of colsum_partial */
 int lf_conv1d_tc_supported(int N, int H, int W, int C);
@@ -210,6 +215,10 @@ int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, int W, int C,
 int lf_wgrad3_tc_bf16_ctas(int N, int H, int W, int C);
 int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
                       float* partial, int nctas, lf_stream_t stream);
+/* lf_wgrad3_tc_bf16 with the layer input x stored as bf16 [N,H,W,C] (dy stays fp32): same results as lf_wgrad3_tc_bf16
+ * on the fp32 copy of x, same arguments, nctas (lf_wgrad3_tc_bf16_ctas) and partial layout. */
+int lf_wgrad3_tc_bf16a(const void* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
+                       float* partial, int nctas, lf_stream_t stream);
 
 /* Weight gradient as a split-K GEMM over pixels:
  *   partial[s][t][cp][cq] = sum_{(n,j,i) in split s} P[n, j*psy+pdy[t], i*psx+pdx[t], cp]
@@ -281,6 +290,10 @@ int lf_bn_eval_prepare(int C, const float* gamma, const float* beta, float eps, 
 int lf_bn_apply(const float* x, long long npix, int C, int pix_per_image, const float* scale,
                 const float* shift, const float* drop, const float* res, int relu, float* y,
                 lf_stream_t stream);
+/* lf_bn_apply storing y as bf16, each element of the fp32 result rounded to nearest even (= torch's .to(torch.bfloat16)) */
+int lf_bn_apply_bf16(const float* x, long long npix, int C, int pix_per_image, const float* scale,
+                     const float* shift, const float* drop, const float* res, int relu, void* y,
+                     lf_stream_t stream);
 int lf_bn_bwd_reduce(const float* dy, const float* ymask, const float* drop, const float* x, long long npix,
                      int C, int pix_per_image, const float* mean, const float* invstd, double* partial,
                      lf_stream_t stream);

@@ -59,7 +59,7 @@ class LfConvArgs(ctypes.Structure):
 class LfConvTcArgs(ctypes.Structure):
     _fields_ = [("inp", _p), ("wpack", _p), ("bias", _p), ("out", _p), ("mask_src", _p), ("add_src", _p),
                 ("add_mask", _p), ("colsum_partial", _p), ("stats_partial", _p), ("mask_scale", _p), ("mask_shift", _p), ("N", _i), ("H", _i), ("W", _i), ("C", _i), ("dy", _i * 3),
-                ("dx", _i * 3), ("relu", _i)]
+                ("dx", _i * 3), ("relu", _i), ("in_dtype", _i), ("out_dtype", _i), ("mask_dtype", _i)]
 
 
 class LfWgradArgs(ctypes.Structure):
@@ -127,6 +127,7 @@ _NET_PROTOS = {
     "lf_wgrad3_tc_x3": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
     "lf_wgrad3_tc_bf16_ctas": (_i, [_i, _i, _i, _i]),
     "lf_wgrad3_tc_bf16": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
+    "lf_wgrad3_tc_bf16a": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
     "lf_wgrad_reduce": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "lf_vec_reduce": (_i, [_p, _i, _i, _i, _p, _p]),
     "lf_colsum_blocks": (_i, [ctypes.c_longlong]),
@@ -140,6 +141,7 @@ _NET_PROTOS = {
                             _p, _p]),
     "lf_bn_eval_prepare": (_i, [_i, _p, _p, ctypes.c_float, _p, _p, _p, _p, _p]),
     "lf_bn_apply": (_i, [_p, ctypes.c_longlong, _i, _i, _p, _p, _p, _p, _i, _p, _p]),
+    "lf_bn_apply_bf16": (_i, [_p, ctypes.c_longlong, _i, _i, _p, _p, _p, _p, _i, _p, _p]),
     "lf_bn_bwd_reduce": (_i, [_p, _p, _p, _p, ctypes.c_longlong, _i, _i, _p, _p, _p, _p]),
     "lf_bn_bwd_finalize": (_i, [_p, _i, ctypes.c_longlong, _i, _p, _p, _p, _p, _p]),
     "lf_bn_bwd_apply": (_i, [_p, _p, _p, _p, ctypes.c_longlong, _i, _i, _p, _p, _p, _p, _p, _p, _p]),

@@ -9,6 +9,11 @@
 //  * BF16 (lf_conv1d_tc_bf16): both operands rounded to bf16 (nearest even) -- the activations while their k16 fragments
 //    are formed (pairs of adjacent channels, one 8-byte load each), the weights by the packer ([Cout][3C] bf16, 64-byte
 //    rows, 64B-swizzled tiles of half the TF32 size: resident wherever the TF32 tiles are); products exact in fp32.
+//    The activations may also arrive as bf16 (template ABF, LfConvTcArgs.in_dtype): the slab is then a bf16 TMA box of
+//    64-byte rows, 64B-swizzled, and each fragment register is one 32-bit load of a ready channel pair -- the same
+//    operand bits as rounding the fp32 copy, so the same results.  The BF16 epilogue can also store `out` as bf16
+//    (nearest even, = torch's .to(torch.bfloat16); column sums / statistics are of the fp32 values) and read a bf16
+//    `mask_src`: the ReLU outputs a non_bottleneck_1d block keeps only as convolution inputs and ReLU masks.
 //
 //   out[n,y,x,co] = epi( sum_{t<3} sum_{ci} in[n, (y,x) + o_t, ci] * Wp[co][t*C + ci] )
 //
@@ -73,13 +78,19 @@ struct TcArgs {
     int relu;                 // bit 0: ReLU on conv + bias (before mask / add); bit 1: ReLU after the residual add
     int n_halves, total_m_tiles;
     int stages, stage_bytes, a_bytes;   // a stage = a_bytes of activations [+ the three weight tiles of its chunk]
+    int out_bf16, mask_bf16;  // BF16 kernels only: `out` / `mask_src` hold bf16
 };
 
-template <int C, int P, bool RES>
+// bytes of one activation slab row (32 channels): fp32, or bf16 (ABF)
+constexpr int tc_a_row(bool abf) { return abf ? 64 : 128; }
+
+template <int C, int P, bool RES, bool ABF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     pdl_trigger();
+    static_assert(!ABF || P == TC_BF16, "bf16 activations need the BF16 kernel");
     constexpr bool X3 = P == TC_X3;
+    constexpr int A_ROW = tc_a_row(ABF);
     constexpr int NCB = C / TC_KCH;
     constexpr int W_ATOM = tc_w_atom(P);   // 3xTF32: hi tile, then lo tile; bf16: half-size tile
     constexpr int B_RES_BYTES = RES ? 3 * NCB * W_ATOM : 0;
@@ -135,7 +146,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     mbar_arrive_expect_tx(&full[stage], a.stage_bytes);
                     // tensor map dims: (ci, cblk, across, along, n)
                     for (int l = 0; l < a.nloads; ++l)
-                        tma_load_5d(&tmA, &full[stage], st + l * a.load_rows * 128, 0, cb, tb * a.TB + a.load_b[l],
+                        tma_load_5d(&tmA, &full[stage], st + l * a.load_rows * A_ROW, 0, cb, tb * a.TB + a.load_b[l],
                                     ta * a.TA + a.load_a[l], n);
                     if (!RES)
                         for (int t = 0; t < 3; ++t) load_w(&full[stage], st + a.a_bytes + t * W_ATOM, t, cb);
@@ -160,6 +171,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const bool pre_mask = a.mask_src != nullptr;
     const bool pre_add = (a.add_src != nullptr) && !pre_mask;  // both given: add_src is read in the loop
     const bool affine_mask = a.mask_scale != nullptr;
+    const bool out_bf = P == TC_BF16 && a.out_bf16, mask_bf = P == TC_BF16 && a.mask_bf16;
     float4 csum = make_float4(0.f, 0.f, 0.f, 0.f), csq = csum, msc = csum, msh = csum, bsv = csum;
     if (a.bias) bsv = __ldg(reinterpret_cast<const float4*>(a.bias + ch0));
     if (affine_mask) {
@@ -187,7 +199,10 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (pre_mask || pre_add) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                if (pre_mask) {
+                if (pre_mask && mask_bf) {   // the raw bf16 bits, widened in the epilogue: converting here would wait for the load
+                    const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(a.mask_src) + roff[j]));
+                    pre[j] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), 0.f, 0.f);
+                } else if (pre_mask) {
                     pre[j] = __ldg(reinterpret_cast<const float4*>(a.mask_src + roff[j]));
                 } else {
                     float4 ad = __ldg(reinterpret_cast<const float4*>(a.add_src + roff[j]));
@@ -211,21 +226,30 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             constexpr int W_TAP = RES ? NCB * W_ATOM : W_ATOM;   // distance between the weight tiles of two taps
 #pragma unroll
             for (int t = 0; t < 3; ++t) {
-                const uint8_t* view = st + a.tap_row[t] * 128;   // 1024-byte aligned: the swizzle phase is the view's row
+                // 8 rows of the swizzle period apart (1024 / 512 bytes): the swizzle phase is the view's row
+                const uint8_t* view = st + a.tap_row[t] * A_ROW;
                 if constexpr (P == TC_BF16) {
-                    // k16 fragments: two adjacent channels per register = one 8-byte load inside a 16-byte chunk
+                    // k16 fragments: two adjacent channels per register = one 8-byte load inside a 16-byte chunk (fp32
+                    // slab), or one 4-byte load of the ready pair (bf16 slab)
                     uint32_t ab[2][4];
 #pragma unroll
                     for (int kk = 0; kk < 2; ++kk) {
                         const int c = 16 * kk + 2 * t4;
-                        const float2 v0 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c));
-                        const float2 v1 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c));
-                        const float2 v2 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c + 8));
-                        const float2 v3 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c + 8));
-                        ab[kk][0] = pack_bf16x2(v0.x, v0.y);
-                        ab[kk][1] = pack_bf16x2(v1.x, v1.y);
-                        ab[kk][2] = pack_bf16x2(v2.x, v2.y);
-                        ab[kk][3] = pack_bf16x2(v3.x, v3.y);
+                        if constexpr (ABF) {
+                            ab[kk][0] = *reinterpret_cast<const uint32_t*>(view + sw64_off(ra, c));
+                            ab[kk][1] = *reinterpret_cast<const uint32_t*>(view + sw64_off(ra + 8, c));
+                            ab[kk][2] = *reinterpret_cast<const uint32_t*>(view + sw64_off(ra, c + 8));
+                            ab[kk][3] = *reinterpret_cast<const uint32_t*>(view + sw64_off(ra + 8, c + 8));
+                        } else {
+                            const float2 v0 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c));
+                            const float2 v1 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c));
+                            const float2 v2 = *reinterpret_cast<const float2*>(view + sw128_off(ra, c + 8));
+                            const float2 v3 = *reinterpret_cast<const float2*>(view + sw128_off(ra + 8, c + 8));
+                            ab[kk][0] = pack_bf16x2(v0.x, v0.y);
+                            ab[kk][1] = pack_bf16x2(v1.x, v1.y);
+                            ab[kk][2] = pack_bf16x2(v2.x, v2.y);
+                            ab[kk][3] = pack_bf16x2(v3.x, v3.y);
+                        }
                     }
                     const uint64_t bd = wgmma_desc_sw64(wbase + t * W_TAP);
                     wgmma_fence();
@@ -297,6 +321,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int j = 0; j < 8; ++j) {
             const int r = r0 + 16 * j;
             const size_t off = roff[j];
+            if (mask_bf) pre[j] = bf16x4_to_f4(make_uint2(__float_as_uint(pre[j].x), __float_as_uint(pre[j].y)));
             float4 o = *reinterpret_cast<const float4*>(&stg_h[r * TC_STG_LD + 4 * c4]);
             o.x += bsv.x; o.y += bsv.y; o.z += bsv.z; o.w += bsv.w;
             if (a.relu & 1) {
@@ -325,7 +350,8 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             if (a.relu & 2) {   // ReLU AFTER the residual add: the closing relu(conv + x) of an eval-mode (BN-folded) block
                 o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
             }
-            *reinterpret_cast<float4*>(a.out + off) = o;
+            if (out_bf) *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.out) + off) = f4_to_bf16x4(o);
+            else *reinterpret_cast<float4*>(a.out + off) = o;
             csum.x += o.x; csum.y += o.y; csum.z += o.z; csum.w += o.w;
             if (affine_mask) {   // pre[j] is the BatchNorm input x
                 csq.x = fmaf(o.x, pre[j].x, csq.x); csq.y = fmaf(o.y, pre[j].y, csq.y);
@@ -378,11 +404,11 @@ static int tc_m_ctas(int N, int C, int tiles_per_image) {
 }
 
 // Shared memory: resident weights when they leave room for two stages, else streamed per stage.
-static bool tc_fit(int C, int prec, TcPlan* p) {
+static bool tc_fit(int C, int prec, bool abf, TcPlan* p) {
     const int w_atom = tc_w_atom(prec);
     const int b_res = 3 * (C / TC_KCH) * w_atom;
     TcArgs& g = p->geo;
-    g.a_bytes = g.nloads * g.load_rows * 128;
+    g.a_bytes = g.nloads * g.load_rows * tc_a_row(abf);
     p->res = TC_FIXED_SMEM + b_res + 2 * g.a_bytes <= TC_SMEM_LIMIT;
     g.stage_bytes = g.a_bytes + (p->res ? 0 : 3 * w_atom);
     const int avail = TC_SMEM_LIMIT - TC_FIXED_SMEM - (p->res ? b_res : 0);
@@ -397,7 +423,7 @@ static bool tc_fit(int C, int prec, TcPlan* p) {
 // Halo-slab plan: taps {-d, 0, +d} (forward) or {+d, 0, -d} (input gradient) along one axis.  TA x TB = 128 pixels with
 // TB a power of two such that the tap shift d*TB is a multiple of the 8-row swizzle period; the slab with the fewest
 // rows wins (tall tiles for the large dilations: halo 2d / TA).
-static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p) {
+static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p, bool abf = false) {
     if (!(C == 64 || C == 128) || N <= 0) return false;
     const bool vert = dy[0] != 0 || dy[2] != 0;
     const int* o = vert ? dy : dx;
@@ -428,13 +454,13 @@ static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* d
     g.load_a[0] = -dil;
     g.load_b[0] = 0;
     for (int t = 0; t < 3; ++t) g.tap_row[t] = (fwd_order ? t : 2 - t) * dil * g.TB;
-    if (!tc_fit(C, prec, p)) return false;
+    if (!tc_fit(C, prec, abf, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
     return tc_get_encode_fn() != nullptr;
 }
 
 // Per-tap plan: any three taps; a bx x by = 128 pixel patch with bx | W, by | H (wide patches preferred).
-static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p) {
+static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* dx, int prec, TcPlan* p, bool abf = false) {
     if (!(C == 64 || C == 128) || N <= 0) return false;
     TcArgs& g = p->geo;
     int sh = 7;
@@ -453,24 +479,24 @@ static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* d
         g.load_b[t] = dx ? dx[t] : 0;
         g.tap_row[t] = t * 128;
     }
-    if (!tc_fit(C, prec, p)) return false;
+    if (!tc_fit(C, prec, abf, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
     return tc_get_encode_fn() != nullptr;
 }
 
-template <int C, int P, bool RES>
+template <int C, int P, bool RES, bool ABF>
 static cudaError_t tc_launch(int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB,
                              const TcArgs& a) {
-    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel<C, P, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT);
+    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel<C, P, RES, ABF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT);
     if (e != cudaSuccess) return e;
-    return lf_launch(conv1d_tc_kernel<C, P, RES>, grid, TC_THREADS, smem_bytes, stream, tmA, tmB, a);
+    return lf_launch(conv1d_tc_kernel<C, P, RES, ABF>, grid, TC_THREADS, smem_bytes, stream, tmA, tmB, a);
 }
 
-template <int P>
+template <int P, bool ABF = false>
 static cudaError_t tc_launch_p(bool res, int C, int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
                                const CUtensorMap& tmB, const TcArgs& a) {
-    if (C == 128) return res ? tc_launch<128, P, true>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<128, P, false>(grid, smem_bytes, stream, tmA, tmB, a);
-    return res ? tc_launch<64, P, true>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<64, P, false>(grid, smem_bytes, stream, tmA, tmB, a);
+    if (C == 128) return res ? tc_launch<128, P, true, ABF>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<128, P, false, ABF>(grid, smem_bytes, stream, tmA, tmB, a);
+    return res ? tc_launch<64, P, true, ABF>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<64, P, false, ABF>(grid, smem_bytes, stream, tmA, tmB, a);
 }
 
 static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
@@ -479,14 +505,18 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     const LfConvTcArgs& p = *args;
     LF_REQUIRE(p.in && p.wpack && p.out);
     LF_REQUIRE(!p.mask_scale || (p.mask_shift && p.mask_src && p.stats_partial));
+    LF_REQUIRE((p.in_dtype == LF_F32 || p.in_dtype == LF_BF16) && (p.out_dtype == LF_F32 || p.out_dtype == LF_BF16) &&
+               (p.mask_dtype == LF_F32 || p.mask_dtype == LF_BF16));
+    if (prec != TC_BF16 && (p.in_dtype | p.out_dtype | p.mask_dtype) != LF_F32) return LF_ERR_UNSUPPORTED;
     const bool x3 = prec == TC_X3;
+    const bool abf = p.in_dtype == LF_BF16;
     TcPlan pl{};
-    // bf16 takes the slab exactly where TF32 does (its smaller weight tiles fit wherever the TF32 ones do), so that
-    // lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for both
+    // bf16 takes the slab exactly where TF32 does (its smaller weight tiles and bf16 slabs fit wherever the TF32 ones
+    // do), so that lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for both
     const bool slab = (x3 || g_tc_variant != 1) &&
                       (prec != TC_BF16 || tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, TC_TF32, &pl)) &&
-                      tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl);
-    if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl))) return LF_ERR_UNSUPPORTED;
+                      tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf);
+    if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf))) return LF_ERR_UNSUPPORTED;
     TcArgs a = pl.geo;
     a.out = p.out; a.bias = p.bias; a.mask_src = p.mask_src; a.add_src = p.add_src; a.add_mask = p.add_mask;
     a.colsum_partial = p.colsum_partial;
@@ -495,20 +525,25 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     a.mask_shift = p.mask_shift;
     a.N = p.N; a.H = p.H; a.W = p.W; a.Ctot = p.C; a.relu = p.relu;
     a.n_halves = p.C / TC_BN;
+    a.out_bf16 = p.out_dtype == LF_BF16;
+    a.mask_bf16 = p.mask_dtype == LF_BF16;
     a.total_m_tiles = p.N * a.tiles_a * a.tiles_b;
 
     TcEncodeTiledFn enc = tc_get_encode_fn();
     CUtensorMap tmA, tmB;
     {
-        // activations [N,H,W,C] viewed as (ci:32, cblk:C/32, across, along, n); one box = the slab or one tap's patch
-        const cuuint64_t sx = (cuuint64_t)p.C * 4, sy = (cuuint64_t)p.W * p.C * 4;
+        // activations [N,H,W,C] viewed as (ci:32, cblk:C/32, across, along, n); one box = the slab or one tap's patch;
+        // bf16: rows of 64 bytes, 64B-swizzled
+        const cuuint64_t esz = abf ? 2 : 4;
+        const cuuint64_t sx = (cuuint64_t)p.C * esz, sy = (cuuint64_t)p.W * p.C * esz;
         cuuint64_t dims[5] = {32, (cuuint64_t)(p.C / 32), (cuuint64_t)(a.vertical ? p.W : p.H),
                               (cuuint64_t)(a.vertical ? p.H : p.W), (cuuint64_t)p.N};
-        cuuint64_t strides[4] = {128, a.vertical ? sx : sy, a.vertical ? sy : sx, (cuuint64_t)p.H * p.W * p.C * 4};
+        cuuint64_t strides[4] = {32 * esz, a.vertical ? sx : sy, a.vertical ? sy : sx, (cuuint64_t)p.H * p.W * p.C * esz};
         cuuint32_t box[5] = {32, 1, (cuuint32_t)a.TB, (cuuint32_t)(a.load_rows / a.TB), 1};
         cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-        CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(p.in), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+        CUresult r = enc(&tmA, abf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5,
+                         const_cast<float*>(p.in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         abf ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
@@ -531,6 +566,7 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     const int s = pl.smem_bytes;
     cudaError_t e;
     if (prec == TC_X3) e = tc_launch_p<TC_X3>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
+    else if (prec == TC_BF16 && abf) e = tc_launch_p<TC_BF16, true>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     else if (prec == TC_BF16) e = tc_launch_p<TC_BF16>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     else e = tc_launch_p<TC_TF32>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }

@@ -172,10 +172,12 @@ __global__ void bn_bwd_finalize_sx_kernel(const double* __restrict__ partial, in
 }
 
 // y = relu?( (x*scale+shift) * drop? + res? )
+// BFY: y is bf16, rounded to nearest even
+template <bool BFY>
 __global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ x, long long n4, int C4, int pix_per_image,
                                                        const float* __restrict__ scale, const float* __restrict__ shift,
                                                        const float* __restrict__ drop, const float* __restrict__ res, int relu,
-                                                       float* __restrict__ y) {
+                                                       void* __restrict__ y) {
     pdl_entry();
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
         const int c4 = (int)(i % C4);
@@ -195,7 +197,8 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__
         if (relu) {
             o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
         }
-        reinterpret_cast<float4*>(y)[i] = o;
+        if (BFY) reinterpret_cast<uint2*>(y)[i] = f4_to_bf16x4(o);
+        else reinterpret_cast<float4*>(y)[i] = o;
     }
 }
 
@@ -525,15 +528,26 @@ extern "C" int lf_bn_eval_prepare(int C, const float* gamma, const float* beta, 
     return check_launch();
 }
 
-extern "C" int lf_bn_apply(const float* x, long long npix, int C, int pix_per_image, const float* scale, const float* shift,
-                           const float* drop, const float* res, int relu, float* y, lf_stream_t stream_) {
+template <bool BFY>
+static int bn_apply_run(const float* x, long long npix, int C, int pix_per_image, const float* scale, const float* shift,
+                        const float* drop, const float* res, int relu, void* y, lf_stream_t stream_) {
     STREAM;
     LF_REQUIRE(x && scale && shift && y && pix_per_image > 0);
     int rc = bn_check(npix, C);
     if (rc) return rc;
     const long long n4 = npix * (C / 4);
-    lf_launch(bn_apply_kernel, grid_for(n4, 256), 256, 0, stream, x, n4, C / 4, pix_per_image, scale, shift, drop, res, relu, y);
+    lf_launch(bn_apply_kernel<BFY>, grid_for(n4, 256), 256, 0, stream, x, n4, C / 4, pix_per_image, scale, shift, drop, res, relu, y);
     return check_launch();
+}
+
+extern "C" int lf_bn_apply(const float* x, long long npix, int C, int pix_per_image, const float* scale, const float* shift,
+                           const float* drop, const float* res, int relu, float* y, lf_stream_t stream_) {
+    return bn_apply_run<false>(x, npix, C, pix_per_image, scale, shift, drop, res, relu, y, stream_);
+}
+
+extern "C" int lf_bn_apply_bf16(const float* x, long long npix, int C, int pix_per_image, const float* scale, const float* shift,
+                                const float* drop, const float* res, int relu, void* y, lf_stream_t stream_) {
+    return bn_apply_run<true>(x, npix, C, pix_per_image, scale, shift, drop, res, relu, y, stream_);
 }
 
 extern "C" int lf_bn_bwd_reduce(const float* dy, const float* ymask, const float* drop, const float* x, long long npix, int C,

@@ -250,6 +250,11 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
     return v;
 }
+__device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {   // zero-extended
+    uint32_t v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
 __device__ __forceinline__ float4 lds_f32x4(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
@@ -283,16 +288,18 @@ inline TcEncodeTiledFn tc_get_encode_fn() {
 }
 
 // Strided fp32 view (element strides sx, sy, sn; channels contiguous) as (ci:32, cblk:C/32, x:W, y:H, n:N); one box =
-// [bx*by pixels] x [32 channels] = rows of 128 bytes, 128B-swizzled; out-of-bounds -> zeros
+// [bx*by pixels] x [32 channels] = rows of 128 bytes, 128B-swizzled; out-of-bounds -> zeros.  bf16: a bf16 view, rows of
+// 64 bytes, 64B-swizzled.
 inline bool tc_encode_view(TcEncodeTiledFn enc, CUtensorMap* tm, const float* base, int N, int H, int W, int C, long long sx,
-                           long long sy, long long sn, int bx, int by) {
+                           long long sy, long long sn, int bx, int by, bool bf16 = false) {
+    const cuuint64_t esz = bf16 ? 2 : 4;
     cuuint64_t dims[5] = {32, (cuuint64_t)(C / 32), (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t strides[4] = {128, (cuuint64_t)sx * 4, (cuuint64_t)sy * 4, (cuuint64_t)sn * 4};
+    cuuint64_t strides[4] = {32 * esz, (cuuint64_t)sx * esz, (cuuint64_t)sy * esz, (cuuint64_t)sn * esz};
     cuuint32_t box[5] = {32, 1, (cuuint32_t)bx, (cuuint32_t)by, 1};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return enc(tm, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims,
+               strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, bf16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 

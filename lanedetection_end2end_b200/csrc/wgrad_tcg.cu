@@ -33,6 +33,9 @@
 // their columns.  BF16 wgmma could read B MN-major (imm-trans-b = 1) and skip the transposition, but the K-major tile
 // keeps one B layout and descriptor (wgmma_desc_sw64) for all three tensor-core kernels; double-buffering and the proxy
 // fence are unchanged.  Two wgmma m64nNWk16 per stage.
+// BF16 with a bf16 A view (template ABF, lf_wgrad3_tc_bf16a): the A boxes are [32 px x 32 ch] bf16, 64-byte rows,
+// 64B-swizzled (half the bytes), and an A register is two 16-bit LDS of the ready values -- the bits the fp32 path packs
+// from an fp32 copy of the same values, so the same results.  B stays fp32 and keeps its transposition.
 // The next stage's fragments are not loaded while a stage's wgmma runs: ptxas then reuses the A registers the running
 // wgmma still reads.  Every CTA writes its slice [64 rows][Nn] of one partial; lf_wgrad_reduce sums them in fixed order.
 #include <cuda.h>
@@ -66,12 +69,16 @@ constexpr int wgt_cols(int nn) { return nn <= 64 ? nn : nn / 2; }
 // size, but the region keeps the TF32 size: warpgroup 1 hands its cols/2 fp32 sums per thread over through it at the end.
 constexpr int wgt_wg_bytes(int nn, int prec) { return 2 * (prec == TC_X3 ? 2 : 1) * wgt_cols(nn) * 128; }
 constexpr int wgt_bt_bytes(int nn, int prec) { return 2 * wgt_wg_bytes(nn, prec); }
+// bytes of one A box: fp32, or bf16 (ABF)
+constexpr int wgt_a_box(bool abf) { return abf ? WG_BOX / 2 : WG_BOX; }
 
-template <int NN, int P>
+template <int NN, int P, bool ABF>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmB, const WgtArgs a) {
+    static_assert(!ABF || P == TC_BF16, "a bf16 A view needs the BF16 kernel");
     constexpr bool X3 = P == TC_X3, BF = P == TC_BF16;
+    constexpr int A_BOX = wgt_a_box(ABF);
     constexpr int NW = wgt_cols(NN);                    // B columns per warpgroup = wgmma N
     constexpr bool KSPLIT = NW == NN;                   // warpgroups split the stages, not the columns
     constexpr int BT_TILE = NW * (BF ? 64 : 128);       // one K-major [NW x 32 px] tile (TF32: 1024-, bf16: 512-byte multiple)
@@ -118,11 +125,11 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
             mbar_wait(&empty[stage], phase ^ 1);
             if (leader) {
                 uint8_t* st = smem + (size_t)stage * a.stage_bytes;
-                mbar_arrive_expect_tx(&full[stage], (a.nb_b + na) * WG_BOX);
+                mbar_arrive_expect_tx(&full[stage], a.nb_b * WG_BOX + na * A_BOX);
                 for (int cb = 0; cb < a.nb_b; ++cb) tma_load_5d(&tmB, &full[stage], st + cb * WG_BOX, 0, cb, x0, y0, n);
                 for (int i = 0; i < na; ++i) {
                     const int b = blk0 + i;
-                    tma_load_5d(a.map[b] ? &tmA1 : &tmA0, &full[stage], st + (a.nb_b + i) * WG_BOX, 0, a.cblk[b], x0 + a.dx[b],
+                    tma_load_5d(a.map[b] ? &tmA1 : &tmA0, &full[stage], st + a.nb_b * WG_BOX + i * A_BOX, 0, a.cblk[b], x0 + a.dx[b],
                                 y0 + a.dy[b], n);
                 }
             }
@@ -155,8 +162,17 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         // bf16 (m64k16): register q of step kk holds pixels k0, k0 + 1 (k0 = 16 kk + 2 t4, + 8 for q >= 2) of channel
         // arow (+ 8 for odd q) = two LDS from two box rows; av[kk][q] / av[kk][4 + q] are the low / high halves
         float av[WG_KP / 8][4];
-        const uint32_t abox = st + (a.nb_b + (wl >> 1)) * WG_BOX;
-        if constexpr (BF) {
+        uint32_t ah[WG_KP / 8][4], al[WG_KP / 8][4];
+        const uint32_t abox = st + a.nb_b * WG_BOX + (wl >> 1) * A_BOX;
+        if constexpr (ABF) {
+#pragma unroll
+            for (int kk = 0; kk < WG_KP / 16; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int k0 = 16 * kk + 2 * t4 + 8 * (q >> 1), r = arow + 8 * (q & 1);
+                    ah[kk][q] = rows_ok ? lds_u16(abox + sw64_off(k0, r)) | (lds_u16(abox + sw64_off(k0 + 1, r)) << 16) : 0u;
+                }
+        } else if constexpr (BF) {
 #pragma unroll
             for (int kk = 0; kk < WG_KP / 16; ++kk)
 #pragma unroll
@@ -208,13 +224,12 @@ wgrad_tcg_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                 }
             }
         }
-        uint32_t ah[WG_KP / 8][4], al[WG_KP / 8][4];
 #pragma unroll
         for (int k8 = 0; k8 < WG_KP / 8; ++k8)
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 if (BF) {
-                    if (k8 < WG_KP / 16) ah[k8][q] = pack_bf16x2(av[2 * k8][q], av[2 * k8 + 1][q]);
+                    if (!ABF && k8 < WG_KP / 16) ah[k8][q] = pack_bf16x2(av[2 * k8][q], av[2 * k8 + 1][q]);
                 } else if (X3) {
                     tf32_split(av[k8][q], ah[k8][q], al[k8][q]);
                 } else {
@@ -291,8 +306,8 @@ static bool wgt_pick_patch(int Hs, int Ws, int* bx, int* by) {
     return false;
 }
 
-static bool wgt_encode(TcEncodeTiledFn enc, CUtensorMap* tm, const LfTcgView& v, int N, int C, int bx, int by) {
-    return tc_encode_view(enc, tm, v.ptr, N, v.H, v.W, C, v.sx, v.sy, v.sn, bx, by);
+static bool wgt_encode(TcEncodeTiledFn enc, CUtensorMap* tm, const LfTcgView& v, int N, int C, int bx, int by, bool bf16 = false) {
+    return tc_encode_view(enc, tm, v.ptr, N, v.H, v.W, C, v.sx, v.sy, v.sn, bx, by, bf16);
 }
 
 // split-K slices for `patches` pixel patches and `nblocks` blocks: at least `min_per` patches per slice, and at most as
@@ -313,12 +328,12 @@ static int wgt_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) {
     return wgt_split((long long)N * (Hs / by) * (Ws / bx), 4, nblocks);
 }
 
-template <int NN, int P>
+template <int NN, int P, bool ABF = false>
 static cudaError_t wgt_launch(dim3 grid, int smem_bytes, cudaStream_t stream, const CUtensorMap& tmA0, const CUtensorMap& tmA1,
                               const CUtensorMap& tmB, const WgtArgs& a) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tcg_kernel<NN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tcg_kernel<NN, P, ABF>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return e;
-    return lf_launch(wgrad_tcg_kernel<NN, P>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
+    return lf_launch(wgrad_tcg_kernel<NN, P, ABF>, grid, WG_THREADS, smem_bytes, stream, tmA0, tmA1, tmB, a);
 }
 
 template <int P>
@@ -334,7 +349,8 @@ static cudaError_t wgt_launch_nn(dim3 grid, int smem_bytes, cudaStream_t stream,
 
 // a: A views and their block table, b: the B view; the launch of the generic kernel
 static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int Ws, int Ka, int Nn, int nblocks, const int* map,
-                   const int* dy, const int* dx, const int* cblk, float* partial, int nsplit, int prec, cudaStream_t stream) {
+                   const int* dy, const int* dx, const int* cblk, float* partial, int nsplit, int prec, cudaStream_t stream,
+                   bool abf = false) {
     TcEncodeTiledFn enc = tc_get_encode_fn();
     if (!enc) return LF_ERR_UNSUPPORTED;
     WgtArgs a{};
@@ -348,20 +364,24 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
         two = two || map[b] == 1;
     }
     LF_REQUIRE(!two || av[1].ptr);
+    // a bf16 A view: the 3-tap weight gradients of the bf16 mode (Nn = C)
+    if (abf && (prec != TC_BF16 || !(Nn == 64 || Nn == 128))) return LF_ERR_UNSUPPORTED;
     const int fixed = 1024 + wgt_bt_bytes(Nn, prec) + 256;   // alignment slack + transposed B tiles + barriers
-    a.stage_bytes = (a.nb_b + 2) * WG_BOX;
+    a.stage_bytes = a.nb_b * WG_BOX + 2 * wgt_a_box(abf);   // a multiple of 4 KB: every stage keeps the 1024-byte swizzle phase
     int stages = (WG_SMEM_LIMIT - fixed) / a.stage_bytes;
     if (stages > WG_MAX_STAGES) stages = WG_MAX_STAGES;
     a.stages = stages;
     a.total_patches = N * (Hs / a.by) * (Ws / a.bx);
 
     CUtensorMap tmA0, tmA1, tmB;
-    if (!wgt_encode(enc, &tmA0, av[0], N, Ka, a.bx, a.by)) return LF_ERR_CUDA;
-    if (!wgt_encode(enc, &tmA1, two ? av[1] : av[0], N, Ka, a.bx, a.by)) return LF_ERR_CUDA;
+    if (!wgt_encode(enc, &tmA0, av[0], N, Ka, a.bx, a.by, abf)) return LF_ERR_CUDA;
+    if (!wgt_encode(enc, &tmA1, two ? av[1] : av[0], N, Ka, a.bx, a.by, abf)) return LF_ERR_CUDA;
     if (!wgt_encode(enc, &tmB, bv, N, Nn, a.bx, a.by)) return LF_ERR_CUDA;
     const int smem_bytes = fixed + a.stages * a.stage_bytes;
     const dim3 grid(nsplit, (nblocks + 1) / 2);
-    const cudaError_t e = prec == TC_X3     ? wgt_launch_nn<TC_X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+    const cudaError_t e = abf               ? (Nn == 64 ? wgt_launch<64, TC_BF16, true>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
+                                                        : wgt_launch<128, TC_BF16, true>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a))
+                          : prec == TC_X3   ? wgt_launch_nn<TC_X3>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
                           : prec == TC_BF16 ? wgt_launch_nn<TC_BF16>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a)
                                             : wgt_launch_nn<TC_TF32>(grid, smem_bytes, stream, tmA0, tmA1, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
@@ -397,7 +417,7 @@ static int wgrad3_ctas(int N, int H, int W, int C, int min_per) {
 }
 
 static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                      float* partial, int nctas, int prec, lf_stream_t stream_) {
+                      float* partial, int nctas, int prec, lf_stream_t stream_, bool xbf16 = false) {
     LF_REQUIRE(x && dy && partial && tap_dy && tap_dx && nctas >= 1);
     if (!(C == 64 || C == 128)) return LF_ERR_UNSUPPORTED;
     const LfTcgView xv{x, H, W, (long long)H * W * C, (long long)W * C, C};
@@ -410,7 +430,8 @@ static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int 
             const int b = t * cbs + cb;
             map[b] = 0; bdy[b] = tap_dy[t]; bdx[b] = tap_dx[t]; cblk[b] = cb;
         }
-    return wgt_run(av, gv, N, H, W, C, C, 3 * cbs, map, bdy, bdx, cblk, partial, nctas, prec, reinterpret_cast<cudaStream_t>(stream_));
+    return wgt_run(av, gv, N, H, W, C, C, 3 * cbs, map, bdy, bdx, cblk, partial, nctas, prec, reinterpret_cast<cudaStream_t>(stream_),
+                   xbf16);
 }
 
 extern "C" int lf_wgrad3_tc_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 4); }
@@ -428,4 +449,7 @@ extern "C" int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, 
                                  float* partial, int nctas, lf_stream_t stream) {
     return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_BF16, stream);
 }
-
+extern "C" int lf_wgrad3_tc_bf16a(const void* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
+                                  float* partial, int nctas, lf_stream_t stream) {
+    return wgrad3_run(static_cast<const float*>(x), dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_BF16, stream, true);
+}

@@ -67,9 +67,10 @@ def nb1d(x, mod):
         return res
 
     (wp2, b2), (wp4, b4) = _cached(mod, [c2.weight, c2.bias, c4.weight, c4.bias] + _bn_tensors(mod.bn1) + _bn_tensors(mod.bn2), build)
-    t = o.conv3(x, c1.weight, True, 1, False, bias=c1.bias, relu=True)
-    t = o.conv3(t, None, False, 1, False, wp=wp2, bias=b2, relu=True)
-    t = o.conv3(t, c3.weight, True, dil, False, bias=c3.bias, relu=True)
+    sd = o.nb1d_storage_dtype(x, dil)     # the three intermediates are convolution inputs only
+    t = o.conv3(x, c1.weight, True, 1, False, bias=c1.bias, relu=True, dtype=sd)
+    t = o.conv3(t, None, False, 1, False, wp=wp2, bias=b2, relu=True, dtype=sd)
+    t = o.conv3(t, c3.weight, True, dil, False, bias=c3.bias, relu=True, dtype=sd)
     return o.conv3(t, None, False, dil, False, wp=wp4, bias=b4, relu=2, add_src=x)
 
 

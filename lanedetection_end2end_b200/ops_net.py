@@ -7,7 +7,8 @@ no torch operator touches a feature map on this path.
 Training-mode memory plan per non_bottleneck_1d (what backward needs):
   x (block input), t1 = relu(conv3x1_1), t2 = conv1x3_1 (pre-BN), t3 = relu(bn1),
   t4 = relu(conv3x1_2), t5 = conv1x3_2 (pre-BN), y = block output, the two (mean, invstd)
-  pairs and the dropout mask.
+  pairs and the dropout mask.  t1, t3 and t4 are only convolution inputs and ReLU masks: in bf16 mode
+  they are stored as bf16 (nb1d_storage_dtype).
 """
 import ctypes
 import os
@@ -29,7 +30,9 @@ LfConvArgs, LfWgradArgs, LfConvTcArgs = _capi.LfConvArgs, _capi.LfWgradArgs, _ca
 #   "tf32": tensor cores, single-pass TF32 multiply / fp32 accumulate (what cuDNN does for the reference's
 #           fp32 convs on Ampere+ GPUs; 1e-3 from fp32 on the curve coefficients -- a labelled extra);
 #   "bf16": tensor cores, both operands rounded to bf16 (nearest even) inside the kernels, exact products, fp32
-#           accumulate; storage stays fp32 (a labelled fast mode, ~5e-3 from fp64 on the curve coefficients);
+#           accumulate (a labelled fast mode, ~5e-3 from fp64 on the curve coefficients); the non_bottleneck_1d
+#           tensors that only feed convolutions and ReLU masks are stored as bf16 (same results, see
+#           nb1d_storage_dtype), everything else stays fp32;
 #   shapes a tensor-core kernel does not take stay on the fp32 kernel in every mode.
 CONV_MODES = ("fp32", "tf32", "tf32x3", "bf16")
 CONV_MODE = os.environ.get("LANEFIT_CONV_MODE", "tf32x3")
@@ -634,10 +637,11 @@ def run_conv_tc(taps, x, wpack, out, bias=None, relu=False, mask_src=None, add_s
     for t, (dy, dx) in enumerate(taps):
         a.dy[t], a.dx[t] = dy, dx
     a.relu = int(relu)
-    n_operands = 2 + (mask_src is not None) + (add_src is not None) + (add_mask is not None)
+    a.in_dtype, a.out_dtype = _capi.dtype_id(x), _capi.dtype_id(out)
+    a.mask_dtype = _capi.dtype_id(mask_src) if mask_src is not None else _capi.LF_F32
+    width = sum(t.element_size() for t in (x, out, mask_src, add_src, add_mask) if t is not None)
     entry = "lf_conv1d_tc_x3" if x3_mode() else "lf_conv1d_tc_bf16" if bf16_mode() else "lf_conv1d_tc"
-    _capi.call(entry, ctypes.byref(a), _stream(), flops=2 * N * H * W * 3 * C * C,
-               nbytes=4 * n_operands * N * H * W * C)
+    _capi.call(entry, ctypes.byref(a), _stream(), flops=2 * N * H * W * 3 * C * C, nbytes=width * N * H * W * C)
     if part is not None:
         if _DEFERRED is not None:
             _reduce(part, rows, 1, 1, C, 1, C, colsum, 0, 0, 1)
@@ -674,13 +678,14 @@ def _super_conv_launch(taps, xs, w, vertical, transposed, out, N, H, W, C, cs, e
     run_conv_tc(taps, xs, wp, out.view(N, H, W // SUPER, SUPER * C), colsum=cs, **epi_s)
 
 
-def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, **epi):
+def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, dtype=torch.float32, **epi):
     """One factorised 3-tap convolution of non_bottleneck_1d (or its input gradient when
     ``transposed``): dispatches to the tensor-core kernel in tf32 mode, else to the fp32 kernel.
     ``colsum`` ([C] tensor): also produce the per-channel sums of the result.
-    ``wp``: the already packed tensor-core operand (ops_eval's BatchNorm-folded weights) -- tensor-core routes only."""
+    ``wp``: the already packed tensor-core operand (ops_eval's BatchNorm-folded weights) -- tensor-core routes only.
+    ``dtype``: of the result; bf16 (like a bf16 ``x`` or ``mask_src``) only on the bf16 tensor-core routes."""
     N, H, W, C = x.shape
-    out = torch.empty_like(x)
+    out = torch.empty(x.shape, dtype=dtype, device=x.device)
     if super_ok(x, dil):
         xs = x.view(N, H, W // SUPER, SUPER * C)
         sgn = -1 if transposed else 1
@@ -707,6 +712,8 @@ def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, **epi):
         return run_conv_tc(taps, x, wp, out, colsum=colsum, **epi)
     if wp is not None:
         raise _capi.LanefitError("conv3: a pre-packed operand needs a tensor-core route")
+    if any(t.dtype != torch.float32 for t in [x, out] + [v for v in epi.values() if torch.is_tensor(v)]):
+        raise _capi.LanefitError("conv3: bf16 operands need a bf16 tensor-core route")
     kh, kw = (3, 1) if vertical else (1, 3)
     ph, pw = (dil, 0) if vertical else (0, dil)
     dh, dw = (dil, 1) if vertical else (1, dil)
@@ -726,6 +733,11 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
     bias_grad: "compute" (column sums of d_out), or "skip" (the caller gets it elsewhere)."""
     N, H, W, C = x_in.shape
     sfx = "_x3" if wgrad_x3() else "_bf16" if bf16_mode() else ""   # which tensor-core weight-gradient kernel
+    xbf = x_in.dtype == torch.bfloat16                               # a bf16 layer input: the bf16-A kernel
+    if xbf and not bf16_mode():
+        raise _capi.LanefitError("wgrad3: a bf16 layer input needs the bf16 mode")
+    entry = "lf_wgrad3_tc" + sfx + ("a" if xbf else "")
+    nbytes = (x_in.element_size() + 4) * N * H * W * C
     if super_ok(x_in, dil) and d_out.is_contiguous():
         Cs, Ws = SUPER * C, W // SUPER
         nctas = getattr(_lib(), "lf_wgrad3_tc%s_ctas" % sfx)(N, H, Ws, Cs)
@@ -735,8 +747,8 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
             partial = torch.empty(nctas * 3 * Cs * Cs, dtype=torch.float32, device=x_in.device)
             dws = torch.empty(Cs, Cs, 3, dtype=torch.float32, device=x_in.device)
             st = _stream()
-            _capi.call("lf_wgrad3_tc" + sfx, ptr(x_in), ptr(d_out), N, H, Ws, Cs, tdy, tdx, ptr(partial), nctas, st,
-                       flops=2 * N * H * W * 3 * C * C, nbytes=8 * N * H * W * C)
+            _capi.call(entry, ptr(x_in), ptr(d_out), N, H, Ws, Cs, tdy, tdx, ptr(partial), nctas, st,
+                       flops=2 * N * H * W * 3 * C * C, nbytes=nbytes)
             _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 3, Cs, Cs, Cs, Cs, ptr(dws), 1, 3, Cs * 3, st)
             dw = unpack_wgrad_super(dws, vertical).reshape(w.shape)
             db = None
@@ -753,12 +765,14 @@ def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
         tdx = (ctypes.c_int * 3)(*[(0 if vertical else (k - 1) * dil) for k in range(3)])
         partial = torch.empty(nctas * 3 * C * C, dtype=torch.float32, device=x_in.device)
         st = _stream()
-        _capi.call("lf_wgrad3_tc" + sfx, ptr(x_in), ptr(d_out), N, H, W, C, tdy, tdx, ptr(partial), nctas, st,
-                   flops=2 * N * H * W * 3 * C * C, nbytes=8 * N * H * W * C)
+        _capi.call(entry, ptr(x_in), ptr(d_out), N, H, W, C, tdy, tdx, ptr(partial), nctas, st,
+                   flops=2 * N * H * W * 3 * C * C, nbytes=nbytes)
         _reduce(partial, nctas, 3, C, C, C, C, dw, lay[0], lay[1], lay[2])
         if db is not None:
             run_colsum(d_out, C, 0, db)
         return dw, db
+    if xbf:
+        raise _capi.LanefitError("wgrad3: a bf16 layer input needs a tensor-core route")
     kh, kw = (3, 1) if vertical else (1, 3)
     ph, pw = (dil, 0) if vertical else (0, dil)
     dh, dw_ = (dil, 1) if vertical else (1, dil)
@@ -877,21 +891,22 @@ def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running
     if rows > 0:
         part = torch.empty(rows * 2 * C, dtype=torch.float64, device=x.device)
         taps = [(((k - 1) * dil, 0) if vertical else (0, (k - 1) * dil)) for k in range(3)]
-        out = run_conv_tc(taps, x, packed(w, "tc_fwd", pack_tc_fwd, split=pack_split()), torch.empty_like(x), bias=bias,
-                          stats_partial=part)
+        out = run_conv_tc(taps, x, packed(w, "tc_fwd", pack_tc_fwd, split=pack_split()),
+                          torch.empty(x.shape, dtype=torch.float32, device=x.device), bias=bias, stats_partial=part)
         return out, bn_finalize(part, rows, N * H * W, C, gamma, beta, running_mean, running_var)
     out = conv3(x, w, vertical, dil, False, bias=bias)
     return out, bn_forward_stats(out, gamma, beta, running_mean, running_var, training)
 
 
-def bn_apply(x, s, relu, drop=None, res=None):
-    h = _lib()
+def bn_apply(x, s, relu, drop=None, res=None, dtype=torch.float32):
+    """y = relu?((x*scale+shift) * drop? + res?), stored as ``dtype`` (fp32, or bf16 rounded to nearest even)."""
     C = x.shape[-1]
     npix = x.numel() // C
-    y = torch.empty_like(x)
+    y = torch.empty(x.shape, dtype=dtype, device=x.device)
     ppi = x.shape[1] * x.shape[2]
-    _capi.call("lf_bn_apply", ptr(x), npix, C, ppi, ptr(s.scale), ptr(s.shift), ptr(drop), ptr(res), int(relu), ptr(y),
-                              _stream(), nbytes=4 * npix * C * (2 + (res is not None)))
+    entry = "lf_bn_apply_bf16" if dtype == torch.bfloat16 else "lf_bn_apply"
+    _capi.call(entry, ptr(x), npix, C, ppi, ptr(s.scale), ptr(s.shift), ptr(drop), ptr(res), int(relu), ptr(y),
+               _stream(), nbytes=npix * C * (4 * (1 + (res is not None)) + y.element_size()))
     return y
 
 
@@ -1032,15 +1047,33 @@ class DownFunction(torch.autograd.Function):
 # --------------------------------------------------------------------------------------
 # non_bottleneck_1d  (ERFNet.py:25-60)
 # --------------------------------------------------------------------------------------
+def nb1d_storage_dtype(x, dil):
+    """Element type of the non_bottleneck_1d tensors that are only convolution inputs and ReLU masks: t1, t3, t4 of
+    Nb1dFunction and the three intermediates of ops_eval.nb1d.  bf16 in bf16 mode when every launch of the block,
+    forward and backward, runs on the bf16 tensor-core kernels: they round these operands to bf16 (nearest even)
+    anyway, so storing them rounded changes no result (a positive value at most half of bf16's smallest subnormal,
+    2^-134, would round to zero and flip its ReLU mask bit).  fp32 otherwise."""
+    if not bf16_mode():
+        return torch.float32
+    N, H, W, C = x.shape
+    if super_ok(x, dil):
+        ok = _lib().lf_wgrad3_tc_bf16_ctas(N, H, W // SUPER, SUPER * C) > 0
+    else:
+        ok = (all(tc_supported(x, v, d) for v in (True, False) for d in (1, dil))
+              and _lib().lf_wgrad3_tc_bf16_ctas(N, H, W, C) > 0)
+    return torch.bfloat16 if ok else torch.float32
+
+
 class Nb1dFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, b1, w2, b2, g1, be1, w3, b3, w4, b4, g2, be2, rm1, rv1, rm2, rv2, dil, drop, training):
         _capi.require_cuda(x)
         N, H, W, C = x.shape
-        t1 = conv3(x, w1, True, 1, False, bias=b1, relu=True)
+        sd = nb1d_storage_dtype(x, dil)
+        t1 = conv3(x, w1, True, 1, False, bias=b1, relu=True, dtype=sd)
         t2, s1 = conv3_bn_stats(t1, w2, False, 1, b2, g1, be1, rm1, rv1, training)
-        t3 = bn_apply(t2, s1, relu=True)
-        t4 = conv3(t3, w3, True, dil, False, bias=b3, relu=True)
+        t3 = bn_apply(t2, s1, relu=True, dtype=sd)
+        t4 = conv3(t3, w3, True, dil, False, bias=b3, relu=True, dtype=sd)
         t5, s2 = conv3_bn_stats(t4, w4, False, dil, b4, g2, be2, rm2, rv2, training)
         y = bn_apply(t5, s2, relu=True, drop=drop, res=x)
         ctx.save_for_backward(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1.mean, s1.invstd, s2.mean, s2.invstd,

@@ -5,7 +5,9 @@
 For every config the model, loss and batch are built once (bench.py's recipe: kaiming init, random images, synthetic
 targets); each round then re-captures the step in every mode in turn and times `--steps` replays with CUDA events, so the
 modes see the same card, clock and thermal state.  The card name, power limit and max SM clock come from a read-only
-`nvidia-smi --query-gpu` in the same run.  Prints one JSON document (and writes it to --out if given).
+`nvidia-smi --query-gpu` in the same run.  `max_memory_allocated_mb` is torch.cuda.max_memory_allocated() from the
+step's capture through its timed replays (the model, its gradients, the graph's memory pool), per mode, largest over
+the rounds.  Prints one JSON document (and writes it to --out if given).
 """
 import argparse
 import json
@@ -63,11 +65,14 @@ def main():
         hx, hxgt, hvalid = bench.host_batch(cfg, 1234, pinned=False)
         dx, dxgt, dvalid = hx.cuda(), hxgt.cuda(), hvalid.cuda()
         ms = {m: [] for m in a.modes}
+        peak = {m: 0 for m in a.modes}
         losses = {}
         for _ in range(a.rounds):
             for m in a.modes:
                 ops_net.set_conv_mode(m)
                 try:
+                    torch.cuda.synchronize()
+                    torch.cuda.reset_peak_memory_stats()
                     g = GraphedTrainStep(model, crit, cfg["nclasses"], dx, dxgt, dvalid, None)
                     for _ in range(3):
                         g()
@@ -79,6 +84,7 @@ def main():
                     e1.record()
                     torch.cuda.synchronize()
                     ms[m].append(e0.elapsed_time(e1) / a.steps)
+                    peak[m] = max(peak[m], torch.cuda.max_memory_allocated())
                     losses[m] = float(loss)
                     del g
                 finally:
@@ -88,6 +94,7 @@ def main():
             "ms_per_step": {m: [round(v, 3) for v in ms[m]] for m in a.modes},
             "median_ms": {m: round(statistics.median(ms[m]), 3) for m in a.modes},
             "images_per_s": {m: round(cfg["batch"] * 1000.0 / statistics.median(ms[m]), 1) for m in a.modes},
+            "max_memory_allocated_mb": {m: round(peak[m] / 2 ** 20, 1) for m in a.modes},
             "last_loss": losses,
         }
         del model

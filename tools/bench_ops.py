@@ -4,7 +4,8 @@
     python tools/bench_ops.py [--batch 32] [--modes tf32x3 tf32 bf16] > ops.jsonl
 
 One JSON line per (mode, op, shape): mean launch time over `--iters` back-to-back launches on tensors larger than L2 in
-aggregate (each op cycles through `--rot` independent input sets), CUDA events on the launching stream."""
+aggregate (each op cycles through `--rot` independent input sets), CUDA events on the launching stream.  In bf16 mode the
+"bf16 ..." ops read (and the forward writes) the bf16 activations non_bottleneck_1d stores in that mode."""
 import argparse
 import json
 import os
@@ -33,6 +34,7 @@ def main():
     for C, H, W, vertical, dil in SHAPES:
         N = a.batch
         xs = [torch.randn(N, H, W, C, device=dev) for _ in range(a.rot)]
+        xh = [t.bfloat16() for t in xs]
         gs = [torch.randn(N, H, W, C, device=dev) for _ in range(a.rot)]
         kh, kw = (3, 1) if vertical else (1, 3)
         w = torch.randn(C, C, kh, kw, device=dev) / (3 * C) ** 0.5
@@ -51,14 +53,22 @@ def main():
                 wf, wd, tf, td, view, bb = o.pack_tc_fwd(w), o.pack_tc_dgrad(w), taps(1), taps(-1), (lambda t: t), b
             wf, wd = o.tc_operand(wf), o.tc_operand(wd)   # tf32x3: the TF32 hi / lo pair; bf16: bf16 operands
             outs = [torch.empty_like(view(xs[0])) for _ in range(a.rot)]
+            outh = [torch.empty_like(view(xh[0])) for _ in range(a.rot)]
+            # op -> (launch, bytes per element of the activation-sized operands it moves)
             ops = {
-                "fwd_bias_relu": lambda i: o.run_conv_tc(tf, view(xs[i]), wf, outs[i], bias=bb, relu=True),
-                "dgrad_mask": lambda i: o.run_conv_tc(td, view(gs[i]), wd, outs[i], mask_src=view(xs[i])),
-                "dgrad_add": lambda i: o.run_conv_tc(td, view(gs[i]), wd, outs[i], add_src=view(xs[i]),
-                                                      add_mask=view(xs[(i + 1) % a.rot])),
-                "wgrad (+reduce)": lambda i: o.wgrad3(xs[i], gs[i], w, vertical, dil, bias_grad="skip"),
+                "fwd_bias_relu": (lambda i: o.run_conv_tc(tf, view(xs[i]), wf, outs[i], bias=bb, relu=True), 8),
+                "dgrad_mask": (lambda i: o.run_conv_tc(td, view(gs[i]), wd, outs[i], mask_src=view(xs[i])), 12),
+                "dgrad_add": (lambda i: o.run_conv_tc(td, view(gs[i]), wd, outs[i], add_src=view(xs[i]),
+                                                      add_mask=view(xs[(i + 1) % a.rot])), 16),
+                "wgrad (+reduce)": (lambda i: o.wgrad3(xs[i], gs[i], w, vertical, dil, bias_grad="skip"), 8),
             }
-            for name, fn in ops.items():
+            if mode == "bf16":
+                ops.update({
+                    "bf16 fwd_bias_relu (bf16 in, out)": (lambda i: o.run_conv_tc(tf, view(xh[i]), wf, outh[i], bias=bb, relu=True), 4),
+                    "bf16 dgrad_mask (bf16 mask)": (lambda i: o.run_conv_tc(td, view(gs[i]), wd, outs[i], mask_src=view(xh[i])), 10),
+                    "bf16 wgrad (+reduce) (bf16 x)": (lambda i: o.wgrad3(xh[i], gs[i], w, vertical, dil, bias_grad="skip"), 6),
+                })
+            for name, (fn, width) in ops.items():
                 # a.iters launches (cycling through the input sets) captured into a CUDA graph: the replay time is GPU
                 # time, not ctypes launch overhead (~25 us per eager launch)
                 side = torch.cuda.Stream()
@@ -82,7 +92,7 @@ def main():
                 us = e0.elapsed_time(e1) * 1e3 / a.iters
                 del g
                 flops = 2.0 * N * H * W * 3 * C * C
-                nbytes = 4.0 * N * H * W * C * (2 + (name != "fwd_bias_relu") + (name == "dgrad_add"))
+                nbytes = float(width) * N * H * W * C
                 print(json.dumps({"mode": mode, "op": name, "C": C, "H": H, "W": W, "vertical": vertical, "dil": dil, "batch": N,
                                   "us": round(us, 2), "tflops": round(flops / us / 1e6, 1), "gbs": round(nbytes / us / 1e3, 0)}),
                       flush=True)
