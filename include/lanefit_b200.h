@@ -462,6 +462,51 @@ int lf_frame_preprocess(const unsigned char* frames, int N, int Hin, int Win, in
                         int kx, const int* yb, const int* yk, int ky, int Ho, int Wo, const unsigned char* flip, int layout,
                         float* out, lf_stream_t stream);
 
+/* Optimizer update (csrc/optim.cu; replaces the torch.optim.Adam / SGD / RMSprop that BP/Networks/utils.py define_optim
+ * builds, stepped at BP/main.py:262,340): one multi-tensor launch updates every parameter listed in `segs`, in place.
+ * Each tensor stays where it is; the launch splits every segment into chunks of LF_OPTIM_CHUNK elements (the last one
+ * shorter) and maps chunks to CTAs.  A chunk uses 16-byte accesses when all of its pointers are 16-byte aligned, scalar
+ * accesses otherwise, so gradients may be views at any offset into a flat buffer.
+ * Scalars are formed in fp64 from `hyper` and the step counter, then rounded to fp32; the elementwise arithmetic is fp32
+ * in torch's order, each operation an explicit round-to-nearest intrinsic (nothing left for the compiler to contract);
+ * a term a + s*b is one fused multiply-add exactly where torch's CUDA kernels form it as one (add_ with alpha, lerp_,
+ * addcmul_, addcdiv_).  g = grad + wd*p in every algorithm:
+ *   LF_OPTIM_ADAM    state0 = exp_avg, state1 = exp_avg_sq (amsgrad off, L2 weight decay, not AdamW):
+ *                    m = m + (1-b1)(g-m);  v = b2 v + (1-b2) g g;  t += 1;
+ *                    p -= (lr / (1-b1^t)) * m / (sqrt(v) / sqrt(1-b2^t) + eps)
+ *   LF_OPTIM_SGD     state0 = momentum_buffer, state1 unused (NULL; dampening 0, no Nesterov):
+ *                    buf = g on the first step (t = 0 before it), else momentum*buf + g;  p -= lr*buf
+ *   LF_OPTIM_RMSPROP state0 = square_avg, state1 = momentum_buffer (not centred; hyper.beta2 is alpha):
+ *                    sq = alpha sq + (1-alpha) g g;  buf = momentum*buf + g / (sqrt(sq) + eps);  p -= lr*buf
+ * `state->step` is advanced once per launch, by the last CTA to finish (ticket).  `status`: NULL, or a device word
+ * (lf_lsq_fwd's status); when it is nonzero the launch changes no parameter, state tensor or step counter and only
+ * increments `state->skipped` -- the reference skips the batch of a singular system (BP/main.py:289-292) without a host
+ * round trip.  `segs`, `hyper` and `state` are DEVICE pointers; `state` is zeroed once before first use and the ticket is
+ * left at zero by every launch.  Never synchronises; graph-capturable (a replay reads the current `hyper`). */
+#define LF_OPTIM_ADAM 0
+#define LF_OPTIM_SGD 1
+#define LF_OPTIM_RMSPROP 2
+#define LF_OPTIM_CHUNK 2048
+typedef struct LfOptimSeg {
+    float* param;
+    const float* grad;
+    float* state0;
+    float* state1;
+    long long numel;
+    long long chunk0;       /* index of this segment's first chunk: sum of ceil(numel / LF_OPTIM_CHUNK) over the rows before */
+} LfOptimSeg;
+typedef struct LfOptimHyper {
+    double lr, beta1, beta2, eps, weight_decay, momentum;    /* beta2 = alpha for RMSprop; unused fields ignored */
+} LfOptimHyper;
+typedef struct LfOptimState {
+    long long step;         /* updates applied (torch's per-parameter `step`, shared by every parameter) */
+    long long skipped;      /* launches skipped by a nonzero status word */
+    unsigned long long ticket;
+} LfOptimState;
+/* nchunks = total chunks over all rows (the chunk0 of a row one past the last) */
+int lf_optim_step(int algo, const LfOptimSeg* segs, int nsegs, long long nchunks, const LfOptimHyper* hyper,
+                  LfOptimState* state, const int* status, lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

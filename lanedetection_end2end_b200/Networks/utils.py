@@ -204,7 +204,16 @@ class AverageMeter(object):
         self.avg = self.sum / self.count
 
 
-def define_optim(optim, params, lr, weight_decay):
+def define_optim(optim, params, lr, weight_decay, fused=None):
+    """torch.optim's Adam / SGD / RMSprop (BP/Networks/utils.py:451-461), or with ``fused`` the same update as one launch
+    of the library's kernel (lanedetection_end2end_b200.optim.FusedOptimizer, CUDA-graph capturable, same state_dict
+    format).  fused=None reads LANEFIT_FUSED_OPTIM (default 0: the torch optimizer), so the reference's main.py can opt in
+    without edits."""
+    if fused is None:
+        fused = os.environ.get("LANEFIT_FUSED_OPTIM", "0") != "0"
+    if fused and optim in ("adam", "sgd", "rmsprop"):
+        from ._pkg import submodule
+        return submodule("optim").FusedOptimizer(params, optim, lr, weight_decay)
     if optim == "adam":
         return torch.optim.Adam(params, lr=lr, weight_decay=weight_decay)
     if optim == "sgd":

@@ -103,7 +103,25 @@ class LfWgradTcgArgs(ctypes.Structure):
                 ("dx", _i * WGRAD_TCG_MAX_BLOCKS), ("cblk", _i * WGRAD_TCG_MAX_BLOCKS), ("nctas", _i), ("precision", _i)]
 
 
+OPTIM_ADAM, OPTIM_SGD, OPTIM_RMSPROP = 0, 1, 2
+OPTIM_CHUNK = 2048
+
+
+class LfOptimSeg(ctypes.Structure):
+    _fields_ = [("param", _p), ("grad", _p), ("state0", _p), ("state1", _p), ("numel", _ll), ("chunk0", _ll)]
+
+
+class LfOptimHyper(ctypes.Structure):
+    _fields_ = [("lr", _c_double), ("beta1", _c_double), ("beta2", _c_double), ("eps", _c_double),
+                ("weight_decay", _c_double), ("momentum", _c_double)]
+
+
+class LfOptimState(ctypes.Structure):
+    _fields_ = [("step", _ll), ("skipped", _ll), ("ticket", ctypes.c_ulonglong)]
+
+
 _NET_PROTOS = {
+    "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg_ctas_x3": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg_ctas_bf16": (_i, [_i, _i, _i, _i, _i, _i]),

@@ -64,6 +64,16 @@ class FlatGradAllReduce:
         return self.flat
 
 
+def any_rank_nonzero(word, out, group=None):
+    """out[0] = max over the group's ranks of word[0] (int32 status words, >= 0): nonzero iff any rank's word is nonzero.
+    The guarded optimizer update reads it, so that a singular system on one rank skips the update on every rank and the
+    replicas, which apply the same averaged gradients, stay identical.  One capturable all-reduce of one element."""
+    out.copy_(word)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(out, op=dist.ReduceOp.MAX, group=group)
+    return out
+
+
 def broadcast_parameters(module, src=0, group=None):
     """Make every replica start from rank ``src``'s parameters and buffers."""
     if not dist.is_initialized() or dist.get_world_size(group) == 1:

@@ -21,8 +21,22 @@ FUSED_LOSS = os.environ.get("LANEFIT_FUSED_LOSS", "1") != "0"
 
 
 class GraphedTrainStep:
+    """``optimizer``: None (the graph ends with the gradients, the caller steps its optimizer), or an
+    ``optim.FusedOptimizer`` over the model's parameters: the graph then starts by zeroing ``model.lsq_status`` (the
+    status becomes per-step) and ends, after the reducer, with the update guarded by that word -- a batch with a singular
+    system changes no parameter or optimizer state, with no host synchronisation.  With a reducer the guard reads the
+    word's maximum over the ranks (one all-reduce of one element, ddp.any_rank_nonzero), so every rank skips or updates
+    together and the replicas stay identical.  Each call writes the optimizer's
+    hyperparameters first if a param_groups value changed (schedulers work without a recapture)."""
+
     def __init__(self, model, criterion, nclasses, example_x, example_xgt, example_valid, reducer=None, warmup=3,
-                 capture_error_mode="global", extra_loss=None, global_valid=False):
+                 capture_error_mode="global", extra_loss=None, global_valid=False, optimizer=None):
+        if optimizer is not None:
+            from .optim import FusedOptimizer
+            if not isinstance(optimizer, FusedOptimizer):
+                raise TypeError("GraphedTrainStep captures the update of an optim.FusedOptimizer only, got %s"
+                                % type(optimizer).__name__)
+        self.optimizer = optimizer
         self.model = model
         self.global_valid = global_valid  # batch-global sum(valid) normaliser across ranks (ddp.lane_valid_scale)
         self.extra_loss = extra_loss      # callable(forward 9-tuple) -> scalar added to the loss (e.g. the --clas head losses)
@@ -48,6 +62,14 @@ class GraphedTrainStep:
         if reducer is not None and hasattr(reducer, "attach"):
             reducer.attach()          # gradients become views of the flat all-reduce buffer: no pack / unpack copies
         self.grads = [p.grad for p in self.params if p.grad is not None]
+        if optimizer is not None:
+            self.updated = optimizer.grad_params()
+            optimizer.prepare(self.updated)          # state and segment table exist before the capture
+            optimizer.sync_hyperparameters()
+            self.skip_word = torch.zeros(1, dtype=torch.int32, device=dev)   # status word reduced over the ranks
+            # what a replay writes through raw pointers besides the parameters: the BatchNorm running statistics
+            self.written = self.updated + [b for m in model.modules() if isinstance(m, torch.nn.BatchNorm2d)
+                                           for b in (m.running_mean, m.running_var) if b is not None]
         self.graph = torch.cuda.CUDAGraph()
         # with NCCL in the graph use capture_error_mode="thread_local": the process group's watchdog thread polls CUDA
         # events, which the default "global" mode treats as a capture violation
@@ -59,6 +81,8 @@ class GraphedTrainStep:
         if first:
             self.model.zero_grad(set_to_none=True)
         else:
+            if self.optimizer is not None:
+                self.model.lsq_status.zero_()
             torch._foreach_zero_(self.grads)
         out = self.model(self.x, self.gt_line, True)
         scale = None
@@ -81,6 +105,13 @@ class GraphedTrainStep:
         loss.backward()
         if self.reducer is not None:
             self.reducer()
+        if not first and self.optimizer is not None:
+            status = self.model.lsq_status
+            if self.reducer is not None:
+                # data-parallel: the ranks share the averaged gradients, so a singular system on any rank skips every rank
+                from .ddp import any_rank_nonzero
+                status = any_rank_nonzero(status, self.skip_word, getattr(self.reducer, "group", None))
+            self.optimizer.launch(status=status)
         return loss.detach()
 
     def load(self, x, xgt, valid):
@@ -115,7 +146,12 @@ class GraphedTrainStep:
         self._consumed.record(cur)
 
     def __call__(self):
+        if self.optimizer is None:
+            self.graph.replay()
+            return self.loss
+        self.optimizer.sync_hyperparameters()
         self.graph.replay()
+        torch.autograd.graph.increment_version(self.written)    # version-keyed caches (ops_eval) see the update
         return self.loss
 
 

@@ -39,7 +39,10 @@ def synthetic_batch(B, device, seed=0):
     return img.to(device), x_gt.to(device), valid.to(device)
 
 
-def run(steps=40, batch=4, lr=1e-3, seed=0, device="cuda"):
+def run(steps=40, batch=4, lr=1e-3, seed=0, device="cuda", fused=False, graphed=False):
+    """fused: the library's Adam (optim.FusedOptimizer) instead of torch.optim.Adam.  graphed (needs fused): the whole
+    iteration, update included, as one CUDA graph replay per step (engine.GraphedTrainStep); a skipped step is counted
+    from the optimizer's device counter once at the end."""
     from lanedetection_end2end_b200.Networks.LSQ_layer import Net
     from lanedetection_end2end_b200.Networks.utils import define_args, define_init_weights, define_optim
     from lanedetection_end2end_b200.Loss_crit import define_loss_crit
@@ -51,9 +54,16 @@ def run(steps=40, batch=4, lr=1e-3, seed=0, device="cuda"):
         define_init_weights(model, "kaiming")
     model = model.to(device).train()
     criterion, _ = define_loss_crit(args)
-    optimizer = define_optim("adam", model.parameters(), lr, 0)
+    optimizer = define_optim("adam", model.parameters(), lr, 0, fused=fused or graphed)
     x, x_gt, valid = synthetic_batch(batch, device, seed)
     gt_line = torch.zeros(batch, 4)
+    if graphed:
+        from lanedetection_end2end_b200.engine import GraphedTrainStep
+        step = GraphedTrainStep(model, criterion, 2, x, x_gt, valid, optimizer=optimizer)
+        losses = [step().clone() for _ in range(steps)]
+        losses = [float(v) for v in losses]
+        return {"steps": steps, "batch": batch, "skipped": optimizer.skipped, "loss_first": losses[0], "loss_last": losses[-1],
+                "loss_min": min(losses), "losses": [round(v, 2) for v in losses]}
     losses, skipped = [], 0
     for _ in range(steps):
         optimizer.zero_grad()
@@ -74,5 +84,7 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--batch", type=int, default=4)
+    ap.add_argument("--fused-optim", action="store_true", help="step with the library's fused Adam kernel")
+    ap.add_argument("--graphed", action="store_true", help="one CUDA graph replay per iteration (implies --fused-optim)")
     a = ap.parse_args()
-    print(json.dumps(run(a.steps, a.batch)))
+    print(json.dumps(run(a.steps, a.batch, fused=a.fused_optim, graphed=a.graphed)))
