@@ -305,6 +305,24 @@ int lf_bn_bwd_finalize(const double* partial, int nblk, long long npix, int C, f
  * c1 = dbeta/npix, c2 = dgamma/npix = the per-channel constants lf_bn_bwd_apply takes. */
 int lf_bn_bwd_finalize_sx(const double* partial, int nblk, long long npix, int C, int fold, const float* mean,
                           const float* invstd, float* dgamma, float* dbeta, float* c1, float* c2, lf_stream_t stream);
+/* SyncBatchNorm (nn.SyncBatchNorm containers): the statistics of every rank, with the all-reduce between two launches.
+ *  collapse : partial[nblk][2][C*fold] (of lf_bn_stats, the conv epilogue's stats_partial or lf_bn_bwd_reduce) ->
+ *             totals[2C+1] = (sum a [C], sum b [C], npix), each sum in the order the finalize kernels above use
+ *             (fold > 1 as lf_bn_bwd_finalize_sx); local (optional) receives a copy.  All-reduce (SUM) `totals`.
+ *  finalize_tot        : lf_bn_finalize from the summed totals (count = totals[2C], as fp64).
+ *  bwd_finalize_tot    : lf_bn_bwd_finalize; dgamma / dbeta from `local` (this rank's sums), c1 / c2 from `global` and *count
+ *                        (the forward's global count).
+ *  bwd_finalize_sx_tot : the same for lf_bn_bwd_finalize_sx's (sum g, sum g*x), with mean / invstd of the forward.
+ * Each shares its per-channel arithmetic with the kernel it mirrors: totals of one process give the same bits. */
+int lf_bn_collapse(const double* partial, int nblk, int C, int fold, long long npix, double* totals, double* local,
+                   lf_stream_t stream);
+int lf_bn_finalize_tot(const double* totals, int C, const float* gamma, const float* beta, float eps, float momentum,
+                       float* running_mean, float* running_var, float* mean, float* invstd, float* scale, float* shift,
+                       lf_stream_t stream);
+int lf_bn_bwd_finalize_tot(const double* local, const double* global, const double* count, int C, float* dgamma,
+                           float* dbeta, float* c1, float* c2, lf_stream_t stream);
+int lf_bn_bwd_finalize_sx_tot(const double* local, const double* global, const double* count, int C, const float* mean,
+                              const float* invstd, float* dgamma, float* dbeta, float* c1, float* c2, lf_stream_t stream);
 int lf_bn_bwd_apply(const float* dy, const float* ymask, const float* drop, const float* x, long long npix,
                     int C, int pix_per_image, const float* mean, const float* invstd, const float* gamma,
                     const float* c1, const float* c2, float* dx, lf_stream_t stream);

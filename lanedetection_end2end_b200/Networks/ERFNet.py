@@ -5,6 +5,8 @@ and ``define_init_weights`` work unchanged) and forward signatures.  The ``nn.Co
 own forward is never called; every block runs as one autograd Function over the sm_90a
 kernels (ops_net.py).  Feature maps travel between blocks as NHWC memory viewed with the
 reference's NCHW shape (channels_last), so chaining blocks costs no layout change.
+A BatchNorm container converted by ``torch.nn.SyncBatchNorm.convert_sync_batchnorm`` makes its block normalise with the
+statistics of every rank of its ``process_group`` in training mode (ops_net.BNSync); eval mode is unchanged.
 """
 import torch
 import torch.nn as nn
@@ -88,7 +90,8 @@ class DownsamplerBlock(nn.Module):
             if y is not None:
                 return _ops.as_nchw_view(y)
         y = _ops.DownFunction.apply(x, self.ninput, self.conv.weight, self.conv.bias, self.bn.weight, self.bn.bias,
-                                    self.bn.running_mean, self.bn.running_var, self.training, need_dx)
+                                    self.bn.running_mean, self.bn.running_var, self.training, need_dx,
+                                    _ops.bn_sync(self.bn, self.training))
         _track(self.bn, self.training)
         return _ops.as_nchw_view(y)
 
@@ -132,7 +135,8 @@ class non_bottleneck_1d(nn.Module):
             self.bn1.weight, self.bn1.bias, self.conv3x1_2.weight, self.conv3x1_2.bias,
             self.conv1x3_2.weight, self.conv1x3_2.bias, self.bn2.weight, self.bn2.bias,
             self.bn1.running_mean, self.bn1.running_var, self.bn2.running_mean, self.bn2.running_var,
-            self.dilated, self._drop_mask(x), self.training)
+            self.dilated, self._drop_mask(x), self.training, _ops.bn_sync(self.bn1, self.training),
+            _ops.bn_sync(self.bn2, self.training))
         _track(self.bn1, self.training)
         _track(self.bn2, self.training)
         return _ops.as_nchw_view(y)
@@ -199,7 +203,8 @@ class UpsamplerBlock(nn.Module):
             if y is not None:
                 return _ops.as_nchw_view(y)
         y = _ops.UpFunction.apply(x, self.conv.weight, self.conv.bias, self.bn.weight, self.bn.bias,
-                                  self.bn.running_mean, self.bn.running_var, self.training)
+                                  self.bn.running_mean, self.bn.running_var, self.training,
+                                  _ops.bn_sync(self.bn, self.training))
         _track(self.bn, self.training)
         return _ops.as_nchw_view(y)
 

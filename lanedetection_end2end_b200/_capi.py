@@ -186,6 +186,10 @@ _NET_PROTOS = {
     "lf_linear_bwd_data": (_i, [_p, _p, _p, _i, _i, _i, _p, _p]),
     "lf_linear_bwd_weight": (_i, [_p, _p, _p, _i, _i, _i, _p, _p, _p]),
     "lf_bn_bwd_finalize_sx": (_i, [_p, _i, ctypes.c_longlong, _i, _i, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_bn_collapse": (_i, [_p, _i, _i, _i, ctypes.c_longlong, _p, _p, _p]),
+    "lf_bn_finalize_tot": (_i, [_p, _i, _p, _p, ctypes.c_float, ctypes.c_float, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_bn_bwd_finalize_tot": (_i, [_p, _p, _p, _i, _p, _p, _p, _p, _p]),
+    "lf_bn_bwd_finalize_sx_tot": (_i, [_p, _p, _p, _i, _p, _p, _p, _p, _p, _p, _p]),
 }
 PROTOTYPES.update(_NET_PROTOS)
 

@@ -96,17 +96,26 @@ __device__ __forceinline__ void bn_sum_partials(const double* __restrict__ parti
     s2 = warp_sum((b0 + b1) + (b2 + b3));
 }
 
-__global__ void bn_finalize_kernel(const double* __restrict__ partial, int nblk, long long npix, int C,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum,
-                                   float* running_mean, float* running_var, float* mean, float* invstd, float* scale,
-                                   float* shift) {
-    pdl_entry();
-    const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per channel
-    if (c >= C) return;
-    double s1, s2;
-    bn_sum_partials(partial, nblk, C, c, s1, s2);
-    if ((threadIdx.x & 31) != 0) return;
-    const double n = (double)npix;
+// Column groups f*C + c (f < fold) of a [nblk][2][C*fold] partial that map to channel c (fold > 1: super-pixel layers),
+// each summed by bn_sum_partials, then added in group order
+__device__ __forceinline__ void bn_sum_folded(const double* __restrict__ partial, int nblk, int C, int fold, int c, double& s1,
+                                              double& s2) {
+    s1 = 0.0;
+    s2 = 0.0;
+    for (int f = 0; f < fold; ++f) {
+        double a, b;
+        bn_sum_partials(partial, nblk, C * fold, f * C + c, a, b);
+        s1 += a;
+        s2 += b;
+    }
+}
+
+// Per-channel finalize arithmetic, shared by the kernels that sum partials themselves and the ones that read totals
+// (SyncBatchNorm: totals all-reduced over the ranks), so that both give the same bits from the same sums.
+__device__ __forceinline__ void bn_finalize_channel(int c, double s1, double s2, double n, const float* __restrict__ gamma,
+                                                    const float* __restrict__ beta, float eps, float momentum,
+                                                    float* running_mean, float* running_var, float* mean, float* invstd,
+                                                    float* scale, float* shift) {
     const double m = s1 / n;
     double var = s2 / n - m * m;
     if (var < 0.0) var = 0.0;
@@ -117,10 +126,95 @@ __global__ void bn_finalize_kernel(const double* __restrict__ partial, int nblk,
     scale[c] = sc;
     shift[c] = beta[c] - (float)m * sc;
     if (running_mean) {
-        const double unb = (npix > 1) ? var * n / (n - 1.0) : var;
+        const double unb = (n > 1.0) ? var * n / (n - 1.0) : var;
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)m;
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unb;
     }
+}
+
+// Backward constants from (s1, s2) = (sum g, sum g*xhat): dgamma / dbeta from this rank's sums (l), c1 / c2 from the sums
+// over every rank (g) and the global count n.  Single process: l == g.
+__device__ __forceinline__ void bn_bwd_finalize_channel(int c, double s1l, double s2l, double s1g, double s2g, double n,
+                                                        float* dgamma, float* dbeta, float* c1, float* c2) {
+    dbeta[c] = (float)s1l;
+    dgamma[c] = (float)s2l;
+    c1[c] = (float)(s1g / n);
+    c2[c] = (float)(s2g / n);
+}
+
+// The same from (s1, s2) = (sum g, sum g*x) of the conv epilogue: sum g*xhat = invstd*(sum g*x - mean*sum g), linear in the
+// sums, so converting the all-reduced sums with the (global) mean is exact
+__device__ __forceinline__ void bn_bwd_finalize_sx_channel(int c, double s1l, double s2l, double s1g, double s2g, double n,
+                                                           const float* __restrict__ mean, const float* __restrict__ invstd,
+                                                           float* dgamma, float* dbeta, float* c1, float* c2) {
+    const double dgl = (double)invstd[c] * (s2l - (double)mean[c] * s1l);
+    const double dgg = (double)invstd[c] * (s2g - (double)mean[c] * s1g);
+    dbeta[c] = (float)s1l;
+    dgamma[c] = (float)dgl;
+    c1[c] = (float)(s1g / n);
+    c2[c] = (float)(dgg / n);
+}
+
+__global__ void bn_finalize_kernel(const double* __restrict__ partial, int nblk, long long npix, int C,
+                                   const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum,
+                                   float* running_mean, float* running_var, float* mean, float* invstd, float* scale,
+                                   float* shift) {
+    pdl_entry();
+    const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per channel
+    if (c >= C) return;
+    double s1, s2;
+    bn_sum_partials(partial, nblk, C, c, s1, s2);
+    if ((threadIdx.x & 31) != 0) return;
+    bn_finalize_channel(c, s1, s2, (double)npix, gamma, beta, eps, momentum, running_mean, running_var, mean, invstd, scale,
+                        shift);
+}
+
+// SyncBatchNorm, step 1: partial[nblk][2][C*fold] -> totals[2C+1] = (sum a [C], sum b [C], npix), summed exactly as the
+// finalize kernels sum them (fold == 1: bn_sum_partials, else bn_sum_folded).  local (optional): a second copy, kept
+// while `totals` is all-reduced (the backward's dgamma / dbeta are this rank's sums).
+__global__ void bn_collapse_kernel(const double* __restrict__ partial, int nblk, int C, int fold, long long npix,
+                                   double* __restrict__ totals, double* __restrict__ local) {
+    pdl_entry();
+    const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per channel
+    if (c >= C) return;
+    double s1, s2;
+    if (fold == 1) bn_sum_partials(partial, nblk, C, c, s1, s2);
+    else bn_sum_folded(partial, nblk, C, fold, c, s1, s2);
+    if ((threadIdx.x & 31) != 0) return;
+    totals[c] = s1;
+    totals[C + c] = s2;
+    if (c == 0) totals[2 * C] = (double)npix;
+    if (local) {
+        local[c] = s1;
+        local[C + c] = s2;
+        if (c == 0) local[2 * C] = (double)npix;
+    }
+}
+
+// SyncBatchNorm, step 2 (after the all-reduce of totals): the forward finalize from the global sums and count
+__global__ void bn_finalize_tot_kernel(const double* __restrict__ totals, int C, const float* __restrict__ gamma,
+                                       const float* __restrict__ beta, float eps, float momentum, float* running_mean,
+                                       float* running_var, float* mean, float* invstd, float* scale, float* shift) {
+    pdl_entry();
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    bn_finalize_channel(c, totals[c], totals[C + c], totals[2 * C], gamma, beta, eps, momentum, running_mean, running_var, mean,
+                        invstd, scale, shift);
+}
+
+// SX: totals hold (sum g, sum g*x) of the conv epilogue (lf_bn_bwd_finalize_sx), else (sum g, sum g*xhat)
+template <bool SX>
+__global__ void bn_bwd_finalize_tot_kernel(const double* __restrict__ local, const double* __restrict__ global,
+                                           const double* __restrict__ count, int C, const float* __restrict__ mean,
+                                           const float* __restrict__ invstd, float* dgamma, float* dbeta, float* c1, float* c2) {
+    pdl_entry();
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    if (SX)
+        bn_bwd_finalize_sx_channel(c, local[c], local[C + c], global[c], global[C + c], *count, mean, invstd, dgamma, dbeta,
+                                   c1, c2);
+    else
+        bn_bwd_finalize_channel(c, local[c], local[C + c], global[c], global[C + c], *count, dgamma, dbeta, c1, c2);
 }
 
 __global__ void bn_eval_prepare_kernel(int C, const float* gamma, const float* beta, float eps, const float* rm,
@@ -142,10 +236,7 @@ __global__ void bn_bwd_finalize_kernel(const double* __restrict__ partial, int n
     double s1, s2;
     bn_sum_partials(partial, nblk, C, c, s1, s2);
     if ((threadIdx.x & 31) != 0) return;
-    dbeta[c] = (float)s1;
-    dgamma[c] = (float)s2;
-    c1[c] = (float)(s1 / (double)npix);
-    c2[c] = (float)(s2 / (double)npix);
+    bn_bwd_finalize_channel(c, s1, s2, s1, s2, (double)npix, dgamma, dbeta, c1, c2);
 }
 
 // Statistics from the conv epilogue (lf_conv1d_tc[_x3] with mask_scale): [0] = sum g, [1] = sum g*x  ->  sum g*xhat =
@@ -156,19 +247,10 @@ __global__ void bn_bwd_finalize_sx_kernel(const double* __restrict__ partial, in
     pdl_entry();
     const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per channel
     if (c >= C) return;
-    double s1 = 0.0, s2 = 0.0;
-    for (int f = 0; f < fold; ++f) {
-        double a, b;
-        bn_sum_partials(partial, nblk, C * fold, f * C + c, a, b);
-        s1 += a;
-        s2 += b;
-    }
+    double s1, s2;
+    bn_sum_folded(partial, nblk, C, fold, c, s1, s2);
     if ((threadIdx.x & 31) != 0) return;
-    const double dg = (double)invstd[c] * (s2 - (double)mean[c] * s1);
-    dbeta[c] = (float)s1;
-    dgamma[c] = (float)dg;
-    c1[c] = (float)(s1 / (double)npix);
-    c2[c] = (float)(dg / (double)npix);
+    bn_bwd_finalize_sx_channel(c, s1, s2, s1, s2, (double)npix, mean, invstd, dgamma, dbeta, c1, c2);
 }
 
 // y = relu?( (x*scale+shift) * drop? + res? )
@@ -517,6 +599,44 @@ extern "C" int lf_bn_finalize(const double* partial, int nblk, long long npix, i
     LF_REQUIRE((running_mean == nullptr) == (running_var == nullptr));
     lf_launch(bn_finalize_kernel, (C * 32 + 255) / 256, 256, 0, stream, partial, nblk, npix, C, gamma, beta, eps, momentum, running_mean,
                                                             running_var, mean, invstd, scale, shift);
+    return check_launch();
+}
+
+extern "C" int lf_bn_collapse(const double* partial, int nblk, int C, int fold, long long npix, double* totals, double* local,
+                              lf_stream_t stream_) {
+    STREAM;
+    LF_REQUIRE(partial && totals && nblk >= 1 && C >= 1 && fold >= 1 && npix > 0);
+    lf_launch(bn_collapse_kernel, (C * 32 + 255) / 256, 256, 0, stream, partial, nblk, C, fold, npix, totals, local);
+    return check_launch();
+}
+
+extern "C" int lf_bn_finalize_tot(const double* totals, int C, const float* gamma, const float* beta, float eps, float momentum,
+                                  float* running_mean, float* running_var, float* mean, float* invstd, float* scale, float* shift,
+                                  lf_stream_t stream_) {
+    STREAM;
+    LF_REQUIRE(totals && gamma && beta && mean && invstd && scale && shift && C >= 1);
+    LF_REQUIRE((running_mean == nullptr) == (running_var == nullptr));
+    lf_launch(bn_finalize_tot_kernel, (C + 127) / 128, 128, 0, stream, totals, C, gamma, beta, eps, momentum, running_mean,
+              running_var, mean, invstd, scale, shift);
+    return check_launch();
+}
+
+extern "C" int lf_bn_bwd_finalize_tot(const double* local, const double* global, const double* count, int C, float* dgamma,
+                                      float* dbeta, float* c1, float* c2, lf_stream_t stream_) {
+    STREAM;
+    LF_REQUIRE(local && global && count && dgamma && dbeta && c1 && c2 && C >= 1);
+    lf_launch(bn_bwd_finalize_tot_kernel<false>, (C + 127) / 128, 128, 0, stream, local, global, count, C, (const float*)nullptr,
+              (const float*)nullptr, dgamma, dbeta, c1, c2);
+    return check_launch();
+}
+
+extern "C" int lf_bn_bwd_finalize_sx_tot(const double* local, const double* global, const double* count, int C, const float* mean,
+                                         const float* invstd, float* dgamma, float* dbeta, float* c1, float* c2,
+                                         lf_stream_t stream_) {
+    STREAM;
+    LF_REQUIRE(local && global && count && mean && invstd && dgamma && dbeta && c1 && c2 && C >= 1);
+    lf_launch(bn_bwd_finalize_tot_kernel<true>, (C + 127) / 128, 128, 0, stream, local, global, count, C, mean, invstd, dgamma,
+              dbeta, c1, c2);
     return check_launch();
 }
 

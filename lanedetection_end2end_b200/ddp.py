@@ -1,9 +1,13 @@
 """Data-parallel plumbing (new capability -- the reference is single-GPU, SURVEY.md 2.1/8e):
-one process per GPU, full model replica, per-replica BatchNorm statistics, and ONE
-all-reduce (sum, then 1/world) over a single flat fp32 gradient buffer per step
-(2 063 344 elements = 8.25 MB for the 2-lane model).  Parameters whose gradient is None
-(``net.encoder.output_conv``, unused in training -- BP/Networks/ERFNet.py:84,92-93)
-contribute zeros so every rank reduces the same layout.
+one process per GPU, full model replica, and ONE all-reduce (sum, then 1/world) over a
+single flat fp32 gradient buffer per step (2 063 344 elements = 8.25 MB for the 2-lane model).
+Parameters whose gradient is None (``net.encoder.output_conv``, unused in training --
+BP/Networks/ERFNet.py:84,92-93) contribute zeros so every rank reduces the same layout.
+
+BatchNorm statistics are per replica with ``nn.BatchNorm2d`` containers.  After
+``torch.nn.SyncBatchNorm.convert_sync_batchnorm(model, group)`` every BatchNorm normalises with
+the statistics of all ranks of its ``process_group`` (ops_net.BNSync): one small fp64 SUM
+all-reduce (``allreduce_totals``) per BatchNorm forward and one per BatchNorm backward.
 """
 import torch
 import torch.distributed as dist
@@ -72,6 +76,15 @@ def any_rank_nonzero(word, out, group=None):
     if dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(out, op=dist.ReduceOp.MAX, group=group)
     return out
+
+
+def allreduce_totals(totals, group=None):
+    """In-place SUM all-reduce of a SyncBatchNorm totals buffer (fp64 sums and count, lf_bn_collapse) over the group's
+    ranks, on the current stream: NCCL inside a captured step, any backend eagerly.  Without an initialised process group,
+    or with one rank, there is nothing to add and no collective is issued."""
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(totals, op=dist.ReduceOp.SUM, group=group)
+    return totals
 
 
 def broadcast_parameters(module, src=0, group=None):

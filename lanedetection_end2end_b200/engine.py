@@ -20,6 +20,13 @@ import torch
 FUSED_LOSS = os.environ.get("LANEFIT_FUSED_LOSS", "1") != "0"
 
 
+def batchnorm_running_stats(model):
+    """The running statistics of every BatchNorm container (nn.BatchNorm2d, nn.SyncBatchNorm, ...): a replay updates them
+    through raw pointers, so their versions are bumped after it."""
+    return [b for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
+            for b in (m.running_mean, m.running_var) if b is not None]
+
+
 class GraphedTrainStep:
     """``optimizer``: None (the graph ends with the gradients, the caller steps its optimizer), or an
     ``optim.FusedOptimizer`` over the model's parameters: the graph then starts by zeroing ``model.lsq_status`` (the
@@ -68,8 +75,7 @@ class GraphedTrainStep:
             optimizer.sync_hyperparameters()
             self.skip_word = torch.zeros(1, dtype=torch.int32, device=dev)   # status word reduced over the ranks
             # what a replay writes through raw pointers besides the parameters: the BatchNorm running statistics
-            self.written = self.updated + [b for m in model.modules() if isinstance(m, torch.nn.BatchNorm2d)
-                                           for b in (m.running_mean, m.running_var) if b is not None]
+            self.written = self.updated + batchnorm_running_stats(model)
         self.graph = torch.cuda.CUDAGraph()
         # with NCCL in the graph use capture_error_mode="thread_local": the process group's watchdog thread polls CUDA
         # events, which the default "global" mode treats as a capture violation

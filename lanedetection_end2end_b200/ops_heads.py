@@ -132,27 +132,28 @@ class ConvBnReluFunction(torch.autograd.Function):
     """relu(bn(conv(x) + b)) on NHWC fp32 (one stage of Classification.forward, reference :194-197)."""
 
     @staticmethod
-    def forward(ctx, x, w, b, gamma, beta, rm, rv, training, eps):
+    def forward(ctx, x, w, b, gamma, beta, rm, rv, training, eps, sync=None):
+        """sync: ops_net.BNSync (SyncBatchNorm container) or None."""
         _capi.require_cuda(x)
         u = conv_fwd(x, w, b)
-        s = o.bn_forward_stats(u, gamma, beta, rm, rv, training, eps)
+        s = o.bn_forward_stats(u, gamma, beta, rm, rv, training, eps, sync=sync)
         y = o.bn_apply(u, s, relu=True)
-        ctx.save_for_backward(x, w, u, y, gamma, s.mean, s.invstd)
-        ctx.training = training
+        ctx.save_for_backward(x, w, u, y, gamma, s.mean, s.invstd, s.count)
+        ctx.training, ctx.sync = training, sync
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, w, u, y, gamma, mean, invstd = ctx.saved_tensors
+        x, w, u, y, gamma, mean, invstd, count = ctx.saved_tensors
         o._require_training_for_backward(ctx.training)
         s = o.BNState()
-        s.mean, s.invstd = mean, invstd
-        du, dgamma, dbeta = o.bn_backward(dy.contiguous(), y, None, u, s, gamma)
+        s.mean, s.invstd, s.count = mean, invstd, count
+        du, dgamma, dbeta = o.bn_backward(dy.contiguous(), y, None, u, s, gamma, sync=ctx.sync)
         dw = conv_wgrad(x, du, w)
         # the conv feeds a training-mode BatchNorm: sum over pixels of du vanishes identically (DESIGN.md, deviations)
         db = torch.zeros(w.shape[0], dtype=torch.float32, device=x.device)
         dx = conv_dgrad(du, w) if ctx.needs_input_grad[0] else None
-        return dx, dw, db, dgamma, dbeta, None, None, None, None
+        return dx, dw, db, dgamma, dbeta, None, None, None, None, None
 
 
 class MaxPool2FlatFunction(torch.autograd.Function):
@@ -239,6 +240,6 @@ class LinearFunction(torch.autograd.Function):
 
 def conv_bn_relu(x, conv, bn, training, track):
     y = ConvBnReluFunction.apply(x, conv.weight, conv.bias, bn.weight, bn.bias, bn.running_mean, bn.running_var, training,
-                                 bn.eps)
+                                 bn.eps, o.bn_sync(bn, training))
     track(bn, training)
     return y

@@ -847,28 +847,67 @@ def run_colsum(src, C, coff, dst):
 
 
 class BNState:
-    """Per-call BatchNorm2d state: batch (mean, invstd) for backward, (scale, shift) for apply."""
-    __slots__ = ("mean", "invstd", "scale", "shift")
+    """Per-call BatchNorm2d state: batch (mean, invstd) for backward, (scale, shift) for apply; with a BNSync also
+    ``count``, the global pixel count (fp64 [1] on the device) the backward divides by."""
+    __slots__ = ("mean", "invstd", "scale", "shift", "count")
+
+
+class BNSync:
+    """Training-mode BatchNorm synchronised over the ranks of ``group`` (an ``nn.SyncBatchNorm``'s ``process_group``; None =
+    the default group): every rank's partial sums are collapsed into a totals buffer (lf_bn_collapse), SUM all-reduced
+    (ddp.allreduce_totals) and finalized from the totals (lf_bn_*finalize*_tot).  Without a process group or with one rank
+    the same launches run without the collective and give the bits of the plain path."""
+    __slots__ = ("group",)
+
+    def __init__(self, group=None):
+        self.group = group
+
+    def allreduce(self, totals):
+        from .ddp import allreduce_totals
+        allreduce_totals(totals, self.group)
+
+
+def bn_sync(bn, training):
+    """The synchronisation of a BatchNorm container: BNSync(bn.process_group) for an nn.SyncBatchNorm in training mode
+    (what torch.nn.SyncBatchNorm.convert_sync_batchnorm makes), else None (per-process statistics)."""
+    return BNSync(bn.process_group) if training and isinstance(bn, torch.nn.SyncBatchNorm) else None
 
 
 def _bn_state(C, device):
     s = BNState()
     buf = torch.empty(4, C, dtype=torch.float32, device=device)
     s.mean, s.invstd, s.scale, s.shift = buf[0], buf[1], buf[2], buf[3]
+    s.count = None
     return s
 
 
-def bn_finalize(part, nblk, npix, C, gamma, beta, running_mean, running_var, eps=BN_EPS):
-    """part: float64 [nblk][2][C] partial sums / sums of squares -> BNState (+ running-stat update)."""
+def _bn_collapse(part, nblk, npix, C, sync, keep_local=False):
+    """SyncBatchNorm: partials [nblk][2][C] -> all-reduced totals [2C+1] (sums, count); keep_local: also this rank's totals
+    (returned second, before the all-reduce).  The backward reduces only the 2C sums: its count is the forward's."""
+    tot = torch.empty(2 if keep_local else 1, 2 * C + 1, dtype=torch.float64, device=part.device)
+    _capi.call("lf_bn_collapse", ptr(part), nblk, C, 1, npix, ptr(tot[0]), ptr(tot[1]) if keep_local else None, _stream())
+    sync.allreduce(tot[0, :2 * C] if keep_local else tot[0])
+    return (tot[0], tot[1]) if keep_local else tot[0]
+
+
+def bn_finalize(part, nblk, npix, C, gamma, beta, running_mean, running_var, eps=BN_EPS, sync=None):
+    """part: float64 [nblk][2][C] partial sums / sums of squares -> BNState (+ running-stat update); sync: a BNSync for the
+    statistics of every rank, else this process's."""
     s = _bn_state(C, part.device)
+    if sync is not None:
+        tot = _bn_collapse(part, nblk, npix, C, sync)
+        _capi.call("lf_bn_finalize_tot", ptr(tot), C, ptr(gamma), ptr(beta), eps, BN_MOMENTUM, ptr(running_mean),
+                   ptr(running_var), ptr(s.mean), ptr(s.invstd), ptr(s.scale), ptr(s.shift), _stream())
+        s.count = tot[2 * C:]
+        return s
     _capi.call("lf_bn_finalize", ptr(part), nblk, npix, C, ptr(gamma), ptr(beta), eps, BN_MOMENTUM,
                ptr(running_mean), ptr(running_var), ptr(s.mean), ptr(s.invstd), ptr(s.scale), ptr(s.shift), _stream())
     return s
 
 
-def bn_forward_stats(x, gamma, beta, running_mean, running_var, training, eps=BN_EPS):
+def bn_forward_stats(x, gamma, beta, running_mean, running_var, training, eps=BN_EPS, sync=None):
     """x: dense NHWC.  Returns BNState; updates running stats in training mode
-    (nn.BatchNorm2d(eps=1e-3, momentum=0.1), ERFNet.py:17,33,39,102)."""
+    (nn.BatchNorm2d(eps=1e-3, momentum=0.1), ERFNet.py:17,33,39,102).  sync: BNSync (training mode only)."""
     h = _lib()
     C = x.shape[-1]
     npix = x.numel() // C
@@ -876,14 +915,14 @@ def bn_forward_stats(x, gamma, beta, running_mean, running_var, training, eps=BN
         nblk = h.lf_bn_blocks(npix, C)
         part = torch.empty(nblk * 2 * C, dtype=torch.float64, device=x.device)
         _capi.call("lf_bn_stats", ptr(x), npix, C, ptr(part), _stream(), nbytes=4 * npix * C)
-        return bn_finalize(part, nblk, npix, C, gamma, beta, running_mean, running_var, eps)
+        return bn_finalize(part, nblk, npix, C, gamma, beta, running_mean, running_var, eps, sync)
     s = _bn_state(C, x.device)
     _capi.call("lf_bn_eval_prepare", C, ptr(gamma), ptr(beta), eps, ptr(running_mean), ptr(running_var),
                ptr(s.scale), ptr(s.shift), _stream())
     return s
 
 
-def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running_var, training):
+def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running_var, training, sync=None):
     """conv (forward) followed by the BatchNorm statistics of its output -> (out, BNState).  On the tensor-core slab
     kernel the per-channel sums are accumulated in the conv epilogue, saving a full pass over `out`."""
     N, H, W, C = x.shape
@@ -893,9 +932,9 @@ def conv3_bn_stats(x, w, vertical, dil, bias, gamma, beta, running_mean, running
         taps = [(((k - 1) * dil, 0) if vertical else (0, (k - 1) * dil)) for k in range(3)]
         out = run_conv_tc(taps, x, packed(w, "tc_fwd", pack_tc_fwd, split=pack_split()),
                           torch.empty(x.shape, dtype=torch.float32, device=x.device), bias=bias, stats_partial=part)
-        return out, bn_finalize(part, rows, N * H * W, C, gamma, beta, running_mean, running_var)
+        return out, bn_finalize(part, rows, N * H * W, C, gamma, beta, running_mean, running_var, sync=sync)
     out = conv3(x, w, vertical, dil, False, bias=bias)
-    return out, bn_forward_stats(out, gamma, beta, running_mean, running_var, training)
+    return out, bn_forward_stats(out, gamma, beta, running_mean, running_var, training, sync=sync)
 
 
 def bn_apply(x, s, relu, drop=None, res=None, dtype=torch.float32):
@@ -913,9 +952,9 @@ def bn_apply(x, s, relu, drop=None, res=None, dtype=torch.float32):
 PREMASK_RESIDUAL = os.environ.get("LANEFIT_PREMASK_RES", "1") != "0"
 
 
-def bn_backward(dy, ymask, drop, x, s, gamma, want_gated=False):
+def bn_backward(dy, ymask, drop, x, s, gamma, want_gated=False, sync=None):
     """-> (dx, dgamma, dbeta[, gated]).  g = dy*(ymask>0)*drop is recomputed on the fly; want_gated: also return
-    dy*(ymask>0), stored by the apply pass (lf_bn_bwd_apply_gated)."""
+    dy*(ymask>0), stored by the apply pass (lf_bn_bwd_apply_gated).  sync: the forward's BNSync (s.count set)."""
     h = _lib()
     C = x.shape[-1]
     npix = x.numel() // C
@@ -927,7 +966,11 @@ def bn_backward(dy, ymask, drop, x, s, gamma, want_gated=False):
                                    ptr(part), st, nbytes=4 * npix * C * (2 + (ymask is not None)))
     buf = torch.empty(4, C, dtype=torch.float32, device=x.device)
     dgamma, dbeta, c1, c2 = buf[0], buf[1], buf[2], buf[3]
-    _capi.call("lf_bn_bwd_finalize", ptr(part), nblk, npix, C, ptr(dgamma), ptr(dbeta), ptr(c1), ptr(c2), st)
+    if sync is not None:
+        glob, loc = _bn_collapse(part, nblk, npix, C, sync, keep_local=True)
+        _capi.call("lf_bn_bwd_finalize_tot", ptr(loc), ptr(glob), ptr(s.count), C, ptr(dgamma), ptr(dbeta), ptr(c1), ptr(c2), st)
+    else:
+        _capi.call("lf_bn_bwd_finalize", ptr(part), nblk, npix, C, ptr(dgamma), ptr(dbeta), ptr(c1), ptr(c2), st)
     dx = torch.empty_like(x)
     if want_gated:
         gated = torch.empty_like(x)
@@ -947,10 +990,10 @@ def bn_backward(dy, ymask, drop, x, s, gamma, want_gated=False):
 FUSE_BN_BWD = os.environ.get("LANEFIT_FUSE_BN_BWD", "1") != "0"
 
 
-def dgrad_relu_bn_fused(d_out, w, vertical, dil, x, s, gamma):
+def dgrad_relu_bn_fused(d_out, w, vertical, dil, x, s, gamma, sync=None):
     """(dgrad of the 3-tap conv) * (relu(bn(x)) > 0) -> g, then BatchNorm backward -> (dx, dgamma, dbeta); s carries the
-    forward's (mean, invstd, scale, shift).  Returns None when the shapes are not served by the slab kernel (caller takes
-    the two-pass route)."""
+    forward's (mean, invstd, scale, shift[, count]).  Returns None when the shapes are not served by the slab kernel (caller
+    takes the two-pass route).  sync: the forward's BNSync."""
     N, H, W, C = d_out.shape
     rows = tc_rows(d_out, vertical, dil, stats=True) if FUSE_BN_BWD else 0
     if rows <= 0:
@@ -963,8 +1006,13 @@ def dgrad_relu_bn_fused(d_out, w, vertical, dil, x, s, gamma):
     buf = torch.empty(4, C, dtype=torch.float32, device=d_out.device)
     dgamma, dbeta, c1, c2 = buf[0], buf[1], buf[2], buf[3]
     st = _stream()
-    _capi.call("lf_bn_bwd_finalize_sx", ptr(part), rows, npix, C, 1, ptr(s.mean), ptr(s.invstd), ptr(dgamma), ptr(dbeta), ptr(c1),
-               ptr(c2), st)
+    if sync is not None:
+        glob, loc = _bn_collapse(part, rows, npix, C, sync, keep_local=True)
+        _capi.call("lf_bn_bwd_finalize_sx_tot", ptr(loc), ptr(glob), ptr(s.count), C, ptr(s.mean), ptr(s.invstd), ptr(dgamma),
+                   ptr(dbeta), ptr(c1), ptr(c2), st)
+    else:
+        _capi.call("lf_bn_bwd_finalize_sx", ptr(part), rows, npix, C, 1, ptr(s.mean), ptr(s.invstd), ptr(dgamma), ptr(dbeta),
+                   ptr(c1), ptr(c2), st)
     dx = torch.empty_like(x)
     _capi.call("lf_bn_bwd_apply", ptr(g), None, None, ptr(x), npix, C, H * W, ptr(s.mean), ptr(s.invstd), ptr(gamma), ptr(c1),
                ptr(c2), ptr(dx), st, nbytes=4 * npix * C * 3)
@@ -982,8 +1030,8 @@ def _require_training_for_backward(training):
 # --------------------------------------------------------------------------------------
 class DownFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, cin, w, b, gamma, beta, rm, rv, training, need_dx):
-        """x: [N,H,W,Cx] NHWC with Cx >= cin (stem: 3 channels padded to 4)."""
+    def forward(ctx, x, cin, w, b, gamma, beta, rm, rv, training, need_dx, sync=None):
+        """x: [N,H,W,Cx] NHWC with Cx >= cin (stem: 3 channels padded to 4).  sync: BNSync (SyncBatchNorm) or None."""
         _capi.require_cuda(x)
         h = _lib()
         N, H, W, cx = x.shape
@@ -998,16 +1046,16 @@ class DownFunction(torch.autograd.Function):
             wmat = packed(w, "conv_fwd_%d" % cin_gemm, lambda t: pack_conv_fwd(t, cin_gemm))
             run_conv(phases, x, wmat, cin_gemm, cat, cc, 0, bias=b)
         _capi.call("lf_maxpool2_fwd", ptr(x), N, H, W, cin, cx, ptr(cat), cout, cc, _stream())
-        s = bn_forward_stats(cat, gamma, beta, rm, rv, training)
+        s = bn_forward_stats(cat, gamma, beta, rm, rv, training, sync=sync)
         y = bn_apply(cat, s, relu=True)
-        ctx.save_for_backward(x, w, cat, y, gamma, s.mean, s.invstd)
-        ctx.cfg = (cin, training, need_dx)
+        ctx.save_for_backward(x, w, cat, y, gamma, s.mean, s.invstd, s.count)
+        ctx.cfg = (cin, training, need_dx, sync)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, w, cat, y, gamma, mean, invstd = ctx.saved_tensors
-        cin, training, need_dx = ctx.cfg
+        x, w, cat, y, gamma, mean, invstd, count = ctx.saved_tensors
+        cin, training, need_dx, sync = ctx.cfg
         _require_training_for_backward(training)
         h = _lib()
         dy = dy.contiguous()
@@ -1015,8 +1063,8 @@ class DownFunction(torch.autograd.Function):
         cc = w.shape[0]
         cout = cc + cin
         s = BNState()
-        s.mean, s.invstd = mean, invstd
-        dcat, dgamma, dbeta = bn_backward(dy, y, None, cat, s, gamma)
+        s.mean, s.invstd, s.count = mean, invstd, count
+        dcat, dgamma, dbeta = bn_backward(dy, y, None, cat, s, gamma, sync=sync)
         # weight / bias gradient of the conv part (channels [0,cc) of dcat)
         dw = torch.empty_like(w)
         db = _empty((cc,), x)
@@ -1041,7 +1089,7 @@ class DownFunction(torch.autograd.Function):
                 phases, _ = plans.transposed_gather_plan(dcat.shape[1], dcat.shape[2], H, W, 3, 1)
                 run_conv(phases, dcat, wd, cc, dx, cin, 0)
             _capi.call("lf_maxpool2_bwd", ptr(x), N, H, W, cin, cx, ptr(dcat), cout, cc, ptr(dx), cx, 1, _stream())
-        return dx, None, dw, db, dgamma, dbeta, None, None, None, None
+        return dx, None, dw, db, dgamma, dbeta, None, None, None, None, None
 
 
 # --------------------------------------------------------------------------------------
@@ -1066,25 +1114,27 @@ def nb1d_storage_dtype(x, dil):
 
 class Nb1dFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w1, b1, w2, b2, g1, be1, w3, b3, w4, b4, g2, be2, rm1, rv1, rm2, rv2, dil, drop, training):
+    def forward(ctx, x, w1, b1, w2, b2, g1, be1, w3, b3, w4, b4, g2, be2, rm1, rv1, rm2, rv2, dil, drop, training, sync1=None,
+                sync2=None):
+        """sync1 / sync2: BNSync of bn1 / bn2 (SyncBatchNorm containers) or None."""
         _capi.require_cuda(x)
         N, H, W, C = x.shape
         sd = nb1d_storage_dtype(x, dil)
         t1 = conv3(x, w1, True, 1, False, bias=b1, relu=True, dtype=sd)
-        t2, s1 = conv3_bn_stats(t1, w2, False, 1, b2, g1, be1, rm1, rv1, training)
+        t2, s1 = conv3_bn_stats(t1, w2, False, 1, b2, g1, be1, rm1, rv1, training, sync=sync1)
         t3 = bn_apply(t2, s1, relu=True, dtype=sd)
         t4 = conv3(t3, w3, True, dil, False, bias=b3, relu=True, dtype=sd)
-        t5, s2 = conv3_bn_stats(t4, w4, False, dil, b4, g2, be2, rm2, rv2, training)
+        t5, s2 = conv3_bn_stats(t4, w4, False, dil, b4, g2, be2, rm2, rv2, training, sync=sync2)
         y = bn_apply(t5, s2, relu=True, drop=drop, res=x)
         ctx.save_for_backward(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1.mean, s1.invstd, s2.mean, s2.invstd,
-                              drop if drop is not None else x.new_empty(0), s1.scale, s1.shift)
-        ctx.cfg = (dil, training, drop is not None)
+                              drop if drop is not None else x.new_empty(0), s1.scale, s1.shift, s1.count, s2.count)
+        ctx.cfg = (dil, training, drop is not None, sync1, sync2)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        (x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, m1, is1, m2, is2, drop, sc1, sh1) = ctx.saved_tensors
-        dil, training, has_drop = ctx.cfg
+        (x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, m1, is1, m2, is2, drop, sc1, sh1, n1, n2) = ctx.saved_tensors
+        dil, training, has_drop, sync1, sync2 = ctx.cfg
         _require_training_for_backward(training)
         drop = drop if has_drop else None
         dy = dy.contiguous()
@@ -1092,24 +1142,26 @@ class Nb1dFunction(torch.autograd.Function):
         s1, s2 = BNState(), BNState()
         s1.mean, s1.invstd, s2.mean, s2.invstd = m1, is1, m2, is2
         s1.scale, s1.shift = sc1, sh1
+        s1.count, s2.count = n1, n2
 
         global _DEFERRED
         _DEFERRED = jobs = []
         try:
-            return Nb1dFunction._backward_body(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1, s2, drop, dil, dy, jobs)
+            return Nb1dFunction._backward_body(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1, s2, drop, dil, dy, jobs,
+                                               sync1, sync2)
         finally:
             _DEFERRED = None
 
     @staticmethod
-    def _backward_body(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1, s2, drop, dil, dy, jobs):
+    def _backward_body(x, t1, t2, t3, t4, t5, y, w1, w2, w3, w4, g1, g2, s1, s2, drop, dil, dy, jobs, sync1=None, sync2=None):
         N, H, W, C = x.shape
         # y = relu(bn2(t5)*drop + x).  The apply pass also emits gm = dy*(y>0), the gradient of the skip connection, so the
         # block's last conv adds one pre-masked operand instead of reading dy and y again in its epilogue.
         gm = None
         if PREMASK_RESIDUAL and tc_mode():
-            d5, dg2, dbe2, gm = bn_backward(dy, y, drop, t5, s2, g2, want_gated=True)
+            d5, dg2, dbe2, gm = bn_backward(dy, y, drop, t5, s2, g2, want_gated=True, sync=sync2)
         else:
-            d5, dg2, dbe2 = bn_backward(dy, y, drop, t5, s2, g2)
+            d5, dg2, dbe2 = bn_backward(dy, y, drop, t5, s2, g2, sync=sync2)
         # Bias gradients.  conv1x3_1 / conv1x3_2 feed a BatchNorm: sum_pixels(BN backward output) == 0
         # identically (the reference's autograd returns pure round-off there), so db2 = db4 = 0.
         # conv3x1_1 / conv3x1_2 feed a ReLU: db = column sums of the masked input gradient, which the
@@ -1122,13 +1174,13 @@ class Nb1dFunction(torch.autograd.Function):
         d4 = conv3(d5, w4, False, dil, True, colsum=db3, mask_src=t4)
         # conv3x1_2 (dilated)
         dw3, _ = wgrad3(t3, d4, w3, True, dil, bias_grad="skip")
-        fused = dgrad_relu_bn_fused(d4, w3, True, dil, t2, s1, g1)
+        fused = dgrad_relu_bn_fused(d4, w3, True, dil, t2, s1, g1, sync=sync1)
         if fused is not None:
             d2, dg1, dbe1 = fused          # dgrad + relu mask + BatchNorm reductions in one launch, then apply
         else:
             d3 = conv3(d4, w3, True, dil, True, mask_src=t3)
             # bn1 (+relu already applied through mask_src=t3)
-            d2, dg1, dbe1 = bn_backward(d3, None, None, t2, s1, g1)
+            d2, dg1, dbe1 = bn_backward(d3, None, None, t2, s1, g1, sync=sync1)
         # conv1x3_1
         dw2, _ = wgrad3(t1, d2, w2, False, 1, bias_grad="skip")
         d1 = conv3(d2, w2, False, 1, True, colsum=db1, mask_src=t1)
@@ -1138,7 +1190,7 @@ class Nb1dFunction(torch.autograd.Function):
         if jobs:
             flush_deferred_reductions(jobs)
         return (dx, dw1, db1, dw2, db2, dg1, dbe1, dw3, db3, dw4, db4, dg2, dbe2, None, None, None, None, None, None,
-                None)
+                None, None, None)
 
 
 # --------------------------------------------------------------------------------------
@@ -1146,7 +1198,8 @@ class Nb1dFunction(torch.autograd.Function):
 # --------------------------------------------------------------------------------------
 class UpFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w, b, gamma, beta, rm, rv, training):
+    def forward(ctx, x, w, b, gamma, beta, rm, rv, training, sync=None):
+        """sync: BNSync (SyncBatchNorm) or None."""
         _capi.require_cuda(x)
         N, H, W, ci = x.shape
         co = w.shape[1]
@@ -1157,22 +1210,22 @@ class UpFunction(torch.autograd.Function):
             u = run_tcg_s2convT(x, ci, wgs, co, _empty((N, Ho, Wo, co), x), bias2=packed(b, "tile2", lambda t: t.repeat(2)))
         else:
             u = run_conv(phases, x, packed(w, "convT_fwd", pack_convT_fwd), ci, _empty((N, Ho, Wo, co), x), co, bias=b)
-        s = bn_forward_stats(u, gamma, beta, rm, rv, training)
+        s = bn_forward_stats(u, gamma, beta, rm, rv, training, sync=sync)
         y = bn_apply(u, s, relu=True)
-        ctx.save_for_backward(x, w, u, y, gamma, s.mean, s.invstd)
-        ctx.training = training
+        ctx.save_for_backward(x, w, u, y, gamma, s.mean, s.invstd, s.count)
+        ctx.training, ctx.sync = training, sync
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, w, u, y, gamma, mean, invstd = ctx.saved_tensors
+        x, w, u, y, gamma, mean, invstd, count = ctx.saved_tensors
         _require_training_for_backward(ctx.training)
         dy = dy.contiguous()
         N, H, W, ci = x.shape
         co = w.shape[1]
         s = BNState()
-        s.mean, s.invstd = mean, invstd
-        du, dgamma, dbeta = bn_backward(dy, y, None, u, s, gamma)
+        s.mean, s.invstd, s.count = mean, invstd, count
+        du, dgamma, dbeta = bn_backward(dy, y, None, u, s, gamma, sync=ctx.sync)
         dw, db = torch.empty_like(w), _empty((co,), x)
         if wgrad_tcg_ok(du, co, x, ci):
             dw = wgrad_tcg_convT(x, ci, du, co)
@@ -1184,7 +1237,7 @@ class UpFunction(torch.autograd.Function):
         else:
             pd, _ = plans.convT_dgrad_plan(2 * H, 2 * W, H, W, 3, 1)
             dx = run_conv(pd, du, packed(w, "convT_dgrad", pack_convT_dgrad), co, torch.empty_like(x), ci)
-        return dx, dw, db, dgamma, dbeta, None, None, None
+        return dx, dw, db, dgamma, dbeta, None, None, None, None
 
 
 # --------------------------------------------------------------------------------------
