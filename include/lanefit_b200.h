@@ -525,6 +525,47 @@ typedef struct LfOptimState {
 int lf_optim_step(int algo, const LfOptimSeg* segs, int nsegs, long long nchunks, const LfOptimHyper* hyper,
                   LfOptimState* state, const int* status, lf_stream_t stream);
 
+/* Baseline JPEG decode (csrc/jpeg.cu; replaces Image.open(f).convert('RGB') of BP/Dataloader/Load_Data_new.py:118-119):
+ * a batch of same-size baseline (SOF0 / 8-bit SOF1, Huffman) single-scan JPEGs, YCbCr 4:4:4 / 4:2:2 / 4:2:0 or grayscale,
+ * with or without restart markers -> uint8 RGB [N][H][W][3], bit-identical to Pillow (libjpeg-turbo: ISLOW IDCT, fancy
+ * upsampling, fixed-point YCbCr->RGB).  The markers are parsed on the host (lanedetection_end2end_b200/jpeg.py), which
+ * fills one LfJpegImage per image; the entropy-coded bytes are unstuffed and decoded on the device.
+ * The device blob is LfJpegImage[N] followed by the compressed bytes (ecs_off counts from the blob start).
+ * lf_jpeg_workspace_bytes (HOST): checks the descriptors, fills their layout fields (in place) and returns the scratch
+ *   bytes `workspace` needs (0 = invalid descriptors); *coef_bytes receives the size of the coefficient buffer, which the
+ *   caller zeroes once before first use and which every launch leaves zeroed.
+ * lf_jpeg_decode: three launches (entropy decode, dequantise + IDCT, upsample + colour); corrupt entropy data ORs
+ *   LF_STATUS_JPEG_CORRUPT into *status.  Calls sharing `coef` / `workspace` must be ordered by the caller. */
+#define LF_STATUS_JPEG_CORRUPT 8
+#define LF_JPEG_PIECE_BYTES 128   /* size of one piece of the unstuffed bitstream a thread decodes */
+#define LF_JPEG_MAX_BPM 6         /* blocks per MCU (4:2:0) */
+typedef struct LfJpegHuff {
+    unsigned short look[512];     /* 9-bit lookahead: (code length << 8) | symbol, 0 = longer code */
+    int maxcode[18];              /* largest code of each length 1..16, -1 if none; [17] sentinel */
+    int valoff[18];               /* symbol index - code, per length */
+    unsigned char val[256];
+} LfJpegHuff;
+typedef struct LfJpegImage {
+    long long ecs_off;            /* entropy-coded segment: blob offset and length in bytes */
+    int ecs_len;
+    int W, H, ncomp;              /* ncomp 1 (grayscale) or 3 (YCbCr) */
+    int mcux, mcuy, bpm;          /* MCUs per row / column, blocks per MCU */
+    int restart, nint;            /* restart interval in MCUs (0 = none), number of intervals */
+    int hs[3], vs[3];             /* sampling factors; comp_w / comp_h: component size in samples */
+    int comp_w[3], comp_h[3];
+    int qtab[3];                  /* quantisation table of each component */
+    int blk_comp[LF_JPEG_MAX_BPM], blk_dx[LF_JPEG_MAX_BPM], blk_dy[LF_JPEG_MAX_BPM];
+    int blk_dc[LF_JPEG_MAX_BPM], blk_ac[LF_JPEG_MAX_BPM]; /* Huffman tables of each block of the MCU (0..3 each) */
+    /* layout, filled by lf_jpeg_workspace_bytes: byte offsets into workspace, block offset into coef */
+    long long stream_off, x_off, b_off, us_off, pb_off, plane_off[3], block_off;
+    int plane_stride[3], npieces_max;
+    unsigned short qt[4][64];     /* quantisation tables, natural order */
+    LfJpegHuff dc[4], ac[4];
+} LfJpegImage;
+size_t lf_jpeg_workspace_bytes(LfJpegImage* images, int N, size_t* coef_bytes);
+int lf_jpeg_decode(const void* blob, int N, int W, int H, unsigned char* out, int* status, void* coef, size_t coef_bytes,
+                   void* workspace, size_t workspace_bytes, lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

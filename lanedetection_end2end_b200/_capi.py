@@ -120,7 +120,28 @@ class LfOptimState(ctypes.Structure):
     _fields_ = [("step", _ll), ("skipped", _ll), ("ticket", ctypes.c_ulonglong)]
 
 
+STATUS_JPEG_CORRUPT = 8
+JPEG_PIECE_BYTES = 128
+JPEG_MAX_BPM = 6
+
+
+class LfJpegHuff(ctypes.Structure):
+    _fields_ = [("look", ctypes.c_ushort * 512), ("maxcode", _i * 18), ("valoff", _i * 18), ("val", ctypes.c_ubyte * 256)]
+
+
+class LfJpegImage(ctypes.Structure):
+    _fields_ = [("ecs_off", _ll), ("ecs_len", _i), ("W", _i), ("H", _i), ("ncomp", _i), ("mcux", _i), ("mcuy", _i), ("bpm", _i),
+                ("restart", _i), ("nint", _i), ("hs", _i * 3), ("vs", _i * 3), ("comp_w", _i * 3), ("comp_h", _i * 3),
+                ("qtab", _i * 3), ("blk_comp", _i * JPEG_MAX_BPM), ("blk_dx", _i * JPEG_MAX_BPM), ("blk_dy", _i * JPEG_MAX_BPM),
+                ("blk_dc", _i * JPEG_MAX_BPM), ("blk_ac", _i * JPEG_MAX_BPM),
+                ("stream_off", _ll), ("x_off", _ll), ("b_off", _ll), ("us_off", _ll), ("pb_off", _ll), ("plane_off", _ll * 3),
+                ("block_off", _ll), ("plane_stride", _i * 3), ("npieces_max", _i), ("qt", (ctypes.c_ushort * 64) * 4),
+                ("dc", LfJpegHuff * 4), ("ac", LfJpegHuff * 4)]
+
+
 _NET_PROTOS = {
+    "lf_jpeg_workspace_bytes": (_c_size_t, [_p, _i, _p]),
+    "lf_jpeg_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p, _c_size_t, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg_ctas_x3": (_i, [_i, _i, _i, _i, _i, _i]),
