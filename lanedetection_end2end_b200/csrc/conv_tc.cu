@@ -28,8 +28,11 @@
 //  * B: the weights of this CTA's 64 output channels, K-major 128B-swizzled [64 x 32] tiles (hi and lo tiles for 3xTF32).
 //    Resident in shared memory for the whole persistent CTA when they leave room for two slab stages, else streamed
 //    next to the slab of their 32-channel chunk.
-//  * MMA: wgmma m64n64k8 TF32.  Two consumer warpgroups own 64 pixel rows each; they load their A fragments from the
-//    swizzled slab (split into hi / lo in registers for 3xTF32) and take B from shared memory through a descriptor.
+//  * MMA: wgmma m64n64k8 TF32.  Two consumer warpgroups own 64 pixel rows each and take A and B from shared memory
+//    through descriptors.  Once a stage has landed, the 256 consumer threads make one elementwise pass over its slab:
+//    each word becomes its TF32 rounding in place and, for 3xTF32, the rounded remainder goes to the same offset of a
+//    lo buffer outside the ring (two when shared memory allows, else one; else one laid over the staging tile), so
+//    every tap view is a descriptor into the slab, 1024-byte aligned like the B tiles.  (BF16 keeps register A.)
 //    Accumulators stay in registers: each tap's products are summed by the tensor core from zero and added to the
 //    running fp32 sum with a rounded FADD (the tensor core's own accumulation does not round like IEEE adds); 3xTF32
 //    keeps the sum of the two small correction terms apart and adds it in the epilogue (small terms first).
@@ -78,6 +81,9 @@ struct TcArgs {
     int relu;                 // bit 0: ReLU on conv + bias (before mask / add); bit 1: ReLU after the residual add
     int n_halves, total_m_tiles;
     int stages, stage_bytes, a_bytes;   // a stage = a_bytes of activations [+ the three weight tiles of its chunk]
+    // 3xTF32: n_lo (1 or 2) lo slab buffers in the lo_bytes after the ring, or (lo_stg = 1) one that ends where the
+    // staging tile ends: it overlaps the staging tile and whatever it needs beyond it is the lo_bytes before it
+    int n_lo, lo_stg, lo_bytes;
     int out_bf16, mask_bf16;  // BF16 kernels only: `out` / `mask_src` hold bf16
 };
 
@@ -98,7 +104,8 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sB = smem;
     uint8_t* sA = smem + B_RES_BYTES;
-    float* stg = reinterpret_cast<float*>(sA + (size_t)a.stages * a.stage_bytes);
+    uint8_t* sLo = sA + (size_t)a.stages * a.stage_bytes;
+    float* stg = reinterpret_cast<float*>(sLo + a.lo_bytes);
     uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + 2 * TC_STG_BYTES);
     uint64_t* empty = full + TC_MAX_STAGES;
     uint64_t* bfull = empty + TC_MAX_STAGES;
@@ -172,42 +179,37 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const bool pre_add = (a.add_src != nullptr) && !pre_mask;  // both given: add_src is read in the loop
     const bool affine_mask = a.mask_scale != nullptr;
     const bool out_bf = P == TC_BF16 && a.out_bf16, mask_bf = P == TC_BF16 && a.mask_bf16;
-    float4 csum = make_float4(0.f, 0.f, 0.f, 0.f), csq = csum, msc = csum, msh = csum, bsv = csum;
-    if (a.bias) bsv = __ldg(reinterpret_cast<const float4*>(a.bias + ch0));
-    if (affine_mask) {
-        msc = __ldg(reinterpret_cast<const float4*>(a.mask_scale + ch0));
-        msh = __ldg(reinterpret_cast<const float4*>(a.mask_shift + ch0));
-    }
+    float4 csum = make_float4(0.f, 0.f, 0.f, 0.f), csq = csum;
     const int ra = 64 * wg + 16 * wl + g;   // this thread's fragment rows ra, ra + 8
     if (RES) mbar_wait(bfull, 0);
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, chunk = 0;
     for (int mt = cta_m; mt < a.total_m_tiles; mt += m_stride) {
         const int ta = mt % a.tiles_a;
         const int tb = (mt / a.tiles_a) % a.tiles_b;
         const int n = mt / (a.tiles_a * a.tiles_b);
-        size_t roff[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        // element offset of phase-2 row r0 + 16 j: formed again in the epilogue, not held through the main loop
+        auto roff = [&](int j) {
             const int r = r0 + 16 * j;
             const int ap = r >> a.tb_shift, bp = r & (a.TB - 1);
             const int pa = ta * a.TA + ap, pb = tb * a.TB + bp;
             const int y = a.vertical ? pa : pb, x = a.vertical ? pb : pa;
-            roff[j] = ((size_t)(n * a.H + y) * a.W + x) * a.Ctot + ch0;
-        }
+            return ((size_t)(n * a.H + y) * a.W + x) * a.Ctot + ch0;
+        };
         float4 pre[8];
         if (pre_mask || pre_add) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
+                const size_t off = roff(j);
                 if (pre_mask && mask_bf) {   // the raw bf16 bits, widened in the epilogue: converting here would wait for the load
-                    const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(a.mask_src) + roff[j]));
+                    const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(a.mask_src) + off));
                     pre[j] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), 0.f, 0.f);
                 } else if (pre_mask) {
-                    pre[j] = __ldg(reinterpret_cast<const float4*>(a.mask_src + roff[j]));
+                    pre[j] = __ldg(reinterpret_cast<const float4*>(a.mask_src + off));
                 } else {
-                    float4 ad = __ldg(reinterpret_cast<const float4*>(a.add_src + roff[j]));
+                    float4 ad = __ldg(reinterpret_cast<const float4*>(a.add_src + off));
                     if (a.add_mask) {
-                        const float4 mk = __ldg(reinterpret_cast<const float4*>(a.add_mask + roff[j]));
+                        const float4 mk = __ldg(reinterpret_cast<const float4*>(a.add_mask + off));
                         ad.x = mk.x > 0.f ? ad.x : 0.f; ad.y = mk.y > 0.f ? ad.y : 0.f;
                         ad.z = mk.z > 0.f ? ad.z : 0.f; ad.w = mk.w > 0.f ? ad.w : 0.f;
                     }
@@ -221,8 +223,31 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < 32; ++i) acc[i] = acs[i] = part[i] = 0.f;
         for (int cb = 0; cb < NCB; ++cb) {
             mbar_wait(&full[stage], phase);
-            const uint8_t* st = sA + (size_t)stage * a.stage_bytes;
+            uint8_t* st = sA + (size_t)stage * a.stage_bytes;
             const uint32_t wbase = RES ? smem_u32(sB + cb * W_ATOM) : smem_u32(st + a.a_bytes);
+            uint8_t* lo = nullptr;   // 3xTF32: this chunk's lo buffer
+            if (X3)
+                lo = a.lo_stg ? reinterpret_cast<uint8_t*>(stg) + 2 * TC_STG_BYTES - a.a_bytes
+                              : sLo + (size_t)(chunk & (a.n_lo - 1)) * a.a_bytes;
+            if constexpr (P != TC_BF16) {
+                // The slab as the tensor core reads it, one elementwise pass over the swizzled bytes: each word v -> hi =
+                // tf32_rna(v) in place and (3xTF32) lo = tf32_rna(v - hi) at the same offset of the lo buffer.  A single
+                // lo buffer may still be read by the other warpgroup's MMAs of the previous chunk; with two, the barrier
+                // below of the previous chunk already waited for the MMAs that read this one.
+                if (X3 && a.n_lo != 2) named_bar_sync(1, 256);
+                const uint32_t s_st = smem_u32(st), s_lo = X3 ? smem_u32(lo) : 0;
+                for (uint32_t o = 16 * threadIdx.x; o < (uint32_t)a.a_bytes; o += 16 * 256) {
+                    const float4 v = lds_f32x4(s_st + o);
+                    const uint4 h = make_uint4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
+                    sts_u32x4(s_st + o, h);
+                    if (X3)
+                        sts_u32x4(s_lo + o, make_uint4(tf32_rna(v.x - __uint_as_float(h.x)), tf32_rna(v.y - __uint_as_float(h.y)),
+                                                       tf32_rna(v.z - __uint_as_float(h.z)), tf32_rna(v.w - __uint_as_float(h.w))));
+                }
+                fence_proxy_async_smem();   // the generic stores above, before the wgmma (async proxy) reads
+                named_bar_sync(1, 256);     // the two warpgroups' tap views overlap in the halo rows
+            }
+            ++chunk;
             constexpr int W_TAP = RES ? NCB * W_ATOM : W_ATOM;   // distance between the weight tiles of two taps
 #pragma unroll
             for (int t = 0; t < 3; ++t) {
@@ -261,31 +286,20 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
                     for (int i = 0; i < 32; ++i) acc[i] += part[i];
                 } else {
-                    uint32_t ah[4][4], al[4][4];
-#pragma unroll
-                    for (int k8 = 0; k8 < 4; ++k8) {
-                        const int c = 8 * k8 + t4;
-                        const float v[4] = {*reinterpret_cast<const float*>(view + sw128_off(ra, c)),
-                                            *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c)),
-                                            *reinterpret_cast<const float*>(view + sw128_off(ra, c + 4)),
-                                            *reinterpret_cast<const float*>(view + sw128_off(ra + 8, c + 4))};
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            if (X3) {
-                                tf32_split(v[q], ah[k8][q], al[k8][q]);
-                            } else {
-                                ah[k8][q] = tf32_rna(v[q]);
-                            }
-                        }
-                    }
-                    const uint64_t bd = wgmma_desc_sw128(wbase + t * W_TAP);
+                    // this warpgroup's 64 rows of the view (hi) and of the same rows of the lo buffer; k8 = 32 bytes along K
+                    // (descriptors formed at each MMA from 32-bit addresses: fewer live registers than 64-bit descriptors)
+                    const uint32_t va = smem_u32(view) + 64 * wg * 128;
+                    const uint32_t vl = X3 ? va - smem_u32(st) + smem_u32(lo) : 0;
+                    const uint32_t vb = wbase + t * W_TAP;
                     wgmma_fence();
 #pragma unroll
                     for (int k8 = 0; k8 < 4; ++k8) {
-                        wgmma_m64n64k8_tf32(part, ah[k8], bd + 2 * k8, k8);   // k8 = 0: part = product (previous tap dropped)
+                        const uint32_t k = 32 * k8;
+                        // k8 = 0: part = product (previous tap dropped)
+                        wgmma_m64n64k8_tf32_ss(part, wgmma_desc_sw128(va + k), wgmma_desc_sw128(vb + k), k8);
                         if (X3) {
-                            wgmma_m64n64k8_tf32(acs, ah[k8], bd + (TC_ATOM >> 4) + 2 * k8, 1);   // a_hi * w_lo
-                            wgmma_m64n64k8_tf32(acs, al[k8], bd + 2 * k8, 1);                    // a_lo * w_hi
+                            wgmma_m64n64k8_tf32_ss(acs, wgmma_desc_sw128(va + k), wgmma_desc_sw128(vb + TC_ATOM + k), 1);   // a_hi * w_lo
+                            wgmma_m64n64k8_tf32_ss(acs, wgmma_desc_sw128(vl + k), wgmma_desc_sw128(vb + k), 1);             // a_lo * w_hi
                         }
                     }
                     wgmma_commit();
@@ -307,7 +321,15 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
 
+        // phase-2 channel vectors: loaded per tile (cache hits), not held through the main loop
+        float4 bsv = make_float4(0.f, 0.f, 0.f, 0.f), msc = bsv, msh = bsv;
+        if (a.bias) bsv = __ldg(reinterpret_cast<const float4*>(a.bias + ch0));
+        if (affine_mask) {
+            msc = __ldg(reinterpret_cast<const float4*>(a.mask_scale + ch0));
+            msh = __ldg(reinterpret_cast<const float4*>(a.mask_shift + ch0));
+        }
         // ---- phase 1: accumulator fragments -> staging tile (both halves)
+        if (X3 && a.lo_stg) named_bar_sync(1, 256);   // the other warpgroup's last MMAs may still read the lo buffer there
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
             const int row = ra + 8 * ((i >> 1) & 1);
@@ -320,7 +342,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int r = r0 + 16 * j;
-            const size_t off = roff[j];
+            const size_t off = roff(j);
             if (mask_bf) pre[j] = bf16x4_to_f4(make_uint2(__float_as_uint(pre[j].x), __float_as_uint(pre[j].y)));
             float4 o = *reinterpret_cast<const float4*>(&stg_h[r * TC_STG_LD + 4 * c4]);
             o.x += bsv.x; o.y += bsv.y; o.z += bsv.z; o.w += bsv.w;
@@ -403,7 +425,9 @@ static int tc_m_ctas(int N, int C, int tiles_per_image) {
     return (int)(m_ctas < 1 ? 1 : m_ctas);
 }
 
-// Shared memory: resident weights when they leave room for two stages, else streamed per stage.
+// Shared memory: resident weights when they leave room for two stages, else streamed per stage.  3xTF32 also needs lo
+// buffers of one slab each, outside the ring: two when two stages still fit next to them, else one, else one laid over
+// the staging tile (idle during the main loop; slabs larger than it reach back into the space before it).
 static bool tc_fit(int C, int prec, bool abf, TcPlan* p) {
     const int w_atom = tc_w_atom(prec);
     const int b_res = 3 * (C / TC_KCH) * w_atom;
@@ -412,11 +436,21 @@ static bool tc_fit(int C, int prec, bool abf, TcPlan* p) {
     p->res = TC_FIXED_SMEM + b_res + 2 * g.a_bytes <= TC_SMEM_LIMIT;
     g.stage_bytes = g.a_bytes + (p->res ? 0 : 3 * w_atom);
     const int avail = TC_SMEM_LIMIT - TC_FIXED_SMEM - (p->res ? b_res : 0);
-    int stages = avail / g.stage_bytes;
+    g.n_lo = g.lo_stg = g.lo_bytes = 0;
+    if (prec == TC_X3) {
+        g.n_lo = 2;
+        while (g.n_lo > 0 && avail - g.n_lo * g.a_bytes < 2 * g.stage_bytes) --g.n_lo;
+        g.lo_bytes = g.n_lo * g.a_bytes;
+        if (g.n_lo == 0) {
+            g.n_lo = g.lo_stg = 1;
+            g.lo_bytes = g.a_bytes > 2 * TC_STG_BYTES ? g.a_bytes - 2 * TC_STG_BYTES : 0;
+        }
+    }
+    int stages = (avail - g.lo_bytes) / g.stage_bytes;
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages < 1) return false;
     g.stages = stages;
-    p->smem_bytes = TC_FIXED_SMEM + (p->res ? b_res : 0) + stages * g.stage_bytes;
+    p->smem_bytes = TC_FIXED_SMEM + (p->res ? b_res : 0) + stages * g.stage_bytes + g.lo_bytes;
     return true;
 }
 

@@ -88,7 +88,7 @@ __device__ __forceinline__ uint32_t sw128_off(int r, int c) { return (uint32_t)(
 // groups 1024 bytes apart) = exactly what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B.  Descriptor: start >> 4 (bits 0-13),
 // LBO >> 4 (16-29; unused for swizzled K-major), SBO >> 4 (32-45), layout 1 = SWIZZLE_128B (bits 62-63).  The tile base
 // must be 1024-byte aligned; the k-th group of 8 TF32 along K starts 32*k bytes later (+2 in the start field).
-// A operand: registers, the m64k8 TF32 fragment of this thread:
+// A operand: registers (or shared memory, wgmma_m64n64k8_tf32_ss), the m64k8 TF32 fragment of this thread:
 //   a[0] = A[16w + g][t], a[1] = A[16w + g + 8][t], a[2] = A[16w + g][t + 4], a[3] = A[16w + g + 8][t + 4]
 // (w = warp within the warpgroup, g = lane / 4, t = lane % 4).  Accumulator fragment of m64nN, register i:
 //   row 16w + g + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2t + (i & 1).
@@ -119,6 +119,21 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], const uint32
           "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
           "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// The same with A from shared memory: adesc describes a K-major, 128B-swizzled [64 x 32] fp32 tile exactly like B (rows =
+// the 64 M rows; wgmma_desc_sw128 of a 1024-byte aligned base, +2 per k8).  The words must already be TF32 values.
+__device__ __forceinline__ void wgmma_m64n64k8_tf32_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 // D[64 x 48] (+)= A[64 x 8] * B[48 x 8]^T
 __device__ __forceinline__ void wgmma_m64n48k8_tf32(float (&d)[24], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
@@ -262,6 +277,9 @@ __device__ __forceinline__ float4 lds_f32x4(uint32_t addr) {
 }
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
     asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts_u32x4(uint32_t addr, uint4 v) {
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 // orders this thread's generic-proxy shared-memory stores before later async-proxy (wgmma, TMA) accesses
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
