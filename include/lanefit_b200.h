@@ -175,6 +175,14 @@ typedef struct LfConvTcArgs {
                                 a bf16 `out` is the fp32 result rounded to nearest even (colsum / stats are of the fp32
                                 values); a bf16 `mask_src` gates like its fp32 copy.  Same shapes and slab cases as fp32. */
 } LfConvTcArgs;
+/* Arguments of lf_conv1d_tc_fp8: the LfConvTcArgs of the launch (unchanged layout) followed by the fp8 scales. */
+typedef struct LfConvTcFp8Args {
+    LfConvTcArgs conv;
+    const float* x_amax;     /* [N] per-image max |in| over the stored input values (the activation scale) */
+    const float* w_scale;    /* [C] per-output-channel dequantisation factors of the e4m3 `wpack` (a_w / 448) */
+    float* out_amax;         /* [N] per-image max |out| of the stored values, reduced with atomicMax on the float bits:
+                                the caller zeroes it; it is the `x_amax` of the next convolution */
+} LfConvTcFp8Args;
 /* 0 = unsupported shape, else the number of CTA rows of colsum_partial */
 int lf_conv1d_tc_supported(int N, int H, int W, int C);
 /* 3xTF32 variant (csrc/conv_tc.cu): same arguments and epilogue, but `wpack` is the pre-split operand
@@ -191,6 +199,17 @@ int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream);
  * accumulate.  It serves exactly the shapes of lf_conv1d_tc and runs on the slab kernel exactly where lf_conv1d_tc does,
  * so lf_conv1d_tc_supported and lf_conv1d_tc_slab_ok answer for it. */
 int lf_conv1d_tc_bf16(const LfConvTcArgs* args, lf_stream_t stream);
+/* FP8 variant (inference only): conv.wpack is a [C][3*C] e4m3 operand quantised per output channel (w_scale), the
+ * activations (fp32, or bf16 with in_dtype = LF_BF16) are quantised per image in the kernel: q = e4m3(v * (448 /
+ * x_amax[n])), round to nearest even with saturation (0 when x_amax[n] = 0).  Each tap's products of one 32-channel
+ * chunk are summed from zero by the tensor core and added to the fp32 sum; then
+ *   out = epi( acc * ((x_amax[n] / 448) * w_scale[co]) + bias )     (each operation rounded to nearest in fp32)
+ * and out_amax[n] receives the per-image max |stored out|.  x_amax, w_scale and out_amax are required; colsum_partial,
+ * stats_partial and mask_scale are not taken.  Same shapes and slab cases as lf_conv1d_tc. */
+int lf_conv1d_tc_fp8(const LfConvTcFp8Args* args, lf_stream_t stream);
+/* amax[n] = max(amax[n], max |x[n, ...]|) over the `per_image` elements of each of the N images of x (fp32, or bf16
+ * with dtype = LF_BF16), by atomicMax on the float bits: zero amax first for the plain per-image max. */
+int lf_amax_per_image(const void* x, int dtype, long long per_image, int N, float* amax, lf_stream_t stream);
 /* 2 (default) = halo-slab kernel (one TMA slab per 32-channel chunk shared by the three taps);
  * 1 = first version (one TMA box per tap).  Same results; process-wide switch for A/B measurements. */
 void lf_conv1d_tc_set_variant(int variant);

@@ -85,6 +85,8 @@ class DownsamplerBlock(nn.Module):
             x = _ops.image_to_nhwc_pad(input, (self.ninput + 3) // 4 * 4)
         else:
             x = _ops.as_nhwc(input)
+        if _ops.fp8_mode():
+            _ops.require_inference_mode(self.training, x, self.conv.weight)
         if not self.training and x.is_cuda and EVAL_FUSED and _eval.inference_only(x, self.conv.weight):
             y = _eval.down(x, self)
             if y is not None:
@@ -126,6 +128,8 @@ class non_bottleneck_1d(nn.Module):
 
     def forward(self, input):
         x = _ops.as_nhwc(input)
+        if _ops.fp8_mode():             # fp8: the folded eval path below or an error (Nb1dFunction refuses the mode)
+            _ops.require_inference_mode(self.training, x, self.conv3x1_1.weight)
         if not self.training and x.is_cuda and EVAL_FUSED and _eval.inference_only(x, self.conv3x1_1.weight):
             y = _eval.nb1d(x, self)                  # BatchNorm folded into the weights: 4 conv launches, nothing else
             if y is not None:
@@ -198,6 +202,8 @@ class UpsamplerBlock(nn.Module):
 
     def forward(self, input):
         x = _ops.as_nhwc(input)
+        if _ops.fp8_mode():
+            _ops.require_inference_mode(self.training, x, self.conv.weight)
         if not self.training and x.is_cuda and EVAL_FUSED and _eval.inference_only(x, self.conv.weight):
             y = _eval.up(x, self)
             if y is not None:
@@ -254,6 +260,8 @@ class Net(nn.Module):
 
     def forward(self, input, flag, only_encode=False):
         global _PENDING_COUNTERS
+        if _ops.fp8_mode():             # inference-only mode: refuse a training or autograd forward before any launch
+            _ops.require_inference_mode(self.training, input, *self.parameters())
         if only_encode:
             return self.encoder.forward(input, predict=True)
         _PENDING_COUNTERS = []

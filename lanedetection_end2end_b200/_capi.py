@@ -62,6 +62,10 @@ class LfConvTcArgs(ctypes.Structure):
                 ("dx", _i * 3), ("relu", _i), ("in_dtype", _i), ("out_dtype", _i), ("mask_dtype", _i)]
 
 
+class LfConvTcFp8Args(ctypes.Structure):
+    _fields_ = [("conv", LfConvTcArgs), ("x_amax", _p), ("w_scale", _p), ("out_amax", _p)]
+
+
 class LfWgradArgs(ctypes.Structure):
     _fields_ = [("P", _p), ("Q", _p), ("partial", _p), ("qsum_partial", _p),
                 ("N", _i), ("Hs", _i), ("Ws", _i),
@@ -157,6 +161,8 @@ _NET_PROTOS = {
     "lf_conv1d_tc_supported": (_i, [_i, _i, _i, _i]),
     "lf_conv1d_tc_x3": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
     "lf_conv1d_tc_bf16": (_i, [ctypes.POINTER(LfConvTcArgs), _p]),
+    "lf_conv1d_tc_fp8": (_i, [ctypes.POINTER(LfConvTcFp8Args), _p]),
+    "lf_amax_per_image": (_i, [_p, _i, ctypes.c_longlong, _i, _p, _p]),
     "lf_conv1d_tc_x3_rows": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_conv1d_tc_set_variant": (None, [_i]),
     "lf_conv1d_tc_slab_ok": (_i, [_i, _i, _i, _i, _i, _i]),

@@ -14,6 +14,14 @@
 //    operand bits as rounding the fp32 copy, so the same results.  The BF16 epilogue can also store `out` as bf16
 //    (nearest even, = torch's .to(torch.bfloat16); column sums / statistics are of the fp32 values) and read a bf16
 //    `mask_src`: the ReLU outputs a non_bottleneck_1d block keeps only as convolution inputs and ReLU masks.
+//  * FP8 (lf_conv1d_tc_fp8, inference only): e4m3 operands with fp32 scales.  The weights arrive quantised per output
+//    channel ([Cout][3C] e4m3, 32-byte rows, 32B-swizzled [64 x 32] tiles of a quarter of the TF32 size) with their
+//    dequantisation factors w_scale[co]; the activations are quantised per image while their k32 fragments are formed:
+//    q = e4m3(v * inv[n]), inv[n] = 448 / x_amax[n] (4 adjacent channels per register: one 16-byte load from the fp32
+//    slab or 8 bytes from the bf16 slab, two cvt.rn.satfinite.e4m3x2).  One k32 MMA per tap and 32-channel chunk.  The
+//    epilogue computes, in this fp32 order, y = acc * (s_x[n] * w_scale[co]) + bias with s_x[n] = x_amax[n] / 448,
+//    then the usual ReLU / residual steps, and reduces the per-image max |stored value| into out_amax[n] (a warp max,
+//    one shared-memory atomicMax per warp, one global atomicMax per CTA and tile).  Every tile lies within one image.
 //
 //   out[n,y,x,co] = epi( sum_{t<3} sum_{ci} in[n, (y,x) + o_t, ci] * Wp[co][t*C + ci] )
 //
@@ -56,8 +64,13 @@ constexpr int TC_STG_BYTES = 128 * TC_STG_LD * 4; // 18 KB per half
 constexpr int TC_ATOM = TC_BN * 128;              // one [64 out x 32 in] weight tile, 8 KB
 constexpr int TC_SMEM_LIMIT = 227 * 1024;
 constexpr int TC_FIXED_SMEM = 1024 + 2 * TC_STG_BYTES + 256;   // alignment slack + staging + barriers
-// bytes of one [64 out x 32 in] weight tile in precision P: TF32, TF32 hi + lo, or bf16 (64-byte rows, 64B-swizzled)
-constexpr int tc_w_atom(int P) { return P == TC_X3 ? 2 * TC_ATOM : P == TC_BF16 ? TC_ATOM / 2 : TC_ATOM; }
+// bytes of one [64 out x 32 in] weight tile in precision P: TF32, TF32 hi + lo, bf16 (64-byte rows, 64B-swizzled) or
+// e4m3 (32-byte rows, 32B-swizzled)
+constexpr int tc_w_atom(int P) {
+    return P == TC_X3 ? 2 * TC_ATOM : P == TC_BF16 ? TC_ATOM / 2 : P == TC_FP8 ? TC_ATOM / 4 : TC_ATOM;
+}
+// the precisions whose kernels read bf16 activations / write bf16 outputs
+constexpr bool tc_takes_bf16(int P) { return P == TC_BF16 || P == TC_FP8; }
 
 static int g_tc_variant = 2;  // 2 = halo slab, 1 = one box per tap
 
@@ -84,7 +97,10 @@ struct TcArgs {
     // 3xTF32: n_lo (1 or 2) lo slab buffers in the lo_bytes after the ring, or (lo_stg = 1) one that ends where the
     // staging tile ends: it overlaps the staging tile and whatever it needs beyond it is the lo_bytes before it
     int n_lo, lo_stg, lo_bytes;
-    int out_bf16, mask_bf16;  // BF16 kernels only: `out` / `mask_src` hold bf16
+    int out_bf16, mask_bf16;  // BF16 and FP8 kernels only: `out` / `mask_src` hold bf16
+    const float* x_amax;      // FP8 only: [N] per-image max |in|, [Ctot] per-channel weight scales, [N] per-image max
+    const float* w_scale;     //   |out| (atomicMax on the float bits: zeroed by the caller)
+    float* out_amax;
 };
 
 // bytes of one activation slab row (32 channels): fp32, or bf16 (ABF)
@@ -94,8 +110,9 @@ template <int C, int P, bool RES, bool ABF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     pdl_trigger();
-    static_assert(!ABF || P == TC_BF16, "bf16 activations need the BF16 kernel");
+    static_assert(!ABF || tc_takes_bf16(P), "bf16 activations need the BF16 or FP8 kernel");
     constexpr bool X3 = P == TC_X3;
+    constexpr bool FP8 = P == TC_FP8;
     constexpr int A_ROW = tc_a_row(ABF);
     constexpr int NCB = C / TC_KCH;
     constexpr int W_ATOM = tc_w_atom(P);   // 3xTF32: hi tile, then lo tile; bf16: half-size tile
@@ -109,6 +126,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + 2 * TC_STG_BYTES);
     uint64_t* empty = full + TC_MAX_STAGES;
     uint64_t* bfull = empty + TC_MAX_STAGES;
+    uint32_t* amax_slot = reinterpret_cast<uint32_t*>(bfull + 1);   // FP8: this CTA's per-tile max |out|, two tiles deep
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_half = blockIdx.x % a.n_halves;
@@ -123,6 +141,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             mbar_init(&empty[s], 8);   // one arrive per consumer warp
         }
         mbar_init(bfull, 1);
+        amax_slot[0] = amax_slot[1] = 0u;
         fence_barrier_init();
     }
     __syncthreads();
@@ -178,16 +197,26 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const bool pre_mask = a.mask_src != nullptr;
     const bool pre_add = (a.add_src != nullptr) && !pre_mask;  // both given: add_src is read in the loop
     const bool affine_mask = a.mask_scale != nullptr;
-    const bool out_bf = P == TC_BF16 && a.out_bf16, mask_bf = P == TC_BF16 && a.mask_bf16;
+    const bool out_bf = tc_takes_bf16(P) && a.out_bf16, mask_bf = tc_takes_bf16(P) && a.mask_bf16;
     float4 csum = make_float4(0.f, 0.f, 0.f, 0.f), csq = csum;
     const int ra = 64 * wg + 16 * wl + g;   // this thread's fragment rows ra, ra + 8
     if (RES) mbar_wait(bfull, 0);
     int stage = 0;
-    uint32_t phase = 0, chunk = 0;
+    uint32_t phase = 0, chunk = 0, tile_par = 0;
+    const int tiles_img = a.tiles_a * a.tiles_b;
+    // FP8: max |in| of the next tile's image, loaded one tile ahead (its latency would stall the first fragment)
+    float ax_next = FP8 && cta_m < a.total_m_tiles ? __ldg(a.x_amax + cta_m / tiles_img) : 0.f;
     for (int mt = cta_m; mt < a.total_m_tiles; mt += m_stride) {
         const int ta = mt % a.tiles_a;
         const int tb = (mt / a.tiles_a) % a.tiles_b;
-        const int n = mt / (a.tiles_a * a.tiles_b);
+        const int n = mt / tiles_img;   // the tile's image (a tile never crosses one: host plan)
+        // FP8: the image's activation quantisation factor, 448 / max |in| (0 for an all-zero image: every q = 0)
+        float inv = 0.f, ax = 0.f;
+        if (FP8) {
+            ax = ax_next;
+            inv = ax > 0.f ? __fdiv_rn(448.f, ax) : 0.f;
+            if (mt + m_stride < a.total_m_tiles) ax_next = __ldg(a.x_amax + (mt + m_stride) / tiles_img);
+        }
         // element offset of phase-2 row r0 + 16 j: formed again in the epilogue, not held through the main loop
         auto roff = [&](int j) {
             const int r = r0 + 16 * j;
@@ -229,7 +258,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             if (X3)
                 lo = a.lo_stg ? reinterpret_cast<uint8_t*>(stg) + 2 * TC_STG_BYTES - a.a_bytes
                               : sLo + (size_t)(chunk & (a.n_lo - 1)) * a.a_bytes;
-            if constexpr (P != TC_BF16) {
+            if constexpr (P == TC_TF32 || P == TC_X3) {
                 // The slab as the tensor core reads it, one elementwise pass over the swizzled bytes: each word v -> hi =
                 // tf32_rna(v) in place and (3xTF32) lo = tf32_rna(v - hi) at the same offset of the lo buffer.  A single
                 // lo buffer may still be read by the other warpgroup's MMAs of the previous chunk; with two, the barrier
@@ -253,7 +282,26 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int t = 0; t < 3; ++t) {
                 // 8 rows of the swizzle period apart (1024 / 512 bytes): the swizzle phase is the view's row
                 const uint8_t* view = st + a.tap_row[t] * A_ROW;
-                if constexpr (P == TC_BF16) {
+                if constexpr (FP8) {
+                    // k32 fragment: four adjacent channels per register = one 16-byte load (fp32 slab) or one 8-byte
+                    // load (bf16 slab); q = e4m3(v * inv), the product rounded to nearest in fp32 first
+                    uint32_t aq[4];
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        const int row = ra + 8 * (r & 1), c = 4 * t4 + 16 * (r >> 1);
+                        float4 v;
+                        if constexpr (ABF) v = bf16x4_to_f4(*reinterpret_cast<const uint2*>(view + sw64_off(row, c)));
+                        else v = *reinterpret_cast<const float4*>(view + sw128_off(row, c));
+                        aq[r] = pack_e4m3x4(__fmul_rn(v.x, inv), __fmul_rn(v.y, inv), __fmul_rn(v.z, inv), __fmul_rn(v.w, inv));
+                    }
+                    wgmma_fence();
+                    wgmma_m64n64k32_e4m3(part, aq, wgmma_desc_sw32(wbase + t * W_TAP), 0);
+                    wgmma_commit();
+                    wgmma_wait0();
+                    reg_fence(part);
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) acc[i] += part[i];
+                } else if constexpr (P == TC_BF16) {
                     // k16 fragments: two adjacent channels per register = one 8-byte load inside a 16-byte chunk (fp32
                     // slab), or one 4-byte load of the ready pair (bf16 slab)
                     uint32_t ab[2][4];
@@ -324,6 +372,13 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         // phase-2 channel vectors: loaded per tile (cache hits), not held through the main loop
         float4 bsv = make_float4(0.f, 0.f, 0.f, 0.f), msc = bsv, msh = bsv;
         if (a.bias) bsv = __ldg(reinterpret_cast<const float4*>(a.bias + ch0));
+        float4 dqs = make_float4(0.f, 0.f, 0.f, 0.f);   // FP8: dequantisation factors s_x[n] * w_scale[co]
+        if (FP8) {
+            const float sx = __fdiv_rn(ax, 448.f);
+            const float4 ws = __ldg(reinterpret_cast<const float4*>(a.w_scale + ch0));
+            dqs = make_float4(__fmul_rn(sx, ws.x), __fmul_rn(sx, ws.y), __fmul_rn(sx, ws.z), __fmul_rn(sx, ws.w));
+        }
+        float amax = 0.f;                                 // FP8: max |stored value| of this thread's part of the tile
         if (affine_mask) {
             msc = __ldg(reinterpret_cast<const float4*>(a.mask_scale + ch0));
             msh = __ldg(reinterpret_cast<const float4*>(a.mask_shift + ch0));
@@ -345,6 +400,9 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const size_t off = roff(j);
             if (mask_bf) pre[j] = bf16x4_to_f4(make_uint2(__float_as_uint(pre[j].x), __float_as_uint(pre[j].y)));
             float4 o = *reinterpret_cast<const float4*>(&stg_h[r * TC_STG_LD + 4 * c4]);
+            if (FP8) {   // acc * (s_x * s_w), rounded, then + bias (never contracted into an FMA)
+                o.x = __fmul_rn(o.x, dqs.x); o.y = __fmul_rn(o.y, dqs.y); o.z = __fmul_rn(o.z, dqs.z); o.w = __fmul_rn(o.w, dqs.w);
+            }
             o.x += bsv.x; o.y += bsv.y; o.z += bsv.z; o.w += bsv.w;
             if (a.relu & 1) {
                 o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
@@ -374,6 +432,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             if (out_bf) *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.out) + off) = f4_to_bf16x4(o);
             else *reinterpret_cast<float4*>(a.out + off) = o;
+            if (FP8) amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
             csum.x += o.x; csum.y += o.y; csum.z += o.z; csum.w += o.w;
             if (affine_mask) {   // pre[j] is the BatchNorm input x
                 csq.x = fmaf(o.x, pre[j].x, csq.x); csq.y = fmaf(o.y, pre[j].y, csq.y);
@@ -383,7 +442,21 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 csq.z = fmaf(o.z, o.z, csq.z); csq.w = fmaf(o.w, o.w, csq.w);
             }
         }
-        named_bar_sync(1, 256);   // staging tile may be overwritten
+        if (FP8) {
+            // a bf16 `out` stores the rounded values: rounding to nearest is monotonic, so their max is the rounded max
+            if (out_bf) amax = __uint_as_float(f4_to_bf16x4(make_float4(amax, 0.f, 0.f, 0.f)).x << 16);
+            const uint32_t wmax = __reduce_max_sync(0xffffffffu, __float_as_uint(amax));   // |v| >= 0: ordered as uint
+            if (lane == 0) atomicMax(&amax_slot[tile_par], wmax);
+        }
+        named_bar_sync(1, 256);   // staging tile may be overwritten (FP8: and the tile's max is complete)
+        if (FP8) {
+            if (threadIdx.x == 0) {   // the tile's image: one global atomic per CTA and tile; the slot is free again
+                const uint32_t m = amax_slot[tile_par];
+                if (m) atomicMax(reinterpret_cast<unsigned int*>(a.out_amax) + n, m);
+                amax_slot[tile_par] = 0u;
+            }
+            tile_par ^= 1u;
+        }
     }
     if (a.colsum_partial || a.stats_partial) {
         // 16 threads share each float4 column of the half: combine them through the (now free) staging half
@@ -533,7 +606,7 @@ static cudaError_t tc_launch_p(bool res, int C, int grid, int smem_bytes, cudaSt
     return res ? tc_launch<64, P, true, ABF>(grid, smem_bytes, stream, tmA, tmB, a) : tc_launch<64, P, false, ABF>(grid, smem_bytes, stream, tmA, tmB, a);
 }
 
-static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
+static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec, const LfConvTcFp8Args* f8 = nullptr) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!args) return LF_ERR_INVALID_ARGUMENT;
     const LfConvTcArgs& p = *args;
@@ -541,17 +614,26 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     LF_REQUIRE(!p.mask_scale || (p.mask_shift && p.mask_src && p.stats_partial));
     LF_REQUIRE((p.in_dtype == LF_F32 || p.in_dtype == LF_BF16) && (p.out_dtype == LF_F32 || p.out_dtype == LF_BF16) &&
                (p.mask_dtype == LF_F32 || p.mask_dtype == LF_BF16));
-    if (prec != TC_BF16 && (p.in_dtype | p.out_dtype | p.mask_dtype) != LF_F32) return LF_ERR_UNSUPPORTED;
+    if (!tc_takes_bf16(prec) && (p.in_dtype | p.out_dtype | p.mask_dtype) != LF_F32) return LF_ERR_UNSUPPORTED;
+    const bool fp8 = prec == TC_FP8;
+    // FP8 is an inference epilogue: scales in, per-image max out, no gradient-side outputs
+    if (fp8) LF_REQUIRE(f8 && f8->x_amax && f8->w_scale && f8->out_amax && !p.colsum_partial && !p.stats_partial && !p.mask_scale);
     const bool x3 = prec == TC_X3;
     const bool abf = p.in_dtype == LF_BF16;
     TcPlan pl{};
-    // bf16 takes the slab exactly where TF32 does (its smaller weight tiles and bf16 slabs fit wherever the TF32 ones
-    // do), so that lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for both
+    // bf16 and fp8 take the slab exactly where TF32 does (their smaller weight tiles and bf16 slabs fit wherever the
+    // TF32 ones do), so that lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for all three
     const bool slab = (x3 || g_tc_variant != 1) &&
-                      (prec != TC_BF16 || tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, TC_TF32, &pl)) &&
+                      (!tc_takes_bf16(prec) || tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, TC_TF32, &pl)) &&
                       tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf);
     if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf))) return LF_ERR_UNSUPPORTED;
     TcArgs a = pl.geo;
+    // FP8 scales and maxima are per image: every tile must lie within one image (tiles cover each image exactly)
+    if (fp8 && (a.tiles_a * a.TA != (a.vertical ? p.H : p.W) || a.tiles_b * a.TB != (a.vertical ? p.W : p.H)))
+        return LF_ERR_UNSUPPORTED;
+    a.x_amax = fp8 ? f8->x_amax : nullptr;
+    a.w_scale = fp8 ? f8->w_scale : nullptr;
+    a.out_amax = fp8 ? f8->out_amax : nullptr;
     a.out = p.out; a.bias = p.bias; a.mask_src = p.mask_src; a.add_src = p.add_src; a.add_mask = p.add_mask;
     a.colsum_partial = p.colsum_partial;
     a.stats_partial = p.stats_partial;
@@ -583,17 +665,18 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     }
     {
         // packed weights [Cout][3*C] (K contiguous); 3xTF32: [2][Cout][3*C] (hi, lo) as one [2*Cout][3*C] matrix;
-        // bf16: [Cout][3*C] bf16, [64 x 32] boxes of 64-byte rows, 64B-swizzled
+        // bf16: [Cout][3*C] bf16, [64 x 32] boxes of 64-byte rows, 64B-swizzled; fp8: [Cout][3*C] e4m3 bytes, boxes of
+        // 32-byte rows, 32B-swizzled
         const bool bf = prec == TC_BF16;
-        const int esz = bf ? 2 : 4;
+        const int esz = fp8 ? 1 : bf ? 2 : 4;
         cuuint64_t dims[2] = {(cuuint64_t)(3 * p.C), (cuuint64_t)((x3 ? 2 : 1) * p.C)};
         cuuint64_t strides[1] = {(cuuint64_t)(3 * p.C) * esz};
         cuuint32_t box[2] = {32, TC_BN};
         cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmB, bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+        CUresult r = enc(&tmB, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                          const_cast<float*>(p.wpack), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         bf ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         fp8 ? CU_TENSOR_MAP_SWIZZLE_32B : bf ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return LF_ERR_CUDA;
     }
     const int grid = pl.m_ctas * a.n_halves;
@@ -602,6 +685,8 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec) {
     if (prec == TC_X3) e = tc_launch_p<TC_X3>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     else if (prec == TC_BF16 && abf) e = tc_launch_p<TC_BF16, true>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     else if (prec == TC_BF16) e = tc_launch_p<TC_BF16>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
+    else if (fp8 && abf) e = tc_launch_p<TC_FP8, true>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
+    else if (fp8) e = tc_launch_p<TC_FP8>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     else e = tc_launch_p<TC_TF32>(pl.res, p.C, grid, s, stream, tmA, tmB, a);
     if (e != cudaSuccess) { set_last_cuda_error(e); return LF_ERR_CUDA; }
     return check_launch();
@@ -640,3 +725,6 @@ extern "C" int lf_conv1d_tc_x3_rows(int N, int H, int W, int C, int vertical, in
 extern "C" int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_TF32); }
 extern "C" int lf_conv1d_tc_x3(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_X3); }
 extern "C" int lf_conv1d_tc_bf16(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_BF16); }
+extern "C" int lf_conv1d_tc_fp8(const LfConvTcFp8Args* args, lf_stream_t stream) {
+    return args ? tc_run(&args->conv, stream, TC_FP8, args) : LF_ERR_INVALID_ARGUMENT;
+}

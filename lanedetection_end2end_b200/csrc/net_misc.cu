@@ -554,6 +554,32 @@ __global__ void batched_transpose_kernel(const float* __restrict__ in, int R, in
     }
 }
 
+// Per-image max |x| (the activation scale of an fp8 convolution whose input is not another fp8 convolution's output):
+// grid (blocks per image, N); 16-byte loads, a warp max, one atomicMax on the float bits per warp.
+template <bool BF>
+__global__ void __launch_bounds__(256) amax_per_image_kernel(const void* __restrict__ x, long long per_image, float* amax) {
+    pdl_entry();
+    const int n = blockIdx.y;
+    const long long nvec = per_image / 8;   // 8 elements per step: two float4 or one uint4 of bf16
+    float m = 0.f;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+        float4 u, v;
+        if (BF) {
+            const uint4 r = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(x) + (size_t)n * per_image) + i);
+            u = bf16x4_to_f4(make_uint2(r.x, r.y));
+            v = bf16x4_to_f4(make_uint2(r.z, r.w));
+        } else {
+            const float4* p = reinterpret_cast<const float4*>(static_cast<const float*>(x) + (size_t)n * per_image) + 2 * i;
+            u = __ldg(p);
+            v = __ldg(p + 1);
+        }
+        m = fmaxf(m, fmaxf(fmaxf(fmaxf(fabsf(u.x), fabsf(u.y)), fmaxf(fabsf(u.z), fabsf(u.w))),
+                           fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)))));
+    }
+    const uint32_t w = __reduce_max_sync(0xffffffffu, __float_as_uint(m));   // |x| >= 0: ordered as uint
+    if ((threadIdx.x & 31) == 0 && w) atomicMax(reinterpret_cast<unsigned int*>(amax) + n, w);
+}
+
 static inline int grid_for(long long n, int threads, int maxblocks = 0) {
     if (maxblocks <= 0) maxblocks = device_sms() * 16;
     long long b = (n + threads - 1) / threads;
@@ -856,5 +882,18 @@ extern "C" int lf_nchw_to_nhwc(const float* in, int N, int C, int H, int W, floa
     const int R = C, S = H * W;  // [C][HW] -> [HW][C]
     dim3 grid((S + 31) / 32, (R + 31) / 32, N), block(32, 8);
     lf_launch(batched_transpose_kernel, grid, block, 0, stream, in, R, S, out);
+    return check_launch();
+}
+
+extern "C" int lf_amax_per_image(const void* x, int dtype, long long per_image, int N, float* amax, lf_stream_t stream_) {
+    STREAM;
+    LF_REQUIRE(x && amax && N > 0 && N <= 65535 && per_image > 0 && per_image % 8 == 0);
+    LF_REQUIRE(dtype == LF_F32 || dtype == LF_BF16);
+    int bx = (device_sms() * 4 + N - 1) / N;   // about four CTAs per SM over the whole batch
+    const long long need = (per_image / 8 + 255) / 256;
+    if (bx > need) bx = (int)need;
+    dim3 grid(bx < 1 ? 1 : bx, N);
+    if (dtype == LF_BF16) lf_launch(amax_per_image_kernel<true>, grid, 256, 0, stream, x, per_image, amax);
+    else lf_launch(amax_per_image_kernel<false>, grid, 256, 0, stream, x, per_image, amax);
     return check_launch();
 }

@@ -180,7 +180,7 @@ __device__ __forceinline__ void wgmma_m64k8_tf32(float (&d)[N / 2], const uint32
 // BF16 operands (the "bf16" convolution mode): both operands rounded to bf16 (round to nearest even), products exact in
 // fp32, fp32 accumulate.  Operand precision of the tensor-core kernel templates (= the `precision` fields of the C ABI):
 // ------------------------------------------------------------------------------------------
-enum TcPrec : int { TC_TF32 = 0, TC_X3 = 1, TC_BF16 = 2 };
+enum TcPrec : int { TC_TF32 = 0, TC_X3 = 1, TC_BF16 = 2, TC_FP8 = 3 };
 
 // bf16x2 of (lo, hi), round to nearest even: `lo` in bits 0-15 (the lower K index of a fragment register)
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -257,6 +257,47 @@ __device__ __forceinline__ void wgmma_m64k16_bf16(float (&d)[N / 2], const uint3
     else if constexpr (N == 32) wgmma_m64n32k16_bf16(d, a, bdesc, accumulate);
     else if constexpr (N == 48) wgmma_m64n48k16_bf16(d, a, bdesc, accumulate);
     else wgmma_m64n64k16_bf16(d, a, bdesc, accumulate);
+}
+
+// ------------------------------------------------------------------------------------------
+// FP8 e4m3 operands (the inference-only "fp8" convolution mode): products of two e4m3 values are exact in fp32.
+// ------------------------------------------------------------------------------------------
+// e4m3x4 of (c0, c1, c2, c3), each rounded to nearest even with saturation to +-448 (cvt.rn.satfinite): c0 in bits 0-7
+// (the lowest K index of a fragment register).  cvt ... e4m3x2 d, a, b puts a in the upper byte of d, b in the lower.
+__device__ __forceinline__ uint32_t pack_e4m3x4(float c0, float c1, float c2, float c3) {
+    uint32_t r;
+    asm("{\n\t.reg .b16 lo, hi;\n\t"
+        "cvt.rn.satfinite.e4m3x2.f32 lo, %2, %1;\n\t"
+        "cvt.rn.satfinite.e4m3x2.f32 hi, %4, %3;\n\t"
+        "mov.b32 %0, {lo, hi};\n\t}"
+        : "=r"(r)
+        : "f"(c0), "f"(c1), "f"(c2), "f"(c3));
+    return r;
+}
+// B operand: K-major, 32B-swizzled e4m3 tile in shared memory (rows of 32 bytes = one k32 step, 8-row groups 256
+// bytes apart) = what TMA writes for a [rows x 32] uint8 box with CU_TENSOR_MAP_SWIZZLE_32B.  Descriptor: layout 3 =
+// SWIZZLE_32B, SBO = 256; the tile base must be 256-byte aligned.  A k32 MMA reads the whole row: no K advance.
+__device__ __forceinline__ uint64_t wgmma_desc_sw32(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(256 >> 4) << 32) | (3ull << 62);
+}
+// A operand: registers, the m64k32 8-bit fragment of this thread (PTX ISA, "Register fragment for matrix A" of
+// wgmma .m64nNk32), four e4m3 per register, the lowest K index in the lowest byte:
+//   a[0] = A[16w + g][4t .. 4t+3],      a[1] = A[16w + g + 8][4t .. 4t+3],
+//   a[2] = A[16w + g][4t+16 .. 4t+19],  a[3] = A[16w + g + 8][4t+16 .. 4t+19]
+// (w, g, t as for TF32).  The accumulator fragment is the one of the TF32 instructions.
+// D[64 x 64] (+)= A[64 x 32] * B[64 x 32]^T, e4m3 in, fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n64k32_e4m3(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 
 // Shared-state-space accesses (addresses from smem_u32): LDS / STS without generic-address translation.

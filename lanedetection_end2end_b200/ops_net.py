@@ -33,8 +33,12 @@ LfConvArgs, LfWgradArgs, LfConvTcArgs = _capi.LfConvArgs, _capi.LfWgradArgs, _ca
 #           accumulate (a labelled fast mode, ~5e-3 from fp64 on the curve coefficients); the non_bottleneck_1d
 #           tensors that only feed convolutions and ReLU masks are stored as bf16 (same results, see
 #           nb1d_storage_dtype), everything else stays fp32;
+#   "fp8": INFERENCE ONLY (an eval-mode forward without autograd, ops_eval.py): the four 3-tap convolutions of every
+#           non_bottleneck_1d run on FP8 e4m3 operands (weights scaled per output channel, activations per image,
+#           lf_conv1d_tc_fp8); every other layer runs exactly as in bf16 mode (bf16_mode() is true in fp8 mode).  A
+#           training forward or one that builds an autograd graph raises (require_inference_mode);
 #   shapes a tensor-core kernel does not take stay on the fp32 kernel in every mode.
-CONV_MODES = ("fp32", "tf32", "tf32x3", "bf16")
+CONV_MODES = ("fp32", "tf32", "tf32x3", "bf16", "fp8")
 CONV_MODE = os.environ.get("LANEFIT_CONV_MODE", "tf32x3")
 
 
@@ -46,8 +50,8 @@ def set_conv_mode(mode):
 
 
 def tc_mode():
-    """True when the dense convolutions run on tensor cores (TF32, 3xTF32 or BF16)."""
-    return CONV_MODE in ("tf32", "tf32x3", "bf16")
+    """True when the dense convolutions run on tensor cores (TF32, 3xTF32, BF16 or FP8)."""
+    return CONV_MODE in ("tf32", "tf32x3", "bf16", "fp8")
 
 
 def x3_mode():
@@ -55,7 +59,21 @@ def x3_mode():
 
 
 def bf16_mode():
-    return CONV_MODE == "bf16"
+    """True when the layers run with bf16 operands: the bf16 mode, and every layer of the fp8 mode except the
+    non_bottleneck_1d 3-tap convolutions of ops_eval."""
+    return CONV_MODE in ("bf16", "fp8")
+
+
+def fp8_mode():
+    return CONV_MODE == "fp8"
+
+
+def require_inference_mode(training, *tensors):
+    """The fp8 mode serves eval-mode forwards without autograd only: raise for a training forward or one that would
+    build an autograd graph (any of `tensors` requiring grad with grad mode on), instead of running another mode."""
+    if fp8_mode() and (training or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors))):
+        raise RuntimeError("conv mode 'fp8' is inference-only: run the model in eval mode under torch.no_grad() "
+                           "(or torch.inference_mode()), or set another conv mode for training")
 
 
 def pack_split():
@@ -614,9 +632,11 @@ def _taps_axis(taps):
 
 
 def run_conv_tc(taps, x, wpack, out, bias=None, relu=False, mask_src=None, add_src=None, add_mask=None, colsum=None,
-                mask_affine=None, stats_partial=None):
+                mask_affine=None, stats_partial=None, fp8=None):
     """3-tap convolution on tensor cores.  taps: [(dy, dx)] * 3 in weight-slot order.  colsum: optional [C]
-    tensor receiving the column sums of `out` (bias gradient), accumulated in the kernel's epilogue."""
+    tensor receiving the column sums of `out` (bias gradient), accumulated in the kernel's epilogue.
+    fp8: (x_amax [N], w_scale [C], out_amax [N]) with an e4m3 `wpack` (uint8 storage): lf_conv1d_tc_fp8, the fp8 mode's
+    only 3-tap route; out_amax receives max |out| per image and must be zeroed by the caller."""
     N, H, W, C = x.shape
     a = LfConvTcArgs()
     a.inp, a.wpack, a.out = x.data_ptr(), wpack.data_ptr(), out.data_ptr()
@@ -640,8 +660,16 @@ def run_conv_tc(taps, x, wpack, out, bias=None, relu=False, mask_src=None, add_s
     a.in_dtype, a.out_dtype = _capi.dtype_id(x), _capi.dtype_id(out)
     a.mask_dtype = _capi.dtype_id(mask_src) if mask_src is not None else _capi.LF_F32
     width = sum(t.element_size() for t in (x, out, mask_src, add_src, add_mask) if t is not None)
-    entry = "lf_conv1d_tc_x3" if x3_mode() else "lf_conv1d_tc_bf16" if bf16_mode() else "lf_conv1d_tc"
-    _capi.call(entry, ctypes.byref(a), _stream(), flops=2 * N * H * W * 3 * C * C, nbytes=width * N * H * W * C)
+    if fp8 is not None:
+        f = _capi.LfConvTcFp8Args()
+        f.conv = a
+        f.x_amax, f.w_scale, f.out_amax = (t.data_ptr() for t in fp8)
+        entry, arg = "lf_conv1d_tc_fp8", f
+    elif fp8_mode():
+        raise _capi.LanefitError("run_conv_tc: the fp8 mode runs 3-tap convolutions only with fp8 operands (ops_eval)")
+    else:
+        entry, arg = "lf_conv1d_tc_x3" if x3_mode() else "lf_conv1d_tc_bf16" if bf16_mode() else "lf_conv1d_tc", a
+    _capi.call(entry, ctypes.byref(arg), _stream(), flops=2 * N * H * W * 3 * C * C, nbytes=width * N * H * W * C)
     if part is not None:
         if _DEFERRED is not None:
             _reduce(part, rows, 1, 1, C, 1, C, colsum, 0, 0, 1)
@@ -1033,6 +1061,7 @@ class DownFunction(torch.autograd.Function):
     def forward(ctx, x, cin, w, b, gamma, beta, rm, rv, training, need_dx, sync=None):
         """x: [N,H,W,Cx] NHWC with Cx >= cin (stem: 3 channels padded to 4).  sync: BNSync (SyncBatchNorm) or None."""
         _capi.require_cuda(x)
+        require_inference_mode(training)
         h = _lib()
         N, H, W, cx = x.shape
         cc = w.shape[0]                      # conv output channels = noutput - ninput
@@ -1097,7 +1126,8 @@ class DownFunction(torch.autograd.Function):
 # --------------------------------------------------------------------------------------
 def nb1d_storage_dtype(x, dil):
     """Element type of the non_bottleneck_1d tensors that are only convolution inputs and ReLU masks: t1, t3, t4 of
-    Nb1dFunction and the three intermediates of ops_eval.nb1d.  bf16 in bf16 mode when every launch of the block,
+    Nb1dFunction and the three intermediates of ops_eval.nb1d (also in fp8 mode, whose kernels take either and
+    quantise them per image).  bf16 in bf16 mode when every launch of the block,
     forward and backward, runs on the bf16 tensor-core kernels: they round these operands to bf16 (nearest even)
     anyway, so storing them rounded changes no result (a positive value at most half of bf16's smallest subnormal,
     2^-134, would round to zero and flip its ReLU mask bit).  fp32 otherwise."""
@@ -1118,6 +1148,9 @@ class Nb1dFunction(torch.autograd.Function):
                 sync2=None):
         """sync1 / sync2: BNSync of bn1 / bn2 (SyncBatchNorm containers) or None."""
         _capi.require_cuda(x)
+        if fp8_mode():
+            raise RuntimeError("conv mode 'fp8' is inference-only: non_bottleneck_1d runs it on the folded eval path "
+                               "(ops_eval.nb1d) only")
         N, H, W, C = x.shape
         sd = nb1d_storage_dtype(x, dil)
         t1 = conv3(x, w1, True, 1, False, bias=b1, relu=True, dtype=sd)
@@ -1201,6 +1234,7 @@ class UpFunction(torch.autograd.Function):
     def forward(ctx, x, w, b, gamma, beta, rm, rv, training, sync=None):
         """sync: BNSync (SyncBatchNorm) or None."""
         _capi.require_cuda(x)
+        require_inference_mode(training)
         N, H, W, ci = x.shape
         co = w.shape[1]
         phases, (Ho, Wo) = plans.transposed_gather_plan(H, W, 2 * H, 2 * W, 3, 1)
