@@ -585,6 +585,41 @@ size_t lf_jpeg_workspace_bytes(LfJpegImage* images, int N, size_t* coef_bytes);
 int lf_jpeg_decode(const void* blob, int N, int W, int H, unsigned char* out, int* status, void* coef, size_t coef_bytes,
                    void* workspace, size_t workspace_bytes, lf_stream_t stream);
 
+/* PNG decode of label maps (csrc/png.cu; replaces Image.open(f).convert('P') of BP/Dataloader/Load_Data_new.py:120-121):
+ * a batch of same-size non-interlaced PNGs, 8-bit grayscale or 1/2/4/8-bit palette -> uint8 [N][H][W] holding the gray
+ * values or palette indices, bit-identical to Pillow.  The chunks are walked on the host (lanedetection_end2end_b200/png.py),
+ * which checks the 2-byte zlib header and fills one LfPngImage per image; the DEFLATE data is inflated, unfiltered and
+ * unpacked on the device.  The device blob is LfPngImage[N] followed by each image's zlib stream (its IDAT payloads
+ * concatenated; zoff counts from the blob start).
+ * lf_png_workspace_bytes (HOST): checks the descriptors, fills rowbytes and raw_off (in place) and returns the scratch
+ *   bytes `workspace` needs (0 = invalid descriptors).
+ * lf_png_decode: two launches (inflate; unfilter + unpack); a corrupt stream (invalid code or code-length set, distance
+ *   before the start of the output, output longer or shorter than H * (1 + rowbytes), stream ending before its final block,
+ *   Adler-32 mismatch, filter type above 4) ORs LF_STATUS_PNG_CORRUPT into *status; that image's frame is undefined.
+ *   Calls sharing `workspace` must be ordered by the caller. */
+#define LF_STATUS_PNG_CORRUPT 16
+typedef struct LfPngImage {
+    long long zoff;               /* zlib stream (2-byte header, DEFLATE data, Adler-32): blob offset and length */
+    int zlen;
+    int W, H;
+    int depth;                    /* bits per sample: 8 (grayscale or palette) or 1, 2, 4 (palette) */
+    /* layout, filled by lf_png_workspace_bytes */
+    int rowbytes;                 /* (W * depth + 7) / 8: a scanline is one filter-type byte + rowbytes */
+    int reserved;
+    long long raw_off;            /* workspace offset of the H * (1 + rowbytes) inflated (still filtered) bytes */
+} LfPngImage;
+size_t lf_png_workspace_bytes(LfPngImage* images, int N);
+int lf_png_decode(const void* blob, int N, int W, int H, unsigned char* out, int* status, void* workspace, size_t workspace_bytes,
+                  lf_stream_t stream);
+
+/* Label-map transform of the reference loader (csrc/input_pipe.cu; BP/Dataloader/Load_Data_new.py:129,131,160-184): uint8
+ * maps [N][Hin][Win] -> int64 [N][1][Ho][Wo] = the collated `gt`.  Row oy of the output reads source row crop_y0 + ys[oy],
+ * column ox reads xs[ox] (Pillow's NEAREST resize, tables from input_pipeline.nearest_table).  nclasses < 3 turns 3 and 4
+ * into 0.  A flipped image (flip[n] != 0; flip may be NULL) is mirrored with 1 and 2 swapped, and then every pixel where the
+ * UNFLIPPED resized map held 3 / 4 is set to 4 / 3, as the reference does (its masks are taken before the flip). */
+int lf_label_preprocess(const unsigned char* maps, int N, int Hin, int Win, int crop_y0, const int* xs, const int* ys, int Ho,
+                        int Wo, int nclasses, const unsigned char* flip, long long* out, lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -143,7 +143,18 @@ class LfJpegImage(ctypes.Structure):
                 ("dc", LfJpegHuff * 4), ("ac", LfJpegHuff * 4)]
 
 
+STATUS_PNG_CORRUPT = 16
+
+
+class LfPngImage(ctypes.Structure):
+    _fields_ = [("zoff", _ll), ("zlen", _i), ("W", _i), ("H", _i), ("depth", _i), ("rowbytes", _i), ("reserved", _i),
+                ("raw_off", _ll)]
+
+
 _NET_PROTOS = {
+    "lf_png_workspace_bytes": (_c_size_t, [_p, _i]),
+    "lf_png_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p]),
+    "lf_label_preprocess": (_i, [_p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _p, _p]),
     "lf_jpeg_workspace_bytes": (_c_size_t, [_p, _i, _p]),
     "lf_jpeg_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p, _c_size_t, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),

@@ -64,9 +64,47 @@ __global__ void __launch_bounds__(256) frame_preprocess_kernel(const uint8_t* __
     }
 }
 
+// Label map of the loader (Load_Data_new.py:129,131,160-184): crop + Pillow NEAREST resize through the index tables,
+// nclasses < 3 zeroes 3 and 4, a flip mirrors and swaps 1 <-> 2, and then -- the reference's masks being taken before the
+// flip -- every pixel whose UNFLIPPED value was 3 / 4 becomes 4 / 3.  One thread = one output pixel.
+__global__ void __launch_bounds__(256) label_preprocess_kernel(const uint8_t* __restrict__ maps, int N, int Hin, int Win, int y0,
+                                                               const int* __restrict__ xs, const int* __restrict__ ys, int Ho,
+                                                               int Wo, int nclasses, const uint8_t* __restrict__ flip,
+                                                               long long* __restrict__ out) {
+    pdl_entry();
+    const long long total = (long long)N * Ho * Wo;
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const int ox = (int)(idx % Wo);
+        const int oy = (int)((idx / Wo) % Ho);
+        const int n = (int)(idx / ((long long)Wo * Ho));
+        const uint8_t* row = maps + ((size_t)n * Hin + y0 + __ldg(ys + oy)) * Win;
+        const int v0 = row[__ldg(xs + ox)];
+        const bool fl = flip && flip[n];
+        int v = fl ? row[__ldg(xs + Wo - 1 - ox)] : v0;
+        if (nclasses < 3 && (v == 3 || v == 4)) v = 0;
+        if (fl) {
+            v = v == 1 ? 2 : (v == 2 ? 1 : v);
+            v = v0 == 3 ? 4 : (v0 == 4 ? 3 : v);
+        }
+        out[idx] = v;
+    }
+}
+
 }  // namespace lf
 
 using namespace lf;
+
+extern "C" int lf_label_preprocess(const unsigned char* maps, int N, int Hin, int Win, int crop_y0, const int* xs, const int* ys, int Ho,
+                                   int Wo, int nclasses, const unsigned char* flip, long long* out, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(maps && xs && ys && out && N >= 1 && Hin >= 1 && Win >= 1 && Ho >= 1 && Wo >= 1 && crop_y0 >= 0 && crop_y0 < Hin);
+    const long long total = (long long)N * Ho * Wo;
+    const long long cap = (long long)device_sms() * 16;
+    const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
+    lf_launch(label_preprocess_kernel, grid, 256, 0, stream, (const uint8_t*)maps, N, Hin, Win, crop_y0, xs, ys, Ho, Wo, nclasses,
+              (const uint8_t*)flip, out);
+    return check_launch();
+}
 
 extern "C" int lf_frame_preprocess(const unsigned char* frames, int N, int Hin, int Win, int crop_y0, int crop_rows, const int* xb,
                                    const int* xk, int kx, const int* yb, const int* yk, int ky, int Ho, int Wo,
