@@ -216,29 +216,6 @@ void lf_conv1d_tc_set_variant(int variant);
 /* 1 if a call with taps {-dil,0,+dil} along y (vertical) or x runs on the slab kernel, i.e. may ask for stats_partial */
 int lf_conv1d_tc_slab_ok(int N, int H, int W, int C, int vertical, int dil);
 
-/* Tensor-core weight gradient of the same 3-tap convolutions:
- *   partial[cta][t][ci][co] = sum over this CTA's pixel range of x[n,y+dy[t],x+dx[t],ci] * dy[n,y,x,co]
- * nctas = lf_wgrad3_tc_ctas(...) (0 = unsupported shape); finish with
- * lf_wgrad_reduce(partial, nctas, 3, C, C, C, C, dst, st, sp, sq). */
-int lf_wgrad3_tc_ctas(int N, int H, int W, int C);
-int lf_wgrad3_tc(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                 float* partial, int nctas, lf_stream_t stream);
-/* 3xTF32 variant (csrc/wgrad_tcg.cu): same arguments and partial layout; both operands are split into TF32 hi / lo
- * parts on the fly and every product is x_hi*g_hi + (x_hi*g_lo + x_lo*g_hi), fp32 accumulate -- results agree with
- * lf_wgrad_f32 to fp32 round-off (the weight gradient the reference's autograd forms in fp32). */
-int lf_wgrad3_tc_x3_ctas(int N, int H, int W, int C);
-int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                    float* partial, int nctas, lf_stream_t stream);
-/* BF16 variant: same arguments and partial layout; both operands rounded to bf16 (nearest even) in the kernel, fp32
- * accumulate. */
-int lf_wgrad3_tc_bf16_ctas(int N, int H, int W, int C);
-int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                      float* partial, int nctas, lf_stream_t stream);
-/* lf_wgrad3_tc_bf16 with the layer input x stored as bf16 [N,H,W,C] (dy stays fp32): same results as lf_wgrad3_tc_bf16
- * on the fp32 copy of x, same arguments, nctas (lf_wgrad3_tc_bf16_ctas) and partial layout. */
-int lf_wgrad3_tc_bf16a(const void* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                       float* partial, int nctas, lf_stream_t stream);
-
 /* Weight gradient as a split-K GEMM over pixels:
  *   partial[s][t][cp][cq] = sum_{(n,j,i) in split s} P[n, j*psy+pdy[t], i*psx+pdx[t], cp]
  *                                                  * Q[n, j*qsy+qdy[t], i*qsx+qdx[t], cq]
@@ -397,11 +374,15 @@ typedef struct LfConvTcgArgs {
 int lf_conv_tcg_supported(int N, int Hs, int Ws, int Kc, int Ng);
 int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream);
 
-/* Weight gradients of the same layers on tensor cores (csrc/wgrad_tcg.cu), over the same views:
+/* Weight gradients on tensor cores (csrc/wgrad_tcg.cu), over the views above -- of these layers, of the Classification
+ * heads' stride-1 convolutions and of the factorised 3-tap convolutions of non_bottleneck_1d:
  *   D[blk*32 + c][n] = sum_{img,y,x} A_{map[blk]}(img, y+dy[blk], x+dx[blk], cblk[blk]*32 + c) * B(img, y, x, n)
  * for blk < nblocks (<= LF_WGRAD_TCG_MAX_BLOCKS), c < 32, n < Nn (multiple of 32, <= 128; ceil(nblocks/4)*Nn <= 512).
- * partial: [nctas][nblocks*32][Nn] per-CTA partial sums (nctas from lf_wgrad_tcg_ctas); reduce with lf_wgrad_reduce
- * (ntaps = 1, Cp = nblocks*32, Cq = Nn), then gather into [Co,Ci,3,3] (ops_net.wgrad_tcg_*). */
+ * partial: [nctas][nblocks*32][Nn] per-CTA partial sums; reduce with lf_wgrad_reduce (ntaps = 1, Cp = nblocks*32, Cq = Nn),
+ * then gather into [Co,Ci,3,3] (ops_net.wgrad_tcg_*), or for a 3-tap convolution with blk = t*C/32 + cb
+ * (ntaps = 3, Cp = Cq = C) straight into the weight layout.
+ * nctas = lf_wgrad_tcg_ctas(..., min_patches): split-K slices of at least min_patches 32-pixel patches each, at most one
+ * wave of CTAs (0 = unsupported shape).  The split count fixes the order in which the partials are summed. */
 #define LF_WGRAD_TCG_MAX_BLOCKS 24
 typedef struct LfWgradTcgArgs {
     LfTcgView a[2];
@@ -413,10 +394,11 @@ typedef struct LfWgradTcgArgs {
     int nctas;
     int precision;          /* 0 = TF32 multiply; 1 = 3xTF32 (both operands split in shared memory, fp32-grade);
                                2 = BF16 multiply (both operands rounded to bf16 in the kernel) */
+    int a_dtype;            /* element type of the A views: LF_F32, or LF_BF16 (the bf16-stored layer inputs of the bf16
+                               mode: same results as their fp32 copy) -- precision 2 and Nn in {64, 128} only, else
+                               LF_ERR_UNSUPPORTED; B stays fp32 */
 } LfWgradTcgArgs;
-int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);
-int lf_wgrad_tcg_ctas_x3(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);     /* same, for precision 1 */
-int lf_wgrad_tcg_ctas_bf16(int N, int Hs, int Ws, int Ka, int Nn, int nblocks);   /* same, for precision 2 */
+int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks, int min_patches);
 int lf_wgrad_tcg(const LfWgradTcgArgs* args, lf_stream_t stream);
 
 /* Batched weight packing (host side: ops_net.WeightPackCache).  The reference keeps Conv2d / ConvTranspose2d

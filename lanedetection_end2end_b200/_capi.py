@@ -104,7 +104,8 @@ WGRAD_TCG_MAX_BLOCKS = 24
 class LfWgradTcgArgs(ctypes.Structure):
     _fields_ = [("a", LfTcgView * 2), ("b", LfTcgView), ("partial", _p), ("N", _i), ("Hs", _i), ("Ws", _i), ("Ka", _i),
                 ("Nn", _i), ("nblocks", _i), ("map", _i * WGRAD_TCG_MAX_BLOCKS), ("dy", _i * WGRAD_TCG_MAX_BLOCKS),
-                ("dx", _i * WGRAD_TCG_MAX_BLOCKS), ("cblk", _i * WGRAD_TCG_MAX_BLOCKS), ("nctas", _i), ("precision", _i)]
+                ("dx", _i * WGRAD_TCG_MAX_BLOCKS), ("cblk", _i * WGRAD_TCG_MAX_BLOCKS), ("nctas", _i), ("precision", _i),
+                ("a_dtype", _i)]
 
 
 OPTIM_ADAM, OPTIM_SGD, OPTIM_RMSPROP = 0, 1, 2
@@ -158,9 +159,7 @@ _NET_PROTOS = {
     "lf_jpeg_workspace_bytes": (_c_size_t, [_p, _i, _p]),
     "lf_jpeg_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p, _c_size_t, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
-    "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i]),
-    "lf_wgrad_tcg_ctas_x3": (_i, [_i, _i, _i, _i, _i, _i]),
-    "lf_wgrad_tcg_ctas_bf16": (_i, [_i, _i, _i, _i, _i, _i]),
+    "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg": (_i, [ctypes.POINTER(LfWgradTcgArgs), _p]),
     "lf_reduce_multi": (_i, [ctypes.POINTER(LfReduceJob), _i, _p]),
     "lf_conv_tcg_supported": (_i, [_i, _i, _i, _i, _i]),
@@ -177,13 +176,6 @@ _NET_PROTOS = {
     "lf_conv1d_tc_x3_rows": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_conv1d_tc_set_variant": (None, [_i]),
     "lf_conv1d_tc_slab_ok": (_i, [_i, _i, _i, _i, _i, _i]),
-    "lf_wgrad3_tc_ctas": (_i, [_i, _i, _i, _i]),
-    "lf_wgrad3_tc": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
-    "lf_wgrad3_tc_x3_ctas": (_i, [_i, _i, _i, _i]),
-    "lf_wgrad3_tc_x3": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
-    "lf_wgrad3_tc_bf16_ctas": (_i, [_i, _i, _i, _i]),
-    "lf_wgrad3_tc_bf16": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
-    "lf_wgrad3_tc_bf16a": (_i, [_p, _p, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _p, _i, _p]),
     "lf_wgrad_reduce": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "lf_vec_reduce": (_i, [_p, _i, _i, _i, _p, _p]),
     "lf_colsum_blocks": (_i, [ctypes.c_longlong]),
@@ -266,12 +258,13 @@ def check(rc, what):
 
 
 LAUNCHES = 0          # kernels launched through the C ABI since import (every call below = 1 launch)
-TRACE = None          # set to a list to record (name, start_event, end_event, flops, bytes) per launch
+TRACE = None          # set to a list to record (label, start_event, end_event, flops, bytes) per launch
 
 
-def call(name, *args, flops=0, nbytes=0):
+def call(name, *args, flops=0, nbytes=0, label=None):
     """Invoke one launching entry point: counts it, optionally brackets it with CUDA events on
-    the current stream (bench.py's per-kernel roofline), and raises on a non-zero return."""
+    the current stream (bench.py's per-kernel roofline), and raises on a non-zero return.
+    label: the name the launch is traced under (default: the entry point's)."""
     global LAUNCHES
     fn = getattr(lib(), name)
     if TRACE is None:
@@ -282,7 +275,7 @@ def call(name, *args, flops=0, nbytes=0):
         e0.record()
         rc = fn(*args)
         e1.record()
-        TRACE.append((name, e0, e1, flops, nbytes))
+        TRACE.append((label or name, e0, e1, flops, nbytes))
     LAUNCHES += 1
     check(rc, name)
 

@@ -3,12 +3,12 @@
 //     D[blk*32 + c][n] = sum_{img,y,x} A_{map[blk]}(img, y + dy[blk], x + dx[blk], cblk[blk]*32 + c) * B(img, y, x, n)
 //
 // i.e. one 32-channel block of one tap per `blk` (up to 24 blocks), n < Nn (multiple of 32, <= 128), over strided NHWC
-// views.  Its callers:
-//  * lf_wgrad_tcg: the resolution-changing layers (3x3 stride-2 Conv2d of DownsamplerBlock, 3x3 stride-2 ConvTranspose2d
-//    of UpsamplerBlock; BP/Networks/ERFNet.py:15,101) on the pair-pixel / row-parity views of conv_tcg.cu, and the
+// views.  Its one entry point, lf_wgrad_tcg, takes the block table from the host (ops_net.run_wgrad_tcg) for
+//  * the resolution-changing layers (3x3 stride-2 Conv2d of DownsamplerBlock, 3x3 stride-2 ConvTranspose2d of
+//    UpsamplerBlock; BP/Networks/ERFNet.py:15,101) on the pair-pixel / row-parity views of conv_tcg.cu, and the
 //    Classification heads;
-//  * lf_wgrad3_tc / lf_wgrad3_tc_x3: the factorised 3-tap convolutions (C in {64,128}), dW[t][ci][co] = block t*C/32 + cb
-//    of X shifted by tap t against dY -- the partial layout [3][C][C] is the block layout above.
+//  * the factorised 3-tap convolutions (C in {64,128}; C = 16 on the super-pixel view), dW[t][ci][co] = block
+//    t*C/32 + cb of X shifted by tap t against dY -- the partial layout [3][C][C] is the block layout above.
 // The K dimension of these GEMMs is the pixel index, so both operands lie MN-major in the NHWC boxes TMA loads.  wgmma
 // takes A (rows = x-channels, k = pixels) from registers, which the threads load from the swizzled box like any other
 // fragment; it reads TF32 B only K-major from shared memory, so the dY boxes are transposed in shared memory first.
@@ -33,9 +33,9 @@
 // their columns.  BF16 wgmma could read B MN-major (imm-trans-b = 1) and skip the transposition, but the K-major tile
 // keeps one B layout and descriptor (wgmma_desc_sw64) for all three tensor-core kernels; double-buffering and the proxy
 // fence are unchanged.  Two wgmma m64nNWk16 per stage.
-// BF16 with a bf16 A view (template ABF, lf_wgrad3_tc_bf16a): the A boxes are [32 px x 32 ch] bf16, 64-byte rows,
-// 64B-swizzled (half the bytes), and an A register is two 16-bit LDS of the ready values -- the bits the fp32 path packs
-// from an fp32 copy of the same values, so the same results.  B stays fp32 and keeps its transposition.
+// BF16 with a bf16 A view (template ABF, LfWgradTcgArgs.a_dtype = LF_BF16): the A boxes are [32 px x 32 ch] bf16,
+// 64-byte rows, 64B-swizzled (half the bytes), and an A register is two 16-bit LDS of the ready values -- the bits the
+// fp32 path packs from an fp32 copy of the same values, so the same results.  B stays fp32 and keeps its transposition.
 // The next stage's fragments are not loaded while a stage's wgmma runs: ptxas then reuses the A registers the running
 // wgmma still reads.  Every CTA writes its slice [64 rows][Nn] of one partial; lf_wgrad_reduce sums them in fixed order.
 #include <cuda.h>
@@ -320,12 +320,12 @@ static int wgt_split(long long patches, int min_per, int nblocks) {
     return (int)(s < 1 ? 1 : s);
 }
 
-static int wgt_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) {
+static int wgt_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks, int min_patches) {
     int bx, by;
     if (N <= 0 || Ka % 32 != 0 || Ka < 32 || Nn % 32 != 0 || Nn < 32 || Nn > 128 || nblocks < 1 || nblocks > WG_MAXB) return 0;
-    if (!wgt_pick_patch(Hs, Ws, &bx, &by)) return 0;
+    if (min_patches < 1 || !wgt_pick_patch(Hs, Ws, &bx, &by)) return 0;
     if (!tc_get_encode_fn()) return 0;
-    return wgt_split((long long)N * (Hs / by) * (Ws / bx), 4, nblocks);
+    return wgt_split((long long)N * (Hs / by) * (Ws / bx), min_patches, nblocks);
 }
 
 template <int NN, int P, bool ABF = false>
@@ -350,7 +350,7 @@ static cudaError_t wgt_launch_nn(dim3 grid, int smem_bytes, cudaStream_t stream,
 // a: A views and their block table, b: the B view; the launch of the generic kernel
 static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int Ws, int Ka, int Nn, int nblocks, const int* map,
                    const int* dy, const int* dx, const int* cblk, float* partial, int nsplit, int prec, cudaStream_t stream,
-                   bool abf = false) {
+                   bool abf) {
     TcEncodeTiledFn enc = tc_get_encode_fn();
     if (!enc) return LF_ERR_UNSUPPORTED;
     WgtArgs a{};
@@ -393,63 +393,17 @@ static int wgt_run(const LfTcgView* av, const LfTcgView& bv, int N, int Hs, int 
 using namespace lf;
 
 // number of split-K slices (= partials) lf_wgrad_tcg will use, 0 = unsupported
-extern "C" int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
-extern "C" int lf_wgrad_tcg_ctas_x3(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
-extern "C" int lf_wgrad_tcg_ctas_bf16(int N, int Hs, int Ws, int Ka, int Nn, int nblocks) { return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks); }
+extern "C" int lf_wgrad_tcg_ctas(int N, int Hs, int Ws, int Ka, int Nn, int nblocks, int min_patches) {
+    return wgt_ctas(N, Hs, Ws, Ka, Nn, nblocks, min_patches);
+}
 
 extern "C" int lf_wgrad_tcg(const LfWgradTcgArgs* args, lf_stream_t stream_) {
     if (!args) return LF_ERR_INVALID_ARGUMENT;
     const LfWgradTcgArgs& p = *args;
     LF_REQUIRE(p.a[0].ptr && p.b.ptr && p.partial && p.nctas >= 1);
     LF_REQUIRE(p.precision == TC_TF32 || p.precision == TC_X3 || p.precision == TC_BF16);
-    if (!wgt_ctas(p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks)) return LF_ERR_UNSUPPORTED;
+    LF_REQUIRE(p.a_dtype == LF_F32 || p.a_dtype == LF_BF16);
+    if (!wgt_ctas(p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks, 1)) return LF_ERR_UNSUPPORTED;
     return wgt_run(p.a, p.b, p.N, p.Hs, p.Ws, p.Ka, p.Nn, p.nblocks, p.map, p.dy, p.dx, p.cblk, p.partial, p.nctas, p.precision,
-                   reinterpret_cast<cudaStream_t>(stream_));
-}
-
-// ---- factorised 3-tap convolutions: partial[cta][t][ci][co] = blocks t*C/32 + cb of X shifted by tap t against dY
-static int wgrad3_ctas(int N, int H, int W, int C, int min_per) {
-    int bx, by;
-    if (!(C == 64 || C == 128) || N <= 0) return 0;
-    if (!wgt_pick_patch(H, W, &bx, &by)) return 0;
-    if (!tc_get_encode_fn()) return 0;
-    return wgt_split((long long)N * (H / by) * (W / bx), min_per, 3 * C / 32);
-}
-
-static int wgrad3_run(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                      float* partial, int nctas, int prec, lf_stream_t stream_, bool xbf16 = false) {
-    LF_REQUIRE(x && dy && partial && tap_dy && tap_dx && nctas >= 1);
-    if (!(C == 64 || C == 128)) return LF_ERR_UNSUPPORTED;
-    const LfTcgView xv{x, H, W, (long long)H * W * C, (long long)W * C, C};
-    const LfTcgView gv{dy, H, W, (long long)H * W * C, (long long)W * C, C};
-    const LfTcgView av[2] = {xv, xv};
-    const int cbs = C / 32;
-    int map[12], bdy[12], bdx[12], cblk[12];
-    for (int t = 0; t < 3; ++t)
-        for (int cb = 0; cb < cbs; ++cb) {
-            const int b = t * cbs + cb;
-            map[b] = 0; bdy[b] = tap_dy[t]; bdx[b] = tap_dx[t]; cblk[b] = cb;
-        }
-    return wgt_run(av, gv, N, H, W, C, C, 3 * cbs, map, bdy, bdx, cblk, partial, nctas, prec, reinterpret_cast<cudaStream_t>(stream_),
-                   xbf16);
-}
-
-extern "C" int lf_wgrad3_tc_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 4); }
-extern "C" int lf_wgrad3_tc_x3_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 8); }
-extern "C" int lf_wgrad3_tc_bf16_ctas(int N, int H, int W, int C) { return wgrad3_ctas(N, H, W, C, 4); }
-extern "C" int lf_wgrad3_tc(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                            float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_TF32, stream);
-}
-extern "C" int lf_wgrad3_tc_x3(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                               float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_X3, stream);
-}
-extern "C" int lf_wgrad3_tc_bf16(const float* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                                 float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(x, dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_BF16, stream);
-}
-extern "C" int lf_wgrad3_tc_bf16a(const void* x, const float* dy, int N, int H, int W, int C, const int* tap_dy, const int* tap_dx,
-                                  float* partial, int nctas, lf_stream_t stream) {
-    return wgrad3_run(static_cast<const float*>(x), dy, N, H, W, C, tap_dy, tap_dx, partial, nctas, TC_BF16, stream, true);
+                   reinterpret_cast<cudaStream_t>(stream_), p.a_dtype == LF_BF16);
 }

@@ -77,42 +77,10 @@ def _wgrad_tcg_dense(x, dy, taps):
     """-> [ntaps*Ci][Co]: row t*Ci + ci = sum over pixels of x[pixel + tap t][ci] * dy[pixel][:], or None if unsupported."""
     N, H, W, Ci = x.shape
     Co = dy.shape[-1]
-    if not (o.WGRAD_TCG and o.tc_mode() and Ci % 32 == 0 and Co % 32 == 0 and Co <= 128 and x.is_contiguous() and dy.is_contiguous()):
+    if not (o.tc_mode() and Ci % 32 == 0 and Co % 32 == 0 and Co <= 128 and x.is_contiguous() and dy.is_contiguous()):
         return None
-    per_tap = Ci // 32
-    max_taps = 0
-    for tpl in range(len(taps), 0, -1):
-        nb = tpl * per_tap
-        if ((nb + 3) // 4) * Co <= 512 and nb <= _capi.WGRAD_TCG_MAX_BLOCKS and o._wgrad_tcg_ctas(N, H, W, Ci, Co, nb) > 0:
-            max_taps = tpl
-            break
-    if max_taps == 0:
-        return None
-    res = torch.empty(len(taps) * Ci, Co, dtype=torch.float32, device=x.device)
-    st = o._stream()
-    t0 = 0
-    while t0 < len(taps):
-        tpl = min(max_taps, len(taps) - t0)
-        nblocks = tpl * per_tap
-        nctas = o._wgrad_tcg_ctas(N, H, W, Ci, Co, nblocks)
-        if nctas <= 0:
-            return None
-        partial = torch.empty(nctas * nblocks * 32 * Co, dtype=torch.float32, device=x.device)
-        a = _capi.LfWgradTcgArgs()
-        a.a[0] = o._tcg_view(x, H, W, H * W * Ci, W * Ci, Ci)
-        a.a[1] = a.a[0]
-        a.b = o._tcg_view(dy, H, W, H * W * Co, W * Co, Co)
-        a.partial, a.N, a.Hs, a.Ws, a.Ka, a.Nn, a.nblocks, a.nctas = partial.data_ptr(), N, H, W, Ci, Co, nblocks, nctas
-        a.precision = o.wgrad_precision()
-        for i in range(nblocks):
-            dyy, dxx = taps[t0 + i // per_tap]
-            a.map[i], a.dy[i], a.dx[i], a.cblk[i] = 0, dyy, dxx, i % per_tap
-        _capi.call("lf_wgrad_tcg", ctypes.byref(a), st, flops=2 * N * H * W * nblocks * 32 * Co,
-                   nbytes=4 * N * H * W * (nblocks * 32 + Co))
-        _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 1, nblocks * 32, Co, nblocks * 32, Co,
-                   res.data_ptr() + 4 * t0 * Ci * Co, 0, Co, 1, st)
-        t0 += tpl
-    return res
+    return o.wgrad_tcg_rows([o._tcg_view(x, H, W, H * W * Ci, W * Ci, Ci)], o._tcg_view(dy, H, W, H * W * Co, W * Co, Co),
+                            [(0, ty, tx) for ty, tx in taps], N, H, W, Ci, Co, range(len(taps), 0, -1), x.device)
 
 
 def conv_wgrad(x, dy, w):

@@ -100,13 +100,9 @@ def tcg_precision(wg):
 WGRAD_SINGLE_PASS = os.environ.get("LANEFIT_WGRAD_TF32", "0") == "1"
 
 
-def wgrad_x3():
-    return x3_mode() and not WGRAD_SINGLE_PASS
-
-
 def wgrad_precision():
     """LfWgradTcgArgs.precision of the active mode (0 = TF32, 1 = 3xTF32, 2 = BF16)."""
-    return 2 if bf16_mode() else int(wgrad_x3())
+    return 2 if bf16_mode() else int(x3_mode() and not WGRAD_SINGLE_PASS)
 
 
 def split_tf32(t):
@@ -298,77 +294,96 @@ def _tcg_wgrad_index(kind, C, O, Nn, device):
     return _TCG_WGRAD_IDX[key]
 
 
-WGRAD_TCG = os.environ.get("LANEFIT_WGRAD_TCG", "1") != "0"
+def wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, three_tap=False):
+    """Split-K CTA count (= partials) of one lf_wgrad_tcg launch in the active mode, 0 = unsupported.  Each CTA takes at
+    least 8 32-pixel patches for the 3xTF32 weight gradients of the 3-tap convolutions (three_tap), 4 for every other
+    launch.  The split count fixes the order in which the partials are summed, so these values are part of the results."""
+    min_patches = 8 if three_tap and wgrad_precision() == 1 else 4
+    return int(_lib().lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, min_patches))
+
+
+def run_wgrad_tcg(av, bv, blocks, N, Hs, Ws, Ka, Nn, device, a_dtype=_capi.LF_F32, three_tap=False, label=None, flops=None,
+                  nbytes=None):
+    """One lf_wgrad_tcg launch in the active mode's precision -> (partial [nctas][len(blocks)*32][Nn], nctas), which the
+    caller reduces.  av: the A views (one or two LfTcgView, elements of a_dtype), bv: the B view, blocks: the block table
+    [(view, dy, dx, channel block)]; three_tap: see wgrad_tcg_ctas.  label / flops / nbytes: what the launch is traced as
+    (default: lf_wgrad_tcg, the products of the block table and one fp32 read of every operand element)."""
+    nblocks = len(blocks)
+    nctas = wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, three_tap)
+    partial = torch.empty(nctas * nblocks * 32 * Nn, dtype=torch.float32, device=device)
+    a = _capi.LfWgradTcgArgs()
+    for i, v in enumerate(av):
+        a.a[i] = v
+    a.b = bv
+    a.partial, a.N, a.Hs, a.Ws, a.Ka, a.Nn, a.nblocks, a.nctas = partial.data_ptr(), N, Hs, Ws, Ka, Nn, nblocks, nctas
+    a.precision, a.a_dtype = wgrad_precision(), a_dtype
+    for i, (m, dy, dx, cb) in enumerate(blocks):
+        a.map[i], a.dy[i], a.dx[i], a.cblk[i] = m, dy, dx, cb
+    _capi.call("lf_wgrad_tcg", ctypes.byref(a), _stream(), label=label,
+               flops=2 * N * Hs * Ws * nblocks * 32 * Nn if flops is None else flops,
+               nbytes=4 * N * Hs * Ws * (nblocks * 32 + Nn) if nbytes is None else nbytes)
+    return partial, nctas
+
+
+def wgrad_tcg_taps_per_launch(N, Hs, Ws, Ka, Nn, candidates):
+    """The first tap count of `candidates` whose block table (Ka/32 blocks per tap) one lf_wgrad_tcg launch takes, 0 = none."""
+    for tpl in candidates:
+        nb = tpl * (Ka // 32)
+        if ((nb + 3) // 4) * Nn <= 512 and nb <= _capi.WGRAD_TCG_MAX_BLOCKS and wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nb) > 0:
+            return tpl
+    return 0
+
+
+def wgrad_tcg_rows(av, bv, taps, N, Hs, Ws, Ka, Nn, candidates, device):
+    """-> reduced [len(taps)*Ka][Nn] tensor: row (t*Ka + k) = sum over pixels of A_{view}(pixel + (dy, dx))[k] * B(pixel)[:Nn]
+    for taps[t] = (view, dy, dx), in launches of the first tap count of `candidates` one launch takes; None if none does."""
+    tpl = wgrad_tcg_taps_per_launch(N, Hs, Ws, Ka, Nn, candidates)
+    if tpl == 0:
+        return None
+    res = torch.empty(len(taps) * Ka, Nn, dtype=torch.float32, device=device)
+    for t0 in range(0, len(taps), tpl):
+        blocks = [(m, dy, dx, cb) for m, dy, dx in taps[t0:t0 + tpl] for cb in range(Ka // 32)]
+        partial, nctas = run_wgrad_tcg(av, bv, blocks, N, Hs, Ws, Ka, Nn, device)
+        rows = len(blocks) * 32
+        _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 1, rows, Nn, rows, Nn, res.data_ptr() + 4 * t0 * Ka * Nn, 0, Nn, 1,
+                   _stream())
+    return res
+
+
+# the stride-2 layers: 6, 3 or 2 of the six pair-pixel taps per launch
+_S2_TAPS_PER_LAUNCH = (6, 3, 2)
 
 
 def wgrad_tcg_ok(a_t, C, b_t, Nn):
     """A = dense [N,2Hs,2Ws,C] tensor (pair view 2C channels), B = [N,Hs,Ws,>=Nn] tensor."""
     N, H2, W2, ca = a_t.shape
-    if not (WGRAD_TCG and tc_mode() and ca == C and (2 * C) % 32 == 0 and H2 % 2 == 0 and W2 % 2 == 0 and Nn % 32 == 0 and Nn <= 128
+    if not (tc_mode() and ca == C and (2 * C) % 32 == 0 and H2 % 2 == 0 and W2 % 2 == 0 and Nn % 32 == 0 and Nn <= 128
             and b_t.shape[-1] >= Nn and b_t.shape[1] == H2 // 2 and b_t.shape[2] == W2 // 2
             and a_t.is_contiguous() and b_t.is_contiguous()):
         return False
-    per_tap = (2 * C) // 32
-    taps_per_launch = _wgrad_tcg_taps_per_launch(N, H2 // 2, W2 // 2, C, Nn)
-    return taps_per_launch > 0
+    return wgrad_tcg_taps_per_launch(N, H2 // 2, W2 // 2, 2 * C, Nn, _S2_TAPS_PER_LAUNCH) > 0
 
 
-def _wgrad_tcg_ctas(*args):
-    return int((_lib().lf_wgrad_tcg_ctas_bf16 if bf16_mode() else _lib().lf_wgrad_tcg_ctas_x3 if wgrad_x3()
-                else _lib().lf_wgrad_tcg_ctas)(*args))
-
-
-def _wgrad_tcg_taps_per_launch(N, Hs, Ws, C, Nn):
-    """6, 3 or 2 taps per launch (block table and shared-memory stages permitting), 0 = unsupported."""
-    per_tap = (2 * C) // 32
-    for tpl in (6, 3, 2):
-        nb = tpl * per_tap
-        if ((nb + 3) // 4) * Nn <= 512 and nb <= _capi.WGRAD_TCG_MAX_BLOCKS and _wgrad_tcg_ctas(N, Hs, Ws, 2 * C, Nn, nb) > 0:
-            return tpl
-    return 0
-
-
-def run_wgrad_tcg(a_t, C, b_t, Nn):
+def _s2_wgrad_rows(a_t, C, b_t, Nn):
     """-> reduced [6*2C][Nn] tensor: row (t*2C + k) = sum over pixels of A_t(pixel + tap t)[k] * B(pixel)[:Nn]
     with the six pair-pixel taps of TCG_S2CONV_TAPS."""
     N, H2, W2, _ = a_t.shape
-    Hs, Ws = H2 // 2, W2 // 2
-    Ka = 2 * C
-    per_tap = Ka // 32
-    cb_tot = b_t.shape[-1]
-    taps_per_launch = _wgrad_tcg_taps_per_launch(N, Hs, Ws, C, Nn)
-    res = torch.empty(6 * Ka, Nn, dtype=torch.float32, device=a_t.device)
-    st = _stream()
-    for t0 in range(0, 6, taps_per_launch):
-        nblocks = taps_per_launch * per_tap
-        nctas = _wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks)
-        partial = torch.empty(nctas * nblocks * 32 * Nn, dtype=torch.float32, device=a_t.device)
-        a = _capi.LfWgradTcgArgs()
-        a.a[0] = _tcg_view(a_t, Hs, Ws, H2 * W2 * C, 2 * W2 * C, 2 * C)
-        a.a[1] = _tcg_view(a_t, Hs, Ws, H2 * W2 * C, 2 * W2 * C, 2 * C, W2 * C)
-        a.b = _tcg_view(b_t, Hs, Ws, Hs * Ws * cb_tot, Ws * cb_tot, cb_tot)
-        a.partial, a.N, a.Hs, a.Ws, a.Ka, a.Nn, a.nblocks, a.nctas = partial.data_ptr(), N, Hs, Ws, Ka, Nn, nblocks, nctas
-        a.precision = wgrad_precision()
-        for i in range(nblocks):
-            m, dy, dx = TCG_S2CONV_TAPS[t0 + i // per_tap]
-            a.map[i], a.dy[i], a.dx[i], a.cblk[i] = m, dy, dx, i % per_tap
-        _capi.call("lf_wgrad_tcg", ctypes.byref(a), st, flops=2 * N * Hs * Ws * nblocks * 32 * Nn,
-                   nbytes=4 * N * Hs * Ws * (nblocks * 32 + Nn))
-        _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 1, nblocks * 32, Nn, nblocks * 32, Nn,
-                   res.data_ptr() + 4 * t0 * Ka * Nn, 0, Nn, 1, st)
-    return res
+    Hs, Ws, cb = H2 // 2, W2 // 2, b_t.shape[-1]
+    av = [_tcg_view(a_t, Hs, Ws, H2 * W2 * C, 2 * W2 * C, 2 * C), _tcg_view(a_t, Hs, Ws, H2 * W2 * C, 2 * W2 * C, 2 * C, W2 * C)]
+    bv = _tcg_view(b_t, Hs, Ws, Hs * Ws * cb, Ws * cb, cb)
+    return wgrad_tcg_rows(av, bv, TCG_S2CONV_TAPS, N, Hs, Ws, 2 * C, Nn, _S2_TAPS_PER_LAUNCH, a_t.device)
 
 
 def wgrad_tcg_conv(x, cin, dcat, cc):
     """dW [cc, cin, 3, 3] of the stride-2 Conv2d (DownsamplerBlock): A = x, B = dcat[..., :pad32(cc)]."""
     Nn = plans.pad_to(cc, 32)
-    res = run_wgrad_tcg(x, cin, dcat, Nn)
+    res = _s2_wgrad_rows(x, cin, dcat, Nn)
     return res.reshape(-1)[_tcg_wgrad_index("conv", cin, cc, Nn, x.device)].view(cc, cin, 3, 3)
 
 
 def wgrad_tcg_convT(x, ci, du, co):
     """dW [ci, co, 3, 3] of the stride-2 ConvTranspose2d (UpsamplerBlock): A = du (output gradient), B = x."""
-    res = run_wgrad_tcg(du, co, x, ci)
+    res = _s2_wgrad_rows(du, co, x, ci)
     return res.reshape(-1)[_tcg_wgrad_index("convT", co, ci, ci, x.device)].view(ci, co, 3, 3)
 
 
@@ -756,55 +771,54 @@ def conv3(x, w, vertical, dil, transposed, colsum=None, wp=None, dtype=torch.flo
     return out
 
 
+def wgrad3_tcg_ok(N, H, W, C):
+    """Does lf_wgrad_tcg take the weight gradient of a 3-tap convolution on [N,H,W,C] (the super-pixel view for C = 16)?"""
+    return tc_mode() and C in (64, 128) and wgrad_tcg_ctas(N, H, W, C, C, 3 * C // 32, three_tap=True) > 0
+
+
+def _wgrad3_tcg(x, d_out, H, W, C, taps):
+    """lf_wgrad_tcg over the three taps [(dy, dx)] of a 3-tap convolution, x / d_out read as dense [N,H,W,C] (block
+    t*C/32 + cb = tap t, channel block cb) -> (partial [nctas][3][C][C], nctas).  Traced as lf_wgrad3_tc[_x3 | _bf16][a]
+    (a: bf16 x) with the products of the convolution and one read of x and d_out."""
+    label = "lf_wgrad3_tc" + ("", "_x3", "_bf16")[wgrad_precision()] + ("a" if x.dtype == torch.bfloat16 else "")
+    blocks = [(0, dy, dx, cb) for dy, dx in taps for cb in range(C // 32)]
+    return run_wgrad_tcg([_tcg_view(x, H, W, H * W * C, W * C, C)], _tcg_view(d_out, H, W, H * W * C, W * C, C), blocks,
+                         x.shape[0], H, W, C, C, x.device, a_dtype=_capi.dtype_id(x), three_tap=True, label=label,
+                         flops=6 * x.numel() * x.shape[-1], nbytes=(x.element_size() + 4) * x.numel())
+
+
 def wgrad3(x_in, d_out, w, vertical, dil, bias_grad="compute"):
     """Weight + bias gradient of one factorised 3-tap convolution -> (dw [Co,Ci,kh,kw], db [Co] or None).
     bias_grad: "compute" (column sums of d_out), or "skip" (the caller gets it elsewhere)."""
     N, H, W, C = x_in.shape
-    sfx = "_x3" if wgrad_x3() else "_bf16" if bf16_mode() else ""   # which tensor-core weight-gradient kernel
-    xbf = x_in.dtype == torch.bfloat16                               # a bf16 layer input: the bf16-A kernel
+    xbf = x_in.dtype == torch.bfloat16                               # a bf16 layer input: a bf16 A view
     if xbf and not bf16_mode():
         raise _capi.LanefitError("wgrad3: a bf16 layer input needs the bf16 mode")
-    entry = "lf_wgrad3_tc" + sfx + ("a" if xbf else "")
-    nbytes = (x_in.element_size() + 4) * N * H * W * C
-    if super_ok(x_in, dil) and d_out.is_contiguous():
-        Cs, Ws = SUPER * C, W // SUPER
-        nctas = getattr(_lib(), "lf_wgrad3_tc%s_ctas" % sfx)(N, H, Ws, Cs)
-        if nctas > 0:
-            tdy = (ctypes.c_int * 3)(*[((k - 1) if vertical else 0) for k in range(3)])
-            tdx = (ctypes.c_int * 3)(*[(0 if vertical else (k - 1)) for k in range(3)])
-            partial = torch.empty(nctas * 3 * Cs * Cs, dtype=torch.float32, device=x_in.device)
-            dws = torch.empty(Cs, Cs, 3, dtype=torch.float32, device=x_in.device)
-            st = _stream()
-            _capi.call(entry, ptr(x_in), ptr(d_out), N, H, Ws, Cs, tdy, tdx, ptr(partial), nctas, st,
-                       flops=2 * N * H * W * 3 * C * C, nbytes=nbytes)
-            _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 3, Cs, Cs, Cs, Cs, ptr(dws), 1, 3, Cs * 3, st)
-            dw = unpack_wgrad_super(dws, vertical).reshape(w.shape)
-            db = None
-            if bias_grad == "compute":
-                db = torch.empty(C, dtype=torch.float32, device=x_in.device)
-                run_colsum(d_out, C, 0, db)
-            return dw, db
-    dw = torch.empty_like(w)
     db = torch.empty(C, dtype=torch.float32, device=x_in.device) if bias_grad == "compute" else None
     lay = (1, 3, C * 3)                                   # (tap, ci, co) strides of [Co,Ci,3] weights
-    nctas = getattr(_lib(), "lf_wgrad3_tc%s_ctas" % sfx)(N, H, W, C) if (tc_mode() and C in (64, 128)) else 0
-    if nctas > 0:
-        tdy = (ctypes.c_int * 3)(*[((k - 1) * dil if vertical else 0) for k in range(3)])
-        tdx = (ctypes.c_int * 3)(*[(0 if vertical else (k - 1) * dil) for k in range(3)])
-        partial = torch.empty(nctas * 3 * C * C, dtype=torch.float32, device=x_in.device)
-        st = _stream()
-        _capi.call(entry, ptr(x_in), ptr(d_out), N, H, W, C, tdy, tdx, ptr(partial), nctas, st,
-                   flops=2 * N * H * W * 3 * C * C, nbytes=nbytes)
+    if super_ok(x_in, dil) and d_out.is_contiguous() and wgrad3_tcg_ok(N, H, W // SUPER, SUPER * C):
+        Cs = SUPER * C
+        taps = [((k - 1, 0) if vertical else (0, k - 1)) for k in range(3)]
+        partial, nctas = _wgrad3_tcg(x_in, d_out, H, W // SUPER, Cs, taps)
+        dws = torch.empty(Cs, Cs, 3, dtype=torch.float32, device=x_in.device)
+        _capi.call("lf_wgrad_reduce", ptr(partial), nctas, 3, Cs, Cs, Cs, Cs, ptr(dws), 1, 3, Cs * 3, _stream())
+        dw = unpack_wgrad_super(dws, vertical).reshape(w.shape)
+    elif wgrad3_tcg_ok(N, H, W, C):
+        taps = [(((k - 1) * dil, 0) if vertical else (0, (k - 1) * dil)) for k in range(3)]
+        partial, nctas = _wgrad3_tcg(x_in, d_out, H, W, C, taps)
+        dw = torch.empty_like(w)
         _reduce(partial, nctas, 3, C, C, C, C, dw, lay[0], lay[1], lay[2])
-        if db is not None:
-            run_colsum(d_out, C, 0, db)
+    else:
+        if xbf:
+            raise _capi.LanefitError("wgrad3: a bf16 layer input needs a tensor-core route")
+        kh, kw = (3, 1) if vertical else (1, 3)
+        ph, pw = (dil, 0) if vertical else (0, dil)
+        dh, dw_ = (dil, 1) if vertical else (1, dil)
+        dw = torch.empty_like(w)
+        run_wgrad(plans.conv_wgrad_plan(H, W, kh, kw, 1, ph, pw, dh, dw_), x_in, C, d_out, C, 0, N, dw, lay, db)
         return dw, db
-    if xbf:
-        raise _capi.LanefitError("wgrad3: a bf16 layer input needs a tensor-core route")
-    kh, kw = (3, 1) if vertical else (1, 3)
-    ph, pw = (dil, 0) if vertical else (0, dil)
-    dh, dw_ = (dil, 1) if vertical else (1, dil)
-    run_wgrad(plans.conv_wgrad_plan(H, W, kh, kw, 1, ph, pw, dh, dw_), x_in, C, d_out, C, 0, N, dw, lay, db)
+    if db is not None:
+        run_colsum(d_out, C, 0, db)
     return dw, db
 
 
@@ -1135,10 +1149,9 @@ def nb1d_storage_dtype(x, dil):
         return torch.float32
     N, H, W, C = x.shape
     if super_ok(x, dil):
-        ok = _lib().lf_wgrad3_tc_bf16_ctas(N, H, W // SUPER, SUPER * C) > 0
+        ok = wgrad3_tcg_ok(N, H, W // SUPER, SUPER * C)
     else:
-        ok = (all(tc_supported(x, v, d) for v in (True, False) for d in (1, dil))
-              and _lib().lf_wgrad3_tc_bf16_ctas(N, H, W, C) > 0)
+        ok = all(tc_supported(x, v, d) for v in (True, False) for d in (1, dil)) and wgrad3_tcg_ok(N, H, W, C)
     return torch.bfloat16 if ok else torch.float32
 
 

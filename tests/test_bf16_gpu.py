@@ -269,8 +269,8 @@ def test_bf16_heads_dense_convolutions(Ci, Co, k):
 @pytest.mark.parametrize("C", [64, 128])
 @pytest.mark.parametrize("vertical", [True, False])
 @pytest.mark.parametrize("dil", [1, 2, 4, 8, 16])
-def test_bf16_wgrad3_exact_operands(C, vertical, dil):
-    """lf_wgrad3_tc_bf16 vs torch-CPU fp64 autograd."""
+def test_bf16_wgrad3_tcg_exact_operands(C, vertical, dil):
+    """The bf16 3-tap weight gradient (lf_wgrad_tcg precision 2, traced as lf_wgrad3_tc_bf16) vs torch-CPU fp64 autograd."""
     o = ops()
     g = torch.Generator().manual_seed(C + dil + 100 * vertical)
     N, H, W = 2, 32, 64
@@ -278,7 +278,7 @@ def test_bf16_wgrad3_exact_operands(C, vertical, dil):
     dy = bx(torch.randn(N, H, W, C, generator=g)).cuda()
     kh, kw = (3, 1) if vertical else (1, 3)
     w = torch.zeros(C, C, kh, kw, device="cuda")
-    assert in_mode("bf16", lambda: o._lib().lf_wgrad3_tc_bf16_ctas(N, H, W, C)) > 0
+    assert in_mode("bf16", lambda: o.wgrad3_tcg_ok(N, H, W, C))
     dw, db = in_mode("bf16", lambda: o.wgrad3(x, dy, w, vertical, dil))
     wd = torch.zeros(C, C, kh, kw, dtype=torch.float64, requires_grad=True)
     pad = (dil, 0) if vertical else (0, dil)

@@ -131,7 +131,8 @@ def test_bf16_storage_c16_super_pixel_layers(bf16, vertical):
 @pytest.mark.parametrize("vertical", [True, False])
 @pytest.mark.parametrize("dil", DILS)
 def test_bf16a_weight_gradient_equals_fp32_a(bf16, C, vertical, dil):
-    """lf_wgrad3_tc_bf16a (bf16 layer input, fp32 output gradient) == lf_wgrad3_tc_bf16 on the fp32 copy."""
+    """The 3-tap weight gradient with a bf16 A view (bf16 layer input, fp32 output gradient; traced as lf_wgrad3_tc_bf16a) ==
+    the one on the fp32 copy."""
     from lanedetection_end2end_b200 import _capi
     o = bf16
     x, w, _, (dy, _) = _case(C, 32, 64, vertical, 7 * C + dil + vertical)

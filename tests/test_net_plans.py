@@ -320,15 +320,18 @@ def test_tcg_pair_pixel_forms_match_torch_convs(monkeypatch):
 
 def _emulate_wgrad_tcg(a, tensors):
     """CPU restatement of the lf_wgrad_tcg contract: every CTA's partial holds 1/nctas of the total (so that the
-    reduction that follows is exercised), computed in fp64."""
+    reduction that follows is exercised), computed in fp64.  The A views hold elements of a.a_dtype, B is fp32."""
+    from lanedetection_end2end_b200 import _capi
+
     def locate(ptr):
         for t in tensors:
-            if t.data_ptr() <= ptr < t.data_ptr() + t.numel() * 4:
-                return t, (ptr - t.data_ptr()) // 4
+            if t.data_ptr() <= ptr < t.data_ptr() + t.numel() * t.element_size():
+                return t, (ptr - t.data_ptr()) // t.element_size()
         raise AssertionError("pointer outside the known tensors")
 
-    def gather(v, dy, dx, c0, nc):
+    def gather(v, dy, dx, c0, nc, dtype):
         base, off = locate(v.ptr)
+        assert base.dtype == dtype, (base.dtype, dtype)
         flat = base.reshape(-1).double()
         ys, xs = torch.arange(a.Hs) + dy, torch.arange(a.Ws) + dx
         ok = ((ys >= 0) & (ys < v.H)).view(1, -1, 1, 1) & ((xs >= 0) & (xs < v.W)).view(1, 1, -1, 1)
@@ -336,17 +339,29 @@ def _emulate_wgrad_tcg(a, tensors):
                + xs.clamp(0, v.W - 1).view(1, 1, -1, 1) * v.sx + (c0 + torch.arange(nc)).view(1, 1, 1, -1))
         return flat[idx] * ok
 
-    B = gather(a.b, 0, 0, 0, a.Nn)
+    a_dtype = {_capi.LF_F32: torch.float32, _capi.LF_BF16: torch.bfloat16}[a.a_dtype]
+    B = gather(a.b, 0, 0, 0, a.Nn, torch.float32)
     D = torch.zeros(a.nblocks * 32, a.Nn, dtype=torch.float64)
     for blk in range(a.nblocks):
-        A = gather(a.a[a.map[blk]], a.dy[blk], a.dx[blk], a.cblk[blk] * 32, 32)
+        A = gather(a.a[a.map[blk]], a.dy[blk], a.dx[blk], a.cblk[blk] * 32, 32, a_dtype)
         D[blk * 32:(blk + 1) * 32] = torch.einsum("nyxc,nyxo->co", A, B)
     pt, poff = locate(a.partial)
     part = pt.reshape(-1)[poff:poff + a.nctas * D.numel()].view(a.nctas, *D.shape)
     part[:] = (D / a.nctas).float()
 
 
-def test_tcg_weight_gradients_match_torch(monkeypatch):
+def _emulate_wgrad_reduce(args, tensors):
+    """CPU restatement of lf_wgrad_reduce: dst[t*st + p*sp + q*sq] = sum over splits of partial[s][t][p][q]."""
+    partial, nsplit, ntaps, cp, cq, cpp, cqp, dst, st_, sp, sq, _stream = args
+    src = next(t for t in tensors if t.data_ptr() == partial)
+    red = src.reshape(-1)[:nsplit * ntaps * cpp * cqp].view(nsplit, ntaps, cpp, cqp)[:, :, :cp, :cq].double().sum(0).float()
+    res = next(t for t in tensors if t.data_ptr() <= dst < t.data_ptr() + t.numel() * 4)
+    idx = ((dst - res.data_ptr()) // 4 + torch.arange(ntaps).view(-1, 1, 1) * st_ + torch.arange(cp).view(1, -1, 1) * sp
+           + torch.arange(cq).view(1, 1, -1) * sq)
+    res.reshape(-1)[idx.reshape(-1)] = red.reshape(-1)
+
+
+def test_tcg_weight_gradients_through_one_launcher_match_torch(monkeypatch):
     """wgrad_tcg_conv / wgrad_tcg_convT (pair-pixel taps, block lists, split launches, partial reduction, final gather)
     against autograd's weight gradients of the stride-2 Conv2d / ConvTranspose2d, with the kernel replaced by a literal
     restatement of its contract."""
@@ -357,19 +372,15 @@ def test_tcg_weight_gradients_match_torch(monkeypatch):
 
     class FakeLib:
         @staticmethod
-        def lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks):
+        def lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, min_patches):
+            assert min_patches == 4
             return 3 if ((nblocks + 3) // 4) * Nn <= 512 else 0
 
     def fake_call(name, *args, **kw):
         if name == "lf_wgrad_tcg":
             _emulate_wgrad_tcg(args[0]._obj, live)
         elif name == "lf_wgrad_reduce":
-            partial, nsplit, ntaps, cp, cq, cpp, cqp, dst, st_, sp, sq, _stream = args
-            src = next(t for t in live if t.data_ptr() == partial)
-            red = src.view(nsplit, cp, cq).double().sum(0).float()
-            res = next(t for t in live if t.data_ptr() <= dst < t.data_ptr() + t.numel() * 4)
-            off = (dst - res.data_ptr()) // 4
-            res.reshape(-1)[off:off + cp * cq] = red.reshape(-1)
+            _emulate_wgrad_reduce(args, live)
         else:
             raise AssertionError(name)
 
@@ -410,7 +421,7 @@ def test_tcg_weight_gradients_match_torch(monkeypatch):
         assert torch.allclose(dw.double(), w.grad, atol=1e-4, rtol=1e-5), (I, O)
 
 
-def test_heads_dense_conv_forms_match_torch(monkeypatch):
+def test_heads_dense_conv_and_wgrad_tcg_forms_match_torch(monkeypatch):
     """ops_heads: the Classification heads' 1x1 / 3x3 stride-1 convolutions, their input gradients and weight gradients are
     expressed as run-time-tap launches of lf_conv_tcg / lf_wgrad_tcg (tap lists, packed operands, split launches, the final
     view / permute).  Run that host code on the CPU with the two kernels replaced by literal restatements of their contracts
@@ -425,7 +436,8 @@ def test_heads_dense_conv_forms_match_torch(monkeypatch):
             return 1
 
         @staticmethod
-        def lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks):
+        def lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, min_patches):
+            assert min_patches == 4
             return 3 if ((nblocks + 3) // 4) * Nn <= 512 else 0
 
     def fake_call(name, *args, **kw):
@@ -434,12 +446,7 @@ def test_heads_dense_conv_forms_match_torch(monkeypatch):
         elif name == "lf_wgrad_tcg":
             _emulate_wgrad_tcg(args[0]._obj, live)
         elif name == "lf_wgrad_reduce":
-            partial, nsplit, ntaps, cp, cq, cpp, cqp, dst, st_, sp, sq, _stream = args
-            src = next(t for t in live if t.data_ptr() == partial)
-            red = src.view(nsplit, cp, cq).double().sum(0).float()
-            res = next(t for t in live if t.data_ptr() <= dst < t.data_ptr() + t.numel() * 4)
-            off = (dst - res.data_ptr()) // 4
-            res.reshape(-1)[off:off + cp * cq] = red.reshape(-1)
+            _emulate_wgrad_reduce(args, live)
         else:
             raise AssertionError(name)
 
@@ -453,7 +460,7 @@ def test_heads_dense_conv_forms_match_torch(monkeypatch):
     monkeypatch.setattr(o, "_stream", lambda: None)
     monkeypatch.setattr(o, "_lib", lambda: FakeLib)
     monkeypatch.setattr(_capi, "lib", lambda: FakeLib)
-    monkeypatch.setattr(hd, "ptr", lambda t: t.data_ptr() if t is not None else None)
+    monkeypatch.setattr(o, "ptr", lambda t: t.data_ptr() if t is not None else None)
     monkeypatch.setattr(_capi, "call", fake_call)
     monkeypatch.setattr(o, "CONV_MODE", "tf32")            # single operands (the hi/lo split is a pure re-encoding of the same matrix)
     monkeypatch.setattr(torch, "empty", tracking_empty)
@@ -483,3 +490,76 @@ def _keep(live, t):
     """Register a freshly packed operand so that the emulators can resolve its pointer."""
     live.append(t)
     return t
+
+
+def test_wgrad3_matches_torch(monkeypatch):
+    """ops_net.wgrad3 on its tensor-core route (the 3-tap block table, the super-pixel view of C = 16 and its unpacking,
+    the reduction into the [Co,Ci,3] weight layout, a bf16 A view) against fp64 autograd, with lf_wgrad_tcg replaced by a
+    literal restatement of its contract; per mode also the launch's precision, its trace label and the split policy (at
+    least 8 patches per CTA for the 3xTF32 weight gradients, 4 otherwise)."""
+    import torch.nn.functional as F
+    from lanedetection_end2end_b200 import ops_net as o, _capi
+    live, launches = [], []
+
+    class FakeLib:
+        @staticmethod
+        def lf_wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nblocks, min_patches):
+            launches.append(("ctas", min_patches))
+            return 3 if ((nblocks + 3) // 4) * Nn <= 512 else 0
+
+        @staticmethod
+        def lf_conv1d_tc_supported(N, H, W, C):
+            return 1
+
+        @staticmethod
+        def lf_conv1d_tc_x3_rows(N, H, W, C, vertical, dil):
+            return 1
+
+    def fake_call(name, *args, **kw):
+        if name == "lf_wgrad_tcg":
+            launches.append((kw["label"], args[0]._obj.precision))
+            _emulate_wgrad_tcg(args[0]._obj, live)
+        elif name == "lf_wgrad_reduce":
+            _emulate_wgrad_reduce(args, live)
+        else:
+            raise AssertionError(name)
+
+    def tracking(fn):
+        def alloc(*a_, **kw):
+            t = fn(*a_, **kw)
+            live.append(t)
+            return t
+        return alloc
+
+    monkeypatch.setattr(o, "_stream", lambda: None)
+    monkeypatch.setattr(o, "_lib", lambda: FakeLib)
+    monkeypatch.setattr(o, "ptr", lambda t: t.data_ptr() if t is not None else None)
+    monkeypatch.setattr(_capi, "call", fake_call)
+    monkeypatch.setattr(torch, "empty", tracking(torch.empty))
+    monkeypatch.setattr(torch, "empty_like", tracking(torch.empty_like))
+    g = torch.Generator().manual_seed(5)
+    # (mode, single-pass weight gradients, layer input dtype) -> (precision, trace label, fewest patches per CTA)
+    modes = {("tf32", False, torch.float32): (0, "lf_wgrad3_tc", 4),
+             ("tf32x3", False, torch.float32): (1, "lf_wgrad3_tc_x3", 8),
+             ("tf32x3", True, torch.float32): (0, "lf_wgrad3_tc", 4),
+             ("bf16", False, torch.float32): (2, "lf_wgrad3_tc_bf16", 4),
+             ("bf16", False, torch.bfloat16): (2, "lf_wgrad3_tc_bf16a", 4)}
+    for (mode, single, dtype), (prec, label, min_patches) in modes.items():
+        monkeypatch.setattr(o, "CONV_MODE", mode)
+        monkeypatch.setattr(o, "WGRAD_SINGLE_PASS", single)
+        for (C, vertical, dil) in [(64, True, 1), (64, False, 2), (128, True, 2), (128, False, 1), (16, True, 1), (16, False, 1)]:
+            N, H, W = 2, 8, 16
+            x = torch.randn(N, H, W, C, generator=g).to(dtype)
+            dy = torch.randn(N, H, W, C, generator=g)
+            kh, kw = (3, 1) if vertical else (1, 3)
+            w = torch.zeros(C, C, kh, kw)
+            live[:] = [x, dy]
+            launches.clear()
+            dw, db = o.wgrad3(x, dy, w, vertical, dil, bias_grad="skip")
+            assert db is None and launches[-1] == (label, prec), (mode, C, launches)
+            assert {m for kind, m in launches if kind == "ctas"} == {min_patches}, (mode, C, launches)
+            wd = torch.zeros(C, C, kh, kw, dtype=torch.float64, requires_grad=True)
+            pad, dl = ((dil, 0), (dil, 1)) if vertical else ((0, dil), (1, dil))
+            F.conv2d(x.double().permute(0, 3, 1, 2), wd, None, 1, pad, dl).backward(dy.double().permute(0, 3, 1, 2))
+            assert dw.shape == w.shape and torch.allclose(dw.double(), wd.grad, atol=1e-4, rtol=1e-5), (mode, dtype, C,
+                                                                                                           vertical, dil)

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Diagnostic (GPU): non_bottleneck_1d(128, dil) at 32x64 in tf32x3 and fp32 modes vs the fp64 oracle: per-parameter gradient
-errors, ReLU-flip counts, and the x3-vs-fp32 difference; plus lf_wgrad3_tc_x3 alone on the block's own (t3, d4) operands."""
+errors, ReLU-flip counts, and the x3-vs-fp32 difference; plus the 3xTF32 weight gradient (ops_net.wgrad3) alone on the
+block's own (t3, d4) operands."""
 import json
 import os
 import sys
