@@ -377,7 +377,8 @@ int lf_conv_tcg(const LfConvTcgArgs* args, lf_stream_t stream);
 /* Weight gradients on tensor cores (csrc/wgrad_tcg.cu), over the views above -- of these layers, of the Classification
  * heads' stride-1 convolutions and of the factorised 3-tap convolutions of non_bottleneck_1d:
  *   D[blk*32 + c][n] = sum_{img,y,x} A_{map[blk]}(img, y+dy[blk], x+dx[blk], cblk[blk]*32 + c) * B(img, y, x, n)
- * for blk < nblocks (<= LF_WGRAD_TCG_MAX_BLOCKS), c < 32, n < Nn (multiple of 32, <= 128; ceil(nblocks/4)*Nn <= 512).
+ * for blk < nblocks (<= LF_WGRAD_TCG_MAX_BLOCKS, any Nn: a CTA takes one pair of blocks), c < 32, n < Nn (multiple of
+ * 32, <= 128).
  * partial: [nctas][nblocks*32][Nn] per-CTA partial sums; reduce with lf_wgrad_reduce (ntaps = 1, Cp = nblocks*32, Cq = Nn),
  * then gather into [Co,Ci,3,3] (ops_net.wgrad_tcg_*), or for a 3-tap convolution with blk = t*C/32 + cb
  * (ntaps = 3, Cp = Cq = C) straight into the weight layout.

@@ -326,7 +326,10 @@ def run_wgrad_tcg(av, bv, blocks, N, Hs, Ws, Ka, Nn, device, a_dtype=_capi.LF_F3
 
 
 def wgrad_tcg_taps_per_launch(N, Hs, Ws, Ka, Nn, candidates):
-    """The first tap count of `candidates` whose block table (Ka/32 blocks per tap) one lf_wgrad_tcg launch takes, 0 = none."""
+    """The first tap count of `candidates` whose block table (Ka/32 blocks per tap) one lf_wgrad_tcg launch takes, 0 = none.
+    lf_wgrad_tcg takes up to 24 blocks at any Nn; the launches here stay at ceil(blocks/4)*Nn <= 512 (at most 16 blocks at
+    Nn = 128), a split policy: the Upsampler's 24-block table at Nn = 128 in one launch was not faster than in two on an
+    H100, and the split count fixes the order in which the partials are summed."""
     for tpl in candidates:
         nb = tpl * (Ka // 32)
         if ((nb + 3) // 4) * Nn <= 512 and nb <= _capi.WGRAD_TCG_MAX_BLOCKS and wgrad_tcg_ctas(N, Hs, Ws, Ka, Nn, nb) > 0:

@@ -8,6 +8,9 @@ import torch.nn.functional as F
 
 from lanedetection_end2end_b200 import net_plans as plans
 from lanedetection_end2end_b200 import ops_net as ops
+from tcg_contract import emulate_conv_tcg as _emulate_conv_tcg
+from tcg_contract import emulate_wgrad_reduce as _emulate_wgrad_reduce
+from tcg_contract import emulate_wgrad_tcg as _emulate_wgrad_tcg
 
 torch.manual_seed(0)
 DT = torch.float64
@@ -225,41 +228,6 @@ def test_weight_pack_gather_tables_reproduce_every_packer():
         assert torch.equal(got, ref), (fn, shape)
 
 
-def _emulate_conv_tcg(a, tensors):
-    """CPU restatement of the lf_conv_tcg contract (include/lanefit_b200.h) on the exact views / strides the host
-    code put into LfConvTcgArgs; `tensors` = the CPU tensors the pointers refer to."""
-    def locate(ptr):
-        for t in tensors:
-            if t.data_ptr() <= ptr < t.data_ptr() + t.numel() * 4:
-                return t, (ptr - t.data_ptr()) // 4
-        raise AssertionError("pointer outside the known tensors")
-
-    K = a.ntaps * a.Kc
-    wt, woff = locate(a.wg)
-    Wg = wt.reshape(-1)[woff:woff + a.Ng * K].view(a.Ng, K).double()
-    acc = torch.zeros(a.N, a.Hs, a.Ws, a.Ng, dtype=torch.float64)
-    for t in range(a.ntaps):
-        v = a.a[a.map[t]]
-        base, off = locate(v.ptr)
-        # as_strided must stay inside the storage: gather explicitly with bounds checks (zero outside [0,H)x[0,W))
-        flat = base.reshape(-1).double()
-        ys = torch.arange(a.Hs) + a.dy[t]
-        xs = torch.arange(a.Ws) + a.dx[t]
-        ok = ((ys >= 0) & (ys < v.H)).view(1, -1, 1, 1) & ((xs >= 0) & (xs < v.W)).view(1, 1, -1, 1)
-        idx = (off + torch.arange(a.N).view(-1, 1, 1, 1) * v.sn + ys.clamp(0, v.H - 1).view(1, -1, 1, 1) * v.sy
-               + xs.clamp(0, v.W - 1).view(1, 1, -1, 1) * v.sx + torch.arange(a.Kc).view(1, 1, 1, -1))
-        A = flat[idx] * ok
-        acc += torch.einsum("nyxk,ck->nyxc", A, Wg[:, t * a.Kc:(t + 1) * a.Kc])
-    if a.bias:
-        bt, boff = locate(a.bias)
-        acc += bt.reshape(-1)[boff:boff + a.Ng].double()
-    ot, ooff = locate(a.out)
-    oflat = ot.reshape(-1)
-    oidx = (ooff + torch.arange(a.N).view(-1, 1, 1, 1) * a.osn + (torch.arange(a.Hs) * a.oy_mul + a.oy0).view(1, -1, 1, 1) * a.osy
-            + torch.arange(a.Ws).view(1, 1, -1, 1) * a.osx + torch.arange(a.Ng).view(1, 1, 1, -1))
-    oflat[oidx.reshape(-1)] = acc.reshape(-1).float()
-
-
 def test_tcg_pair_pixel_forms_match_torch_convs(monkeypatch):
     """The four layer forms served by lf_conv_tcg (Down forward / input gradient, Up forward / input gradient) are
     re-expressed as unit-stride gathers over pair-pixel / row-parity views.  Run the host code on CPU with the kernel
@@ -316,49 +284,6 @@ def test_tcg_pair_pixel_forms_match_torch_convs(monkeypatch):
         xin = x.permute(0, 3, 1, 2).double().requires_grad_(True)
         F.conv_transpose2d(xin, w.double(), stride=2, padding=1, output_padding=1).backward(du.permute(0, 3, 1, 2).double())
         assert torch.allclose(dx.double(), xin.grad.permute(0, 2, 3, 1), atol=1e-5), (I, O)
-
-
-def _emulate_wgrad_tcg(a, tensors):
-    """CPU restatement of the lf_wgrad_tcg contract: every CTA's partial holds 1/nctas of the total (so that the
-    reduction that follows is exercised), computed in fp64.  The A views hold elements of a.a_dtype, B is fp32."""
-    from lanedetection_end2end_b200 import _capi
-
-    def locate(ptr):
-        for t in tensors:
-            if t.data_ptr() <= ptr < t.data_ptr() + t.numel() * t.element_size():
-                return t, (ptr - t.data_ptr()) // t.element_size()
-        raise AssertionError("pointer outside the known tensors")
-
-    def gather(v, dy, dx, c0, nc, dtype):
-        base, off = locate(v.ptr)
-        assert base.dtype == dtype, (base.dtype, dtype)
-        flat = base.reshape(-1).double()
-        ys, xs = torch.arange(a.Hs) + dy, torch.arange(a.Ws) + dx
-        ok = ((ys >= 0) & (ys < v.H)).view(1, -1, 1, 1) & ((xs >= 0) & (xs < v.W)).view(1, 1, -1, 1)
-        idx = (off + torch.arange(a.N).view(-1, 1, 1, 1) * v.sn + ys.clamp(0, v.H - 1).view(1, -1, 1, 1) * v.sy
-               + xs.clamp(0, v.W - 1).view(1, 1, -1, 1) * v.sx + (c0 + torch.arange(nc)).view(1, 1, 1, -1))
-        return flat[idx] * ok
-
-    a_dtype = {_capi.LF_F32: torch.float32, _capi.LF_BF16: torch.bfloat16}[a.a_dtype]
-    B = gather(a.b, 0, 0, 0, a.Nn, torch.float32)
-    D = torch.zeros(a.nblocks * 32, a.Nn, dtype=torch.float64)
-    for blk in range(a.nblocks):
-        A = gather(a.a[a.map[blk]], a.dy[blk], a.dx[blk], a.cblk[blk] * 32, 32, a_dtype)
-        D[blk * 32:(blk + 1) * 32] = torch.einsum("nyxc,nyxo->co", A, B)
-    pt, poff = locate(a.partial)
-    part = pt.reshape(-1)[poff:poff + a.nctas * D.numel()].view(a.nctas, *D.shape)
-    part[:] = (D / a.nctas).float()
-
-
-def _emulate_wgrad_reduce(args, tensors):
-    """CPU restatement of lf_wgrad_reduce: dst[t*st + p*sp + q*sq] = sum over splits of partial[s][t][p][q]."""
-    partial, nsplit, ntaps, cp, cq, cpp, cqp, dst, st_, sp, sq, _stream = args
-    src = next(t for t in tensors if t.data_ptr() == partial)
-    red = src.reshape(-1)[:nsplit * ntaps * cpp * cqp].view(nsplit, ntaps, cpp, cqp)[:, :, :cp, :cq].double().sum(0).float()
-    res = next(t for t in tensors if t.data_ptr() <= dst < t.data_ptr() + t.numel() * 4)
-    idx = ((dst - res.data_ptr()) // 4 + torch.arange(ntaps).view(-1, 1, 1) * st_ + torch.arange(cp).view(1, -1, 1) * sp
-           + torch.arange(cq).view(1, 1, -1) * sq)
-    res.reshape(-1)[idx.reshape(-1)] = red.reshape(-1)
 
 
 def test_tcg_weight_gradients_through_one_launcher_match_torch(monkeypatch):
