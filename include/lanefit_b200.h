@@ -603,6 +603,22 @@ int lf_png_decode(const void* blob, int N, int W, int H, unsigned char* out, int
 int lf_label_preprocess(const unsigned char* maps, int N, int Hin, int Win, int crop_y0, const int* xs, const int* ys, int Ho,
                         int Wo, int nclasses, const unsigned char* flip, long long* out, lf_stream_t stream);
 
+/* TuSimple test-set scoring of one batch (csrc/tusimple.cu; replaces the lane gating of BP/test.py:66-89 and
+ * LaneEval.bench of BP/eval_lane.py:27-57): one launch, no host synchronisation, graph-capturable.
+ *   x_cal [B][P][S] f64: Projections.compute_all's output (1280-wide pixels); line_pred [B][4] f32: the rounded sigmoid in the
+ *   head's order (the launch applies the reference's [1, 2, 0, 3] permutation; needs P == 4), or NULL; horizon_pred [B] int32
+ *   (720p rows), or NULL.
+ *   Ground-truth table of the whole file (N rows, table width G <= LF_TUSIMPLE_MAX_GT lanes): gt_x [N][G][S] int32,
+ *   gt_lanes [N] (lanes per row), thresh [N][G] f64 (20 / cos(arctan(k)) of each lane, LaneEval.get_angle's value).
+ *   pos: device int32, the file row of slot 0.  Rows pos .. min(pos + B, N) - 1 are scored; *pos += B afterwards.
+ *   lanes [N][P][S] int32: the gated, rounded lanes the reference writes into its JSON (-2 = no point; a NaN becomes -2);
+ *   per_image [N][3] f64: (accuracy, fp, fn) of each row as LaneEval.bench returns them, bit-identical. */
+#define LF_TUSIMPLE_MAX_GT 8
+#define LF_TUSIMPLE_MAX_S 64
+int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* horizon_pred, int B, int P, int S, const int* gt_x,
+                      const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes, double* per_image,
+                      lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -152,7 +152,11 @@ class LfPngImage(ctypes.Structure):
                 ("raw_off", _ll)]
 
 
+TUSIMPLE_MAX_GT = 8
+TUSIMPLE_MAX_S = 64
+
 _NET_PROTOS = {
+    "lf_tusimple_score": (_i, [_p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "lf_png_workspace_bytes": (_c_size_t, [_p, _i]),
     "lf_png_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p]),
     "lf_label_preprocess": (_i, [_p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _p, _p]),

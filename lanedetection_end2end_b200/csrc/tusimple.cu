@@ -1,0 +1,122 @@
+// TuSimple test-set scoring of one batch in one launch (replaces BP/test.py:66-99 and LaneEval.bench of
+// BP/eval_lane.py:27-57 for the rows of that batch):
+//
+//   gate   lane j -> -2 when 1 - line_pred[perm[j]] != 0 (perm = [1, 2, 0, 3]); the first max(int((h - 160) / 10), 0)
+//          samples -> -2; values > 1279 or < 0 -> -2 (before rounding); the rest rounded half to even (np.round)
+//   score  per ground-truth lane g: max over predictions p of the line accuracy (#samples with |p' - g'| < thresh[g]) / S,
+//          where a negative sample counts as -100; matched when >= 0.85.  (a, fp, fn) as LaneEval.bench forms them, the
+//          lane sum sequential in lane order, float64.
+//
+// The ground-truth angle thresholds depend on the ground truth alone and come in precomputed (inference.TuSimpleScorer,
+// bit-identical to LaneEval.get_angle); everything here is integer counting, compares and a few float64 additions and
+// divisions, so the result equals LaneEval's bit for bit.  One CTA per launch, one warp per image: a latency-bound launch.
+// The batch covers file rows pos .. pos + B - 1; rows >= N are not scored, and the launch advances *pos by B so a
+// captured graph can be replayed once per batch.
+#include "lf_common.cuh"
+
+namespace lf {
+
+constexpr int TS_WARPS = 8;
+constexpr int TS_MAXP = 4;      // predicted lanes (the reference's 4-lane --clas model)
+
+__global__ void __launch_bounds__(TS_WARPS * 32) tusimple_score_kernel(
+    const double* __restrict__ x_cal, const float* __restrict__ line_pred, const int* __restrict__ horizon_pred, int B, int P,
+    int S, const int* __restrict__ gt_x, const int* __restrict__ gt_lanes, const double* __restrict__ thresh, int N, int G,
+    int* pos, int* __restrict__ lanes, double* __restrict__ per_image) {
+    pdl_entry();
+    __shared__ int s_pred[TS_WARPS][TS_MAXP * LF_TUSIMPLE_MAX_S];
+    __shared__ double s_acc[TS_WARPS][LF_TUSIMPLE_MAX_GT * TS_MAXP];
+    __shared__ long long s_pos;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) s_pos = *pos;
+    __syncthreads();
+    const long long p0 = s_pos;
+    for (int b = warp; b < B; b += TS_WARPS) {
+        const long long row = p0 + b;
+        if (row < 0 || row >= N) continue;
+        // ---- gating (lanes_from_predictions): the same compares on the same float32 / float64 values
+        int cut = 0;
+        if (horizon_pred) {
+            const float bound = (float)(horizon_pred[b] - 160) / 10.0f;     // torch true division of an int32 tensor
+            cut = bound >= (float)S ? S : (bound >= 1.0f ? (int)bound : 0);  // max(int(bound), 0), capped by the slice
+        }
+        unsigned off = 0;       // bit p: lane p switched off by the line-type head
+        if (line_pred) {
+            const int perm[TS_MAXP] = {1, 2, 0, 3};
+#pragma unroll
+            for (int p = 0; p < TS_MAXP; ++p)
+                if (1.0f - line_pred[(size_t)b * TS_MAXP + perm[p]] != 0.0f) off |= 1u << p;
+        }
+        int* out = lanes + (size_t)row * P * S;
+        for (int i = lane; i < P * S; i += 32) {
+            const int p = i / S, s = i - p * S;
+            double v = x_cal[(size_t)b * P * S + i];
+            if (((off >> p) & 1u) || s < cut) v = -2.0;
+            // > 1279 or < 0 -> -2; NaN (a singular fit, reported through the LSQ status word) -> -2 as well
+            const int q = (v >= 0.0 && v <= 1279.0) ? __double2int_rn(v) : -2;
+            out[i] = q;
+            s_pred[warp][i] = q;
+        }
+        __syncwarp();
+        // ---- LaneEval.bench: one thread per (ground-truth lane, prediction) pair
+        const int g_n = min(max(gt_lanes[row], 0), G);
+        const bool early = g_n + 2 < P;           // LaneEval's early return (0, 0, 1)
+        if (!early && lane < g_n * P) {
+            const int g = lane / P, p = lane - g * P;
+            const int* gx = gt_x + ((size_t)row * G + g) * S;
+            const double th = thresh[(size_t)row * G + g];
+            int cnt = 0;
+            for (int s = 0; s < S; ++s) {
+                const long long pv = s_pred[warp][p * S + s] >= 0 ? s_pred[warp][p * S + s] : -100;
+                const long long gv = gx[s] >= 0 ? gx[s] : -100;
+                cnt += (double)llabs(pv - gv) < th ? 1 : 0;
+            }
+            s_acc[warp][lane] = (double)cnt / (double)S;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            double* r = per_image + (size_t)row * 3;
+            if (early) {
+                r[0] = 0.0;
+                r[1] = 0.0;
+                r[2] = 1.0;
+            } else {
+                double sum = 0.0, mn = 0.0, fn = 0.0, matched = 0.0;
+                for (int g = 0; g < g_n; ++g) {
+                    double m = s_acc[warp][g * P];
+                    for (int p = 1; p < P; ++p) m = s_acc[warp][g * P + p] > m ? s_acc[warp][g * P + p] : m;
+                    if (m < 0.85) fn += 1.0;
+                    else matched += 1.0;
+                    sum += m;
+                    mn = (g == 0 || m < mn) ? m : mn;
+                }
+                const double fp = (double)P - matched;
+                if (g_n > 4 && fn > 0.0) fn -= 1.0;
+                if (g_n > 4) sum -= mn;
+                const double den = fmax(fmin(4.0, (double)g_n), 1.0);
+                r[0] = sum / den;
+                r[1] = fp / (double)P;
+                r[2] = fn / den;
+            }
+        }
+        __syncwarp();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *pos = (int)(p0 + B);
+}
+
+}  // namespace lf
+
+using namespace lf;
+
+extern "C" int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* horizon_pred, int B, int P, int S,
+                                 const int* gt_x, const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes,
+                                 double* per_image, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(x_cal && gt_x && gt_lanes && thresh && pos && lanes && per_image);
+    LF_REQUIRE(B > 0 && P >= 1 && P <= TS_MAXP && S >= 1 && S <= LF_TUSIMPLE_MAX_S && N > 0 && G >= 1 && G <= LF_TUSIMPLE_MAX_GT);
+    LF_REQUIRE(!line_pred || P == TS_MAXP);
+    lf_launch(tusimple_score_kernel, 1, TS_WARPS * 32, 0, stream, x_cal, line_pred, horizon_pred, B, P, S, gt_x, gt_lanes, thresh,
+              N, G, pos, lanes, per_image);
+    return check_launch();
+}

@@ -166,24 +166,31 @@ class GraphedInference:
     what the reference's validate() / test_model() loops do per batch (BP/main.py:452, BP/test.py:53-55), without the ~25 us
     of ctypes / Python per launch.  ``infer(x)`` copies the batch into the static input and replays; the returned 9-tuple
     (beta0..3, masked, output, line, horizon, output_seg) aliases static buffers that the next call overwrites.
-    ``model.lsq_status`` (device int32, OR-ed) reports singular systems; `check()` reads it (one sync)."""
+    ``model.lsq_status`` (device int32, OR-ed) reports singular systems; `check()` reads it (one sync).
+    ``post``: optional callable(9-tuple) captured right after the forward (and run by every warm-up pass); its return value
+    is ``self.post_out``, static like ``self.out``."""
 
-    def __init__(self, model, example_x, warmup=2):
+    def __init__(self, model, example_x, warmup=2, post=None):
         self.model = model.eval()
         model.defer_status_check = True
         self.x = example_x.clone()
         self.gt_line = torch.zeros(example_x.shape[0], 4)
+        self.post_out = None
         dev = example_x.device
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(max(1, warmup)):             # builds and caches the folded operands outside the capture
-                model(self.x, self.gt_line, True)
+                out = model(self.x, self.gt_line, True)
+                if post is not None:
+                    post(out)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(self.graph):
             self.out = model(self.x, self.gt_line, True)
+            if post is not None:
+                self.post_out = post(self.out)
 
     def infer(self, x):
         self.x.copy_(x, non_blocking=True)

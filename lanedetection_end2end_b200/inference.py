@@ -6,6 +6,11 @@ curve coefficients after ``model(input, ...)``.
   lanes_from_predictions     BP/test.py:66-86    gate lanes by the line-type / horizon heads, clip to the image
   write_tusimple_predictions BP/test.py:88-99    one JSON line per image in the TuSimple submission format
 
+  lane_threshold             eval_lane.py:15-24,39  LaneEval's per-lane pixel threshold, bit-identical
+  TuSimpleScorer             BP/test.py:66-99 + eval_lane.py:27-95  gating and LaneEval scoring on the GPU, one launch
+                                                 (lf_tusimple_score, csrc/tusimple.cu) per batch
+  test_model                 BP/test.py:23-129   the per-epoch test-set evaluation, one CUDA-graph replay per batch
+
 ``Projections.compute_coordinates`` keeps the reference's name, argument and result ([B, order+1, 1] float64 -> [B, 56]
 float64, in 1280x720 pixels); on a CUDA tensor it is ONE launch of lf_backproj_loss (csrc/loss.cu, the kernel that
 evaluates the training loss: same per-point code, x_cal output only) instead of two bmm's, a stack/permute and two
@@ -13,6 +18,7 @@ divisions; ``compute_all`` does all lanes of the batch in that one launch.
 """
 import ctypes
 import json
+import os
 
 import numpy as np
 import torch
@@ -23,6 +29,10 @@ if __package__:
 else:                                   # imported top-level next to the reference's main.py / test.py
     import _capi
     from Loss_crit import backprojection_loss
+
+TUSIMPLE_SAMPLES = 56                   # h_samples 160..710 step 10: what Projections predicts
+TUSIMPLE_LANES = 4                      # predicted lanes of the 4-lane --clas model
+PIXEL_THRESH = 20                       # LaneEval.pixel_thresh (pt_thresh 0.85 lives in the kernel)
 
 
 def resize_coordinates(array):
@@ -88,3 +98,199 @@ def write_tusimple_predictions(json_file, gt_lines, lanes_pred, first_index, run
         line["run_time"] = run_time
         json.dump(line, json_file)
         json_file.write("\n")
+
+
+def lane_threshold(xs, h_samples):
+    """LaneEval's pixel threshold of one ground-truth lane (eval_lane.py:15-24,39): 20 / cos(arctan(k)), k the slope of the
+    least-squares line x = k y + c through the samples with x >= 0 (theta 0 below two of them).  sklearn's LinearRegression
+    fits that line by centring y and x and calling scipy.linalg.lstsq; the same call here gives the same bits."""
+    import scipy.linalg
+    xs, ys = np.asarray(xs), np.asarray(h_samples)
+    keep = xs >= 0
+    theta = 0
+    if int(keep.sum()) > 1:
+        y = ys[keep].astype(np.float64)[:, None]
+        x = xs[keep].astype(np.float64)
+        y = y - np.average(y, axis=0)
+        x = x - np.average(x)
+        theta = np.arctan(scipy.linalg.lstsq(y, x, cond=1e-6)[0][0])
+    return float(PIXEL_THRESH / np.cos(theta))
+
+
+class TuSimpleScorer:
+    """The TuSimple metric of a test pass on the GPU (BP/test.py:66-99 then LaneEval.bench_one_submit, eval_lane.py:59-95).
+
+    Construction parses the ground truth (a test_label.json path or its parsed rows) once: every row must have 56
+    h_samples (the rows Projections predicts; TuSimple's 48-sample 0313 clips are rejected, as LaneEval rejects them), lanes
+    of len(h_samples) samples, at most 8 lanes and a unique raw_file; each lane's threshold is computed here
+    (lane_threshold).  ``score`` is one lf_tusimple_score launch per batch: it gates and rounds the batch's lanes exactly as
+    lanes_from_predictions does and scores them against rows pos .. pos + B - 1 exactly as LaneEval.bench does, then
+    advances pos by B on the device, so it can be captured into a CUDA graph and replayed once per batch.  ``result``
+    returns [accuracy, fp, fn] bit-identical to bench_one_submit on the file ``write_json`` writes."""
+
+    def __init__(self, gt_rows_or_path, device="cuda"):
+        if isinstance(gt_rows_or_path, (str, bytes, os.PathLike)):
+            with open(gt_rows_or_path) as f:
+                rows = [json.loads(line) for line in f.readlines()]
+        else:
+            rows = list(gt_rows_or_path)
+        N, G, S = len(rows), _capi.TUSIMPLE_MAX_GT, TUSIMPLE_SAMPLES
+        if N == 0:
+            raise ValueError("the ground truth has no rows")
+        gt_x = np.full((N, G, S), -2, np.int32)
+        gt_n = np.zeros(N, np.int32)
+        thresh = np.zeros((N, G), np.float64)
+        seen = set()
+        for i, row in enumerate(rows):
+            name = row.get("raw_file")
+            if name is None or "lanes" not in row or "h_samples" not in row:
+                raise ValueError("ground-truth row %d lacks raw_file, lanes or h_samples" % i)
+            if name in seen:
+                raise ValueError("%s: duplicate raw_file in the ground truth" % name)
+            seen.add(name)
+            h, lanes = row["h_samples"], row["lanes"]
+            if len(h) != S:
+                raise ValueError("%s: %d h_samples; the predictions have %d (LaneEval raises 'Format of lanes error')"
+                                 % (name, len(h), S))
+            if len(lanes) > G:
+                raise ValueError("%s: %d lanes, the table holds %d" % (name, len(lanes), G))
+            for j, lane in enumerate(lanes):
+                if len(lane) != len(h):
+                    raise ValueError("%s: lane %d has %d samples for %d h_samples" % (name, j, len(lane), len(h)))
+                arr = np.asarray(lane)
+                if arr.dtype.kind not in "iu" or arr.min() < -2 ** 31 or arr.max() >= 2 ** 31:
+                    raise ValueError("%s: lane %d holds values that are not int32 pixel columns" % (name, j))
+                gt_x[i, j] = arr
+                thresh[i, j] = lane_threshold(arr, h)
+            gt_n[i] = len(lanes)
+        dev = torch.device(device)
+        self.rows, self.N = rows, N
+        self.gt_x = torch.from_numpy(gt_x).to(dev)
+        self.gt_lanes = torch.from_numpy(gt_n).to(dev)
+        self.thresh = torch.from_numpy(thresh).to(dev)
+        self.lanes = torch.full((N, TUSIMPLE_LANES, S), -2, dtype=torch.int32, device=dev)
+        # per_image rows and pos share one buffer so that result() is one device-to-host copy
+        self._out = torch.zeros(N * 3 + 1, dtype=torch.float64, device=dev)
+        self.per_image = self._out[:N * 3].view(N, 3)
+        self.pos = self._out[N * 3:].view(torch.int32)[:1]
+
+    def score(self, x_cal, line_pred=None, horizon_pred=None):
+        """x_cal [B, 4, 56] float64 (Projections.compute_all), line_pred [B, 4] float32 in the head's order (rounded
+        sigmoid), horizon_pred [B] int32 (720p rows): one launch, no synchronisation."""
+        B = x_cal.shape[0]
+        if x_cal.dtype != torch.float64 or tuple(x_cal.shape[1:]) != (TUSIMPLE_LANES, TUSIMPLE_SAMPLES):
+            raise ValueError("x_cal must be float64 [B, %d, %d], got %s %s" % (TUSIMPLE_LANES, TUSIMPLE_SAMPLES, x_cal.dtype,
+                                                                               tuple(x_cal.shape)))
+        if line_pred is not None and (line_pred.dtype != torch.float32 or tuple(line_pred.shape) != (B, TUSIMPLE_LANES)):
+            raise ValueError("line_pred must be float32 [B, 4], got %s %s" % (line_pred.dtype, tuple(line_pred.shape)))
+        if horizon_pred is not None and (horizon_pred.dtype != torch.int32 or tuple(horizon_pred.shape) != (B,)):
+            raise ValueError("horizon_pred must be int32 [B], got %s %s" % (horizon_pred.dtype, tuple(horizon_pred.shape)))
+        _capi.require_cuda(x_cal, line_pred, horizon_pred)
+        c = lambda t: None if t is None else t.contiguous()
+        x_cal, line_pred, horizon_pred = c(x_cal), c(line_pred), c(horizon_pred)
+        p = _capi.ptr
+        _capi.call("lf_tusimple_score", p(x_cal), p(line_pred), p(horizon_pred), B, TUSIMPLE_LANES, TUSIMPLE_SAMPLES,
+                   p(self.gt_x), p(self.gt_lanes), p(self.thresh), self.N, _capi.TUSIMPLE_MAX_GT, p(self.pos), p(self.lanes),
+                   p(self.per_image), _capi.stream_ptr())
+
+    def reset(self):
+        """Start a new pass at file row 0 (on the current stream)."""
+        self.pos.zero_()
+
+    def result(self):
+        """[accuracy, fp, fn] of the pass as bench_one_submit returns them: the per-image rows summed in file order.  Raises
+        unless every row was scored."""
+        out = self._out.cpu().numpy()
+        scored = min(int(out[self.N * 3:].view(np.int32)[0]), self.N)
+        if scored != self.N:
+            raise RuntimeError("scored %d of the %d ground-truth rows: LaneEval needs a prediction for every test image"
+                               % (scored, self.N))
+        accuracy, fp, fn = 0., 0., 0.
+        for a, p, n in out[:self.N * 3].reshape(self.N, 3).tolist():
+            accuracy += a
+            fp += p
+            fn += n
+        return [accuracy / self.N, fp / self.N, fn / self.N]
+
+    def predictions(self):
+        """The gated integer lanes of every row (one copy), as lanes_from_predictions returns them."""
+        return self.lanes.cpu().tolist()
+
+    def write_json(self, json_file):
+        write_tusimple_predictions(json_file, self.rows, self.predictions(), 0)
+
+
+_SCORERS = {}           # (absolute path, device) -> (file stamp, TuSimpleScorer): one table build per ground-truth file
+
+
+def _scorer_for(gt_file, device):
+    st = os.stat(gt_file)
+    key, stamp = (os.path.abspath(gt_file), str(device)), (st.st_mtime_ns, st.st_size)
+    hit = _SCORERS.get(key)
+    if hit is None or hit[0] != stamp:
+        hit = _SCORERS[key] = (stamp, TuSimpleScorer(gt_file, device))
+    return hit[1]
+
+
+def test_model(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0):
+    """The reference's per-epoch test-set evaluation (BP/test.py:23-129), same signature and return value (the TuSimple
+    accuracy).  Reads args.test_dir/test_label.json, writes args.save_path/test_set_predictions.json.
+
+    Each batch is one CUDA-graph replay of the eval forward, the heads' post-processing (the reference's torch ops),
+    Projections.compute_all and TuSimpleScorer.score; the host only copies the batch into the static input (a shorter last
+    batch fills the leading slots and only its rows are scored).  Nothing synchronises until the end of the pass, where a
+    singular least-squares system raises the RuntimeError the reference raises at its batch, the file is written and the
+    accuracy line is printed.  Only the end-to-end 4-lane --clas model is scored, as in the reference; draw_testset (cv2
+    drawing) is not supported."""
+    if not (args.end_to_end and args.clas and args.nclasses == 4):
+        raise ValueError("test_model scores the end-to-end 4-lane --clas model (end_to_end=%s, clas=%s, nclasses=%s)"
+                         % (args.end_to_end, args.clas, args.nclasses))
+    if args.draw_testset:
+        raise NotImplementedError("draw_testset is not supported")
+    if __package__:
+        from .engine import GraphedInference
+    else:
+        from engine import GraphedInference
+    dev = next(model.parameters()).device
+    scorer = _scorer_for(os.path.join(args.test_dir, "test_label.json"), dev)
+    params = Projections(args)
+
+    def post(out):
+        horizon_pred = torch.sigmoid(out[7]).sum(dim=1)
+        horizon_pred = (torch.round((resize_coordinates(horizon_pred) + 80) / 10) * 10).int()
+        line_pred = torch.round(torch.sigmoid(out[6]))
+        scorer.score(params.compute_all(out[:4]), line_pred, horizon_pred)
+
+    deferred = model.defer_status_check
+    graph, images, batches = None, 0, 0
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    try:
+        with torch.no_grad():
+            for batch in loader:
+                n = batch.shape[0]
+                if graph is None:
+                    graph = GraphedInference(model, batch.to(dev, torch.float32), post=post)
+                    scorer.reset()
+                    model.lsq_status.zero_()
+                    start.record()
+                elif n > graph.x.shape[0]:
+                    raise ValueError("batch of %d images after a first batch of %d" % (n, graph.x.shape[0]))
+                graph.x[:n].copy_(batch, non_blocking=True)
+                graph.graph.replay()
+                images += n
+                batches += 1
+            end.record()
+        if graph is None:
+            raise ValueError("the test loader yielded no batch")
+        graph.check()
+    finally:
+        model.defer_status_check = deferred
+    if images != scorer.N:
+        raise RuntimeError("We do not get the predictions of all the test tasks: %d images for %d ground-truth rows"
+                           % (images, scorer.N))
+    with open(os.path.join(args.save_path, "test_set_predictions.json"), "w") as f:
+        scorer.write_json(f)
+    acc_seg = scorer.result()
+    print(acc_seg)
+    print("===> Average ACC on TESTSET is {:.8} in {:.6}s for a batch".format(acc_seg[0], start.elapsed_time(end) / 1e3 / batches))
+    return acc_seg[0]
