@@ -619,6 +619,33 @@ int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* ho
                       const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes, double* per_image,
                       lf_stream_t stream);
 
+/* The TuSimple loader's device cache (csrc/loader.cu; Dataloader/Load_Data_new.py of this package, replacing the per-sample
+ * work of BP/Dataloader/Load_Data_new.py:110-197 after decoding).  A cache is two slot-addressed uint8 buffers of resized,
+ * UNFLIPPED samples: frames [S][Ho][Wo][3] and label maps [S][Ho][Wo].
+ * lf_loader_stage: frames uint8 [N][Hin][Win][3] (decoded RGB) and maps uint8 [N][Hin][Win] (decoded label maps; NULL =
+ *   frames only, for a test set) -> rows [crop_y0, crop_y0+crop_rows) -> frame n into cache_frames[slots[n]] by Pillow's
+ *   BILINEAR (xb/xk/yb/yk as lf_frame_preprocess takes them) and map n into cache_maps[slots[n]] by Pillow's NEAREST (xs/ys
+ *   as lf_label_preprocess takes them).  slots: device int32 [N].  One launch; bit-identical to what lf_frame_preprocess /
+ *   lf_label_preprocess read before their flip.
+ * lf_loader_assemble: one collated batch, one launch.  sample: device int32 [N][3] = (slot, table row, flip).
+ *   image [N][3][Ho][Wo] f32 = cache_frames / 255 (__fdiv_rn, ToTensor's value), mirrored when flip != 0;
+ *   gt [N][1][Ho][Wo] int64 = the class rules of lf_label_preprocess (nclasses, flip, the 3 / 4 quirk) on the cached map;
+ *   per-row tables over nrows rows, flip state f = (flip != 0):
+ *     lanes [N][4][56] f64 = lanes_tab[f][row]   (lanes_tab [2][nrows][4][56])
+ *     valid [N][4][56] f64 = valid_tab[row]      (valid_tab [nrows][4][56]: not flipped, as the reference leaves it)
+ *     horizon [N][Ho] f32 = 1 for y < horizon_tab[row], else 0 (horizon_tab [nrows] int32)
+ *     line [N][4] f32 = line_tab[f][row]         (line_tab [2][nrows][4])
+ *   Every output may be NULL (not written); the tables and caches an output needs must not be.  Needs Ho * Wo >= 224. */
+#define LF_LOADER_LANES 4
+#define LF_LOADER_POINTS 56
+int lf_loader_stage(const unsigned char* frames, const unsigned char* maps, int N, int Hin, int Win, int crop_y0, int crop_rows,
+                    const int* xb, const int* xk, int kx, const int* yb, const int* yk, int ky, const int* xs, const int* ys, int Ho,
+                    int Wo, const int* slots, unsigned char* cache_frames, unsigned char* cache_maps, lf_stream_t stream);
+int lf_loader_assemble(const unsigned char* cache_frames, const unsigned char* cache_maps, int N, int Ho, int Wo, int nclasses,
+                       const int* sample, int nrows, const double* lanes_tab, const double* valid_tab, const int* horizon_tab,
+                       const float* line_tab, float* image, long long* gt, double* lanes, double* valid, float* horizon, float* line,
+                       lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,20 +6,14 @@
 // of it): a separable triangle filter widened by the down-scale factor, evaluated in FIXED POINT -- integer coefficients
 // (22 fractional bits), accumulator 2^21 + sum(pixel * coeff), clip8(acc >> 22), horizontal pass first with an 8-bit
 // intermediate, then the vertical pass.  The coefficient tables depend on the sizes only and are built once on the host
-// (input_pipeline.py, float64 like Pillow); the kernel does the integer arithmetic, so the result is bit-identical to
+// (input_pipeline.py, float64 like Pillow); the kernel does the integer arithmetic (resample.cuh, shared with the loader's
+// staging kernel in loader.cu), so the result is bit-identical to
 // PIL's (tests: tests/test_input_pipeline_*.py).  One thread = one output pixel (3 channels); the horizontal value of a
 // source row is recomputed by the ~2.5 output rows that use it (integer MACs on L1/L2-resident bytes; the kernel reads
 // each frame byte from HBM once: 2.4 MB per 1280x640 crop).
-#include "lf_common.cuh"
+#include "resample.cuh"
 
 namespace lf {
-
-constexpr int IP_BITS = 22;
-
-__device__ __forceinline__ int ip_clip8(int acc) {
-    const int v = acc >> IP_BITS;
-    return v < 0 ? 0 : (v > 255 ? 255 : v);
-}
 
 __global__ void __launch_bounds__(256) frame_preprocess_kernel(const uint8_t* __restrict__ frames, int N, int Hin, int Win, int y0,
                                                                const int* __restrict__ xb, const int* __restrict__ xk, int kx,
@@ -33,25 +27,9 @@ __global__ void __launch_bounds__(256) frame_preprocess_kernel(const uint8_t* __
         const int oy = (int)((idx / Wo) % Ho);
         const int n = (int)(idx / ((long long)Wo * Ho));
         const int sx = (flip && flip[n]) ? Wo - 1 - ox : ox;        // F.hflip of the resized image
-        const int xmin = __ldg(xb + 2 * sx), nx = __ldg(xb + 2 * sx + 1);
-        const int ymin = __ldg(yb + 2 * oy), ny = __ldg(yb + 2 * oy + 1);
-        int av0 = 1 << (IP_BITS - 1), av1 = av0, av2 = av0;
-        for (int j = 0; j < ny; ++j) {
-            const uint8_t* row = frames + ((size_t)((size_t)n * Hin + y0 + ymin + j) * Win + xmin) * 3;
-            int a0 = 1 << (IP_BITS - 1), a1 = a0, a2 = a0;
-            for (int i = 0; i < nx; ++i) {
-                const int k = __ldg(xk + sx * kx + i);
-                a0 += (int)row[3 * i] * k;
-                a1 += (int)row[3 * i + 1] * k;
-                a2 += (int)row[3 * i + 2] * k;
-            }
-            const int kyv = __ldg(yk + oy * ky + j);
-            av0 += ip_clip8(a0) * kyv;
-            av1 += ip_clip8(a1) * kyv;
-            av2 += ip_clip8(a2) * kyv;
-        }
-        const float r = __fdiv_rn((float)ip_clip8(av0), 255.f), g = __fdiv_rn((float)ip_clip8(av1), 255.f),
-                    b = __fdiv_rn((float)ip_clip8(av2), 255.f);
+        int c0, c1, c2;
+        ip_bilinear_rgb(frames + ((size_t)n * Hin + y0) * Win * 3, Win, xb, xk, kx, yb, yk, ky, sx, oy, c0, c1, c2);
+        const float r = __fdiv_rn((float)c0, 255.f), g = __fdiv_rn((float)c1, 255.f), b = __fdiv_rn((float)c2, 255.f);
         if (layout == 1) {   // NHWC, 3 channels padded to 4 (what the stem convolution reads)
             reinterpret_cast<float4*>(out)[idx] = make_float4(r, g, b, 0.f);
         } else {             // NCHW (what the reference's loader returns)
@@ -80,13 +58,8 @@ __global__ void __launch_bounds__(256) label_preprocess_kernel(const uint8_t* __
         const uint8_t* row = maps + ((size_t)n * Hin + y0 + __ldg(ys + oy)) * Win;
         const int v0 = row[__ldg(xs + ox)];
         const bool fl = flip && flip[n];
-        int v = fl ? row[__ldg(xs + Wo - 1 - ox)] : v0;
-        if (nclasses < 3 && (v == 3 || v == 4)) v = 0;
-        if (fl) {
-            v = v == 1 ? 2 : (v == 2 ? 1 : v);
-            v = v0 == 3 ? 4 : (v0 == 4 ? 3 : v);
-        }
-        out[idx] = v;
+        const int v = fl ? row[__ldg(xs + Wo - 1 - ox)] : v0;
+        out[idx] = ip_label_rules(v, v0, fl, nclasses);
     }
 }
 

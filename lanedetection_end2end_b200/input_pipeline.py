@@ -11,9 +11,9 @@ LabelPreprocessor does the same for the ground-truth label map (:129,131,160-184
 
     gt = LabelPreprocessor(256, nclasses=4)(maps_u8, flip=mask)   # [N,720,1280] uint8 cuda -> [N,1,256,512] int64
 
-Decoding is outside this module (jpeg.JpegDecoder and png.PngDecoder deliver the frames and maps); the lane labels of the
-loader (lane coordinates / 2.5, valid-point mask, horizon vector, line types; :133-160) are O(100) scalars per image and
-stay on the host."""
+Decoding is outside this module (jpeg.JpegDecoder and png.PngDecoder deliver the frames and maps).  Dataloader/Load_Data_new.py
+joins the decoders, these tables and the lane labels of the loader (lane coordinates / 2.5, valid-point mask, horizon
+vector, line types; :133-160) into a loader with a device cache (csrc/loader.cu)."""
 import math
 
 import numpy as np
