@@ -466,6 +466,11 @@ int lf_linear_bwd_weight(const float* dy, const float* relu_out, const float* x,
  * BP/main.py:258,307): target [B][H][W] int64, weight [C] or NULL; partial = 2*lf_ce2d_blocks() doubles of scratch, sums = 2
  * doubles (weighted loss sum, weight sum) kept for the backward, loss = 1 double; dx = gout * dloss/dx (gout NULL = 1). */
 int lf_seg_lane_maps(const float* out, int B, int C, int H, int W, int nl, int mask_rows, float* maps, lf_stream_t stream);
+/* lf_seg_lane_maps plus the gt_line substitution of BP/Networks/LSQ_layer.py:308-311 (`masked[gt_mask] = masked[0, 0]...`):
+ * gt_line [B][nl] float on the device, or NULL (then the output is lf_seg_lane_maps'); where gt_line[b][k] != 0, maps[b][k] is
+ * image 0 / lane 0's map as lf_seg_lane_maps computes it. */
+int lf_seg_lane_maps_line(const float* out, int B, int C, int H, int W, int nl, int mask_rows, const float* gt_line, float* maps,
+                          lf_stream_t stream);
 int lf_ce2d_blocks(int B, int H, int W);
 int lf_ce2d_fwd(const float* x, const long long* target, const float* weight, int B, int C, int H, int W, double* partial, double* sums,
                 double* loss, lf_stream_t stream);

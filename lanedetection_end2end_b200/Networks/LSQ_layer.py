@@ -233,14 +233,22 @@ class Net(nn.Module):
             # detached; fitted without gradient
             nl = 2 if self.nclasses < 3 else 4
             _capi.require_cuda(output)
-            # argmax + per-lane label maps + row mask in one launch (csrc/seg.cu: lf_seg_lane_maps)
+            # argmax + per-lane label maps + row mask + the gt_line substitution of :308-311 in one launch
+            # (csrc/seg.cu: lf_seg_lane_maps_line), with no host read of a device gt_line
             od = output.detach().contiguous().float()
-            masked = torch.empty(od.shape[0], nl, od.shape[2], od.shape[3], dtype=torch.float32, device=od.device)
-            _capi.call("lf_seg_lane_maps", _capi.ptr(od), od.shape[0], od.shape[1], od.shape[2], od.shape[3], nl,
-                       self.zero_rows, _capi.ptr(masked), _capi.stream_ptr())
-            if gt_line.sum() != 0:                                       # :308-311
-                gt_mask = gt_line[:, :, None, None].bool().expand_as(masked).to(masked.device)
-                masked[gt_mask] = masked[0, 0].unsqueeze(0).repeat(int(gt_line.sum().item()), 1, 1).view(-1)
+            B = od.shape[0]
+            masked = torch.empty(B, nl, od.shape[2], od.shape[3], dtype=torch.float32, device=od.device)
+            gl = gt_line
+            if not gl.is_cuda and not bool(gl.ne(0).any()):             # a host gt_line is checked on the host
+                gl = None
+            if gl is not None and tuple(gl.shape) != (B, nl):
+                # not one flag per map: the reference broadcasts its mask when gt_line is nonzero, and raises where it
+                # cannot (4 line flags for 2 lanes); this needs the host read the [B, nl] case avoids
+                gl = gl[:, :, None, None].expand_as(masked)[:, :, 0, 0] if gl.sum() != 0 else None
+            if gl is not None:
+                gl = gl.to(od.device, torch.float32, non_blocking=True).contiguous()
+            _capi.call("lf_seg_lane_maps_line", _capi.ptr(od), B, od.shape[1], od.shape[2], od.shape[3], nl,
+                       self.zero_rows, _capi.ptr(gl), _capi.ptr(masked), _capi.stream_ptr())
             with torch.no_grad():
                 beta, _ = self.ls_layer.forward_all(masked, grid, status_out=status, max_order=3)
         else:

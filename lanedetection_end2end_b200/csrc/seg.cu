@@ -2,6 +2,7 @@
 //  * lf_seg_lane_maps  -- BP/Networks/LSQ_layer.py:279-293,301: argmax over the L+1 class planes of the decoder output,
 //    one map per lane holding the label value where that lane wins (left = label * (label == 1), ...), top rows zeroed;
 //    the maps then go through the same LSQ kernel as the end-to-end path (no gradient on this branch).
+//    lf_seg_lane_maps_line adds the gt_line substitution of :308-311 in the same launch, so it needs no host read of gt_line.
 //  * lf_ce2d_*         -- the weighted pixel-wise nn.CrossEntropyLoss(weights) of BP/Loss_crit.py:64-65 on the planar
 //    [B, C, H, W] logits (BP/main.py:258,307): loss = sum_i w[t_i] (lse_i - x_{t_i}) / sum_i w[t_i], and its gradient
 //    w[t_i] (softmax_c - [c == t_i]) / sum w, recomputed from the logits (nothing saved but the two sums).
@@ -14,24 +15,40 @@ namespace lf {
 constexpr int SEG_MAXC = 8;
 constexpr int SEG_THREADS = 256;
 
+__device__ __forceinline__ int seg_argmax(const float* __restrict__ o, int C, long long HW) {
+    float best = o[0];
+    int arg = 0;
+    for (int c = 1; c < C; ++c) {
+        const float v = o[(size_t)c * HW];
+        if (v > best) {   // first maximum wins
+            best = v;
+            arg = c;
+        }
+    }
+    return arg;
+}
+
+// gt_line (NULL or [B][nl]): where gt_line[b][k] != 0, map (b, k) is image 0 / lane 0's map instead (LSQ_layer.py:308-311).
+// The replacement is read from the logits, not from `maps`, so it is the map before any replacement, as the reference's
+// right-hand side masked[0, 0] is evaluated before its boolean assignment.
 __global__ void __launch_bounds__(SEG_THREADS) seg_lane_maps_kernel(const float* __restrict__ out, int B, int C, long long HW, int W,
-                                                                    int nl, int mask_rows, float* __restrict__ maps) {
+                                                                    int nl, int mask_rows, const float* __restrict__ gt_line,
+                                                                    float* __restrict__ maps) {
     pdl_entry();
     const long long total = (long long)B * HW;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const long long b = i / HW, p = i - b * HW;
-        const float* o = out + (size_t)b * C * HW + p;
-        float best = o[0];
-        int arg = 0;
-        for (int c = 1; c < C; ++c) {
-            const float v = o[(size_t)c * HW];
-            if (v > best) {   // first maximum wins
-                best = v;
-                arg = c;
-            }
-        }
+        const int arg = seg_argmax(out + (size_t)b * C * HW + p, C, HW);
         const bool masked = (int)(p / W) < mask_rows;
-        for (int k = 0; k < nl; ++k) maps[((size_t)b * nl + k) * HW + p] = (!masked && arg == k + 1) ? (float)(k + 1) : 0.f;
+        int arg0 = -1;    // image 0's winner at p, computed once if a lane of image b is replaced
+        for (int k = 0; k < nl; ++k) {
+            float v = (!masked && arg == k + 1) ? (float)(k + 1) : 0.f;
+            if (gt_line && gt_line[b * nl + k] != 0.f) {
+                if (arg0 < 0) arg0 = seg_argmax(out + p, C, HW);
+                v = (!masked && arg0 == 1) ? 1.f : 0.f;
+            }
+            maps[((size_t)b * nl + k) * HW + p] = v;
+        }
     }
 }
 
@@ -125,12 +142,17 @@ static int seg_blocks(long long total) {
 
 using namespace lf;
 
-extern "C" int lf_seg_lane_maps(const float* out, int B, int C, int H, int W, int nl, int mask_rows, float* maps, lf_stream_t stream_) {
+extern "C" int lf_seg_lane_maps_line(const float* out, int B, int C, int H, int W, int nl, int mask_rows, const float* gt_line,
+                                     float* maps, lf_stream_t stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     LF_REQUIRE(out && maps && B >= 1 && C >= 2 && H >= 1 && W >= 1 && nl >= 1 && nl < C && mask_rows >= 0);
     const long long HW = (long long)H * W;
-    lf_launch(seg_lane_maps_kernel, seg_blocks(B * HW), SEG_THREADS, 0, stream, out, B, C, HW, W, nl, mask_rows, maps);
+    lf_launch(seg_lane_maps_kernel, seg_blocks(B * HW), SEG_THREADS, 0, stream, out, B, C, HW, W, nl, mask_rows, gt_line, maps);
     return check_launch();
+}
+
+extern "C" int lf_seg_lane_maps(const float* out, int B, int C, int H, int W, int nl, int mask_rows, float* maps, lf_stream_t stream_) {
+    return lf_seg_lane_maps_line(out, B, C, H, W, nl, mask_rows, nullptr, maps, stream_);
 }
 
 extern "C" int lf_ce2d_blocks(int B, int H, int W) { return seg_blocks((long long)B * H * W); }

@@ -11,6 +11,7 @@ The graph only contains our C-ABI kernels, a handful of tiny float64 torch ops o
 graph-safe Philox draws for the Dropout2d masks, and (optionally) the NCCL all-reduce.
 """
 import os
+import time
 
 import torch
 
@@ -34,10 +35,17 @@ class GraphedTrainStep:
     system changes no parameter or optimizer state, with no host synchronisation.  With a reducer the guard reads the
     word's maximum over the ranks (one all-reduce of one element, ddp.any_rank_nonzero), so every rank skips or updates
     together and the replicas stay identical.  Each call writes the optimizer's
-    hyperparameters first if a param_groups value changed (schedulers work without a recapture)."""
+    hyperparameters first if a param_groups value changed (schedulers work without a recapture).
+
+    ``gt_line``: optional example [B, 4] tensor, cloned into a static buffer ``self.gt_line`` that the forward reads (the
+    segmentation branch's substitution, end_to_end=False); default a host tensor of zeros.  ``loss_fn``: optional
+    callable(forward 9-tuple) -> scalar loss that replaces the lane criterion and ``extra_loss``.  ``post``: optional
+    callable(forward 9-tuple, detached loss) run at the end of every step, after the update (its return value is
+    ``self.post_out``); the warm-up steps run it too."""
 
     def __init__(self, model, criterion, nclasses, example_x, example_xgt, example_valid, reducer=None, warmup=3,
-                 capture_error_mode="global", extra_loss=None, global_valid=False, optimizer=None):
+                 capture_error_mode="global", extra_loss=None, global_valid=False, optimizer=None, gt_line=None,
+                 end_to_end=True, loss_fn=None, post=None):
         if optimizer is not None:
             from .optim import FusedOptimizer
             if not isinstance(optimizer, FusedOptimizer):
@@ -54,7 +62,11 @@ class GraphedTrainStep:
         self.x = example_x.clone()
         self.xgt = example_xgt.clone()
         self.valid = example_valid.clone()
-        self.gt_line = torch.zeros(example_x.shape[0], 4)
+        self.gt_line = torch.zeros(example_x.shape[0], 4) if gt_line is None else gt_line.clone()
+        self.end_to_end = end_to_end
+        self.loss_fn = loss_fn
+        self.post = post
+        self.post_out = None
         model.defer_status_check = True
         self.params = [p for p in model.parameters() if p.requires_grad]
 
@@ -90,12 +102,14 @@ class GraphedTrainStep:
             if self.optimizer is not None:
                 self.model.lsq_status.zero_()
             torch._foreach_zero_(self.grads)
-        out = self.model(self.x, self.gt_line, True)
+        out = self.model(self.x, self.gt_line, self.end_to_end)
         scale = None
         if self.global_valid:
             from .ddp import lane_valid_scale
             scale = lane_valid_scale(self.valid, self.L)
-        if FUSED_LOSS and hasattr(self.crit, "_fused_host_constants"):
+        if self.loss_fn is not None:
+            loss = self.loss_fn(out)
+        elif FUSED_LOSS and hasattr(self.crit, "_fused_host_constants"):
             from .Loss_crit import fused_backprojection_loss
             loss, _ = fused_backprojection_loss(self.crit, out[:self.L], self.xgt, self.valid, lane_scale=scale)
         elif hasattr(self.crit, "forward_lanes"):
@@ -106,7 +120,7 @@ class GraphedTrainStep:
                 ll, _ = self.crit(out[l], self.xgt[:, l], self.valid[:, l])
                 loss = loss + ll
             loss = loss / self.L
-        if self.extra_loss is not None:
+        if self.extra_loss is not None and self.loss_fn is None:
             loss = loss + self.extra_loss(out)
         loss.backward()
         if self.reducer is not None:
@@ -118,7 +132,10 @@ class GraphedTrainStep:
                 from .ddp import any_rank_nonzero
                 status = any_rank_nonzero(status, self.skip_word, getattr(self.reducer, "group", None))
             self.optimizer.launch(status=status)
-        return loss.detach()
+        loss = loss.detach()
+        if self.post is not None:
+            self.post_out = self.post(out, loss)
+        return loss
 
     def load(self, x, xgt, valid):
         """Stage a new batch (device or pinned-host tensors) into the static input buffers."""
@@ -168,27 +185,29 @@ class GraphedInference:
     (beta0..3, masked, output, line, horizon, output_seg) aliases static buffers that the next call overwrites.
     ``model.lsq_status`` (device int32, OR-ed) reports singular systems; `check()` reads it (one sync).
     ``post``: optional callable(9-tuple) captured right after the forward (and run by every warm-up pass); its return value
-    is ``self.post_out``, static like ``self.out``."""
+    is ``self.post_out``, static like ``self.out``.
+    ``gt_line`` (optional example [B, 4] tensor, cloned into the static ``self.gt_line``) and ``end_to_end`` are the
+    forward's arguments; by default host zeros and True."""
 
-    def __init__(self, model, example_x, warmup=2, post=None):
+    def __init__(self, model, example_x, warmup=2, post=None, gt_line=None, end_to_end=True):
         self.model = model.eval()
         model.defer_status_check = True
         self.x = example_x.clone()
-        self.gt_line = torch.zeros(example_x.shape[0], 4)
+        self.gt_line = torch.zeros(example_x.shape[0], 4) if gt_line is None else gt_line.clone()
         self.post_out = None
         dev = example_x.device
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(max(1, warmup)):             # builds and caches the folded operands outside the capture
-                out = model(self.x, self.gt_line, True)
+                out = model(self.x, self.gt_line, end_to_end)
                 if post is not None:
                     post(out)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(self.graph):
-            self.out = model(self.x, self.gt_line, True)
+            self.out = model(self.x, self.gt_line, end_to_end)
             if post is not None:
                 self.post_out = post(self.out)
 
@@ -202,3 +221,196 @@ class GraphedInference:
         if st:
             self.model.lsq_status.zero_()
             raise RuntimeError("status word %d (1 singular / 2 non-finite / 4 not positive definite normal matrix)" % st)
+
+
+class DeviceMeters:
+    """The reference's AverageMeters (BP/Networks/utils.py AverageMeter) on the device: one float64 (val, sum, count) row per
+    name, updated as ``sum += val * n; count += n`` -- AverageMeter.update's Python-float arithmetic -- so the averages come
+    out bit for bit.  ``update`` is guarded by a device bool (no synchronisation, capturable); ``read`` is one copy."""
+
+    def __init__(self, names, device):
+        self.names = list(names)
+        self.t = torch.zeros(len(self.names), 3, dtype=torch.float64, device=device)
+
+    def update(self, name, val, ok, n=1):
+        row = self.t[self.names.index(name)]
+        v = val.detach().reshape(()).double()
+        row[0].copy_(torch.where(ok, v, row[0]))
+        row[1].add_(torch.where(ok, v * n, 0.0))
+        row[2].add_(ok.double() * n)
+
+    def read(self):
+        """name -> (val, avg) as AverageMeter holds them (0, 0 before the first update)."""
+        return {k: (v, s / c) if c else (0, 0) for k, (v, s, c) in zip(self.names, self.t.tolist())}
+
+
+class BatchStatus:
+    """A device log of each batch's LSQ status word: ``record`` (capturable) appends ``status`` at a device position and
+    zeroes it for the next batch.  ``skipped`` reads it once: the host labels of the batches whose word was nonzero."""
+
+    def __init__(self, capacity, device):
+        self.log = torch.zeros(max(1, capacity), dtype=torch.int32, device=device)
+        self.pos = torch.zeros(1, dtype=torch.int64, device=device)
+
+    def check(self, i):
+        if i >= self.log.numel():
+            raise ValueError("the loader yielded more batches than its len() of %d" % self.log.numel())
+
+    def record(self, status):
+        self.log.index_copy_(0, self.pos, status.reshape(1))
+        self.pos.add_(1)
+
+    def print_skipped(self, labels):
+        """The reference's line for each skipped batch, in order (BP/main.py:289-292: the batch's idx, then the error)."""
+        from .ops_lsq import status_message
+        for st, idx in zip(self.log[:len(labels)].tolist(), labels):
+            if st:
+                print("Batch with idx {} skipped due to singular matrix".format(idx.numpy()))
+                print(status_message(st))
+
+
+def lane_losses(criterion, out, lanes, vp, L):
+    """The lane loop of BP/main.py:296-305 (and :309-317, :460-469) with its ops in its order: the mean over lanes of the
+    per-lane criterion calls, and the four x_cal (None past L lanes)."""
+    x_cal2 = x_cal3 = None
+    loss_left, x_cal0 = criterion(out[0], lanes[:, 0, :], vp[:, 0])
+    loss_right, x_cal1 = criterion(out[1], lanes[:, 1, :], vp[:, 1])
+    if L > 3:
+        loss_left1, x_cal2 = criterion(out[2], lanes[:, 2, :], vp[:, 2])
+        loss_right1, x_cal3 = criterion(out[3], lanes[:, 3, :], vp[:, 3])
+        loss_left += loss_left1
+        loss_right += loss_right1
+    return (loss_left + loss_right) / L, [x_cal0, x_cal1, x_cal2, x_cal3]
+
+
+def _reporting(i, freq):
+    return freq > 0 and (i + 1) % freq == 0
+
+
+def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch):
+    """One training epoch of the reference's main.py loop (BP/main.py:225-359), each batch one replay of a
+    GraphedTrainStep that holds the forward, the loss, the backward, the fused optimizer's update and the meter updates.
+    Returns (losses.avg, rmse_metric.avg) -- rmse_metric is updated with --end_to_end False only, as in the reference.
+
+    The loader yields the train loader's 7-tuples (input, gt, lanes, idx, gt_line, gt_horizon, valid_points), on the
+    device as Dataloader.Load_Data_new gives them (host tensors are copied in); every batch has the first one's size (the
+    train loader drops its last batch).  ``optimizer`` must be an optim.FusedOptimizer (define_optim(..., fused=True)): the
+    update sits in the graph, guarded by the LSQ status word, so a batch with a singular system changes no parameter, no
+    optimizer state and no meter, without a host synchronisation; the reference's line for each such batch is printed at the
+    end of the epoch.  The host synchronises only at the print_freq lines, at save_weightmap('train', ...) every save_freq
+    batches and at the end.
+
+    Loss: end-to-end, the fused lf_backproj_loss (Loss_crit.fused_backprojection_loss), whose lane sum is reassociated
+    against main.py:296-305's per-lane criterion calls (equal to about 1e-12 relative); with --clas, ``loss * weight_fit +
+    (bce_line.double() + bce_horizon.double()) * weight_class``.  --end_to_end False: criterion_seg(output, gt), with the
+    least-squares fit and the rmse metric computed without gradient (main.py:306-318).  clip_grad_norm is accepted and does
+    nothing: main.py:334-335 clips the gradients of the previous batch before zero_grad() discards them, so it never changes
+    an update.  --pretrained (the skip_epochs segmentation phase and the switch of parameter sets) raises ValueError: a
+    FusedOptimizer keeps one parameter set.  Dropout masks are drawn in the graph from torch's graph-safe Philox offsets;
+    they do not repeat an eager run's masks.  BatchNorm running statistics are those of the epoch's batches (the capture's
+    warm-up steps leave them as they were)."""
+    from .optim import FusedOptimizer
+    from .Loss_crit import fused_backprojection_loss
+    from .Networks import utils as nutils
+    if not isinstance(optimizer, FusedOptimizer):
+        raise TypeError("train_epoch runs the update in the graph: it needs an optim.FusedOptimizer "
+                        "(define_optim(..., fused=True)), got %s" % type(optimizer).__name__)
+    if args.pretrained:
+        raise ValueError("train_epoch does not run --pretrained: its segmentation phase and the switch to end-to-end change "
+                         "the parameter set, which a FusedOptimizer refuses")
+    if args.clas and not args.end_to_end:
+        raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
+    e2e, L = bool(args.end_to_end), args.nclasses
+    if not e2e and L != 4:
+        raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
+                         "loader's 4 line flags over %d lane maps" % L)
+    dev = next(model.parameters()).device
+    model.train()
+    meters = DeviceMeters(("loss", "rmse"), dev)
+    status = BatchStatus(len(loader), dev)
+    static = {}
+
+    def loss_fn(out):
+        if not e2e:
+            with torch.no_grad():
+                static["rmse"], static["x_cal"] = lane_losses(criterion, out, static["lanes"], static["valid"], L)
+            return criterion_seg(out[5], static["gt"])
+        loss, x_cal = fused_backprojection_loss(criterion, out[:L], static["lanes"], static["valid"])
+        static["x_cal"] = [x_cal[:, l] for l in range(L)] + [None] * (4 - L)
+        if args.clas:
+            loss_horizon = criterion_horizon(out[7], static["gt_horizon"]).double()
+            loss_line = criterion_line_class(out[6], static["gt_line"]).double()
+            loss = loss * args.weight_fit + (loss_line + loss_horizon) * args.weight_class
+        return loss
+
+    def post(out, loss):
+        if not torch.cuda.is_current_stream_capturing():
+            return None                      # warm-up steps: no meter or log entry
+        ok = model.lsq_status.reshape(()).eq(0)
+        n = static["input"].shape[0]
+        if not e2e:
+            meters.update("rmse", static["rmse"], ok, n)
+        meters.update("loss", loss, ok, n)
+        status.record(model.lsq_status)
+        return out[4]
+
+    step, labels = None, []
+    bt_sum, bt_n, end = 0.0, 0, time.time()
+    deferred = model.defer_status_check
+    try:
+        for i, (input, gt, lanes, idx, gt_line, gt_horizon, valid_points) in enumerate(loader):
+            batch = {"input": input, "gt": gt.squeeze(1), "lanes": lanes, "gt_line": gt_line, "gt_horizon": gt_horizon,
+                     "valid": valid_points}
+            if step is None:
+                for k, v in batch.items():
+                    static[k] = v.to(dev, non_blocking=True).clone()
+                static["input"] = static["input"].float()
+                static["gt"] = static["gt"].long()
+                # the warm-up steps are training forwards: keep the BatchNorm running statistics they would move
+                bns = [m for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)]
+                saved = [[t.clone() if t is not None else None for t in (m.running_mean, m.running_var, m.num_batches_tracked)]
+                         for m in bns]
+                step = GraphedTrainStep(model, criterion, L, static["input"], static["lanes"], static["valid"],
+                                        optimizer=optimizer, gt_line=None if e2e else static["gt_line"], end_to_end=e2e,
+                                        loss_fn=loss_fn, post=post)
+                for m, ts in zip(bns, saved):
+                    for t, v in zip((m.running_mean, m.running_var, m.num_batches_tracked), ts):
+                        if t is not None:
+                            t.copy_(v)
+                static["input"] = step.x              # the step's own copies are what its forward reads
+                if not e2e:
+                    static["gt_line"] = step.gt_line
+            else:
+                if input.shape[0] != step.x.shape[0]:
+                    raise ValueError("batch of %d images after a first batch of %d: train_epoch replays one batch size"
+                                     % (input.shape[0], step.x.shape[0]))
+                for k, v in batch.items():
+                    static[k].copy_(v, non_blocking=True)
+            status.check(i)
+            labels.append(idx)
+            step()
+            now = time.time()
+            bt_val, end = now - end, now
+            bt_sum, bt_n = bt_sum + bt_val, bt_n + 1
+            if not (_reporting(i, args.print_freq) or _reporting(i, args.save_freq)) or int(status.log[i]):
+                continue                             # a skipped batch reports nothing, as main.py's `continue`
+            m = meters.read()
+            if _reporting(i, args.print_freq):
+                print('Epoch: [{0}][{1}/{2}]\t'
+                      'Time {3:.3f} ({4:.3f})\t'
+                      'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                      'rmse_metric {rmse[0]:.8f} ({rmse[1]:.8f})'.format(
+                          epoch + 1, i + 1, len(loader), bt_val, bt_sum / bt_n, loss=m["loss"], rmse=m["rmse"]))
+            if _reporting(i, args.save_freq):
+                lanes = static["lanes"]
+                nutils.save_weightmap('train', step.post_out, *static["x_cal"],
+                                      lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :], lanes[:, 3, :], static["gt"], 0, i,
+                                      static["input"], args.no_ortho, args.resize, args.save_path, args.nclasses,
+                                      args.no_mapping)
+    finally:
+        model.defer_status_check = deferred
+    if step is None:
+        return 0, 0
+    m = meters.read()
+    status.print_skipped(labels)
+    return m["loss"][1], m["rmse"][1]

@@ -294,3 +294,119 @@ def test_model(loader, model, criterion, criterion_seg, criterion_line_class, cr
     print(acc_seg)
     print("===> Average ACC on TESTSET is {:.8} in {:.6}s for a batch".format(acc_seg[0], start.elapsed_time(end) / 1e3 / batches))
     return acc_seg[0]
+
+
+def validate(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0):
+    """The reference's validation pass (BP/main.py:419-526), same return value: (losses.avg, acc_hor_tot.avg,
+    acc_line_tot.avg, rmse_metric_valid.avg).  ``args`` is main.py's global args, passed in.
+
+    The loader yields the valid loader's 8-tuples (input, gt, lanes, idx, gt_line, gt_horizon, index, valid_points), on the
+    device as Dataloader.Load_Data_new gives them (host tensors are copied in).  Each batch is one replay of a
+    GraphedInference whose post= hook holds the per-lane criterion calls in main.py's order, with --clas the rounded-sigmoid
+    accuracies (divided by resize * val_batch_size and nclasses * val_batch_size, also for a short batch), with --end_to_end
+    False criterion_seg and the rmse metric, and the meter updates (engine.DeviceMeters) guarded by the LSQ status word: a
+    batch with a singular system updates no meter, as main.py's `continue` does, and its line is printed at the end of the
+    pass.  A batch shorter than the first (a loader that keeps its last batch) is replayed by a second graph of its size,
+    so its losses are the ones main.py computes on it.  The host synchronises only at the print_freq lines, at
+    save_weightmap('valid', ...) every 25 batches (called with the static outputs) and at the end.  The --clas BCE losses
+    main.py adds after losses.update change nothing it returns and are not computed."""
+    if __package__:
+        from .engine import GraphedInference, DeviceMeters, BatchStatus, lane_losses, _reporting
+        from .Networks import utils as nutils
+    else:
+        from engine import GraphedInference, DeviceMeters, BatchStatus, lane_losses, _reporting
+        from Networks import utils as nutils
+    if args.clas and not args.end_to_end:
+        raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
+    e2e, L = bool(args.end_to_end), args.nclasses
+    if not e2e and L != 4:
+        raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
+                         "loader's 4 line flags over %d lane maps" % L)
+    dev = next(model.parameters()).device
+    meters = DeviceMeters(("loss", "acc_hor", "acc_line", "rmse"), dev)
+    status = BatchStatus(len(loader), dev)
+    graphs = {}                     # rows -> (GraphedInference, static batch tensors)
+
+    def build(batch):
+        st = {k: v.to(dev, non_blocking=True).clone() for k, v in batch.items()}
+        st["input"], st["gt"] = st["input"].float(), st["gt"].long()
+        n = st["input"].shape[0]
+
+        def post(out):
+            lanes, vp = st["lanes"], st["valid"]
+            if e2e:
+                loss, x_cal = lane_losses(criterion, out, lanes, vp, L)
+            else:
+                loss = criterion_seg(out[5], st["gt"])
+                loss_metric, x_cal = lane_losses(criterion, out, lanes, vp, L)
+            if not torch.cuda.is_current_stream_capturing():
+                return x_cal                 # warm-up passes: no meter or log entry
+            ok = model.lsq_status.reshape(()).eq(0)
+            if not e2e:
+                meters.update("rmse", loss_metric, ok, n)
+            meters.update("loss", loss, ok, n)
+            if args.clas:
+                horizon_pred = torch.round(torch.nn.Sigmoid()(out[7]))
+                acc = torch.eq(horizon_pred, st["gt_horizon"])
+                acc_hor = torch.sum(acc).float() / (args.resize * args.val_batch_size)
+                meters.update("acc_hor", acc_hor, ok)
+                line_pred = torch.round(torch.nn.Sigmoid()(out[6]))
+                acc = torch.eq(line_pred, st["gt_line"])
+                acc_line = torch.sum(acc).float() / (args.nclasses * args.val_batch_size)
+                meters.update("acc_line", acc_line, ok)
+            status.record(model.lsq_status)
+            model.lsq_status.zero_()
+            return x_cal
+
+        g = GraphedInference(model, st["input"], post=post, gt_line=None if e2e else st["gt_line"], end_to_end=e2e)
+        st["input"] = g.x
+        if not e2e:
+            st["gt_line"] = g.gt_line        # the forward's substitution and the accuracies read one buffer
+        model.lsq_status.zero_()
+        return g, st
+
+    deferred = model.defer_status_check
+    first, labels = None, []
+    try:
+        with torch.no_grad():
+            for i, (input, gt, lanes, idx, gt_line, gt_horizon, index, valid_points) in enumerate(loader):
+                batch = {"input": input, "gt": gt.squeeze(1), "lanes": lanes, "gt_line": gt_line, "gt_horizon": gt_horizon,
+                         "valid": valid_points}
+                n = input.shape[0]
+                status.check(i)
+                if first is None:
+                    first = n
+                elif n > first:
+                    raise ValueError("batch of %d images after a first batch of %d" % (n, first))
+                if n in graphs:
+                    g, st = graphs[n]
+                    for k, v in batch.items():
+                        st[k].copy_(v, non_blocking=True)
+                else:
+                    g, st = graphs[n] = build(batch)
+                labels.append(idx)
+                g.graph.replay()
+                if not (_reporting(i, args.print_freq) or _reporting(i, 25)) or int(status.log[i]):
+                    continue                     # a skipped batch reports nothing, as main.py's `continue`
+                if _reporting(i, args.print_freq):
+                    m = meters.read()
+                    print('Test: [{0}/{1}]\t'
+                          'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                          'rmse {rmse[0]:.8f} ({rmse[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], rmse=m["rmse"]))
+                if _reporting(i, 25):
+                    lanes = st["lanes"]
+                    nutils.save_weightmap('valid', g.out[4], *g.post_out, lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :],
+                                          lanes[:, 3, :], st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
+                                          args.save_path, args.nclasses, args.no_mapping)
+    finally:
+        model.defer_status_check = deferred
+    m = meters.read()
+    status.print_skipped(labels)
+    if args.evaluate:
+        crit_string = "TOT LOSS" if args.clas else ("MSE" if args.loss_policy == "backproject" and e2e else
+                                                    "AREA**2" if args.loss_policy == "area" and e2e else "ENTROPY")
+        print("===> Average {}-loss on validation set is {:.8}".format(crit_string, m["loss"][1]))
+        if args.clas and len(loader) != 0:
+            print("===> Average HORIZON ACC on val is {:.8}".format(m["acc_hor"][1]))
+            print("===> Average LINE ACC on val is {:.8}".format(m["acc_hor"][1]))
+    return m["loss"][1], m["acc_hor"][1], m["acc_line"][1], m["rmse"][1]
