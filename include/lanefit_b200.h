@@ -651,6 +651,26 @@ int lf_loader_assemble(const unsigned char* cache_frames, const unsigned char* c
                        const float* line_tab, float* image, long long* gt, double* lanes, double* valid, float* horizon, float* line,
                        lf_stream_t stream);
 
+/* The bird's-eye-view loader on the same cache (csrc/loader.cu; bev/Dataloader/Load_Data_new.py of this package, replacing
+ * the per-sample work of BEV/Dataloader/Load_Data_new.py:77-112 after decoding).
+ * lf_loader_label_rows: for each of N staged maps, cache_maps[slots[n]] -> first_row[positions[n]] = the first row holding a
+ *   value outside {0, 3, 4}, or -1 if there is none (the horizon of the reference's gt.nonzero()[0, 1]; a flip does not move
+ *   rows).  slots, positions: device int32 [N]; first_row: device int32 indexed by table row.  One CTA per map.
+ * lf_loader_assemble_bev: one collated batch, one launch.  sample: device int32 [N][3] = (slot, table row, flip).
+ *   image [N][3][Ho][Wo] f32 as lf_loader_assemble;
+ *   gt [N][1][Ho][Wo] int64 = the cached map (mirrored when flip != 0) with 3 and 4 -> 0, then 1 <-> 2 when flip != 0;
+ *   per-row tables over nrows rows, flip state f = (flip != 0):
+ *     params [N][4][3] f32 = params_tab[f][row]  (params_tab [2][nrows][4][3])
+ *     line [N][4] int64 = line_tab[f][row]       (line_tab [2][nrows][4])
+ *     horizon [N][Ho] f32 = 1 for y < first_row[row], else 0
+ *   Every pointer is required.  Needs Ho * Wo >= 12. */
+#define LF_LOADER_BEV_COEFFS 3
+int lf_loader_label_rows(const unsigned char* cache_maps, int N, int Ho, int Wo, const int* slots, const int* positions, int* first_row,
+                         lf_stream_t stream);
+int lf_loader_assemble_bev(const unsigned char* cache_frames, const unsigned char* cache_maps, int N, int Ho, int Wo,
+                           const int* sample, int nrows, const float* params_tab, const long long* line_tab, const int* first_row,
+                           float* image, long long* gt, float* params, long long* line, float* horizon, lf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -130,9 +130,13 @@ def _read(path):
 
 class _SampleStore:
     """Slot-addressed uint8 buffers of resized, unflipped samples on one device, and the decoders that fill them.
-    Slot state: 0 empty, 1 filled in the current epoch (not served until the decoders' check at its end), 2 served."""
+    Slot state: 0 empty, 1 filled in the current epoch (not served until the decoders' check at its end), 2 served.
 
-    def __init__(self, frame_paths, map_paths, resize, device, cache_bytes):
+    label_rows (the bird's-eye-view loader): after staging, lf_loader_label_rows records the first labelled row of each new
+    map in `first_row` (device int32, per dataset position).  The end-of-epoch check copies it to the host and raises
+    ValueError for every map served in the epoch that has no labelled pixel."""
+
+    def __init__(self, frame_paths, map_paths, resize, device, cache_bytes, label_rows=False):
         self.frame_paths, self.map_paths = list(frame_paths), None if map_paths is None else list(map_paths)
         self.P, self.R = len(self.frame_paths), int(resize)
         self.Ho, self.Wo = self.R, 2 * self.R
@@ -141,6 +145,9 @@ class _SampleStore:
         self.cached = 0 < budget and self.P * per <= budget
         self.device = device
         self.state = np.zeros(self.P, np.int8)
+        self.label_rows = label_rows
+        self.first_row_host = np.full(self.P, -2, np.int32) if label_rows else None   # -2: not recorded yet
+        self._served = np.zeros(self.P, bool) if label_rows else None
         self.workers = 0
         self._pool = None
         self._dev = None
@@ -167,6 +174,10 @@ class _SampleStore:
         self._ring_read = [None, None]   # per staging buffer: event of the last assembly that read it
         self._assembled = {}             # consumer stream -> event of its last assembly (cache mode)
         self._decoded = False
+        self.first_row = None
+        if self.label_rows:
+            with torch.cuda.stream(self.side):     # ordered before the side stream's lf_loader_label_rows
+                self.first_row = torch.full((self.P,), -2, dtype=torch.int32, device=dev)
 
     def _alloc(self, S):
         self.frames = torch.empty(S, self.Ho, self.Wo, 3, dtype=torch.uint8, device=self._dev)
@@ -205,6 +216,8 @@ class _SampleStore:
         (slot of each position, event the assembly waits for or None)."""
         self._setup()
         positions = list(positions)
+        if self._served is not None:
+            self._served[positions] = True
         if self.cached:
             slots = positions
             need = [k for k, p in enumerate(positions) if self.state[p] != 2]
@@ -247,20 +260,42 @@ class _SampleStore:
                        p(yb), p(yk), self.fpre.ky, p(self.lpre.xs), p(self.lpre.ys), self.Ho, self.Wo, p(sl), p(self.frames),
                        p(self.maps), _capi.stream_ptr(), nbytes=frames.numel() + (0 if maps is None else maps.numel())
                        + len(need) * self.Ho * self.Wo * 4)
+            if self.first_row is not None:
+                # a position staged again (ring mode, across an epoch boundary) rewrites the same value
+                pos = torch.tensor([positions[k] for k in need], dtype=torch.int32).pin_memory().to(self._dev, non_blocking=True)
+                _capi.call("lf_loader_label_rows", p(self.maps), len(need), self.Ho, self.Wo, p(sl), p(pos), p(self.first_row),
+                           _capi.stream_ptr(), nbytes=len(need) * self.Ho * self.Wo)
             ev = torch.cuda.Event()
             ev.record(side)
         if self.cached:
             self.state[[positions[k] for k in need]] = 1
         return slots, ev
 
-    def assemble(self, slots, rows, flips, staged, nclasses, tables, image_only):
-        """The batch's device elements on the current stream, from the slots (after `staged`)."""
+    def assembly_begin(self, slots, rows, flips, staged):
+        """(current stream, device int32 [N][3] (slot, table row, flip)) for an assembly launch that reads the slots, after
+        the current stream waits for `staged`.  The launch is followed by assembly_end."""
         stream = torch.cuda.current_stream(self._dev)
         if staged is not None:
             stream.wait_event(staged)
-        N = len(slots)
         sample = torch.from_numpy(np.stack([np.asarray(slots), np.asarray(rows), np.asarray(flips)], 1).astype(np.int32))
-        sample = sample.pin_memory().to(self._dev, non_blocking=True)
+        return stream, sample.pin_memory().to(self._dev, non_blocking=True)
+
+    def assembly_end(self, stream, slots):
+        """Record that `stream` read the slots, so staging does not overwrite them before it has."""
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        if self.cached:
+            self._assembled[stream] = ev
+        else:
+            self._ring_read[0 if slots[0] < self.capacity // 2 else 1] = ev
+            for b in (self.frames, self.maps):
+                if b is not None:
+                    b.record_stream(stream)
+
+    def assemble(self, slots, rows, flips, staged, nclasses, tables, image_only):
+        """The batch's device elements on the current stream, from the slots (after `staged`)."""
+        stream, sample = self.assembly_begin(slots, rows, flips, staged)
+        N = len(slots)
         dev, R = self._dev, self.R
         image = torch.empty(N, 3, R, 2 * R, dtype=torch.float32, device=dev)
         out = [image]
@@ -280,22 +315,29 @@ class _SampleStore:
         _capi.call("lf_loader_assemble", p(self.frames), p(self.maps), N, R, 2 * R, nclasses, p(sample), nrows, p(t.get("lanes")),
                    p(t.get("valid")), p(t.get("horizon")), p(t.get("line")), p(image), p(gt), p(lanes), p(valid), p(horizon),
                    p(line), _capi.stream_ptr(), nbytes=sum(o.numel() * o.element_size() for o in out) + N * R * 2 * R * 4)
-        ev = torch.cuda.Event()
-        ev.record(stream)
-        if self.cached:
-            self._assembled[stream] = ev
-        else:
-            self._ring_read[0 if slots[0] < self.capacity // 2 else 1] = ev
-            for b in (self.frames, self.maps):
-                if b is not None:
-                    b.record_stream(stream)
+        self.assembly_end(stream, slots)
         return out
 
     def finish_epoch(self):
         """End of an epoch: read the decoders' status words if anything was decoded since the last read; the slots filled
         since then are served from now on, or, after a corrupt file, emptied (and ValueError raised)."""
-        if self._dev is None or not self._decoded:
+        if self._dev is None:
             return
+        served = None
+        if self._served is not None:
+            served, self._served = self._served, np.zeros(self.P, bool)
+        if self._decoded:
+            self._check_decoders()
+            if self.first_row is not None:
+                with torch.cuda.stream(self.side):
+                    self.first_row_host = self.first_row.cpu().numpy()
+        if served is not None:
+            bad = np.nonzero(served & (self.first_row_host == -1))[0]
+            if len(bad):
+                raise ValueError("%s: no labelled pixel (a value other than 0, 3 and 4) in the resized label map, so the "
+                                 "horizon is undefined" % ", ".join(self.map_paths[i] for i in bad))
+
+    def _check_decoders(self):
         self._decoded = False
         errors = []
         for d in (self.jdec, self.pdec):

@@ -155,10 +155,13 @@ class LfPngImage(ctypes.Structure):
 TUSIMPLE_MAX_GT = 8
 TUSIMPLE_MAX_S = 64
 LOADER_LANES, LOADER_POINTS = 4, 56
+LOADER_BEV_COEFFS = 3
 
 _NET_PROTOS = {
     "lf_loader_stage": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p, _i, _i, _p, _p, _p, _p]),
     "lf_loader_assemble": (_i, [_p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_loader_label_rows": (_i, [_p, _i, _i, _i, _p, _p, _p, _p]),
+    "lf_loader_assemble_bev": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "lf_tusimple_score": (_i, [_p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "lf_png_workspace_bytes": (_c_size_t, [_p, _i]),
     "lf_png_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p]),
