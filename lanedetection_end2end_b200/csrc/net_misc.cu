@@ -623,6 +623,8 @@ extern "C" int lf_bn_finalize(const double* partial, int nblk, long long npix, i
     STREAM;
     LF_REQUIRE(partial && gamma && beta && mean && invstd && scale && shift && nblk >= 1);
     LF_REQUIRE((running_mean == nullptr) == (running_var == nullptr));
+    int rc = bn_check(npix, C);   // the kernel divides by npix and the grid is sized from C
+    if (rc) return rc;
     lf_launch(bn_finalize_kernel, (C * 32 + 255) / 256, 256, 0, stream, partial, nblk, npix, C, gamma, beta, eps, momentum, running_mean,
                                                             running_var, mean, invstd, scale, shift);
     return check_launch();
@@ -714,6 +716,8 @@ extern "C" int lf_bn_bwd_finalize(const double* partial, int nblk, long long npi
                                   float* c1, float* c2, lf_stream_t stream_) {
     STREAM;
     LF_REQUIRE(partial && dgamma && dbeta && c1 && c2 && nblk >= 1);
+    int rc = bn_check(npix, C);
+    if (rc) return rc;
     lf_launch(bn_bwd_finalize_kernel, (C * 32 + 255) / 256, 256, 0, stream, partial, nblk, npix, C, dgamma, dbeta, c1, c2);
     return check_launch();
 }
