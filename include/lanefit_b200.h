@@ -144,7 +144,9 @@ int lf_conv_f32(const LfConvArgs* args, lf_stream_t stream);
  * tensors with C in {64,128} channels in and out:
  *   out[n,y,x,co] = epi( sum_{t<3} sum_ci in[n, y+dy[t], x+dx[t], ci] * wpack[co*3*C + t*C + ci] )
  * epi as in LfConvArgs.  Requires a bx*by = 128 pixel patch with bx | W, by | H
- * (lf_conv1d_tc_supported tells).  Same results as lf_conv_f32 up to TF32 rounding of the operands. */
+ * (lf_conv1d_tc_supported tells).  Same results as lf_conv_f32 up to the TF32 form of the operands: the kernel rounds
+ * the activations to TF32 (nearest, ties away from zero), while `wpack` reaches the tensor core as its fp32 bits, which
+ * wgmma .tf32 truncates (low 13 mantissa bits ignored); pass TF32-rounded weights for rounded ones. */
 typedef struct LfConvTcArgs {
     const float* in;
     const float* wpack;    /* [C][3*C], K contiguous */
@@ -157,7 +159,7 @@ typedef struct LfConvTcArgs {
                               (the bias gradient when `out` is an output gradient); reduce with lf_vec_reduce */
     double* stats_partial; /* NULL, or [lf_conv1d_tc_supported(...)][2][C]: per-CTA sum and sum of squares of `out`
                               = the `partial` input of lf_bn_finalize (replaces an lf_bn_stats pass over `out`);
-                              LF_ERR_UNSUPPORTED when the launch has to use the per-tap variant */
+                              the slab and the per-tap variants fill it alike */
     const float* mask_scale; /* NULL, or [C] together with mask_shift [C] (needs mask_src and stats_partial): mask_src is then
                               a PRE-activation x, the ReLU-backward mask bit is fma(x, mask_scale[c], mask_shift[c]) > 0
                               (bit-identical to the forward's relu(bn(x)) when scale / shift are lf_bn_finalize's), and the
@@ -213,8 +215,17 @@ int lf_amax_per_image(const void* x, int dtype, long long per_image, int N, floa
 /* 2 (default) = halo-slab kernel (one TMA slab per 32-channel chunk shared by the three taps);
  * 1 = first version (one TMA box per tap).  Same results; process-wide switch for A/B measurements. */
 void lf_conv1d_tc_set_variant(int variant);
-/* 1 if a call with taps {-dil,0,+dil} along y (vertical) or x runs on the slab kernel, i.e. may ask for stats_partial */
+/* 1 if a call with taps {-dil,0,+dil} along y (vertical) or x runs on the slab kernel */
 int lf_conv1d_tc_slab_ok(int N, int H, int W, int C, int vertical, int dil);
+/* The plan lf_conv1d_tc (prec 0), _x3 (1), _bf16 (2) or _fp8 (3) selects for these arguments (in_dtype: of `in`), with
+ * the variant set now; no device needed.  LF_OK and info[LF_TC_PLAN_INFO] = {slab (1) or one box per tap (0), weights
+ * resident (1) or streamed per stage (0), pipeline stages, 3xTF32 lo buffers (0 otherwise), lo buffer over the staging
+ * tile (1), lo bytes outside the ring, tile extent along the conv axis TA, across it TB (pixels), vertical, CTAs per
+ * 64-channel half (= rows of colsum_partial / stats_partial), dynamic shared memory bytes, activation bytes per stage};
+ * LF_ERR_UNSUPPORTED where the launch would return it, LF_ERR_INVALID_ARGUMENT for N, H, W < 1 or a bad prec / dtype.
+ * Tile m = (image * tiles across + tile across) * tiles along + tile along runs on CTA row m % CTAs. */
+#define LF_TC_PLAN_INFO 12
+int lf_conv1d_tc_plan(int prec, int in_dtype, int N, int H, int W, int C, const int* dy, const int* dx, int* info);
 
 /* Weight gradient as a split-K GEMM over pixels:
  *   partial[s][t][cp][cq] = sum_{(n,j,i) in split s} P[n, j*psy+pdy[t], i*psx+pdx[t], cp]

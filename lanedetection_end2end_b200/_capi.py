@@ -62,6 +62,11 @@ class LfConvTcArgs(ctypes.Structure):
                 ("dx", _i * 3), ("relu", _i), ("in_dtype", _i), ("out_dtype", _i), ("mask_dtype", _i)]
 
 
+TC_PLAN_INFO = 12       # LF_TC_PLAN_INFO: entries lf_conv1d_tc_plan fills
+TC_PLAN_FIELDS = ("slab", "res", "stages", "n_lo", "lo_stg", "lo_bytes", "TA", "TB", "vertical", "m_ctas", "smem_bytes",
+                  "a_bytes")
+
+
 class LfConvTcFp8Args(ctypes.Structure):
     _fields_ = [("conv", LfConvTcArgs), ("x_amax", _p), ("w_scale", _p), ("out_amax", _p)]
 
@@ -186,6 +191,7 @@ _NET_PROTOS = {
     "lf_conv1d_tc_x3_rows": (_i, [_i, _i, _i, _i, _i, _i]),
     "lf_conv1d_tc_set_variant": (None, [_i]),
     "lf_conv1d_tc_slab_ok": (_i, [_i, _i, _i, _i, _i, _i]),
+    "lf_conv1d_tc_plan": (_i, [_i, _i, _i, _i, _i, _i, _p, _p, _p]),
     "lf_wgrad_reduce": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "lf_vec_reduce": (_i, [_p, _i, _i, _i, _p, _p]),
     "lf_colsum_blocks": (_i, [ctypes.c_longlong]),

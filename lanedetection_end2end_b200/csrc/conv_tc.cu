@@ -563,7 +563,7 @@ static bool tc_plan_slab(int N, int H, int W, int C, const int* dy, const int* d
     for (int t = 0; t < 3; ++t) g.tap_row[t] = (fwd_order ? t : 2 - t) * dil * g.TB;
     if (!tc_fit(C, prec, abf, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
-    return tc_get_encode_fn() != nullptr;
+    return true;
 }
 
 // Per-tap plan: any three taps; a bx x by = 128 pixel patch with bx | W, by | H (wide patches preferred).
@@ -588,7 +588,22 @@ static bool tc_plan_taps(int N, int H, int W, int C, const int* dy, const int* d
     }
     if (!tc_fit(C, prec, abf, p)) return false;
     p->m_ctas = tc_m_ctas(N, C, g.tiles_a * g.tiles_b);
-    return tc_get_encode_fn() != nullptr;
+    return true;
+}
+
+// The plan tc_run launches (and lf_conv1d_tc_plan reports): the halo slab where it serves the taps -- bf16 and fp8 take
+// it exactly where TF32 does (their smaller weight tiles and bf16 slabs fit wherever the TF32 ones do), so that
+// lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for all three -- else the per-tap boxes (not for 3xTF32).
+static int tc_select(int prec, bool abf, int N, int H, int W, int C, const int* dy, const int* dx, TcPlan* pl, bool* slab) {
+    *slab = (prec == TC_X3 || g_tc_variant != 1) &&
+            (!tc_takes_bf16(prec) || tc_plan_slab(N, H, W, C, dy, dx, TC_TF32, pl)) &&
+            tc_plan_slab(N, H, W, C, dy, dx, prec, pl, abf);
+    if (!*slab && (prec == TC_X3 || !tc_plan_taps(N, H, W, C, dy, dx, prec, pl, abf))) return LF_ERR_UNSUPPORTED;
+    const TcArgs& a = pl->geo;
+    // FP8 scales and maxima are per image: every tile must lie within one image (tiles cover each image exactly)
+    if (prec == TC_FP8 && (a.tiles_a * a.TA != (a.vertical ? H : W) || a.tiles_b * a.TB != (a.vertical ? W : H)))
+        return LF_ERR_UNSUPPORTED;
+    return LF_OK;
 }
 
 template <int C, int P, bool RES, bool ABF>
@@ -615,22 +630,19 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec, const
     LF_REQUIRE((p.in_dtype == LF_F32 || p.in_dtype == LF_BF16) && (p.out_dtype == LF_F32 || p.out_dtype == LF_BF16) &&
                (p.mask_dtype == LF_F32 || p.mask_dtype == LF_BF16));
     if (!tc_takes_bf16(prec) && (p.in_dtype | p.out_dtype | p.mask_dtype) != LF_F32) return LF_ERR_UNSUPPORTED;
+    LF_REQUIRE(p.N >= 1 && p.H >= 1 && p.W >= 1);
     const bool fp8 = prec == TC_FP8;
     // FP8 is an inference epilogue: scales in, per-image max out, no gradient-side outputs
     if (fp8) LF_REQUIRE(f8 && f8->x_amax && f8->w_scale && f8->out_amax && !p.colsum_partial && !p.stats_partial && !p.mask_scale);
     const bool x3 = prec == TC_X3;
     const bool abf = p.in_dtype == LF_BF16;
     TcPlan pl{};
-    // bf16 and fp8 take the slab exactly where TF32 does (their smaller weight tiles and bf16 slabs fit wherever the
-    // TF32 ones do), so that lf_conv1d_tc_supported / lf_conv1d_tc_slab_ok answer for all three
-    const bool slab = (x3 || g_tc_variant != 1) &&
-                      (!tc_takes_bf16(prec) || tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, TC_TF32, &pl)) &&
-                      tc_plan_slab(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf);
-    if (!slab && (x3 || !tc_plan_taps(p.N, p.H, p.W, p.C, p.dy, p.dx, prec, &pl, abf))) return LF_ERR_UNSUPPORTED;
+    bool slab = false;
+    const int rc = tc_select(prec, abf, p.N, p.H, p.W, p.C, p.dy, p.dx, &pl, &slab);
+    if (rc != LF_OK) return rc;
+    TcEncodeTiledFn enc = tc_get_encode_fn();
+    if (!enc) return LF_ERR_UNSUPPORTED;
     TcArgs a = pl.geo;
-    // FP8 scales and maxima are per image: every tile must lie within one image (tiles cover each image exactly)
-    if (fp8 && (a.tiles_a * a.TA != (a.vertical ? p.H : p.W) || a.tiles_b * a.TB != (a.vertical ? p.W : p.H)))
-        return LF_ERR_UNSUPPORTED;
     a.x_amax = fp8 ? f8->x_amax : nullptr;
     a.w_scale = fp8 ? f8->w_scale : nullptr;
     a.out_amax = fp8 ? f8->out_amax : nullptr;
@@ -645,7 +657,6 @@ static int tc_run(const LfConvTcArgs* args, lf_stream_t stream_, int prec, const
     a.mask_bf16 = p.mask_dtype == LF_BF16;
     a.total_m_tiles = p.N * a.tiles_a * a.tiles_b;
 
-    TcEncodeTiledFn enc = tc_get_encode_fn();
     CUtensorMap tmA, tmB;
     {
         // activations [N,H,W,C] viewed as (ci:32, cblk:C/32, across, along, n); one box = the slab or one tap's patch;
@@ -703,7 +714,7 @@ extern "C" void lf_conv1d_tc_set_variant(int v) { g_tc_variant = (v == 1) ? 1 : 
 // calls the slab does not fit.  The bf16 entry serves exactly the shapes and slab cases of the TF32 one.
 extern "C" int lf_conv1d_tc_supported(int N, int H, int W, int C) {
     TcPlan pl{};
-    return tc_plan_taps(N, H, W, C, nullptr, nullptr, TC_TF32, &pl) ? pl.m_ctas : 0;
+    return tc_get_encode_fn() && tc_plan_taps(N, H, W, C, nullptr, nullptr, TC_TF32, &pl) ? pl.m_ctas : 0;
 }
 
 // 1 if a TF32 (or bf16) call with these taps runs on the halo-slab path
@@ -711,7 +722,7 @@ extern "C" int lf_conv1d_tc_slab_ok(int N, int H, int W, int C, int vertical, in
     if (g_tc_variant == 1 || dil < 1) return 0;
     TcPlan pl{};
     const int zero[3] = {0, 0, 0}, off[3] = {-dil, 0, dil};
-    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_TF32, &pl) ? 1 : 0;
+    return tc_get_encode_fn() && tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_TF32, &pl) ? 1 : 0;
 }
 
 // rows of colsum_partial / stats_partial (= CTAs per 64-channel half), 0 if a 3xTF32 call with these taps is not served
@@ -719,7 +730,24 @@ extern "C" int lf_conv1d_tc_x3_rows(int N, int H, int W, int C, int vertical, in
     if (dil < 1) return 0;
     TcPlan pl{};
     const int zero[3] = {0, 0, 0}, off[3] = {-dil, 0, dil};
-    return tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_X3, &pl) ? pl.m_ctas : 0;
+    return tc_get_encode_fn() && tc_plan_slab(N, H, W, C, vertical ? off : zero, vertical ? zero : off, TC_X3, &pl) ? pl.m_ctas : 0;
+}
+
+// The plan tc_run would launch for these arguments (the same selection, no device needed): see the header
+extern "C" int lf_conv1d_tc_plan(int prec, int in_dtype, int N, int H, int W, int C, const int* dy, const int* dx, int* info) {
+    LF_REQUIRE(prec >= TC_TF32 && prec <= TC_FP8 && dy && dx && info);
+    LF_REQUIRE(N >= 1 && H >= 1 && W >= 1);
+    LF_REQUIRE(in_dtype == LF_F32 || in_dtype == LF_BF16);
+    if (in_dtype == LF_BF16 && !tc_takes_bf16(prec)) return LF_ERR_UNSUPPORTED;
+    TcPlan pl{};
+    bool slab = false;
+    const int rc = tc_select(prec, in_dtype == LF_BF16, N, H, W, C, dy, dx, &pl, &slab);
+    if (rc != LF_OK) return rc;
+    const TcArgs& g = pl.geo;
+    const int v[LF_TC_PLAN_INFO] = {slab ? 1 : 0, pl.res ? 1 : 0, g.stages, g.n_lo, g.lo_stg, g.lo_bytes,
+                                    g.TA, g.TB, g.vertical, pl.m_ctas, pl.smem_bytes, g.a_bytes};
+    for (int i = 0; i < LF_TC_PLAN_INFO; ++i) info[i] = v[i];
+    return LF_OK;
 }
 
 extern "C" int lf_conv1d_tc(const LfConvTcArgs* args, lf_stream_t stream) { return tc_run(args, stream, TC_TF32); }

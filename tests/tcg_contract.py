@@ -249,7 +249,7 @@ def emulate_wgrad_reduce(args, tensors):
     partial, nsplit, ntaps, cp, cq, cpp, cqp, dst, st_, sp, sq, _stream = args
     src = next(t for t in tensors if t.data_ptr() == partial)
     red = src.reshape(-1)[:nsplit * ntaps * cpp * cqp].view(nsplit, ntaps, cpp, cqp)[:, :, :cp, :cq].double().sum(0).float()
-    res = next(t for t in tensors if t.data_ptr() <= dst < t.data_ptr() + t.numel() * 4)
+    res, _ = _locate(dst, tensors)   # by each tensor's own byte extent: a bf16 tensor just below dst is not the destination
     idx = ((dst - res.data_ptr()) // 4 + torch.arange(ntaps).view(-1, 1, 1) * st_ + torch.arange(cp).view(1, -1, 1) * sp
            + torch.arange(cq).view(1, 1, -1) * sq)
     res.reshape(-1)[idx.reshape(-1)] = red.reshape(-1)
