@@ -454,6 +454,23 @@ int lf_backproj_loss_host(const double* Y56, const double* yprime, const double*
                           const double* valid, int B, int L, int n, double* lane_loss, double* loss, double* dbeta,
                           double* xcal);
 
+/* Area loss of the bird's-eye-view experiment over all lanes, its gradient and the exact-area metric in one launch
+ * (csrc/loss.cu; replaces Birds_Eye_View_Loss/Loss_crit.py:98-134 summed over the lanes as BEV/main.py:223,237 does, and
+ * the `polynomial.trapezoidal` metric of BEV/main.py:273-280,436-442).  Order 2 only.
+ *   beta [B][L][3], params [B][4][3] (the loader's ground-truth coefficients): float32 DEVICE inputs; L is 2 or 4, B >= 1;
+ *   weight: 0 none (W = 1), 1 linear (W = 1 - y), 2 quadratic (W = 1 - sqrt y); anything else LF_ERR_INVALID_ARGUMENT.
+ *   loss [1] = sum_l mean over the images whose three params[b][l] are all non-zero of int_0^0.7 W (beta - params)^2 dy
+ *     (0 for a lane without such an image): float64 terms, fixed-order sums, one rounding to float32;
+ *   dbeta [B][L][3] = d loss / d beta, same arithmetic;
+ *   exact [B] = (trap(lane 0) + trap(lane 1)) / 2, trap the reference's float32 trapezium rule (101 points on [0, 0.7]),
+ *     bit-identical to polynomial(beta).trapezoidal(polynomial(params)) on the CPU;  exact_mean [1] = its batch mean.
+ *   Every output may be NULL.  One CTA, no atomics, deterministic; no host synchronisation (capturable).
+ * lf_area_loss_host runs the SAME per-image code and summation order on host arrays: a test hook, not a fallback. */
+int lf_area_loss(const float* beta, const float* params, int B, int L, int weight, float* loss, float* dbeta, float* exact,
+                 float* exact_mean, lf_stream_t stream);
+int lf_area_loss_host(const float* beta, const float* params, int B, int L, int weight, float* loss, float* dbeta,
+                      float* exact, float* exact_mean);
+
 /* Fully connected layers of the Classification heads (csrc/linear.cu; replaces nn.Linear at
  * BP/Networks/LSQ_layer.py:188-192,203-206): y[b][o] = bias[o] + sum_k x[b][k] W[o][k], W in nn.Linear's [O][K] layout,
  * fp32, deterministic.  partial: caller-owned scratch of lf_linear_chunks(K)*B*O floats.  relu: apply ReLU to y.

@@ -5,6 +5,8 @@ reference's ``Loss_crit.py`` (BP/Loss_crit.py; BEV: Birds_Eye_View_Loss/Loss_cri
   backprojection_loss   :161-218   (float64; supplies dL/dbeta to the fused LSQ backward)
   Area_Loss             :87-143    (closed-form weighted area between curves)
   MSE_Loss              :146-159
+  polynomial            Birds_Eye_View_Loss/Loss_crit.py:12-35 (the exact-area metric's trapezium rule, CPU)
+  fused_area_loss       Area_Loss over all lanes + the exact-area metric in one launch (lf_area_loss)
 The arithmetic here is O(B*56) float64 -- launch-latency, not bandwidth; fusing it into
 the LSQ kernels' epilogue/prologue is SURVEY.md 8f rank 1 ("next").
 """
@@ -260,3 +262,76 @@ class MSE_Loss(nn.Module):
 
     def forward(self, params, gt_params, compute=True):
         return self.loss_crit(params.squeeze(-1), gt_params)
+
+
+class polynomial:
+    """x(y) = a y^2 + b y + c per image, integrated with the trapezium rule (Birds_Eye_View_Loss/Loss_crit.py:12-35).
+    ``coeffs``: [B, 3] or [B, 3, 1]; ``trapezoidal(other)`` is the area between the two curves on [a, b] in n steps, in
+    the coefficients' dtype -- on float32 CPU tensors the reference's bits (lf_area_loss's exact output restates it)."""
+
+    def __init__(self, coeffs, a=0, b=0.7, n=100):
+        self.a1, self.b1, self.c1 = (t.squeeze() for t in torch.chunk(coeffs, 3, 1))
+        self.a, self.b, self.n = a, b, n
+
+    def calc_pol(self, x):
+        return self.a1 * x ** 2 + self.b1 * x + self.c1
+
+    def trapezoidal(self, other):
+        h = float(self.b - self.a) / self.n
+        s = 0.0 + abs(self.calc_pol(self.a) / 2.0 - other.calc_pol(other.a) / 2.0)
+        for i in range(1, self.n):
+            x = self.a + i * h
+            s += abs(self.calc_pol(x) - other.calc_pol(x))
+        s += abs(self.calc_pol(self.b) / 2.0 - other.calc_pol(self.b) / 2.0)
+        return s * h
+
+
+AREA_WEIGHTS = {"none": 0, "linear": 1, "quadratic": 2}     # lf_area_loss's weight argument
+
+
+class _FusedAreaLoss(torch.autograd.Function):
+    """sum over lanes of Area_Loss (order 2) and the exact-area batch mean, ONE launch (csrc/loss.cu: lf_area_loss)."""
+
+    @staticmethod
+    def forward(ctx, beta, params, weight, exact):
+        _capi.require_cuda(beta, params)
+        B, L, _ = beta.shape
+        out = torch.empty(2 + B * L * 3, dtype=torch.float32, device=beta.device)
+        loss, exact_mean, dbeta = out[0:1], out[1:2], out[2:].view(B, L, 3)
+        p = _capi.ptr
+        _capi.call("lf_area_loss", p(beta), p(params), B, L, weight, p(loss), p(dbeta), None, p(exact_mean) if exact else None,
+                   _capi.stream_ptr())
+        ctx.save_for_backward(dbeta)
+        ctx.mark_non_differentiable(exact_mean)
+        return loss.reshape(()), exact_mean.reshape(())
+
+    @staticmethod
+    def backward(ctx, g, _g_exact):
+        (dbeta,) = ctx.saved_tensors
+        return dbeta * g, None, None, None
+
+
+def fused_area_loss(betas, params, weight_funct, exact=False):
+    """``sum_l Area_Loss(2, weight_funct)(betas[l], params[:, l])`` -- BEV/main.py:223,237 -- and, with ``exact``, the
+    exact-area metric ``((trap_left + trap_right) / 2).mean()`` of BEV/main.py:273-280, in one launch on the device.
+    betas: sequence of L (2 or 4) float32 tensors [B, 3, 1] (Net.forward's beta0..3); params: the loader's [B, 4, 3].
+    Returns (loss, exact_mean or None), float32 0-d tensors; only the loss has a gradient.
+
+    The loss sums float64 terms in a fixed order and rounds once, so it is the reference's value to float32 rounding (not
+    its float32 bits).  A lane that no image has contributes 0, also when none has any lane (where Area_Loss returns the
+    Python 0).  The 4-lane masks of main.py:226-234 multiply by 1 exactly the images Area_Loss selects, so they change
+    neither the value nor the gradient and are not applied.  The per-image metric is the reference's float32 bits; the
+    mean differs from torch's .mean() by summation order only."""
+    if weight_funct not in AREA_WEIGHTS:
+        raise ValueError("unknown weight_funct %r (none, linear or quadratic)" % (weight_funct,))
+    if len(betas) not in (2, 4):
+        raise ValueError("fused_area_loss takes 2 or 4 lanes, got %d" % len(betas))
+    B = params.shape[0]
+    for b in betas:
+        if b.numel() != B * 3:
+            raise ValueError("order 2 only: every beta must be [B, 3, 1], got %s" % (tuple(b.shape),))
+    if tuple(params.shape) != (B, 4, 3):
+        raise ValueError("params must be [B, 4, 3], got %s" % (tuple(params.shape),))
+    beta = torch.stack([b.reshape(B, 3) for b in betas], 1).float().contiguous()
+    loss, exact_mean = _FusedAreaLoss.apply(beta, params.float().contiguous(), AREA_WEIGHTS[weight_funct], bool(exact))
+    return loss, (exact_mean if exact else None)

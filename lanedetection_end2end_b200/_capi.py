@@ -220,6 +220,8 @@ _NET_PROTOS = {
     "lf_pack_gather": (_i, [_p, _i, _i, _p]),
     "lf_backproj_loss": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
     "lf_backproj_loss_host": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p]),
+    "lf_area_loss": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "lf_area_loss_host": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p]),
     "lf_seg_lane_maps": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p]),
     "lf_seg_lane_maps_line": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p, _p]),
     "lf_ce2d_blocks": (_i, [_i, _i, _i]),

@@ -1,5 +1,5 @@
-"""Birds_Eye_View_Loss/Loss_crit.py mirror: Area_Loss (:78-134) and MSE_Loss (:137-150) are shared
-with the BP mirror."""
+"""Birds_Eye_View_Loss/Loss_crit.py mirror: polynomial (:12-35), Area_Loss (:78-134) and MSE_Loss (:137-150) are shared
+with the BP mirror, with fused_area_loss (the lanes' Area_Loss and the exact-area metric in one launch)."""
 import importlib
 import os
 import sys
@@ -13,3 +13,5 @@ except ImportError:
 Area_Loss = _L.Area_Loss
 MSE_Loss = _L.MSE_Loss
 define_loss_crit = _L.define_loss_crit
+polynomial = _L.polynomial
+fused_area_loss = _L.fused_area_loss

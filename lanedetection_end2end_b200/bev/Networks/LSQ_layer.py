@@ -68,6 +68,8 @@ Classification = _L.Classification
 
 
 class Net(nn.Module):
+    takes_gt_line = False           # forward(input, end_to_end): engine.model_forward calls it without the BP gt_line
+
     def __init__(self, args):
         super().__init__()
         from . import define_model

@@ -187,3 +187,253 @@ extern "C" int lf_backproj_loss_host(const double* Y56, const double* yprime, co
     *loss = tot / (double)L;
     return LF_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Area loss of the bird's-eye-view experiment over all lanes, its gradient and the exact-area metric in one launch:
+// Birds_Eye_View_Loss/Loss_crit.py:98-134 (`Area_Loss`, order 2) summed over the lanes as BEV/main.py:223,237 does, and
+// `polynomial.trapezoidal` (:12-35) as BEV/main.py:273-280 / :436-442 evaluates it.
+//
+//   d       = beta[b][l] - params[b][l]                    (a, b, c in float64 from the float32 inputs)
+//   f(d)    = int_0^0.7 W(y) (a y^2 + b y + c)^2 dy = sum_ij Q_ij d_i d_j,   Q_ij = int_0^0.7 W(y) y^(p_i + p_j) dy
+//   loss    = sum_l (1 / n_l) sum_{b present in l} f(d)    (n_l images whose three ground-truth coefficients are non-zero;
+//                                                            a lane with none contributes 0)
+//   dbeta   = present ? 2 (Q d) / n_l : 0
+//   exact_b = (trap(beta_0, gt_0) + trap(beta_1, gt_1)) / 2 in the reference's float32 arithmetic, op for op
+//
+// The quadratic form holds the reference's three closed forms (none, linear, quadratic) term by term.  float64 terms,
+// sums in a fixed order (thread t takes images t, t + T, ...; then a fixed tree), one rounding to float32 at the end.
+// `lf_area_loss_host` replays the same per-image code and the same summation order on host arrays (a test hook); the
+// explicit round-to-nearest intrinsics keep nvcc from contracting a multiply and an add into one FMA, which the host
+// code does not do, so both give the same bits.
+namespace lf {
+
+constexpr int AREA_THREADS = 128;
+constexpr int AREA_STEPS = 100;     // polynomial(..., n=100)
+constexpr int AREA_MAXL = 4;
+
+struct AreaConst {
+    double Q[3][3];                 // moments of the weight function (a, b, c order: powers 2, 1, 0)
+    float x[AREA_STEPS + 1];        // float32(x_i), x_i = i * h as Python computes it; x_100 = 0.7 (self.b)
+    float x2[AREA_STEPS + 1];       // float32(x_i ** 2)
+    float h;                        // float32(0.7 / 100)
+};
+
+__host__ __device__ inline float area_fmul(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+
+__host__ __device__ inline float area_fadd(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+__host__ __device__ inline double area_dmul(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+
+__host__ __device__ inline double area_dadd(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+__host__ __device__ inline float area_fsub(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+
+// polynomial.calc_pol: (a1 * x**2 + b1 * x) + c1, every op rounded to float32
+__host__ __device__ inline float area_pol(const float* p, float x2, float x) {
+    return area_fadd(area_fadd(area_fmul(p[0], x2), area_fmul(p[1], x)), p[2]);
+}
+
+// polynomial(pred).trapezoidal(polynomial(gt)) of one image
+__host__ __device__ inline float area_trap(const AreaConst& c, const float* pred, const float* gt) {
+    float s = fabsf(area_fsub(area_fmul(area_pol(pred, c.x2[0], c.x[0]), 0.5f), area_fmul(area_pol(gt, c.x2[0], c.x[0]), 0.5f)));
+    for (int i = 1; i < AREA_STEPS; ++i)
+        s = area_fadd(s, fabsf(area_fsub(area_pol(pred, c.x2[i], c.x[i]), area_pol(gt, c.x2[i], c.x[i]))));
+    const int e = AREA_STEPS;
+    s = area_fadd(s, fabsf(area_fsub(area_fmul(area_pol(pred, c.x2[e], c.x[e]), 0.5f), area_fmul(area_pol(gt, c.x2[e], c.x[e]), 0.5f))));
+    return area_fmul(s, c.h);
+}
+
+// one (image, lane): present flag, f(d) and Q d
+__host__ __device__ inline bool area_term(const AreaConst& c, const float* beta, const float* gt, double* f, double qd[3]) {
+    const double d[3] = {(double)beta[0] - (double)gt[0], (double)beta[1] - (double)gt[1], (double)beta[2] - (double)gt[2]};
+    double s = 0.0;
+    for (int i = 0; i < 3; ++i) {
+        qd[i] = area_dadd(area_dadd(area_dmul(c.Q[i][0], d[0]), area_dmul(c.Q[i][1], d[1])), area_dmul(c.Q[i][2], d[2]));
+        s = area_dadd(s, area_dmul(d[i], qd[i]));
+    }
+    *f = s;
+    return gt[0] != 0.0f && gt[1] != 0.0f && gt[2] != 0.0f;
+}
+
+// per-"thread" partial sums of one image: lane sums, lane counts, exact value (slot 2 * AREA_MAXL)
+__host__ __device__ inline void area_accumulate(const AreaConst& c, const float* beta, const float* params, int b, int L,
+                                                bool want_exact, double acc[2 * AREA_MAXL + 1], float* exact) {
+#pragma unroll
+    for (int l = 0; l < AREA_MAXL; ++l) {      // constant indices: acc stays in registers
+        double f, qd[3];
+        if (l < L && area_term(c, beta + ((size_t)b * L + l) * 3, params + ((size_t)b * 4 + l) * 3, &f, qd)) {
+            acc[l] += f;
+            acc[AREA_MAXL + l] += 1.0;
+        }
+    }
+    if (want_exact) {
+        const float tl = area_trap(c, beta + (size_t)b * L * 3, params + (size_t)b * 12);
+        const float tr = area_trap(c, beta + ((size_t)b * L + 1) * 3, params + ((size_t)b * 4 + 1) * 3);
+        const float e = area_fmul(area_fadd(tl, tr), 0.5f);
+        if (exact) exact[b] = e;
+        acc[2 * AREA_MAXL] += (double)e;
+    }
+}
+
+__host__ __device__ inline void area_gradient(const AreaConst& c, const float* beta, const float* params, int b, int L,
+                                              const double* inv_n, float* dbeta) {
+#pragma unroll
+    for (int l = 0; l < AREA_MAXL; ++l) {
+        if (l >= L) break;
+        double f, qd[3];
+        const bool present = area_term(c, beta + ((size_t)b * L + l) * 3, params + ((size_t)b * 4 + l) * 3, &f, qd);
+        for (int k = 0; k < 3; ++k) dbeta[((size_t)b * L + l) * 3 + k] = present ? (float)area_dmul(area_dmul(2.0, qd[k]), inv_n[l]) : 0.0f;
+    }
+}
+
+// loss from the reduced sums; fills inv_n (0 for a lane without images)
+__host__ __device__ inline float area_finish(const double* acc, int L, double* inv_n) {
+    double loss = 0.0;
+#pragma unroll
+    for (int l = 0; l < AREA_MAXL; ++l) {
+        if (l >= L) {
+            inv_n[l] = 0.0;
+            continue;
+        }
+        const double n = acc[AREA_MAXL + l];
+        inv_n[l] = n == 0.0 ? 0.0 : 1.0 / n;
+        loss = area_dadd(loss, area_dmul(acc[l], inv_n[l]));
+    }
+    return (float)loss;
+}
+
+__global__ void __launch_bounds__(AREA_THREADS) area_loss_kernel(const AreaConst c, const float* __restrict__ beta,
+                                                                  const float* __restrict__ params, int B, int L,
+                                                                  float* __restrict__ loss, float* __restrict__ dbeta,
+                                                                  float* __restrict__ exact, float* __restrict__ exact_mean) {
+    pdl_entry();
+    constexpr int NA = 2 * AREA_MAXL + 1;
+    __shared__ double red[NA][AREA_THREADS];
+    __shared__ double s_inv_n[AREA_MAXL];
+    const int tid = threadIdx.x;
+    const bool want_exact = exact || exact_mean;
+    double acc[NA];
+#pragma unroll
+    for (int j = 0; j < NA; ++j) acc[j] = 0.0;
+    for (int b = tid; b < B; b += AREA_THREADS) area_accumulate(c, beta, params, b, L, want_exact, acc, exact);
+#pragma unroll
+    for (int j = 0; j < NA; ++j) red[j][tid] = acc[j];
+    __syncthreads();
+    for (int w = AREA_THREADS / 2; w > 0; w >>= 1) {     // fixed tree
+        if (tid < w) {
+#pragma unroll
+            for (int j = 0; j < NA; ++j) red[j][tid] += red[j][tid + w];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        double tot[NA], inv_n[AREA_MAXL];
+#pragma unroll
+        for (int j = 0; j < NA; ++j) tot[j] = red[j][0];
+        const float l = area_finish(tot, L, inv_n);
+        if (loss) *loss = l;
+        if (exact_mean) *exact_mean = (float)(tot[2 * AREA_MAXL] / (double)B);
+#pragma unroll
+        for (int j = 0; j < AREA_MAXL; ++j) s_inv_n[j] = inv_n[j];
+    }
+    __syncthreads();
+    if (dbeta)
+        for (int b = tid; b < B; b += AREA_THREADS) area_gradient(c, beta, params, b, L, s_inv_n, dbeta);
+}
+
+static int area_fill_const(int weight, AreaConst* c) {
+    // moments M_k = int_0^t W(y) y^k dy, t = 0.7, of W = 1 (0), 1 - y (1), 1 - sqrt(y) (2)
+    const double t = 0.7;
+    double M[5];
+    for (int k = 0; k <= 4; ++k) {
+        M[k] = pow(t, k + 1.0) / (k + 1.0);
+        if (weight == 1) M[k] -= pow(t, k + 2.0) / (k + 2.0);
+        else if (weight == 2) M[k] -= pow(t, k + 1.5) / (k + 1.5);
+        else if (weight != 0) return LF_ERR_INVALID_ARGUMENT;
+    }
+    const int p[3] = {2, 1, 0};
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) c->Q[i][j] = M[p[i] + p[j]];
+    // polynomial(..., a=0, b=0.7, n=100): h = 0.7 / 100, x_i = 0 + i*h in Python doubles, x ** 2 through libm's pow as
+    // Python's float power does; torch rounds each Python scalar to float32 against a float32 tensor
+    const double h = 0.7 / AREA_STEPS;
+    for (int i = 0; i <= AREA_STEPS; ++i) {
+        const double x = i == AREA_STEPS ? 0.7 : (double)i * h;
+        c->x[i] = (float)x;
+        c->x2[i] = (float)pow(x, 2.0);
+    }
+    c->h = (float)h;
+    return LF_OK;
+}
+
+}  // namespace lf
+
+// beta [B][L][3], params [B][4][3] float32: DEVICE; weight 0 none / 1 linear / 2 quadratic; outputs DEVICE, each optional.
+extern "C" int lf_area_loss(const float* beta, const float* params, int B, int L, int weight, float* loss, float* dbeta,
+                            float* exact, float* exact_mean, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(beta && params && B > 0 && (L == 2 || L == 4));
+    AreaConst c;
+    int rc = area_fill_const(weight, &c);
+    if (rc) return rc;
+    lf_launch(area_loss_kernel, 1, AREA_THREADS, 0, stream, c, beta, params, B, L, loss, dbeta, exact, exact_mean);
+    return check_launch();
+}
+
+// TEST HOOK: the kernel's per-image code and summation order on HOST arrays; never called by the package.
+extern "C" int lf_area_loss_host(const float* beta, const float* params, int B, int L, int weight, float* loss, float* dbeta,
+                                 float* exact, float* exact_mean) {
+    if (!(beta && params && B > 0 && (L == 2 || L == 4))) return LF_ERR_INVALID_ARGUMENT;
+    AreaConst c;
+    int rc = area_fill_const(weight, &c);
+    if (rc) return rc;
+    constexpr int NA = 2 * AREA_MAXL + 1;
+    static thread_local double red[NA][AREA_THREADS];
+    const bool want_exact = exact || exact_mean;
+    for (int t = 0; t < AREA_THREADS; ++t) {
+        double acc[NA] = {0.0};
+        for (int b = t; b < B; b += AREA_THREADS) area_accumulate(c, beta, params, b, L, want_exact, acc, exact);
+        for (int j = 0; j < NA; ++j) red[j][t] = acc[j];
+    }
+    for (int w = AREA_THREADS / 2; w > 0; w >>= 1)
+        for (int t = 0; t < w; ++t)
+            for (int j = 0; j < NA; ++j) red[j][t] += red[j][t + w];
+    double tot[NA], inv_n[AREA_MAXL];
+    for (int j = 0; j < NA; ++j) tot[j] = red[j][0];
+    const float l = area_finish(tot, L, inv_n);
+    if (loss) *loss = l;
+    if (exact_mean) *exact_mean = (float)(tot[2 * AREA_MAXL] / (double)B);
+    if (dbeta)
+        for (int b = 0; b < B; ++b) area_gradient(c, beta, params, b, L, inv_n, dbeta);
+    return LF_OK;
+}

@@ -21,6 +21,14 @@ import torch
 FUSED_LOSS = os.environ.get("LANEFIT_FUSED_LOSS", "1") != "0"
 
 
+def model_forward(model, x, gt_line, end_to_end):
+    """Net.forward of either experiment: the back-projection Net takes (input, gt_line, end_to_end), the bird's-eye-view
+    Net (``takes_gt_line = False``) takes (input, end_to_end)."""
+    if getattr(model, "takes_gt_line", True):
+        return model(x, gt_line, end_to_end)
+    return model(x, end_to_end)
+
+
 def batchnorm_running_stats(model):
     """The running statistics of every BatchNorm container (nn.BatchNorm2d, nn.SyncBatchNorm, ...): a replay updates them
     through raw pointers, so their versions are bumped after it."""
@@ -102,7 +110,7 @@ class GraphedTrainStep:
             if self.optimizer is not None:
                 self.model.lsq_status.zero_()
             torch._foreach_zero_(self.grads)
-        out = self.model(self.x, self.gt_line, self.end_to_end)
+        out = model_forward(self.model, self.x, self.gt_line, self.end_to_end)
         scale = None
         if self.global_valid:
             from .ddp import lane_valid_scale
@@ -200,14 +208,14 @@ class GraphedInference:
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(max(1, warmup)):             # builds and caches the folded operands outside the capture
-                out = model(self.x, self.gt_line, end_to_end)
+                out = model_forward(model, self.x, self.gt_line, end_to_end)
                 if post is not None:
                     post(out)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(self.graph):
-            self.out = model(self.x, self.gt_line, end_to_end)
+            self.out = model_forward(model, self.x, self.gt_line, end_to_end)
             if post is not None:
                 self.post_out = post(self.out)
 
@@ -285,6 +293,20 @@ def lane_losses(criterion, out, lanes, vp, L):
 
 def _reporting(i, freq):
     return freq > 0 and (i + 1) % freq == 0
+
+
+def _keeping_batchnorm_stats(model, build):
+    """``build()`` with the BatchNorm running statistics restored afterwards: a GraphedTrainStep's warm-up steps are
+    training forwards, which would move them."""
+    bns = [m for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)]
+    saved = [[t.clone() if t is not None else None for t in (m.running_mean, m.running_var, m.num_batches_tracked)]
+             for m in bns]
+    out = build()
+    for m, ts in zip(bns, saved):
+        for t, v in zip((m.running_mean, m.running_var, m.num_batches_tracked), ts):
+            if t is not None:
+                t.copy_(v)
+    return out
 
 
 def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch):
@@ -366,17 +388,9 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
                     static[k] = v.to(dev, non_blocking=True).clone()
                 static["input"] = static["input"].float()
                 static["gt"] = static["gt"].long()
-                # the warm-up steps are training forwards: keep the BatchNorm running statistics they would move
-                bns = [m for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)]
-                saved = [[t.clone() if t is not None else None for t in (m.running_mean, m.running_var, m.num_batches_tracked)]
-                         for m in bns]
-                step = GraphedTrainStep(model, criterion, L, static["input"], static["lanes"], static["valid"],
-                                        optimizer=optimizer, gt_line=None if e2e else static["gt_line"], end_to_end=e2e,
-                                        loss_fn=loss_fn, post=post)
-                for m, ts in zip(bns, saved):
-                    for t, v in zip((m.running_mean, m.running_var, m.num_batches_tracked), ts):
-                        if t is not None:
-                            t.copy_(v)
+                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
+                    model, criterion, L, static["input"], static["lanes"], static["valid"], optimizer=optimizer,
+                    gt_line=None if e2e else static["gt_line"], end_to_end=e2e, loss_fn=loss_fn, post=post))
                 static["input"] = step.x              # the step's own copies are what its forward reads
                 if not e2e:
                     static["gt_line"] = step.gt_line
@@ -414,3 +428,129 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     m = meters.read()
     status.print_skipped(labels)
     return m["loss"][1], m["rmse"][1]
+
+
+def check_bev_args(args):
+    """The settings train_epoch_bev and inference.validate_bev run: ValueError naming the first one they do not."""
+    from .Loss_crit import AREA_WEIGHTS
+    if args.clas:
+        raise ValueError("--clas is not supported: the bird's-eye-view Net builds no line-type or horizon heads")
+    if args.pretrained:
+        raise ValueError("--pretrained is not supported: its segmentation phase and the switch to end-to-end change the "
+                         "parameter set, which a FusedOptimizer refuses")
+    if args.loss_policy != "area":
+        raise ValueError("loss_policy %r is not supported: the bird's-eye-view loop runs the area loss" % args.loss_policy)
+    if args.order != 2:
+        raise ValueError("order %d is not supported: the area loss and the exact-area metric take order 2 (three "
+                         "coefficients, as the loader's params)" % args.order)
+    if args.weight_funct not in AREA_WEIGHTS:
+        raise ValueError("unknown weight_funct %r (none, linear or quadratic)" % (args.weight_funct,))
+    if not args.end_to_end and args.nclasses != 2:
+        raise ValueError("--end_to_end False needs 2 lanes: the bird's-eye-view Net's segmentation branch fits two lane "
+                         "maps")
+
+
+def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch):
+    """One training epoch of the bird's-eye-view experiment's main.py loop (Birds_Eye_View_Loss/main.py:186-295), each
+    batch one replay of a GraphedTrainStep that holds the forward, the loss, the backward, the fused optimizer's update
+    and the meter updates.  Returns (losses.avg, avg_area.avg, exact_area.avg).
+
+    The loader yields the BEV train loader's 6-tuples (input, gt, params, idx, gt_line, gt_horizon), on the device as
+    bev.Dataloader.Load_Data_new gives them (host tensors are copied in); every batch has the first one's size.
+    ``optimizer`` must be an optim.FusedOptimizer: the update sits in the graph, guarded by the LSQ status word, so a batch
+    with a singular system changes no parameter, no optimizer state and no meter, without a host synchronisation; the
+    reference's line for each such batch is printed at the end of the epoch.  The host synchronises only at the print_freq
+    lines, at save_weightmap('train', ...) every save_freq batches and at the end.
+
+    End-to-end, the loss is Loss_crit.fused_area_loss over the lanes (main.py:222-237; the 4-lane masks change nothing,
+    see there): float64 terms rounded once, so it equals the reference's float32 sum to rounding.  --end_to_end False:
+    criterion_seg(output, gt), and the 2-lane area without gradient as avg_area (main.py:239-244).  The exact-area metric
+    (main.py:272-280) comes from the same launch, per image bit-identical to the reference's CPU polynomial.  --clas,
+    --pretrained, loss policies other than area, orders other than 2 and other lane counts raise ValueError
+    (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch.  Dropout masks are drawn in the
+    graph; BatchNorm running statistics are those of the epoch's batches."""
+    from .optim import FusedOptimizer
+    from .Loss_crit import fused_area_loss
+    from .Networks import utils as nutils
+    if not isinstance(optimizer, FusedOptimizer):
+        raise TypeError("train_epoch_bev runs the update in the graph: it needs an optim.FusedOptimizer "
+                        "(define_optim(..., fused=True)), got %s" % type(optimizer).__name__)
+    check_bev_args(args)
+    e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
+    dev = next(model.parameters()).device
+    model.train()
+    meters = DeviceMeters(("loss", "area", "exact"), dev)
+    status = BatchStatus(len(loader), dev)
+    static = {}
+
+    def loss_fn(out):
+        if e2e:
+            loss, static["exact"] = fused_area_loss(out[:L], static["params"], wf, exact=True)
+            return loss
+        with torch.no_grad():
+            static["area"], static["exact"] = fused_area_loss(out[:2], static["params"], wf, exact=True)
+        return criterion_seg(out[6], static["gt"])
+
+    def post(out, loss):
+        if not torch.cuda.is_current_stream_capturing():
+            return None                      # warm-up steps: no meter or log entry
+        ok = model.lsq_status.reshape(()).eq(0)
+        n = static["input"].shape[0]
+        if not e2e:
+            meters.update("area", static["area"], ok, n)
+        meters.update("loss", loss, ok, n)
+        meters.update("exact", static["exact"], ok, n)
+        status.record(model.lsq_status)
+        return out
+
+    step, labels, M_inv = None, [], None
+    bt_sum, bt_n, end = 0.0, 0, time.time()
+    deferred = model.defer_status_check
+    try:
+        for i, (input, gt, params, idx, gt_line, gt_horizon) in enumerate(loader):
+            batch = {"input": input, "gt": gt, "params": params}
+            if step is None:
+                for k, v in batch.items():
+                    static[k] = v.to(dev, non_blocking=True).clone()
+                static["input"] = static["input"].float()
+                # the BEV loss reads its batch through loss_fn: the step's lane-sample inputs stay empty
+                none = torch.empty(0, device=dev)
+                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
+                    model, criterion, L, static["input"], none, none, optimizer=optimizer, end_to_end=e2e,
+                    loss_fn=loss_fn, post=post))
+                static["input"] = step.x              # the step's own copy is what its forward reads
+            else:
+                if input.shape[0] != step.x.shape[0]:
+                    raise ValueError("batch of %d images after a first batch of %d: train_epoch_bev replays one batch "
+                                     "size" % (input.shape[0], step.x.shape[0]))
+                for k, v in batch.items():
+                    static[k].copy_(v, non_blocking=True)
+            status.check(i)
+            labels.append(idx)
+            step()
+            now = time.time()
+            bt_val, end = now - end, now
+            bt_sum, bt_n = bt_sum + bt_val, bt_n + 1
+            if not (_reporting(i, args.print_freq) or _reporting(i, args.save_freq)) or int(status.log[i]):
+                continue                             # a skipped batch reports nothing, as main.py's `continue`
+            if _reporting(i, args.print_freq):
+                m = meters.read()
+                print('Epoch: [{0}][{1}/{2}]\t'
+                      'Time {3:.3f} ({4:.3f})\t'
+                      'Loss {loss[0]:.8f} ({loss[1]:.8f})'.format(
+                          epoch + 1, i + 1, len(loader), bt_val, bt_sum / bt_n, loss=m["loss"]))
+            if _reporting(i, args.save_freq):
+                if M_inv is None:
+                    from .Dataloader.Load_Data_new import get_homography
+                    M_inv = get_homography(args.resize)
+                out, p = step.post_out, static["params"]
+                nutils.save_weightmap('train', out[5], M_inv, out[4], *out[:4], p[:, 0, :], p[:, 1, :], p[:, 2, :],
+                                      p[:, 3, :], gt_line, static["gt"], 0, i, static["input"], args.no_ortho, args.resize,
+                                      args.save_path)
+    finally:
+        model.defer_status_check = deferred
+    if step is None:
+        return 0, 0, 0
+    m = meters.read()
+    status.print_skipped(labels)
+    return m["loss"][1], m["area"][1], m["exact"][1]

@@ -10,6 +10,7 @@ curve coefficients after ``model(input, ...)``.
   TuSimpleScorer             BP/test.py:66-99 + eval_lane.py:27-95  gating and LaneEval scoring on the GPU, one launch
                                                  (lf_tusimple_score, csrc/tusimple.cu) per batch
   test_model                 BP/test.py:23-129   the per-epoch test-set evaluation, one CUDA-graph replay per batch
+  validate / validate_bev    BP/main.py:419-526, BEV/main.py:362-501  validation passes, one CUDA-graph replay per batch
 
 ``Projections.compute_coordinates`` keeps the reference's name, argument and result ([B, order+1, 1] float64 -> [B, 56]
 float64, in 1280x720 pixels); on a CUDA tensor it is ONE launch of lf_backproj_loss (csrc/loss.cu, the kernel that
@@ -410,3 +411,102 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
             print("===> Average HORIZON ACC on val is {:.8}".format(m["acc_hor"][1]))
             print("===> Average LINE ACC on val is {:.8}".format(m["acc_hor"][1]))
     return m["loss"][1], m["acc_hor"][1], m["acc_line"][1], m["rmse"][1]
+
+
+def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, M_inv, args, epoch=0):
+    """The bird's-eye-view experiment's validation pass (Birds_Eye_View_Loss/main.py:362-501), same return value:
+    (losses.avg, avg_area.avg, avg_trapezium_rule.avg, acc_hor_tot.avg, acc_line_tot.avg), the accuracies 0 (--clas is
+    refused, engine.check_bev_args).
+
+    The loader yields the BEV valid loader's 7-tuples (input, gt, params, idx, gt_line, gt_horizon, index), on the device
+    as bev.Dataloader.Load_Data_new gives them.  Each batch is one replay of a GraphedInference whose post= hook holds
+    Loss_crit.fused_area_loss (the lanes' area loss and the exact-area metric, one launch), with --end_to_end False
+    criterion_seg and the 2-lane area, and the meter updates guarded by the LSQ status word: a batch with a singular system
+    updates no meter, as main.py's `continue` does, and its line is printed at the end of the pass.  A batch shorter than
+    the first is replayed by a second graph of its size.  The host synchronises only at the print_freq lines, at
+    save_weightmap('valid', ...) every 25 batches and at the end."""
+    if __package__:
+        from .engine import GraphedInference, DeviceMeters, BatchStatus, _reporting, check_bev_args
+        from .Loss_crit import fused_area_loss
+        from .Networks import utils as nutils
+    else:
+        from engine import GraphedInference, DeviceMeters, BatchStatus, _reporting, check_bev_args
+        from Loss_crit import fused_area_loss
+        from Networks import utils as nutils
+    check_bev_args(args)
+    e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
+    dev = next(model.parameters()).device
+    meters = DeviceMeters(("loss", "area", "exact"), dev)
+    status = BatchStatus(len(loader), dev)
+    graphs = {}                     # rows -> (GraphedInference, static batch tensors)
+
+    def build(batch):
+        st = {k: v.to(dev, non_blocking=True).clone() for k, v in batch.items()}
+        st["input"] = st["input"].float()
+        n = st["input"].shape[0]
+
+        def post(out):
+            if e2e:
+                loss, exact = fused_area_loss(out[:L], st["params"], wf, exact=True)
+            else:
+                loss = criterion_seg(out[6], st["gt"])
+                area, exact = fused_area_loss(out[:2], st["params"], wf, exact=True)
+            if not torch.cuda.is_current_stream_capturing():
+                return None                  # warm-up passes: no meter or log entry
+            ok = model.lsq_status.reshape(()).eq(0)
+            if not e2e:
+                meters.update("area", area, ok, n)
+            meters.update("exact", exact, ok, n)
+            meters.update("loss", loss, ok, n)
+            status.record(model.lsq_status)
+            model.lsq_status.zero_()
+            return None
+
+        g = GraphedInference(model, st["input"], post=post, end_to_end=e2e)
+        st["input"] = g.x
+        model.lsq_status.zero_()
+        return g, st
+
+    deferred = model.defer_status_check
+    first, labels = None, []
+    try:
+        with torch.no_grad():
+            for i, (input, gt, params, idx, gt_line, gt_horizon, index) in enumerate(loader):
+                batch = {"input": input, "gt": gt, "params": params}
+                n = input.shape[0]
+                status.check(i)
+                if first is None:
+                    first = n
+                elif n > first:
+                    raise ValueError("batch of %d images after a first batch of %d" % (n, first))
+                if n in graphs:
+                    g, st = graphs[n]
+                    for k, v in batch.items():
+                        st[k].copy_(v, non_blocking=True)
+                else:
+                    g, st = graphs[n] = build(batch)
+                labels.append(idx)
+                g.graph.replay()
+                if not (_reporting(i, args.print_freq) or _reporting(i, 25)) or int(status.log[i]):
+                    continue                     # a skipped batch reports nothing, as main.py's `continue`
+                if _reporting(i, args.print_freq):
+                    m = meters.read()
+                    print('Test: [{0}/{1}]\t'
+                          'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                          'Area {area[0]:.8f} ({area[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], area=m["area"]))
+                if _reporting(i, 25):
+                    out, p = g.out, st["params"]
+                    nutils.save_weightmap('valid', out[5], M_inv, out[4], *out[:4], p[:, 0, :], p[:, 1, :], p[:, 2, :],
+                                          p[:, 3, :], gt_line, st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
+                                          args.save_path)
+    finally:
+        model.defer_status_check = deferred
+    m = meters.read()
+    status.print_skipped(labels)
+    if args.evaluate:
+        crit_string = "AREA**2" if e2e else "ENTROPY"
+        print("===> Average {}-loss on validation set is {:.8}".format(crit_string, m["loss"][1]))
+        print("===> Average exact area on validation set is {:.8}".format(m["exact"][1]))
+        if not e2e:
+            print("===> Average area**2 on validation set is {:.8}".format(m["area"][1]))
+    return m["loss"][1], m["area"][1], m["exact"][1], 0, 0
