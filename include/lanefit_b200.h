@@ -82,16 +82,39 @@ const char* lf_last_cuda_error(void);
  *   ytab     [H*W] f32  const - grid[:,1]              (:94, const = 255 BP / 1 BEV)
  *   yrow     [H]   f32  ytab of each row if ytab is constant along rows (true for every
  *                       homography the reference builds), else NULL -> general kernel
- *   mask_rows           rows [0,mask_rows) get weight zero and are never read
- *   beta     [B,L,order+1] f64 out, highest power first (:100-104)
- *   zinv     [B,L,(order+1)^2] f64 out: (Y^T W^2 Y + reg I)^-1, consumed by lf_lsq_bwd
+ *   mask_rows           rows [0,mask_rows) get weight zero and are never read: NaN or Inf
+ *                       in those rows of o, xtab, ytab or yrow changes no output bit
+ *   beta     [B,L,order+1] f64 out, highest power first (:100-104); NaN for a system
+ *            whose solve sets SINGULAR or NOT_POSDEF
+ *   zinv     [B,L,(order+1)^2] f64 out, row-major: (Y^T W^2 Y + reg I)^-1, consumed by
+ *            lf_lsq_bwd.  Z_ij = S_{2d-i-j} + reg_ls*delta_ij, X_i = T_{d-i} with
+ *            S_k = sum w y^k, T_k = sum w x y^k, w = act(o)^2 over the unmasked rows
+ *   solver   LF_SOLVER_INVERSE (Gauss-Jordan, partial pivoting) or LF_SOLVER_CHOLESKY
  *   masked   [B,L,H,W] f32 out or NULL: activation(o) with masked rows zeroed (output #5
- *            of Net.forward, :315)
- *   status   int32 out: OR of LF_STATUS_* over all B*L systems (caller zeroes it)
+ *            of Net.forward, :315); the masked rows are +0.0
+ *   status   int32 out: OR of LF_STATUS_* over all B*L systems (caller zeroes it; bits
+ *            already set stay set)
  *   workspace: lf_lsq_workspace_bytes() bytes, ZEROED once before first use; the
- *            library leaves it reusable (tickets reset) after every launch.
+ *            library leaves it reusable (tickets reset) after every launch, by any
+ *            later call of any shape.  Calls sharing a workspace must be stream-ordered.
+ * Row-separable kernel (yrow given, W % 4 == 0 for f32 o, W % 8 == 0 for bf16 o): 16-byte
+ * loads and stores, so o, xtab and masked (d_o in the backward) must be 16-byte aligned;
+ * a misaligned pointer is refused with LF_ERR_INVALID_ARGUMENT.  Otherwise the general
+ * kernel runs (ytab required, any alignment of the element type).
+ * lf_lsq_fwd returns LF_ERR_UNSUPPORTED for B*L > 16384 (the workspace's ticket region);
+ * lf_lsq_bwd uses no workspace and has no such limit.
  * ------------------------------------------------------------------------- */
 size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order);
+/* The plan lf_lsq_fwd (bwd = 0) or lf_lsq_bwd (bwd = 1) selects for these arguments (has_yrow / has_ytab: whether
+ * that pointer is non-NULL); no device needed (132 SMs assumed without one).  LF_OK and info[LF_LSQ_PLAN_INFO] =
+ * {row-separable kernel (1) or general (0), activation template (LF_ACT_SQUARE, or -1 = run-time activation), lanes
+ * per CTA NL, lane groups (= grid z), chunks per system (= grid x), resident CTAs per SM the chunk count is fitted to,
+ * byte alignment required of o / xtab / masked / d_o (16, or 0 = element alignment)}; otherwise the code the entry
+ * point returns for the same arguments (pointer and solver checks aside).  Chunk c of a system covers the masked rows
+ * [c*m/n, (c+1)*m/n) and the unmasked rows mask_rows + [c*h/n, (c+1)*h/n), m = mask_rows, h = H - m, n = chunks. */
+#define LF_LSQ_PLAN_INFO 7
+int lf_lsq_plan(int bwd, int o_dtype, int has_yrow, int has_ytab, int B, int L, int H, int W, int order, int mask_rows,
+                int act, int* info);
 int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
                int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
                double* beta, double* zinv, float* masked, int* status,

@@ -38,7 +38,10 @@ PROTOTYPES = {
     "lf_lsq_bwd": (_c_int, [_c_void_p, _c_int, _c_void_p, _c_void_p, _c_void_p,
                             _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int,
                             _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p]),
+    "lf_lsq_plan": (_c_int, [_c_int] * 11 + [_c_void_p]),
 }
+LSQ_PLAN_INFO = 7       # LF_LSQ_PLAN_INFO: entries lf_lsq_plan fills
+LSQ_PLAN_FIELDS = ("rowsep", "act_t", "nl", "groups", "nchunks", "ctas_per_sm", "align")
 
 MAX_TAPS = 9
 

@@ -687,17 +687,6 @@ static int pick_nchunks(int B, int groups, int H, int mask_rows, int ctas_per_sm
     return best;
 }
 
-static int validate(const LsqArgs& a, int o_dtype) {
-    LF_REQUIRE(a.o && a.xtab && (a.ytab || a.yrow));
-    LF_REQUIRE(a.B > 0 && a.L > 0 && a.H > 0 && a.W > 0);
-    LF_REQUIRE(a.order >= 0 && a.order <= LF_MAX_ORDER);
-    LF_REQUIRE(a.mask_rows >= 0 && a.mask_rows <= a.H);
-    LF_REQUIRE(a.act >= LF_ACT_NONE && a.act <= LF_ACT_SOFTPLUS);
-    LF_REQUIRE(o_dtype == LF_F32 || o_dtype == LF_BF16);
-    LF_REQUIRE(a.B <= 65535 && a.L <= 65535);
-    return LF_OK;
-}
-
 }  // namespace lf
 
 using namespace lf;
@@ -705,6 +694,54 @@ using namespace lf;
 // Workspace = [ticket region: LSQ_TICKET_BYTES, fixed so that tickets never alias partials of a call
 // with another shape] [partials].  Tickets are left at zero by every launch.
 constexpr size_t LSQ_TICKET_BYTES = 64 * 1024;
+
+// lanes per CTA: balanced groups of at most LSQ_MAXL (L=6 -> 2 groups of 3, not 4+2)
+static void lsq_lane_groups(int L, int* groups, int* nlg) {
+    *groups = (L + LSQ_MAXL - 1) / LSQ_MAXL;
+    *nlg = (L + *groups - 1) / *groups;
+}
+
+// What one lf_lsq_fwd (bwd = 0) or lf_lsq_bwd (bwd = 1) call launches: the kernel, the activation template, the lanes
+// per CTA and the chunks per system.  Both entry points and lf_lsq_plan take their decisions here, so the query cannot
+// drift from the launch.
+struct LsqPlan {
+    int rowsep, act_t, nl, groups, nchunks, ctas_per_sm, align;
+};
+
+static int lsq_plan(int bwd, int o_dtype, int has_yrow, int has_ytab, int B, int L, int H, int W, int order, int mask_rows,
+                    int act, LsqPlan* p) {
+    LF_REQUIRE(B > 0 && L > 0 && H > 0 && W > 0);
+    LF_REQUIRE(order >= 0 && order <= LF_MAX_ORDER);
+    LF_REQUIRE(mask_rows >= 0 && mask_rows <= H);
+    LF_REQUIRE(act >= LF_ACT_NONE && act <= LF_ACT_SOFTPLUS);
+    LF_REQUIRE(o_dtype == LF_F32 || o_dtype == LF_BF16);
+    LF_REQUIRE(B <= 65535 && L <= 65535);
+    if (!bwd && lf_lsq_workspace_bytes(B, L, H, W, order) == 0) return LF_ERR_UNSUPPORTED;   // ticket region full
+    // the row-separable kernels move 16 bytes per load and store: 4 fp32 or 8 bf16 map elements
+    p->rowsep = has_yrow && W % (o_dtype == LF_BF16 ? 8 : 4) == 0;
+    if (!p->rowsep && !has_ytab) return LF_ERR_INVALID_ARGUMENT;
+    p->act_t = act == LF_ACT_SQUARE ? LF_ACT_SQUARE : LSQ_ACT_RUNTIME;
+    p->groups = L;
+    p->nl = 1;
+    if (p->rowsep) lsq_lane_groups(L, &p->groups, &p->nl);
+    p->ctas_per_sm = bwd ? LSQ_BWD_CTAS_PER_SM : (p->rowsep ? LSQ_FWD_CTAS_PER_SM : 4);
+    p->nchunks = pick_nchunks(B, p->groups, H, mask_rows, p->ctas_per_sm);
+    p->align = p->rowsep ? 16 : 0;
+    return LF_OK;
+}
+
+static bool aligned16(const void* ptr) { return ptr == nullptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+extern "C" int lf_lsq_plan(int bwd, int o_dtype, int has_yrow, int has_ytab, int B, int L, int H, int W, int order,
+                           int mask_rows, int act, int* info) {
+    LF_REQUIRE(info && (bwd == 0 || bwd == 1));
+    LsqPlan p{};
+    const int rc = lsq_plan(bwd, o_dtype, has_yrow != 0, has_ytab != 0, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    const int v[LF_LSQ_PLAN_INFO] = {p.rowsep, p.act_t, p.nl, p.groups, p.nchunks, p.ctas_per_sm, p.align};
+    for (int i = 0; i < LF_LSQ_PLAN_INFO; ++i) info[i] = v[i];
+    return LF_OK;
+}
 
 extern "C" size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order) {
     (void)W;
@@ -755,39 +792,29 @@ extern "C" size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order) 
         }                                                              \
     } while (0)
 
-// lanes per CTA: balanced groups of at most LSQ_MAXL (L=6 -> 2 groups of 3, not 4+2)
-static void lsq_lane_groups(int L, int* groups, int* nlg) {
-    *groups = (L + LSQ_MAXL - 1) / LSQ_MAXL;
-    *nlg = (L + *groups - 1) / *groups;
-}
-
 extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
                           int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
                           double* beta, double* zinv, float* masked, int* status, void* workspace,
                           size_t workspace_bytes, lf_stream_t stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && status && workspace);
+    LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
+    LsqPlan p{};
+    const int rc = lsq_plan(0, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    if (workspace_bytes < lf_lsq_workspace_bytes(B, L, H, W, order)) return LF_ERR_WORKSPACE_TOO_SMALL;
+    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked));
     LsqArgs a{};
     a.o = o; a.xtab = xtab; a.ytab = ytab; a.yrow = yrow;
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
     a.reg_ls = reg_ls; a.beta = beta; a.zinv = zinv; a.masked = masked; a.status = status;
-    int rc = validate(a, o_dtype);
-    if (rc != LF_OK) return rc;
-    LF_REQUIRE(beta && zinv && status && workspace);
-    LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
-    const size_t need = lf_lsq_workspace_bytes(B, L, H, W, order);
-    if (need == 0) return LF_ERR_UNSUPPORTED;
-    if (workspace_bytes < need) return LF_ERR_WORKSPACE_TOO_SMALL;
-    const bool rowsep = (yrow != nullptr) && (W % (o_dtype == LF_BF16 ? 8 : 4) == 0);
-    if (!rowsep && !ytab) return LF_ERR_INVALID_ARGUMENT;
-    int groups = L, nlg = 1;
-    if (rowsep) lsq_lane_groups(L, &groups, &nlg);
-    a.nchunks = pick_nchunks(B, groups, H, mask_rows, rowsep ? LSQ_FWD_CTAS_PER_SM : 4);
+    a.nchunks = p.nchunks;
     a.rows_per_cta = 0;
     a.tickets = reinterpret_cast<int*>(workspace);
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
-    dim3 grid(a.nchunks, B, groups);
-    if (rowsep)
-        LSQ_DISPATCH_NL(lsq_fwd_rowsep_kernel, nlg, grid, a);
+    dim3 grid(a.nchunks, B, p.groups);
+    if (p.rowsep)
+        LSQ_DISPATCH_NL(lsq_fwd_rowsep_kernel, p.nl, grid, a);
     else
         LSQ_DISPATCH(lsq_fwd_general_kernel, grid, a);
     return check_launch();
@@ -797,22 +824,20 @@ extern "C" int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const f
                           int L, int H, int W, int order, int mask_rows, int act, const double* beta,
                           const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && gbeta && d_o);
+    LsqPlan p{};
+    const int rc = lsq_plan(1, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(d_o));
     LsqArgs a{};
     a.o = o; a.xtab = xtab; a.ytab = ytab; a.yrow = yrow;
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act;
     a.beta = const_cast<double*>(beta); a.zinv = const_cast<double*>(zinv); a.gbeta = gbeta; a.d_o = d_o;
-    int rc = validate(a, o_dtype);
-    if (rc != LF_OK) return rc;
-    LF_REQUIRE(beta && zinv && gbeta && d_o);
-    const bool rowsep = (yrow != nullptr) && (W % (o_dtype == LF_BF16 ? 8 : 4) == 0);
-    if (!rowsep && !ytab) return LF_ERR_INVALID_ARGUMENT;
-    int groups = L, nlg = 1;
-    if (rowsep) lsq_lane_groups(L, &groups, &nlg);
-    a.nchunks = pick_nchunks(B, groups, H, mask_rows, LSQ_BWD_CTAS_PER_SM);
+    a.nchunks = p.nchunks;
     a.rows_per_cta = 0;
-    dim3 grid(a.nchunks, B, groups);
-    if (rowsep)
-        LSQ_DISPATCH_NL(lsq_bwd_rowsep_kernel, nlg, grid, a);
+    dim3 grid(a.nchunks, B, p.groups);
+    if (p.rowsep)
+        LSQ_DISPATCH_NL(lsq_bwd_rowsep_kernel, p.nl, grid, a);
     else
         LSQ_DISPATCH(lsq_bwd_general_kernel, grid, a);
     return check_launch();
