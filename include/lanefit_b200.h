@@ -583,6 +583,29 @@ typedef struct LfOptimState {
 int lf_optim_step(int algo, const LfOptimSeg* segs, int nsegs, long long nchunks, const LfOptimHyper* hyper,
                   LfOptimState* state, const int* status, lf_stream_t stream);
 
+/* The same update with one step count per parameter, as torch.optim keeps it: a parameter that misses an update (no
+ * gradient, e.g. the heads while only the segmentation output is trained, BP/main.py:32-43,255-282) keeps its count, and
+ * a parameter that joins later starts at step 1.  Row r of `segs` updates the parameter whose count is steps[slot].
+ * `steps` (DEVICE, nparams counts, zeroed once before first use) outlives the tables built over it, so a parameter that
+ * drops out of a table keeps its count.  `slots` (HOST, nsegs entries) repeats the rows' slots for the argument checks:
+ * every slot in [0, nparams), no slot in two rows; the rows in `segs` must carry the same values.
+ * Two launches on `stream`:
+ *   1. one thread per row: with `status` NULL or zero, forms the row's scalars from steps[slot] (fp64 bias corrections
+ *      rounded to fp32, as lf_optim_step; for SGD `first` is steps[slot] == 0), stores them in `scalars` and increments
+ *      steps[slot]; with a nonzero status it changes nothing and increments *skipped once;
+ *   2. lf_optim_step's chunk loop, each chunk with its row's scalars; nothing when the status is nonzero.
+ * The elementwise arithmetic is lf_optim_step's, one code.  `scalars`: DEVICE workspace of
+ * nsegs * LF_OPTIM_PP_SCALAR_BYTES bytes, 16-byte aligned.  Never synchronises; graph-capturable. */
+#define LF_OPTIM_PP_SCALAR_BYTES 48
+typedef struct LfOptimSegPP {
+    LfOptimSeg seg;
+    int slot;               /* index into `steps` */
+    int reserved;
+} LfOptimSegPP;
+int lf_optim_step_pp(int algo, const LfOptimSegPP* segs, const int* slots, int nsegs, long long nchunks,
+                     const LfOptimHyper* hyper, long long* steps, int nparams, void* scalars, long long* skipped,
+                     const int* status, lf_stream_t stream);
+
 /* Baseline JPEG decode (csrc/jpeg.cu; replaces Image.open(f).convert('RGB') of BP/Dataloader/Load_Data_new.py:118-119):
  * a batch of same-size baseline (SOF0 / 8-bit SOF1, Huffman) single-scan JPEGs, YCbCr 4:4:4 / 4:2:2 / 4:2:0 or grayscale,
  * with or without restart markers -> uint8 RGB [N][H][W][3], bit-identical to Pillow (libjpeg-turbo: ISLOW IDCT, fancy

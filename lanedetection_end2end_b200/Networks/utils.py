@@ -204,16 +204,18 @@ class AverageMeter(object):
         self.avg = self.sum / self.count
 
 
-def define_optim(optim, params, lr, weight_decay, fused=None):
+def define_optim(optim, params, lr, weight_decay, fused=None, per_param_step=False):
     """torch.optim's Adam / SGD / RMSprop (BP/Networks/utils.py:451-461), or with ``fused`` the same update as one launch
     of the library's kernel (lanedetection_end2end_b200.optim.FusedOptimizer, CUDA-graph capturable, same state_dict
     format).  fused=None reads LANEFIT_FUSED_OPTIM (default 0: the torch optimizer), so the reference's main.py can opt in
-    without edits."""
+    without edits.  ``per_param_step``: the FusedOptimizer keeps one step count per parameter, as torch.optim does (needed
+    by --pretrained, whose phases train different parameter sets); the torch optimizers always do, so it changes nothing
+    for them."""
     if fused is None:
         fused = os.environ.get("LANEFIT_FUSED_OPTIM", "0") != "0"
     if fused and optim in ("adam", "sgd", "rmsprop"):
         from ._pkg import submodule
-        return submodule("optim").FusedOptimizer(params, optim, lr, weight_decay)
+        return submodule("optim").FusedOptimizer(params, optim, lr, weight_decay, per_param_step=per_param_step)
     if optim == "adam":
         return torch.optim.Adam(params, lr=lr, weight_decay=weight_decay)
     if optim == "sgd":

@@ -133,6 +133,13 @@ class LfOptimState(ctypes.Structure):
     _fields_ = [("step", _ll), ("skipped", _ll), ("ticket", ctypes.c_ulonglong)]
 
 
+OPTIM_PP_SCALAR_BYTES = 48
+
+
+class LfOptimSegPP(ctypes.Structure):
+    _fields_ = [("seg", LfOptimSeg), ("slot", _i), ("reserved", _i)]
+
+
 STATUS_JPEG_CORRUPT = 8
 JPEG_PIECE_BYTES = 128
 JPEG_MAX_BPM = 6
@@ -177,6 +184,7 @@ _NET_PROTOS = {
     "lf_jpeg_workspace_bytes": (_c_size_t, [_p, _i, _p]),
     "lf_jpeg_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p, _c_size_t, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
+    "lf_optim_step_pp": (_i, [_i, _p, _p, _i, _ll, _p, _p, _i, _p, _p, _p, _p]),
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg": (_i, [ctypes.POINTER(LfWgradTcgArgs), _p]),
     "lf_reduce_multi": (_i, [ctypes.POINTER(LfReduceJob), _i, _p]),

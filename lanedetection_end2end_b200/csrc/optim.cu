@@ -11,6 +11,11 @@
 //    the device hyperparameter block and step counter, so a CUDA graph replay picks up a new learning rate without a
 //    recapture.  The step counter is advanced by the last CTA to arrive (ticket, as in lsq.cu): every CTA reads it before
 //    taking its ticket, so no CTA can see the advanced value.
+//  * lf_optim_step_pp keeps one step count per parameter (torch's per-parameter `step`): a first launch with one thread
+//    per row forms that row's scalars from its own count and advances the count, a second runs the same chunk loop with
+//    each chunk's row scalars.  opt_scalars / opt_elem / opt_chunk are shared, so the arithmetic is the same code.
+#include <vector>
+
 #include "lf_common.cuh"
 
 namespace lf {
@@ -141,6 +146,50 @@ __global__ void __launch_bounds__(OPT_THREADS) optim_kernel(const LfOptimSeg* __
     }
 }
 
+// ---- per-parameter step counts (lf_optim_step_pp) -------------------------------------------------------------------
+static_assert(sizeof(OptScalars) <= LF_OPTIM_PP_SCALAR_BYTES, "LF_OPTIM_PP_SCALAR_BYTES too small");
+constexpr int OPT_PP_SCALAR_THREADS = 128;
+
+// launch 1: row r's scalars from its own count, then the count advances.  Rows name distinct slots (checked on the
+// host), so no two threads touch one count.
+__global__ void __launch_bounds__(OPT_PP_SCALAR_THREADS) optim_pp_scalars_kernel(
+    int algo, const LfOptimSegPP* __restrict__ segs, int nsegs, const LfOptimHyper* __restrict__ hyper, long long* steps,
+    OptScalars* __restrict__ scal, long long* skipped, const int* __restrict__ status) {
+    pdl_entry();
+    const int r = blockIdx.x * OPT_PP_SCALAR_THREADS + threadIdx.x;
+    if (r >= nsegs) return;
+    if (status != nullptr && *status != 0) {
+        if (r == 0) *skipped += 1;
+        return;
+    }
+    const int slot = segs[r].slot;
+    const long long t = steps[slot];
+    opt_scalars(algo, hyper, t, scal + r);
+    steps[slot] = t + 1;
+}
+
+// launch 2: optim_kernel's chunk loop with each chunk's row scalars; no ticket, no count
+template <int ALGO>
+__global__ void __launch_bounds__(OPT_THREADS) optim_pp_kernel(const LfOptimSegPP* __restrict__ segs, int nsegs,
+                                                               long long nchunks, const OptScalars* __restrict__ scal,
+                                                               const int* __restrict__ status) {
+    pdl_entry();
+    if (status != nullptr && *status != 0) return;     // every thread reads the same word launch 1 read
+    for (long long c = blockIdx.x; c < nchunks; c += gridDim.x) {
+        int lo = 0, hi = nsegs - 1;           // last row with chunk0 <= c
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (__ldg(&segs[mid].seg.chunk0) <= c) lo = mid;
+            else hi = mid - 1;
+        }
+        const LfOptimSeg sg = segs[lo].seg;
+        const OptScalars s = scal[lo];
+        const long long base = (c - sg.chunk0) * LF_OPTIM_CHUNK;
+        const long long rem = sg.numel - base;
+        if (rem > 0) opt_chunk<ALGO>(sg, base, rem < LF_OPTIM_CHUNK ? (int)rem : LF_OPTIM_CHUNK, s);
+    }
+}
+
 }  // namespace lf
 
 using namespace lf;
@@ -163,5 +212,36 @@ extern "C" int lf_optim_step(int algo, const LfOptimSeg* segs, int nsegs, long l
     const long long cap = (long long)device_sms() * per_sm;
     const dim3 grid((unsigned)(nchunks < cap ? nchunks : cap));
     lf_launch(kernel, grid, OPT_THREADS, 0, stream, segs, nsegs, nchunks, hyper, state, status);
+    return check_launch();
+}
+
+extern "C" int lf_optim_step_pp(int algo, const LfOptimSegPP* segs, const int* slots, int nsegs, long long nchunks,
+                                const LfOptimHyper* hyper, long long* steps, int nparams, void* scalars, long long* skipped,
+                                const int* status, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(segs && slots && nsegs > 0 && nchunks > 0 && hyper && steps && nparams > 0 && scalars && skipped);
+    LF_REQUIRE(algo == LF_OPTIM_ADAM || algo == LF_OPTIM_SGD || algo == LF_OPTIM_RMSPROP);
+    LF_REQUIRE((reinterpret_cast<uintptr_t>(scalars) & 15) == 0);
+    std::vector<char> used(nparams, 0);
+    for (int r = 0; r < nsegs; ++r) {
+        LF_REQUIRE(slots[r] >= 0 && slots[r] < nparams && !used[slots[r]]);
+        used[slots[r]] = 1;
+    }
+    OptScalars* scal = static_cast<OptScalars*>(scalars);
+    lf_launch(optim_pp_scalars_kernel, dim3((nsegs + OPT_PP_SCALAR_THREADS - 1) / OPT_PP_SCALAR_THREADS),
+              OPT_PP_SCALAR_THREADS, 0, stream, algo, segs, nsegs, hyper, steps, scal, skipped, status);
+    const int rc = check_launch();
+    if (rc != LF_OK) return rc;
+    void (*kernel)(const LfOptimSegPP*, int, long long, const OptScalars*, const int*) =
+        algo == LF_OPTIM_ADAM ? optim_pp_kernel<LF_OPTIM_ADAM> : algo == LF_OPTIM_SGD ? optim_pp_kernel<LF_OPTIM_SGD>
+                                                                                   : optim_pp_kernel<LF_OPTIM_RMSPROP>;
+    int per_sm = 0;                           // one wave, at most one CTA per chunk, as lf_optim_step
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, OPT_THREADS, 0) != cudaSuccess || per_sm < 1) {
+        cudaGetLastError();
+        per_sm = 1;
+    }
+    const long long cap = (long long)device_sms() * per_sm;
+    const dim3 grid((unsigned)(nchunks < cap ? nchunks : cap));
+    lf_launch(kernel, grid, OPT_THREADS, 0, stream, segs, nsegs, nchunks, (const OptScalars*)scal, status);
     return check_launch();
 }

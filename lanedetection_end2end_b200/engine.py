@@ -49,11 +49,15 @@ class GraphedTrainStep:
     segmentation branch's substitution, end_to_end=False); default a host tensor of zeros.  ``loss_fn``: optional
     callable(forward 9-tuple) -> scalar loss that replaces the lane criterion and ``extra_loss``.  ``post``: optional
     callable(forward 9-tuple, detached loss) run at the end of every step, after the update (its return value is
-    ``self.post_out``); the warm-up steps run it too."""
+    ``self.post_out``); the warm-up steps run it too.
+
+    ``early_return=True``: the forward is ``model(x, gt_line, end_to_end, early_return=True)``, the decoder output alone
+    (the segmentation pretraining of --pretrained, BP/main.py:255-258), which ``loss_fn`` and ``post`` then receive in
+    place of the 9-tuple.  Without the least-squares layer no batch can be singular: the update runs unguarded."""
 
     def __init__(self, model, criterion, nclasses, example_x, example_xgt, example_valid, reducer=None, warmup=3,
                  capture_error_mode="global", extra_loss=None, global_valid=False, optimizer=None, gt_line=None,
-                 end_to_end=True, loss_fn=None, post=None):
+                 end_to_end=True, loss_fn=None, post=None, early_return=False):
         if optimizer is not None:
             from .optim import FusedOptimizer
             if not isinstance(optimizer, FusedOptimizer):
@@ -72,6 +76,7 @@ class GraphedTrainStep:
         self.valid = example_valid.clone()
         self.gt_line = torch.zeros(example_x.shape[0], 4) if gt_line is None else gt_line.clone()
         self.end_to_end = end_to_end
+        self.early_return = early_return
         self.loss_fn = loss_fn
         self.post = post
         self.post_out = None
@@ -107,10 +112,13 @@ class GraphedTrainStep:
         if first:
             self.model.zero_grad(set_to_none=True)
         else:
-            if self.optimizer is not None:
+            if self.optimizer is not None and not self.early_return:
                 self.model.lsq_status.zero_()
             torch._foreach_zero_(self.grads)
-        out = model_forward(self.model, self.x, self.gt_line, self.end_to_end)
+        if self.early_return:
+            out = self.model(self.x, self.gt_line, self.end_to_end, early_return=True)
+        else:
+            out = model_forward(self.model, self.x, self.gt_line, self.end_to_end)
         scale = None
         if self.global_valid:
             from .ddp import lane_valid_scale
@@ -134,8 +142,8 @@ class GraphedTrainStep:
         if self.reducer is not None:
             self.reducer()
         if not first and self.optimizer is not None:
-            status = self.model.lsq_status
-            if self.reducer is not None:
+            status = None if self.early_return else self.model.lsq_status
+            if self.reducer is not None and status is not None:
                 # data-parallel: the ranks share the averaged gradients, so a singular system on any rank skips every rank
                 from .ddp import any_rank_nonzero
                 status = any_rank_nonzero(status, self.skip_word, getattr(self.reducer, "group", None))
@@ -327,19 +335,32 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     (bce_line.double() + bce_horizon.double()) * weight_class``.  --end_to_end False: criterion_seg(output, gt), with the
     least-squares fit and the rmse metric computed without gradient (main.py:306-318).  clip_grad_norm is accepted and does
     nothing: main.py:334-335 clips the gradients of the previous batch before zero_grad() discards them, so it never changes
-    an update.  --pretrained (the skip_epochs segmentation phase and the switch of parameter sets) raises ValueError: a
-    FusedOptimizer keeps one parameter set.  Dropout masks are drawn in the graph from torch's graph-safe Philox offsets;
-    they do not repeat an eager run's masks.  BatchNorm running statistics are those of the epoch's batches (the capture's
-    warm-up steps leave them as they were)."""
+    an update.  Dropout masks are drawn in the graph from torch's graph-safe Philox offsets; they do not repeat an eager
+    run's masks.  BatchNorm running statistics are those of the epoch's batches (the capture's warm-up steps leave them as
+    they were).
+
+    --pretrained needs a FusedOptimizer built with per_param_step=True (define_optim(..., fused=True,
+    per_param_step=True)), since its phases train different parameter sets; otherwise it raises ValueError.  The phase
+    comes from ``epoch`` and ``args`` as main.py's get_flags gives it (``args`` is not changed): a skip epoch (epoch <
+    skip_epochs and < pretrain_epochs) replays ``model(input, gt_line, False, early_return=True)`` -- the decoder through
+    output_conv2, no least-squares layer -- with the loss criterion_seg(output, gt) and the update unguarded
+    (main.py:255-282), and returns (losses_skip.avg, 0.0); main.py prints no per-batch line there, and its plot at
+    save_freq is not drawn.  Every other epoch follows ``args.end_to_end``, which the caller's get_flags(epoch) sets:
+    the segmentation branch through output_conv2, or end to end through output_conv and the heads, whose optimizer
+    state starts at step 1 while output_conv2 keeps its state.  --clas with --end_to_end False raises ValueError outside
+    the skip epochs (main.py:320-325 would call the line criterion on None)."""
     from .optim import FusedOptimizer
     from .Loss_crit import fused_backprojection_loss
     from .Networks import utils as nutils
     if not isinstance(optimizer, FusedOptimizer):
         raise TypeError("train_epoch runs the update in the graph: it needs an optim.FusedOptimizer "
                         "(define_optim(..., fused=True)), got %s" % type(optimizer).__name__)
-    if args.pretrained:
-        raise ValueError("train_epoch does not run --pretrained: its segmentation phase and the switch to end-to-end change "
-                         "the parameter set, which a FusedOptimizer refuses")
+    if args.pretrained and not optimizer.per_param_step:
+        raise ValueError("train_epoch runs --pretrained with a per-parameter step count only: its segmentation phase and "
+                         "the switch to end-to-end change the parameter set.  Build the optimizer with "
+                         "define_optim(..., fused=True, per_param_step=True)")
+    if args.pretrained and epoch < args.pretrain_epochs and epoch < args.skip_epochs:
+        return _train_skip_epoch(loader, model, optimizer, criterion_seg, args)
     if args.clas and not args.end_to_end:
         raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
     e2e, L = bool(args.end_to_end), args.nclasses
@@ -428,6 +449,47 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     m = meters.read()
     status.print_skipped(labels)
     return m["loss"][1], m["rmse"][1]
+
+
+def _train_skip_epoch(loader, model, optimizer, criterion_seg, args):
+    """A skip epoch of --pretrained (BP/main.py:255-282) as graph replays: the decoder output through output_conv2, the
+    segmentation loss and the unguarded update; returns (losses_skip.avg, 0.0)."""
+    dev = next(model.parameters()).device
+    model.train()
+    meters = DeviceMeters(("loss_skip",), dev)
+    always = torch.ones((), dtype=torch.bool, device=dev)
+    static = {}
+
+    def post(out, loss):
+        if torch.cuda.is_current_stream_capturing():          # warm-up steps: no meter entry
+            meters.update("loss_skip", loss, always, static["input"].shape[0])
+        return None
+
+    step = None
+    deferred = model.defer_status_check
+    try:
+        for i, (input, gt, lanes, idx, gt_line, gt_horizon, valid_points) in enumerate(loader):
+            if step is None:
+                static["input"] = input.to(dev, non_blocking=True).float()
+                static["gt"] = gt.squeeze(1).to(dev, non_blocking=True).long().clone()
+                none = torch.empty(0, device=dev)     # the loss reads gt through loss_fn: no lane-sample inputs
+                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
+                    model, None, args.nclasses, static["input"], none, none, optimizer=optimizer,
+                    end_to_end=False, loss_fn=lambda out: criterion_seg(out, static["gt"]), post=post,
+                    early_return=True))
+                static["input"] = step.x              # the step's own copy is what its forward reads
+            else:
+                if input.shape[0] != step.x.shape[0]:
+                    raise ValueError("batch of %d images after a first batch of %d: train_epoch replays one batch size"
+                                     % (input.shape[0], step.x.shape[0]))
+                static["input"].copy_(input, non_blocking=True)
+                static["gt"].copy_(gt.squeeze(1), non_blocking=True)
+            step()
+    finally:
+        model.defer_status_check = deferred
+    if step is None:
+        return 0, 0
+    return meters.read()["loss_skip"][1], 0.0
 
 
 def check_bev_args(args):

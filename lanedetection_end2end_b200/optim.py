@@ -9,8 +9,13 @@ for a batch with a singular system, as the reference's skip of that batch does (
 
 ``state_dict()`` / ``load_state_dict()`` use torch.optim's format exactly (``param_groups`` key for key, per-parameter
 ``step`` as a CPU float32 tensor, independent state tensors), so checkpoints move both ways between this class and
-``torch.optim.<Cls>``.  One difference in what can be represented: all parameters share one step count.
+``torch.optim.<Cls>``.  By default all parameters share one step count (csrc/optim.cu: lf_optim_step), so the set of
+parameters with a gradient must not change.  ``per_param_step=True`` keeps one device count per parameter
+(lf_optim_step_pp), as torch.optim does: the set may change between updates, which a --pretrained run does by
+construction (its segmentation epochs train ``output_conv2``, its end-to-end epochs ``output_conv`` and the heads).
 """
+import ctypes
+
 import torch
 
 from . import _capi
@@ -29,17 +34,28 @@ _UNSUPPORTED = ("amsgrad", "nesterov", "centered", "maximize")
 
 
 class FusedOptimizer(torch.optim.Optimizer):
-    """``FusedOptimizer(params, kind, lr, weight_decay)`` with kind in {"adam", "sgd", "rmsprop"}: the arguments and
-    semantics of ``define_optim(kind, params, lr, weight_decay)`` (SGD and RMSprop with momentum 0.9), one parameter group.
+    """``FusedOptimizer(params, kind, lr, weight_decay, per_param_step=False)`` with kind in {"adam", "sgd", "rmsprop"}:
+    the arguments and semantics of ``define_optim(kind, params, lr, weight_decay)`` (SGD and RMSprop with momentum 0.9),
+    one parameter group.
 
     ``step()`` updates the parameters whose ``.grad`` is not None, in one launch on the current stream, without a host
-    synchronisation.  ``skipped`` / ``step_count`` read the device counters (one synchronisation each)."""
+    synchronisation.  ``skipped`` / ``step_count`` / ``step_counts`` read the device counters (one synchronisation each).
 
-    def __init__(self, params, kind="adam", lr=1e-3, weight_decay=0):
+    ``per_param_step=False``: one step count for all parameters (one launch); the set of parameters with a gradient must
+    not change after the first update.  ``per_param_step=True``: one count per parameter (two launches), like torch.optim:
+    the set may change between updates outside CUDA graph capture (the segment table is rebuilt; a graph captured
+    earlier keeps its own table), a parameter without a gradient keeps its state and its count, and checkpoints may hold
+    differing steps and parameters without state.  In this mode ``step_count`` is the largest per-parameter count, i.e.
+    the updates of the parameters that took part in the most of them."""
+
+    def __init__(self, params, kind="adam", lr=1e-3, weight_decay=0, per_param_step=False):
         if kind not in _KINDS:
             raise ValueError("FusedOptimizer kind %r: expected one of %s" % (kind, sorted(_KINDS)))
+        if not isinstance(per_param_step, bool):
+            raise TypeError("FusedOptimizer per_param_step must be True or False, got %r" % (per_param_step,))
         cls, extra, self.algo = _KINDS[kind]
         self.kind = kind
+        self.per_param_step = per_param_step
         # torch's own constructor validates the arguments and gives the exact defaults (= param_groups keys) of this version
         defaults = dict(cls([torch.zeros(1)], lr=lr, weight_decay=weight_decay, **extra).defaults)
         super().__init__(params, defaults)
@@ -50,6 +66,8 @@ class FusedOptimizer(torch.optim.Optimizer):
         dev = plist[0].device
         self._hyper = torch.zeros(6, dtype=torch.float64, device=dev)     # LfOptimHyper
         self._counters = torch.zeros(3, dtype=torch.int64, device=dev)    # LfOptimState: step, skipped, ticket
+        # per_param_step: the count of parameter i (its slot) whatever tables are built over it
+        self._steps = torch.zeros(len(plist), dtype=torch.int64, device=dev) if per_param_step else None
         self._hyper_host = None
         self._table_key = None
         self._captured_tables = []
@@ -99,10 +117,11 @@ class FusedOptimizer(torch.optim.Optimizer):
         if torch.cuda.is_current_stream_capturing():
             raise RuntimeError("FusedOptimizer: the set of gradients changed during CUDA graph capture")
         with_state = {id(p) for p, st in self.state.items() if st}
-        if self._started and with_state != {id(p) for p in params}:
+        if not self.per_param_step and self._started and with_state != {id(p) for p in params}:
             raise ValueError("FusedOptimizer keeps one step count for all parameters: the set of parameters with a "
                              "gradient must not change after the first update")
         names = STATE_KEYS[self.kind]
+        slot = {id(p): i for i, p in enumerate(self.param_groups[0]["params"])}
         rows, chunk = [], 0
         for p in params:
             g = p.grad
@@ -116,20 +135,33 @@ class FusedOptimizer(torch.optim.Optimizer):
                     st[k] = torch.zeros_like(p, memory_format=torch.contiguous_format)
             s = [st[k] for k in names]
             rows.append([p.data_ptr(), g.data_ptr(), s[0].data_ptr(), s[1].data_ptr() if len(s) > 1 else 0, p.numel(), chunk])
+            if self.per_param_step:
+                rows[-1].append(slot[id(p)])          # LfOptimSegPP: slot, then reserved (0) in the high word
             chunk += -(-p.numel() // _capi.OPTIM_CHUNK)
         # the previous table is freed here unless a captured graph reads it (launch() keeps those alive)
         self._table = torch.tensor(rows, dtype=torch.int64).to(self._hyper.device)
         self._nsegs, self._nchunks, self._nelem = len(rows), chunk, sum(p.numel() for p in params)
+        if self.per_param_step:
+            self._slots = (ctypes.c_int * len(rows))(*[r[6] for r in rows])
+            self._scalars = torch.empty(len(rows) * _capi.OPTIM_PP_SCALAR_BYTES // 8, dtype=torch.int64,
+                                        device=self._hyper.device)
         self._table_key = key
 
     def launch(self, status=None):
         """The update over the prepared table on the current stream (capturable); ``status``: optional device int32 word,
         nonzero = skip this update."""
         per_elem = 20 if self.kind == "sgd" else 28
-        if torch.cuda.is_current_stream_capturing() and not any(t is self._table for t in self._captured_tables):
-            self._captured_tables.append(self._table)    # a replay reads it by address for as long as this object lives
-        _capi.call("lf_optim_step", self.algo, ptr(self._table), self._nsegs, self._nchunks, ptr(self._hyper),
-                   ptr(self._counters), ptr(status), _capi.stream_ptr(), nbytes=per_elem * self._nelem)
+        if torch.cuda.is_current_stream_capturing() and not any(t[0] is self._table for t in self._captured_tables):
+            # a replay reads them by address for as long as this object lives
+            self._captured_tables.append((self._table, self._scalars if self.per_param_step else None))
+        if self.per_param_step:
+            skipped = ctypes.c_void_p(self._counters.data_ptr() + self._counters.element_size())    # LfOptimState.skipped
+            _capi.call("lf_optim_step_pp", self.algo, ptr(self._table), self._slots, self._nsegs, self._nchunks,
+                       ptr(self._hyper), ptr(self._steps), self._steps.numel(), ptr(self._scalars), skipped, ptr(status),
+                       _capi.stream_ptr(), nbytes=per_elem * self._nelem)
+        else:
+            _capi.call("lf_optim_step", self.algo, ptr(self._table), self._nsegs, self._nchunks, ptr(self._hyper),
+                       ptr(self._counters), ptr(status), _capi.stream_ptr(), nbytes=per_elem * self._nelem)
         self._started = True
 
     @torch.no_grad()
@@ -150,7 +182,19 @@ class FusedOptimizer(torch.optim.Optimizer):
     # -- counters -------------------------------------------------------------------------------------------------------
     @property
     def step_count(self):
+        """Updates applied: the shared count, or with per_param_step the largest per-parameter count."""
+        if self.per_param_step:
+            return int(self._steps.max().item())
         return int(self._counters[0].item())
+
+    @property
+    def step_counts(self):
+        """Each parameter's count, in parameter order: torch.optim's per-parameter ``step`` (0 for a parameter never
+        updated).  Without per_param_step, the shared count for every parameter that has state."""
+        if self.per_param_step:
+            return self._steps.tolist()
+        step = self.step_count
+        return [step if self.state.get(p) else 0 for p in self.param_groups[0]["params"]]
 
     @property
     def skipped(self):
@@ -158,6 +202,17 @@ class FusedOptimizer(torch.optim.Optimizer):
 
     # -- checkpoints in torch.optim's format ----------------------------------------------------------------------------
     def state_dict(self):
+        if self.per_param_step:
+            counts = self.step_counts
+            for p, n in zip(self.param_groups[0]["params"], counts):
+                st = self.state.get(p)
+                if st and "step" in st:
+                    st["step"] = torch.tensor(float(n), dtype=torch.float32)
+            sd = super().state_dict()
+            for i, n in enumerate(counts):
+                if n == 0:
+                    sd["state"].pop(i, None)      # torch.optim holds no state for a parameter before its first update
+            return sd
         step = self.step_count
         for st in self.state.values():
             if "step" in st:
@@ -180,7 +235,13 @@ class FusedOptimizer(torch.optim.Optimizer):
                 raise ValueError("state of parameter %s lacks %s" % (idx, ", ".join(missing)))
             if "step" in st:
                 steps[idx] = float(st["step"])
-        if self.kind == "sgd":
+        if self.per_param_step:
+            # torch's SGD keeps no step: a momentum buffer means at least one update
+            step = 0
+            counts = [0] * len(self.param_groups[0]["params"])
+            for idx in state_dict["state"]:
+                counts[idx] = 1 if self.kind == "sgd" else int(steps.get(idx, 0))
+        elif self.kind == "sgd":
             step = 1 if state_dict["state"] else 0
         else:
             if len(set(steps.values())) > 1:
@@ -190,7 +251,8 @@ class FusedOptimizer(torch.optim.Optimizer):
                                  "count for all parameters" % (odd, steps[odd], first, steps[first]))
             step = int(next(iter(steps.values()))) if steps else 0
         # Existing state tensors keep their addresses: the loaded values are copied into them, so a segment table that a
-        # captured graph reads stays valid.  A parameter that has state here but none in the dict would need its own step.
+        # captured graph reads stays valid.  A parameter that has state here but none in the dict would need its own step
+        # (per_param_step: it gets one, 0).
         old = {p: [st[k] for k in names] for p, st in self.state.items() if st}
         if step > 0:
             for i, p in enumerate(self.param_groups[0]["params"]):
@@ -209,14 +271,17 @@ class FusedOptimizer(torch.optim.Optimizer):
                 else:         # independent of the caller's tensors (the kernel writes in place)
                     st[k] = st[k].clone(memory_format=torch.contiguous_format)
                     replaced = True
-        for p, tensors in old.items():      # step 0: the dict holds no state, i.e. fresh zero state
+        for p, tensors in old.items():      # no state for p in the dict: fresh zero state
             st = self.state[p]
             if not st:
                 if self.kind != "sgd":
                     st["step"] = torch.tensor(0.0, dtype=torch.float32)
                 for k, t in zip(names, tensors):
                     st[k] = t.zero_()
-        self._counters[0].fill_(step)
+        if self.per_param_step:
+            self._steps.copy_(torch.tensor(counts, dtype=torch.int64))
+        else:
+            self._counters[0].fill_(step)
         if replaced:
             self._table_key = None
         self._hyper_host = None
