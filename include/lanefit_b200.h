@@ -120,6 +120,21 @@ int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab,
                double* beta, double* zinv, float* masked, int* status,
                void* workspace, size_t workspace_bytes, lf_stream_t stream);
 
+/* lf_lsq_fwd on the row-separable kernel (yrow required, no ytab) that also stores, per (image, lane, unmasked row r),
+ * rowsums[b][l][r] = (A_r, B_r, C_r) = sum_c (w, w x, w c), w = (mask * act(o))^2, float32 [B][L][H][3]: what
+ * lf_lsq_grid_grad needs.  Same plan, checks and outputs as lf_lsq_fwd. */
+int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L, int H, int W,
+                       int order, int mask_rows, int act, double reg_ls, int solver, double* beta, double* zinv,
+                       float* masked, int* status, float* rowsums, void* workspace, size_t workspace_bytes,
+                       lf_stream_t stream);
+/* Gradient with respect to row-separable tables x[r][c] = alpha_r c + gamma_r, y_r = const - y'_r (a learned
+ * homography), summed over images and lanes in a fixed order, from lf_lsq_fwd_rowsums' row sums and beta, Z^-1 and
+ * gbeta = dL/dbeta:  dL/dgamma_r = (phi.z) A_r,  dL/dalpha_r = (phi.z) C_r,
+ * dL/dy'_r = -[(phi'.z)(B_r - (phi.beta) A_r) - (phi.z)(phi'.beta) A_r],  z = Z^-1 gbeta, phi = [y^d .. y 1].
+ * g_rowp [H][3] f64 = (alpha, gamma, y'); 0 for the masked rows. */
+int lf_lsq_grid_grad(const float* rowsums, const float* yrow, const double* beta, const double* zinv, const double* gbeta,
+                     int B, int L, int H, int order, int mask_rows, double* g_rowp, lf_stream_t stream);
+
 /* Backward of the above: d_o = dL/d o given gbeta = dL/d beta [B,L,order+1] f64.
  * Replaces autograd through mul/bmm/inverse (BP/Networks/LSQ_layer.py:111-116) ==
  * GELS.backward (BP/Networks/gels.py:18-25) composed with the activation and mask:
@@ -476,6 +491,34 @@ int lf_backproj_loss(const double* Y56, const double* yprime, const double* Minv
 int lf_backproj_loss_host(const double* Y56, const double* yprime, const double* Minv, const double* beta, const double* x_gt,
                           const double* valid, int B, int L, int n, double* lane_loss, double* loss, double* dbeta,
                           double* xcal);
+/* lf_backproj_loss with the warp constants on the DEVICE (a learned homography): yk [56] = y' of the sample rows, Minv [9];
+ * Y56 is built from yk in the kernel.  Also emits g_const [65] = dloss/dM^-1 (9) then dloss/dy'_k (56); g_part [L][65]
+ * is scratch (per-lane gradients).  dbeta is required.  lf_backproj_loss_dev_host: the same arithmetic on host arrays
+ * (test hook). */
+int lf_backproj_loss_dev(const double* yk, const double* Minv, const double* beta, const double* x_gt, const double* valid,
+                         int B, int L, int n, double* lane_loss, double* loss, double* dbeta, double* xcal, double* g_part,
+                         double* g_const, unsigned int* ticket, lf_stream_t stream);
+int lf_backproj_loss_dev_host(const double* yk, const double* Minv, const double* beta, const double* x_gt,
+                              const double* valid, int B, int L, int n, double* lane_loss, double* loss, double* dbeta,
+                              double* xcal, double* g_const);
+
+/* Learned bird's-eye-view homography (csrc/homography.cu): get_homography(resize)'s source corners shifted by theta [5]
+ * float32 (theta_0..3: x of the four corners in units of 2*resize; theta_4: row of the two top corners in units of
+ * resize).  The warp stays row-preserving, M and M^-1 come in closed form.
+ * lf_homography_tables: M [9] and Minv [9] (row-major), rowp [resize][3] f64 (alpha_v, gamma_v, y'_v), xtab
+ * [resize][2*resize] f32 = alpha_v u + gamma_v, yrow [resize] f32 = y_const - y'_v, yk [56] f64 (y' of the loss's sample
+ * rows); an unmasked row (v >= mask_rows) on the vanishing line or beyond it (den_v = m21 v + m22 zero or of the
+ * other sign than the bottom row's) or with a non-finite table entry ORs LF_STATUS_NONFINITE into
+ * *status.  lf_homography_bwd: g_theta [5] f32 = dL/dtheta from dL/drowp [resize][3], dL/dMinv [9], dL/dyk [56] (f64,
+ * each may be NULL).  All DEVICE.  The _host variants are test hooks on host arrays (g_theta f64 there). */
+int lf_homography_tables(const float* theta, int resize, int mask_rows, double y_const, double* M, double* Minv,
+                         double* rowp, float* xtab, float* yrow, double* yk, int* status, lf_stream_t stream);
+int lf_homography_bwd(const float* theta, int resize, int mask_rows, const double* g_rowp, const double* g_minv,
+                      const double* g_yk, float* g_theta, lf_stream_t stream);
+int lf_homography_host(const float* theta, int resize, double* Mpair, double* rowp, double* yk);
+int lf_homography_bwd_host(const float* theta, int resize, int mask_rows, const double* g_rowp, const double* g_minv,
+                           const double* g_yk, double* g_theta);
+
 
 /* Area loss of the bird's-eye-view experiment over all lanes, its gradient and the exact-area metric in one launch
  * (csrc/loss.cu; replaces Birds_Eye_View_Loss/Loss_crit.py:98-134 summed over the lanes as BEV/main.py:223,237 does, and

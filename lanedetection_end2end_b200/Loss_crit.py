@@ -107,6 +107,37 @@ class backprojection_loss(nn.Module):
         self.y_prime = (self.M[1, 1] * y_d + self.M[1, 2]) / (self.M[2, 1] * y_d + self.M[2, 2])
         self.Y = _design(255 - self.y_prime, options.order)            # [56, order+1]  (:176-188)
         self._dev = None
+        # --learn_homography: the warp is the model's (bind), read every call from its last forward
+        self.learn_homography = bool(getattr(options, "learn_homography", False))
+        self.__dict__["_warp"] = None
+
+    def bind(self, model):
+        """Use ``model``'s learned warp (Net.homography, --learn_homography): every call then reads M^-1 and y' of the
+        model's last forward, and the loss's gradient reaches the warp.  A criterion built with --learn_homography raises
+        until it is bound, so it never silently uses the fixed warp."""
+        warp = getattr(model, "homography", None)
+        if warp is None:
+            raise ValueError("bind() needs a model built with --learn_homography (it has no learned warp)")
+        self.__dict__["_warp"] = warp
+        return self
+
+    def warp(self):
+        """The bound model's current warp (homography.WarpTables), or None with a fixed warp."""
+        if not self.learn_homography:
+            return None
+        w = self.__dict__["_warp"]
+        if w is None:
+            raise RuntimeError("backprojection_loss was built with --learn_homography: call criterion.bind(model) first")
+        if w.current is None:
+            raise RuntimeError("backprojection_loss: the bound model has not run a forward yet")
+        return w.current
+
+    def _warp_constants(self, device):
+        """(M^-1 [3,3], Y [56, n], c_num, c_den) of the bound warp, differentiable (the torch path of forward*)."""
+        w = self.warp()
+        Mi, yp = w.Minv.view(3, 3), w.yk
+        Y = _design(255 - yp, self.Y.shape[1] - 1)
+        return Mi, Y, Mi[0, 1] * yp + Mi[0, 2], Mi[2, 1] * yp + Mi[2, 2]
 
     def _to(self, device):
         if self._dev != device:
@@ -127,9 +158,12 @@ class backprojection_loss(nn.Module):
         L = len(betas)
         self._to(betas[0].device)
         p = torch.stack([b.reshape(b.size(0), -1) for b in betas], 1).double()     # [B, L, n]
-        x_prime = p @ self.Y.t()                                                    # [B, L, 56]
-        Mi = self.M_inv
-        x_cal = (Mi[0, 0] * x_prime + self._c_num) / (Mi[2, 0] * x_prime + self._c_den)
+        if self.learn_homography:
+            Mi, Y, c_num, c_den = self._warp_constants(betas[0].device)
+        else:
+            Mi, Y, c_num, c_den = self.M_inv, self.Y, self._c_num, self._c_den
+        x_prime = p @ Y.t()                                                         # [B, L, 56]
+        x_cal = (Mi[0, 0] * x_prime + c_num) / (Mi[2, 0] * x_prime + c_den)
         v = valid_samples[:, :L]
         x_err = (x_gt[:, :L] - x_cal) * v
         nvalid = v.sum(dim=(0, 2))                                                  # per lane, like the per-lane calls
@@ -141,6 +175,9 @@ class backprojection_loss(nn.Module):
 
     def _fused_host_constants(self):
         """(Y56 [56, n], y' [56], M^-1 [9]) as contiguous float64 numpy arrays for lf_backproj_loss."""
+        if self.learn_homography:
+            raise RuntimeError("backprojection_loss with --learn_homography reads its warp on the device "
+                               "(lf_backproj_loss_dev); the fixed warp's host constants do not describe it")
         # keyed on the identity and in-place version of the tensors it was built from: reassigning or editing
         # M_inv / Y / y_prime (e.g. a finetuned homography) rebuilds the host copies
         key = tuple((id(t), t._version) for t in (self.Y, self.y_prime, self.M_inv))
@@ -161,10 +198,13 @@ class backprojection_loss(nn.Module):
     def forward(self, params, x_gt, valid_samples):
         self._to(params.device)
         p = params.reshape(params.size(0), -1).double()
-        x_prime = p @ self.Y.t()                                        # [B,56]   (:205)
-        Mi = self.M_inv
-        num = Mi[0, 0] * x_prime + self._c_num                          # M^-1 [x', y', 1]^T  (:208-210)
-        den = Mi[2, 0] * x_prime + self._c_den
+        if self.learn_homography:
+            Mi, Y, c_num, c_den = self._warp_constants(params.device)
+        else:
+            Mi, Y, c_num, c_den = self.M_inv, self.Y, self._c_num, self._c_den
+        x_prime = p @ Y.t()                                             # [B,56]   (:205)
+        num = Mi[0, 0] * x_prime + c_num                                # M^-1 [x', y', 1]^T  (:208-210)
+        den = Mi[2, 0] * x_prime + c_den
         x_cal = num / den
         x_err = (x_gt - x_cal) * valid_samples                          # (:214)
         nvalid = valid_samples.sum()
@@ -209,12 +249,49 @@ class _FusedBackprojLoss(torch.autograd.Function):
         return dbeta * g, None, None, None, None
 
 
+class _FusedBackprojLossWarp(torch.autograd.Function):
+    """_FusedBackprojLoss on a learned warp's device constants (lf_backproj_loss_dev): also the gradient with respect to
+    M^-1 and y' of the sample rows."""
+
+    @staticmethod
+    def forward(ctx, beta, x_gt, valid, Minv, yk, crit, lane_scale=None):
+        B, L, n = beta.shape
+        dev = beta.device
+        lane = torch.empty(L, dtype=torch.float64, device=dev)
+        loss = torch.empty(1, dtype=torch.float64, device=dev)
+        dbeta = torch.empty_like(beta)
+        xcal = torch.empty(B, L, 56, dtype=torch.float64, device=dev)
+        g_part = torch.empty(L, 65, dtype=torch.float64, device=dev)
+        g_const = torch.empty(65, dtype=torch.float64, device=dev)
+        p = _capi.ptr
+        _capi.call("lf_backproj_loss_dev", p(yk.detach().contiguous()), p(Minv.detach().contiguous()), p(beta), p(x_gt),
+                   p(valid), B, L, n, p(lane), p(loss), p(dbeta), p(xcal), p(g_part), p(g_const), p(crit._fused_ticket(dev)),
+                   _capi.stream_ptr())
+        if lane_scale is not None:      # the kernel's outputs are linear in per-lane factors
+            ls = lane_scale.to(torch.float64)
+            loss = (lane * ls).mean().reshape(1)
+            dbeta = dbeta * ls.view(1, L, 1)
+            g_const = (g_part * ls.view(L, 1)).sum(0)
+        ctx.save_for_backward(dbeta, g_const)
+        ctx.mark_non_differentiable(xcal)
+        return loss.reshape(()), xcal
+
+    @staticmethod
+    def backward(ctx, g, _g_xcal):
+        dbeta, g_const = ctx.saved_tensors
+        return dbeta * g, None, None, g_const[:9] * g, g_const[9:] * g, None, None
+
+
 def fused_backprojection_loss(crit, betas, x_gt, valid, lane_scale=None):
     """``mean_l crit(betas[l], x_gt[:, l], valid[:, l])[0]`` (what BP/main.py:297-305 computes) in one launch.
     betas: sequence of L tensors [B, order+1, 1] float64 (Net.forward's beta0..3); x_gt, valid: [B, >=L, 56] float64.
     Returns (loss scalar, x_cal*valid [B, L, 56])."""
     L = len(betas)
     beta = torch.stack([b.reshape(b.shape[0], -1) for b in betas], 1).double().contiguous()      # [B, L, n]
+    warp = crit.warp() if hasattr(crit, "warp") else None
+    if warp is not None:
+        return _FusedBackprojLossWarp.apply(beta, x_gt[:, :L].double().contiguous(), valid[:, :L].double().contiguous(),
+                                            warp.Minv, warp.yk, crit, lane_scale)
     return _FusedBackprojLoss.apply(beta, x_gt[:, :L].double().contiguous(), valid[:, :L].double().contiguous(), crit, lane_scale)
 
 

@@ -207,6 +207,17 @@ class Net(nn.Module):
             # the heads' conv weights are re-packed by the ERFNet module's one-launch weight packer (plain dict entry:
             # not a second registration of the submodules)
             self.net.__dict__["_pack_extra"] = (self.line_classification, self.horizon_estimation)
+        # --learn_homography: the warp is a parameter (homography.LearnedHomography, state_dict key
+        # homography.offsets) whose tables are built on the device every forward; a fixed-warp checkpoint loads with
+        # strict=False and starts the fine-tuning from the fixed warp (offsets = 0)
+        self.learn_homography = bool(getattr(args, "learn_homography", False))
+        if self.learn_homography:
+            if args.no_mapping:
+                raise ValueError("--learn_homography learns the bird's-eye-view warp; it cannot be combined with --no_mapping")
+            if getattr(args, "loss_policy", "backproject") != "backproject":
+                raise ValueError("--learn_homography needs --loss_policy backproject (the loss that sees the warp), got %r"
+                                 % (args.loss_policy,))
+            self.homography = submodule("homography").LearnedHomography(resize, self.zero_rows)
         if not args.no_cuda:
             self.idx_row = self.idx_row.cuda()
         self.defer_status_check = False
@@ -223,6 +234,10 @@ class Net(nn.Module):
             if self.lsq_status is None or self.lsq_status.device != output.device:
                 self.lsq_status = torch.zeros(1, dtype=torch.int32, device=output.device)
             status = self.lsq_status
+        warp = None
+        if self.learn_homography:
+            st = status if status is not None else torch.zeros(1, dtype=torch.int32, device=output.device)
+            warp = self.homography(st)
         grid = self.grid
         if grid.device != output.device:
             grid = self.grid = grid.to(output.device)
@@ -250,15 +265,35 @@ class Net(nn.Module):
             _capi.call("lf_seg_lane_maps_line", _capi.ptr(od), B, od.shape[1], od.shape[2], od.shape[3], nl,
                        self.zero_rows, _capi.ptr(gl), _capi.ptr(masked), _capi.stream_ptr())
             with torch.no_grad():
-                beta, _ = self.ls_layer.forward_all(masked, grid, status_out=status, max_order=3)
+                if warp is not None:
+                    beta, _ = self._lsq_warp(masked, warp, 0, "none", False, st, status is None)
+                else:
+                    beta, _ = self.ls_layer.forward_all(masked, grid, status_out=status, max_order=3)
         else:
             if self.classification_branch:
                 line = self.line_classification(shared_encoder)
                 horizon = self.horizon_estimation(shared_encoder)
             # activation (:295) + row mask (:301) + least squares (:314) in one launch;
             # `masked` is materialised only because the API returns it (:315)
-            beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows,
-                                                     act=self.activation.kind, want_masked=True,
-                                                     status_out=status, max_order=3)
+            if warp is not None:
+                beta, masked = self._lsq_warp(output, warp, self.zero_rows, self.activation.kind, True, st, status is None)
+            else:
+                beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows,
+                                                         act=self.activation.kind, want_masked=True,
+                                                         status_out=status, max_order=3)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)
         return beta0, beta1, beta2, beta3, masked, output, line, horizon, output_seg
+
+    def _lsq_warp(self, W, warp, mask_rows, act, want_masked, status, check):
+        ls = self.ls_layer
+        if ls.order > 3:
+            raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(ls.order))
+        Wm = W.reshape(-1, ls.nclasses, ls.H, ls.W)
+        beta, masked = _ops.lsq_warp(Wm, warp, ls.order, mask_rows, act, ls.reg_ls_value, ls.use_cholesky, want_masked,
+                                     status)
+        if check:
+            # the status word holds the warp's guard as well as the solve's: one host read, as torch.inverse's raise
+            st = int(status.item())
+            if st:
+                raise RuntimeError(_ops.status_message(st))
+        return beta, masked

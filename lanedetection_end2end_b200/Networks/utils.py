@@ -86,6 +86,7 @@ _FLAGS = [
     ("--weight_funct", dict(type=str, default="none")),
     ("--end_to_end", _B(True)),
     ("--no_mapping", _B(False)),
+    ("--learn_homography", _B(False)),
     ("--gamma", dict(type=float, default=0.0)),
     ("--clas", _B(False)),
     ("--cudnn", _B(True)),

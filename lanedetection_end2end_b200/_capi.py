@@ -231,6 +231,15 @@ _NET_PROTOS = {
     "lf_pack_gather": (_i, [_p, _i, _i, _p]),
     "lf_backproj_loss": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
     "lf_backproj_loss_host": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p]),
+    "lf_backproj_loss_dev": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_backproj_loss_dev_host": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "lf_lsq_fwd_rowsums": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p, _p, _p,
+                                ctypes.c_size_t, _p]),
+    "lf_lsq_grid_grad": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p]),
+    "lf_homography_tables": (_i, [_p, _i, _i, ctypes.c_double, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_homography_bwd": (_i, [_p, _i, _i, _p, _p, _p, _p, _p]),
+    "lf_homography_host": (_i, [_p, _i, _p, _p, _p]),
+    "lf_homography_bwd_host": (_i, [_p, _i, _i, _p, _p, _p, _p]),
     "lf_area_loss": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
     "lf_area_loss_host": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p]),
     "lf_seg_lane_maps": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p]),

@@ -1,0 +1,278 @@
+// Learned bird's-eye-view homography (DESIGN.md "Learned homography"): the warp of get_homography(resize) with its source
+// corners shifted by theta [5] (float32), its tables for the least-squares layer and the back-projection loss built on the
+// device every forward, and the gradient of the loss with respect to theta.
+//
+//   source corners (x0, yt) (x1, yt) (x2, yb) (x3, yb):  x_i = base_i + theta_i * 2R,  yt = base_top + theta_4 * R
+//   destination corners fixed;  M maps source to destination, M^-1 destination to source.
+//
+// Both warps keep the two corner rows level, so they are row-preserving: M = [[a,b,c],[0,e,f],[0,g,1]] in closed form
+// (row_preserving() below), no 8x8 solve.  Row v of the network image then maps to one bird's-eye-view row:
+//   den_v = g v + 1,  alpha_v = a / den_v,  gamma_v = (b v + c) / den_v,  y'_v = (e v + f) / den_v
+//   xtab[v][u] = alpha_v u + gamma_v,  yrow[v] = y_const - y'_v          (BP/Networks/LSQ_layer.py:93-94)
+// The backward runs the same closed form on dual numbers with one tangent per entry of theta (forward-mode
+// differentiation: exact, a few hundred fp64 operations per thread) and sums the chain rule over the rows, the 56 sample
+// rows of the loss and M^-1 in a fixed order.  Everything is fp64; no host synchronisation.
+#include "lf_common.cuh"
+
+namespace lf {
+
+constexpr int HG_THREADS = 128;
+constexpr int HG_BWD_THREADS = 256;
+constexpr int HG_NT = 5;          // entries of theta
+constexpr int HG_SAMPLES = 56;    // the loss's sample rows (h_samples 160..710 step 10)
+
+template <int N>
+struct Dual {
+    double v, d[N];
+    __host__ __device__ Dual(double x = 0.0) : v(x) {
+        for (int i = 0; i < N; ++i) d[i] = 0.0;
+    }
+};
+template <int N>
+__host__ __device__ inline Dual<N> operator+(const Dual<N>& a, const Dual<N>& b) {
+    Dual<N> r(a.v + b.v);
+    for (int i = 0; i < N; ++i) r.d[i] = a.d[i] + b.d[i];
+    return r;
+}
+template <int N>
+__host__ __device__ inline Dual<N> operator-(const Dual<N>& a, const Dual<N>& b) {
+    Dual<N> r(a.v - b.v);
+    for (int i = 0; i < N; ++i) r.d[i] = a.d[i] - b.d[i];
+    return r;
+}
+template <int N>
+__host__ __device__ inline Dual<N> operator*(const Dual<N>& a, const Dual<N>& b) {
+    Dual<N> r(a.v * b.v);
+    for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i];
+    return r;
+}
+template <int N>
+__host__ __device__ inline Dual<N> operator/(const Dual<N>& a, const Dual<N>& b) {
+    const double q = a.v / b.v;
+    Dual<N> r(q);
+    for (int i = 0; i < N; ++i) r.d[i] = (a.d[i] - q * b.d[i]) / b.v;
+    return r;
+}
+
+// Row-preserving homography mapping (sx0, yt), (sx1, yt), (sx2, yb), (sx3, yb) to (dx0, Yt), (dx1, Yt), (dx2, Yb),
+// (dx3, Yb), normalised to m[8] = 1 (as cv2.getPerspectiveTransform).  Per row r the map is affine in x with scale
+// s_r = a / (g y_r + 1) and offset o_r; s_t (g yt + 1) = s_b (g yb + 1) gives g, then (b, c) and (e, f) are 2x2 solves.
+template <class T>
+__host__ __device__ inline void row_preserving(const T* sx, T yt, T yb, const T* dx, T Yt, T Yb, T* m) {
+    const T st = (dx[1] - dx[0]) / (sx[1] - sx[0]), sb = (dx[3] - dx[2]) / (sx[3] - sx[2]);
+    const T ot = dx[0] - st * sx[0], ob = dx[2] - sb * sx[2];
+    const T one(1.0);
+    const T g = (sb - st) / (st * yt - sb * yb);
+    const T kt = g * yt + one, kb = g * yb + one;
+    const T b = (ot * kt - ob * kb) / (yt - yb);
+    const T e = (Yt * kt - Yb * kb) / (yt - yb);
+    m[0] = st * kt;
+    m[1] = b;
+    m[2] = ot * kt - b * yt;
+    m[3] = T(0.0);
+    m[4] = e;
+    m[5] = Yt * kt - e * yt;
+    m[6] = T(0.0);
+    m[7] = g;
+    m[8] = one;
+}
+
+// The corners get_homography(resize) hands cv2 (float32, BP/Networks/utils.py:104-121), shifted by theta.
+template <class T>
+__host__ __device__ inline void warp_corners(const float* theta, int R, T* sx, T& yt, T& yb, T* dx, T& Yt, T& Yb) {
+    const double w = 2.0 * R;
+    const double bx[4] = {(double)(float)(0.45 * w), (double)(float)(0.55 * w), (double)(float)(0.02 * w),
+                          (double)(float)(0.97 * w)};
+    const double dxb[4] = {(double)(float)(0.45 * w), (double)(float)(0.55 * w), (double)(float)(0.45 * w),
+                           (double)(float)(0.55 * w)};
+    const double top = (double)(float)(0.20 * R), bottom = (double)(float)(R - 1);
+    for (int i = 0; i < 4; ++i) {
+        sx[i] = T(bx[i]) + T((double)theta[i]) * T(w);
+        dx[i] = T(dxb[i]);
+    }
+    yt = T(top) + T((double)theta[4]) * T((double)R);
+    yb = T(bottom);
+    Yt = T(top);
+    Yb = T(bottom);
+}
+
+// M (m[0..8]) and M^-1 (m[9..17]) of theta
+template <class T>
+__host__ __device__ inline void warp_pair(const float* theta, int R, T* m) {
+    T sx[4], dx[4], yt, yb, Yt, Yb;
+    warp_corners<T>(theta, R, sx, yt, yb, dx, Yt, Yb);
+    row_preserving<T>(sx, yt, yb, dx, Yt, Yb, m);
+    row_preserving<T>(dx, Yt, Yb, sx, yt, yb, m + 9);
+}
+// the same on dual numbers, seeded so that tangent j is d/dtheta_j
+__host__ __device__ inline void warp_pair_dual(const float* theta, int R, Dual<HG_NT>* m) {
+    const double w = 2.0 * R;
+    Dual<HG_NT> sx[4], dx[4], yt, yb, Yt, Yb;
+    warp_corners<Dual<HG_NT>>(theta, R, sx, yt, yb, dx, Yt, Yb);
+    for (int i = 0; i < 4; ++i) sx[i].d[i] = w;
+    yt.d[4] = (double)R;
+    row_preserving(sx, yt, yb, dx, Yt, Yb, m);
+    row_preserving(dx, Yt, Yb, sx, yt, yb, m + 9);
+}
+
+// image row of the loss's sample s (BP/Loss_crit.py:173; the reference divides by 2.5 whatever --resize is)
+__host__ __device__ inline double sample_row(int s) { return (double)(160 + 10 * s - 80) / 2.5; }
+
+// alpha, gamma, y' of image row v
+template <class T>
+__host__ __device__ inline void row_params(const T* m, double v, T* p) {
+    const T vv(v);
+    const T den = m[7] * vv + m[8];
+    p[0] = m[0] / den;
+    p[1] = (m[1] * vv + m[2]) / den;
+    p[2] = (m[4] * vv + m[5]) / den;
+}
+
+__global__ void __launch_bounds__(HG_THREADS) homography_tables_kernel(const float* __restrict__ theta, int R, int mask_rows,
+                                                                        double y_const, double* __restrict__ M,
+                                                                        double* __restrict__ Minv,
+                                                                        double* __restrict__ rowp, float* __restrict__ xtab,
+                                                                        float* __restrict__ yrow, double* __restrict__ yk,
+                                                                        int* __restrict__ status) {
+    pdl_entry();
+    const int v = blockIdx.x, t = threadIdx.x, W = 2 * R;
+    float th[HG_NT];
+    for (int j = 0; j < HG_NT; ++j) th[j] = theta[j];
+    double m[18];
+    warp_pair<double>(th, R, m);
+    double p[3];
+    row_params<double>(m, (double)v, p);
+    const bool guarded = v >= mask_rows;
+    bool bad = false;
+    for (int u = t; u < W; u += HG_THREADS) {
+        const float x = (float)(p[0] * u + p[1]);
+        xtab[(size_t)v * W + u] = x;
+        bad |= !isfinite(x);
+    }
+    if (t == 0) {
+        // with m22 = 1 the rows below the vanishing line have den < 0: a usable row has the bottom row's sign of den
+        const double den = (m[7] * v + m[8]) * (m[7] * (R - 1) + m[8]);
+        const float y = (float)(y_const - p[2]);
+        rowp[(size_t)v * 3 + 0] = p[0];
+        rowp[(size_t)v * 3 + 1] = p[1];
+        rowp[(size_t)v * 3 + 2] = p[2];
+        yrow[v] = y;
+        bad |= !(den > 0.0) || !isfinite(p[0]) || !isfinite(p[1]) || !isfinite(y);
+    }
+    // an unmasked row at or above the vanishing line: the batch is skipped like a singular system
+    if (guarded && bad) atomicOr(status, LF_STATUS_NONFINITE);
+    if (v == 0) {
+        if (t < 9) M[t] = m[t];
+        if (t >= 9 && t < 18) Minv[t - 9] = m[t];
+        if (t < HG_SAMPLES) {
+            const double y = sample_row(t);
+            yk[t] = (m[4] * y + m[5]) / (m[7] * y + m[8]);
+        }
+    }
+}
+
+// One thread's share of dL/dtheta: rows t, t + T, ... (unmasked rows only), sample t < 56, and M^-1 on thread 0.
+__host__ __device__ inline void homography_bwd_partial(const Dual<HG_NT>* m, int t, int nthreads, int R, int mask_rows,
+                                                       const double* g_rowp, const double* g_minv, const double* g_yk,
+                                                       double* acc) {
+    for (int j = 0; j < HG_NT; ++j) acc[j] = 0.0;
+    if (g_rowp)
+        for (int v = mask_rows + t; v < R; v += nthreads) {
+            Dual<HG_NT> p[3];
+            row_params(m, (double)v, p);
+            for (int k = 0; k < 3; ++k) {
+                const double g = g_rowp[(size_t)v * 3 + k];
+                for (int j = 0; j < HG_NT; ++j) acc[j] += g * p[k].d[j];
+            }
+        }
+    if (g_yk && t < HG_SAMPLES) {
+        const Dual<HG_NT> y(sample_row(t));
+        const Dual<HG_NT> q = (m[4] * y + m[5]) / (m[7] * y + m[8]);
+        for (int j = 0; j < HG_NT; ++j) acc[j] += g_yk[t] * q.d[j];
+    }
+    if (g_minv && t == 0)
+        for (int i = 0; i < 9; ++i)
+            for (int j = 0; j < HG_NT; ++j) acc[j] += g_minv[i] * m[9 + i].d[j];
+}
+
+__global__ void __launch_bounds__(HG_BWD_THREADS) homography_bwd_kernel(const float* __restrict__ theta, int R, int mask_rows,
+                                                                         const double* __restrict__ g_rowp,
+                                                                         const double* __restrict__ g_minv,
+                                                                         const double* __restrict__ g_yk,
+                                                                         float* __restrict__ g_theta) {
+    pdl_entry();
+    __shared__ double red[HG_NT][HG_BWD_THREADS];
+    const int t = threadIdx.x;
+    float th[HG_NT];
+    for (int j = 0; j < HG_NT; ++j) th[j] = theta[j];
+    Dual<HG_NT> m[18];
+    warp_pair_dual(th, R, m);
+    double acc[HG_NT];
+    homography_bwd_partial(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp, g_minv, g_yk, acc);
+    for (int j = 0; j < HG_NT; ++j) red[j][t] = acc[j];
+    __syncthreads();
+    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1) {   // fixed tree
+        if (t < w)
+            for (int j = 0; j < HG_NT; ++j) red[j][t] += red[j][t + w];
+        __syncthreads();
+    }
+    if (t < HG_NT) g_theta[t] = (float)red[t][0];
+}
+
+}  // namespace lf
+
+using namespace lf;
+
+// theta [5] f32, M [9], M^-1 [9] (row-major), rowp [R][3] f64 (alpha, gamma, y'), xtab [R][2R] f32, yrow [R] f32,
+// yk [56] f64, status: one int OR-ed with LF_STATUS_NONFINITE -- all DEVICE.
+extern "C" int lf_homography_tables(const float* theta, int resize, int mask_rows, double y_const, double* M,
+                                    double* Minv, double* rowp, float* xtab, float* yrow, double* yk, int* status, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(theta && M && Minv && rowp && xtab && yrow && yk && status);
+    LF_REQUIRE(resize >= 2 && resize <= 65535 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(homography_tables_kernel, resize, HG_THREADS, 0, stream, theta, resize, mask_rows, y_const, M, Minv, rowp, xtab,
+              yrow, yk, status);
+    return check_launch();
+}
+
+// dL/dtheta [5] f32 from dL/d(alpha, gamma, y') [R][3], dL/dM^-1 [9] and dL/dy'_k [56] (each f64, may be NULL) -- DEVICE.
+extern "C" int lf_homography_bwd(const float* theta, int resize, int mask_rows, const double* g_rowp, const double* g_minv,
+                                 const double* g_yk, float* g_theta, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(theta && g_theta && resize >= 2 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(homography_bwd_kernel, 1, HG_BWD_THREADS, 0, stream, theta, resize, mask_rows, g_rowp, g_minv, g_yk, g_theta);
+    return check_launch();
+}
+
+// TEST HOOKS: the same code on HOST arrays; never called by the package.  lf_homography_host: Mpair [18], and with
+// rowp != NULL the (alpha, gamma, y') of every row and with yk != NULL the 56 sample rows' y'.
+extern "C" int lf_homography_host(const float* theta, int resize, double* Mpair, double* rowp, double* yk) {
+    if (!(theta && Mpair && resize >= 2)) return LF_ERR_INVALID_ARGUMENT;
+    warp_pair<double>(theta, resize, Mpair);
+    if (rowp)
+        for (int v = 0; v < resize; ++v) row_params<double>(Mpair, (double)v, rowp + (size_t)v * 3);
+    if (yk)
+        for (int s = 0; s < HG_SAMPLES; ++s) {
+            const double y = sample_row(s);
+            yk[s] = (Mpair[4] * y + Mpair[5]) / (Mpair[7] * y + Mpair[8]);
+        }
+    return LF_OK;
+}
+
+extern "C" int lf_homography_bwd_host(const float* theta, int resize, int mask_rows, const double* g_rowp,
+                                      const double* g_minv, const double* g_yk, double* g_theta) {
+    if (!(theta && g_theta && resize >= 2 && mask_rows >= 0 && mask_rows <= resize)) return LF_ERR_INVALID_ARGUMENT;
+    Dual<HG_NT> m[18];
+    warp_pair_dual(theta, resize, m);
+    double red[HG_NT][HG_BWD_THREADS];
+    for (int t = 0; t < HG_BWD_THREADS; ++t) {
+        double acc[HG_NT];
+        homography_bwd_partial(m, t, HG_BWD_THREADS, resize, mask_rows, g_rowp, g_minv, g_yk, acc);
+        for (int j = 0; j < HG_NT; ++j) red[j][t] = acc[j];
+    }
+    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1)
+        for (int t = 0; t < w; ++t)
+            for (int j = 0; j < HG_NT; ++j) red[j][t] += red[j][t + w];
+    for (int j = 0; j < HG_NT; ++j) g_theta[j] = red[j][0];
+    return LF_OK;
+}

@@ -189,6 +189,200 @@ extern "C" int lf_backproj_loss_host(const double* Y56, const double* yprime, co
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// The same loss with its warp constants on the DEVICE (a learned homography, csrc/homography.cu): y'_k of the 56 sample
+// rows and M^-1 are read at run time, so a captured graph follows the warp, and the kernel also emits the loss's gradient
+// with respect to them: g_const [65] = dloss/dM^-1 (9, row-major) then dloss/dy'_k (56).  Y56 is built from y'_k as the
+// reference builds it (rows [y^d .. y 1], y = 255 - y'_k, BP/Loss_crit.py:175-188), so y'_k reaches the loss both
+// through the back-projection and through the curve's sample points.
+namespace lf {
+
+constexpr int BP_NG = 9 + BP_S;
+
+// row s of the constants from y'_s (and, for s < 9, entry s of M^-1)
+__host__ __device__ inline void bp_const_row(const double* yk, const double* Minv, int n, int s, BpConst* c) {
+    c->yp[s] = yk[s];
+    const double y = 255.0 - yk[s];
+    double pw = 1.0;
+    for (int k = BP_MAXN - 1; k >= 0; --k) {
+        c->Y[s][k] = k < n ? pw : 0.0;
+        if (k < n) pw *= y;
+    }
+    if (s < 9) c->Mi[s] = Minv[s];
+}
+
+// one (image, sample) point: adds d(err^2)/dM^-1 to gmi[9] and returns d(err^2)/dy'_s (before the 1/nvalid, 1/L factors)
+__host__ __device__ inline double bp_point_const_grad(const BpConst& c, const double* beta, int n, int s, double xgt,
+                                                      double valid, double* gmi) {
+    double xp = 0.0;
+    for (int k = 0; k < n; ++k) xp += c.Y[s][k] * beta[k];
+    const double yk = c.yp[s];
+    const double num = c.Mi[0] * xp + (c.Mi[1] * yk + c.Mi[2]);
+    const double den = c.Mi[6] * xp + (c.Mi[7] * yk + c.Mi[8]);
+    const double xcal = num / den;
+    const double err = (xgt - xcal) * valid;
+    const double id = -2.0 * err * valid / den;      // d(err^2)/dxcal / den
+    gmi[0] += id * xp;
+    gmi[1] += id * yk;
+    gmi[2] += id;
+    gmi[6] -= id * xcal * xp;
+    gmi[7] -= id * xcal * yk;
+    gmi[8] -= id * xcal;
+    // dx'/dy of the sampled curve, y = 255 - y'
+    const double y = 255.0 - yk;
+    double dxp = 0.0, pw = 1.0;
+    for (int k = n - 2; k >= 0; --k) {
+        dxp += beta[k] * (double)(n - 1 - k) * pw;
+        pw *= y;
+    }
+    return id * ((c.Mi[1] - c.Mi[7] * xcal) - (c.Mi[0] - c.Mi[6] * xcal) * dxp);
+}
+
+__global__ void __launch_bounds__(BP_THREADS) backproj_loss_dev_kernel(const double* __restrict__ yk,
+                                                                        const double* __restrict__ Minv,
+                                                                        const double* __restrict__ beta,
+                                                                        const double* __restrict__ x_gt,
+                                                                        const double* __restrict__ valid, int B, int L, int n,
+                                                                        double* __restrict__ lane_loss,
+                                                                        double* __restrict__ dbeta, double* __restrict__ xcal,
+                                                                        double* __restrict__ g_part, unsigned int* ticket,
+                                                                        double* __restrict__ loss, double* __restrict__ g_const) {
+    pdl_entry();
+    __shared__ BpConst c;
+    __shared__ double red_sq[BP_THREADS], red_nv[BP_THREADS];
+    __shared__ double gm[9][BP_S];
+    __shared__ double s_scale;
+    const int l = blockIdx.x;
+    const int tid = threadIdx.x;
+    if (tid < BP_S) bp_const_row(yk, Minv, n, tid, &c);
+    __syncthreads();
+    // pass 1: sum of squared errors and of valid over (b, s), as backproj_loss_kernel
+    double sq = 0.0, nv = 0.0;
+    for (int i = tid; i < B * BP_S; i += BP_THREADS) {
+        const int b = i / BP_S, s = i - b * BP_S;
+        const size_t o = ((size_t)b * L + l) * BP_S + s;
+        double xc, q, dq;
+        bp_point(c, beta + ((size_t)b * L + l) * n, n, s, x_gt[o], valid[o], &xc, &q, &dq);
+        if (xcal) xcal[o] = xc;
+        sq += q;
+        nv += valid[o];
+    }
+    red_sq[tid] = sq;
+    red_nv[tid] = nv;
+    __syncthreads();
+    for (int w = BP_THREADS / 2; w > 0; w >>= 1) {
+        if (tid < w) {
+            red_sq[tid] += red_sq[tid + w];
+            red_nv[tid] += red_nv[tid + w];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const double denom = red_nv[0] == 0.0 ? 1.0 : red_nv[0];
+        lane_loss[l] = red_sq[0] / denom;
+        s_scale = 1.0 / (denom * (double)L);
+    }
+    __syncthreads();
+    const double scale = s_scale;
+    // pass 2: dloss/dbeta, one thread per (b, k)
+    for (int i = tid; i < B * n; i += BP_THREADS) {
+        const int b = i / n, k = i - b * n;
+        const double* bt = beta + ((size_t)b * L + l) * n;
+        double g = 0.0;
+        for (int s = 0; s < BP_S; ++s) {
+            const size_t o = ((size_t)b * L + l) * BP_S + s;
+            double xc, q, dq;
+            bp_point(c, bt, n, s, x_gt[o], valid[o], &xc, &q, &dq);
+            g += dq * c.Y[s][k];
+        }
+        dbeta[((size_t)b * L + l) * n + k] = g * scale;
+    }
+    // pass 3: dloss/dy'_s (thread s, images in order) and dloss/dM^-1 (per-sample partials, summed in sample order)
+    if (tid < BP_S) {
+        double gmi[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        double gy = 0.0;
+        for (int b = 0; b < B; ++b) {
+            const size_t o = ((size_t)b * L + l) * BP_S + tid;
+            gy += bp_point_const_grad(c, beta + ((size_t)b * L + l) * n, n, tid, x_gt[o], valid[o], gmi);
+        }
+        g_part[(size_t)l * BP_NG + 9 + tid] = gy * scale;
+        for (int i = 0; i < 9; ++i) gm[i][tid] = gmi[i];
+    }
+    __syncthreads();
+    if (tid < 9) {
+        double g = 0.0;
+        for (int s = 0; s < BP_S; ++s) g += gm[tid][s];
+        g_part[(size_t)l * BP_NG + tid] = g * scale;
+    }
+    // the last lane CTA sums the lane losses and the lanes' constant gradients in lane order
+    __threadfence();
+    __syncthreads();
+    __shared__ bool last;
+    if (tid == 0) last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    if (tid < BP_NG) {
+        double g = 0.0;
+        for (int j = 0; j < L; ++j) g += __ldcg(g_part + (size_t)j * BP_NG + tid);
+        g_const[tid] = g;
+    }
+    if (tid == 0) {
+        double tot = 0.0;
+        for (int j = 0; j < L; ++j) tot += __ldcg(lane_loss + j);
+        *loss = tot / (double)L;
+        *ticket = 0u;
+    }
+}
+
+}  // namespace lf
+
+// yk [56], Minv [9]: DEVICE constants; beta, x_gt, valid, lane_loss, loss, dbeta, xcal (or NULL), ticket as
+// lf_backproj_loss; g_part [L][65] scratch (the per-lane gradients, scaled like dbeta), g_const [65] -- all DEVICE.
+extern "C" int lf_backproj_loss_dev(const double* yk, const double* Minv, const double* beta, const double* x_gt,
+                                    const double* valid, int B, int L, int n, double* lane_loss, double* loss, double* dbeta,
+                                    double* xcal, double* g_part, double* g_const, unsigned int* ticket, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(yk && Minv && beta && x_gt && valid && lane_loss && loss && dbeta && g_part && g_const && ticket);
+    LF_REQUIRE(B > 0 && L > 0 && L <= 65535 && n >= 1 && n <= BP_MAXN);
+    lf_launch(backproj_loss_dev_kernel, L, BP_THREADS, 0, stream, yk, Minv, beta, x_gt, valid, B, L, n, lane_loss, dbeta, xcal,
+              g_part, ticket, loss, g_const);
+    return check_launch();
+}
+
+// TEST HOOK: lf_backproj_loss_dev's arithmetic on HOST arrays (g_const [65] may be NULL); never called by the package.
+extern "C" int lf_backproj_loss_dev_host(const double* yk, const double* Minv, const double* beta, const double* x_gt,
+                                         const double* valid, int B, int L, int n, double* lane_loss, double* loss,
+                                         double* dbeta, double* xcal, double* g_const) {
+    if (!(yk && Minv && beta && x_gt && valid && lane_loss && loss && B > 0 && L > 0 && n >= 1 && n <= BP_MAXN))
+        return LF_ERR_INVALID_ARGUMENT;
+    BpConst c;
+    for (int s = 0; s < BP_S; ++s) bp_const_row(yk, Minv, n, s, &c);
+    double Y56[BP_S * BP_MAXN];
+    for (int s = 0; s < BP_S; ++s)
+        for (int k = 0; k < n; ++k) Y56[s * n + k] = c.Y[s][k];
+    const int rc = lf_backproj_loss_host(Y56, c.yp, c.Mi, beta, x_gt, valid, B, L, n, lane_loss, loss, dbeta, xcal);
+    if (rc || !g_const) return rc;
+    for (int i = 0; i < BP_NG; ++i) g_const[i] = 0.0;
+    for (int l = 0; l < L; ++l) {
+        double nv = 0.0;
+        for (int b = 0; b < B; ++b)
+            for (int s = 0; s < BP_S; ++s) nv += valid[((size_t)b * L + l) * BP_S + s];
+        const double scale = 1.0 / ((nv == 0.0 ? 1.0 : nv) * (double)L);
+        double gm[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int s = 0; s < BP_S; ++s) {
+            double gy = 0.0;
+            for (int b = 0; b < B; ++b) {
+                const size_t o = ((size_t)b * L + l) * BP_S + s;
+                gy += bp_point_const_grad(c, beta + ((size_t)b * L + l) * n, n, s, x_gt[o], valid[o], gm);
+            }
+            g_const[9 + s] += gy * scale;
+        }
+        for (int i = 0; i < 9; ++i) g_const[i] += gm[i] * scale;
+    }
+    return LF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Area loss of the bird's-eye-view experiment over all lanes, its gradient and the exact-area metric in one launch:
 // Birds_Eye_View_Loss/Loss_crit.py:98-134 (`Area_Loss`, order 2) summed over the lanes as BEV/main.py:223,237 does, and
 // `polynomial.trapezoidal` (:12-35) as BEV/main.py:273-280 / :436-442 evaluates it.

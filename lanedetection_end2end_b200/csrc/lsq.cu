@@ -375,8 +375,11 @@ __device__ __forceinline__ int packed_holder(int i) {
 // ---------------------------------------------------------------------------------
 // NL = lanes per CTA (compile time, so the loads of all lanes and column steps of a row are in flight
 // together: the kernel is latency-bound otherwise -- long-scoreboard stalls).
-template <int ACT_T, bool BF16, int NL>
-__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_kernel(const LsqArgs a) {
+// ROWSUMS: also accumulate C_r = sum_c w c and store (A_r, B_r, C_r) of every unmasked row in rowsums [B][L][H][3] --
+// what the gradient with respect to a learned homography's tables needs (lsq_grid_grad_kernel).  `rowsums` is a kernel
+// parameter of its own, not an LsqArgs field, so the other kernels' argument block stays as it was.
+template <int ACT_T, bool BF16, int NL, bool ROWSUMS>
+__device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* rowsums) {
     pdl_entry();
     __shared__ double red[LSQ_WARPS][LSQ_MAXL][LSQ_MAXNM];
     __shared__ double mom[LSQ_MAXL][LSQ_MAXNM];
@@ -418,7 +421,7 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
 #pragma unroll
     for (int l = 0; l < NL; ++l) map_base[l] = ((size_t)(b * a.L + min(l0 + l, a.L - 1)) * a.H) * a.W;
     for (int r = r_begin + warp * RU; r < r_end; r += LSQ_WARPS * RU) {
-        float A[RU][NL], Bx[RU][NL];
+        float A[RU][NL], Bx[RU][NL], Cx[RU][NL];
         size_t rowoff[RU];
         bool rvalid[RU];
 #pragma unroll
@@ -426,7 +429,7 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
             rvalid[u] = r + u < r_end;
             rowoff[u] = (size_t)(rvalid[u] ? r + u : r) * a.W;
 #pragma unroll
-            for (int l = 0; l < NL; ++l) A[u][l] = Bx[u][l] = 0.f;
+            for (int l = 0; l < NL; ++l) A[u][l] = Bx[u][l] = Cx[u][l] = 0.f;
         }
 #pragma unroll UNR
         for (int cv = lane; cv < WV; cv += 32) {
@@ -439,7 +442,7 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
                     const size_t off = map_base[l] + rowoff[u] + (size_t)V * cv;
                     float o[V];
                     load_mapv<BF16>(a.o, off, o);
-                    float sa = 0.f, sb = 0.f;
+                    float sa = 0.f, sb = 0.f, sc = 0.f;
                     // (the backward kernel writes its math with the f2_* pair helpers of lf_common.cuh; on sm_90a they are
                     // two scalar ops each, rounded identically)
 #pragma unroll
@@ -448,6 +451,7 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
                         const float w = o[e] * o[e];
                         sa += w;
                         sb = fmaf(w, x[e], sb);
+                        if constexpr (ROWSUMS) sc = fmaf(w, (float)(V * cv + e), sc);
                     }
                     if (a.masked && l < nl && rvalid[u]) {
 #pragma unroll
@@ -457,6 +461,7 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
                     }
                     A[u][l] += sa;
                     Bx[u][l] += sb;
+                    if constexpr (ROWSUMS) Cx[u][l] += sc;
                 }
             }
         }
@@ -482,6 +487,20 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
                 const float s = __shfl_sync(0xffffffffu, tot, packed_holder<NV>((useB ? NLP : 0) + l));
                 acc[l] = fma(pw, (double)s, acc[l]);
             }
+            if constexpr (ROWSUMS) {
+#pragma unroll
+                for (int l = 0; l < NL; ++l) {
+                    const float sa = __shfl_sync(0xffffffffu, tot, packed_holder<NV>(l));
+                    const float sb = __shfl_sync(0xffffffffu, tot, packed_holder<NV>(NLP + l));
+                    const float sc = warp_sum(Cx[u][l]);
+                    if (lane == 0 && l < nl) {
+                        float* rs = rowsums + ((size_t)(b * a.L + l0 + l) * a.H + r + u) * 3;
+                        rs[0] = sa;
+                        rs[1] = sb;
+                        rs[2] = sc;
+                    }
+                }
+            }
         }
     }
     if (lane < LSQ_MAXNM) {
@@ -489,6 +508,72 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
         for (int l = 0; l < NL; ++l) red[warp][l][lane] = (lane < NM && l < nl) ? acc[l] : 0.0;
     }
     lsq_chunk_tail(a, red, mom, chunk, b, lg, l0, nl);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_kernel(const LsqArgs a) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, false>(a, nullptr);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsums_kernel(const LsqArgs a, float* rowsums) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, true>(a, rowsums);
+}
+
+// ---------------------------------------------------------------------------------
+// Gradient of the loss with respect to the row-separable tables x_{r,c} = alpha_r c + gamma_r, y_r = const - y'_r,
+// from the forward's row sums (DESIGN.md "Learned homography"), summed over images and lanes in a fixed order:
+//   dL/dgamma_r = (phi_r.z) A_r ,  dL/dalpha_r = (phi_r.z) C_r ,
+//   dL/dy_r     = (phi'_r.z)(B_r - (phi_r.beta) A_r) - (phi_r.z)(phi'_r.beta) A_r ,   dL/dy'_r = -dL/dy_r
+// with phi_r = [y^d .. y 1], z = Z^-1 g.  One thread per row; masked rows get 0.  g_rowp [H][3] = (alpha, gamma, y').
+// ---------------------------------------------------------------------------------
+constexpr int LSQ_GG_THREADS = 128;
+
+__global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const float* __restrict__ rowsums,
+                                                                        const float* __restrict__ yrow,
+                                                                        const double* __restrict__ beta,
+                                                                        const double* __restrict__ zinv,
+                                                                        const double* __restrict__ gbeta, int B, int L,
+                                                                        int H, int order, int mask_rows,
+                                                                        double* __restrict__ g_rowp) {
+    pdl_entry();
+    const int r = blockIdx.x * LSQ_GG_THREADS + threadIdx.x;
+    if (r >= H) return;
+    const int n = order + 1;
+    double ga = 0.0, gg = 0.0, gy = 0.0;
+    if (r >= mask_rows) {
+        const double y = (double)yrow[r];
+        double phi[LF_MAX_ORDER + 1], dphi[LF_MAX_ORDER + 1];   // index i: power d - i
+        double pw = 1.0, pwm = 0.0;                                 // y^k, k y^(k-1)
+        for (int i = order; i >= 0; --i) {
+            phi[i] = pw;
+            dphi[i] = pwm;
+            pwm = pwm * y + pw;
+            pw *= y;
+        }
+        for (int bl = 0; bl < B * L; ++bl) {
+            const double* bt = beta + (size_t)bl * n;
+            const double* zi = zinv + (size_t)bl * n * n;
+            const double* g = gbeta + (size_t)bl * n;
+            double pz = 0.0, dz = 0.0, pb = 0.0, db = 0.0;
+            for (int i = 0; i < n; ++i) {
+                double z = 0.0;
+                for (int j = 0; j < n; ++j) z += zi[i * n + j] * g[j];
+                pz += phi[i] * z;
+                dz += dphi[i] * z;
+                pb += phi[i] * bt[i];
+                db += dphi[i] * bt[i];
+            }
+            const float* rs = rowsums + ((size_t)bl * H + r) * 3;
+            const double A = rs[0], Bs = rs[1], C = rs[2];
+            gg += pz * A;
+            ga += pz * C;
+            gy += dz * (Bs - pb * A) - pz * db * A;
+        }
+    }
+    g_rowp[(size_t)r * 3 + 0] = ga;
+    g_rowp[(size_t)r * 3 + 1] = gg;
+    g_rowp[(size_t)r * 3 + 2] = -gy;
 }
 
 // ---------------------------------------------------------------------------------
@@ -817,6 +902,58 @@ extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const f
         LSQ_DISPATCH_NL(lsq_fwd_rowsep_kernel, p.nl, grid, a);
     else
         LSQ_DISPATCH(lsq_fwd_general_kernel, grid, a);
+    return check_launch();
+}
+
+template <int ACT_T, bool BF16>
+static void launch_rowsums(int nl, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums) {
+    switch (nl) {
+        case 1: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 1>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
+        case 2: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 2>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
+        case 3: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 3>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
+        default: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 4>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
+    }
+}
+
+// lf_lsq_fwd on the row-separable kernel that also stores the row sums: same arguments and plan, yrow required,
+// rowsums [B][L][H][3] float32 (rows >= mask_rows written).
+extern "C" int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L, int H,
+                                  int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
+                                  double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                                  size_t workspace_bytes, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(o && xtab && yrow && beta && zinv && status && rowsums && workspace);
+    LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
+    LsqPlan p{};
+    const int rc = lsq_plan(0, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    if (workspace_bytes < lf_lsq_workspace_bytes(B, L, H, W, order)) return LF_ERR_WORKSPACE_TOO_SMALL;
+    LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked));
+    LsqArgs a{};
+    a.o = o; a.xtab = xtab; a.yrow = yrow;
+    a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
+    a.reg_ls = reg_ls; a.beta = beta; a.zinv = zinv; a.masked = masked; a.status = status;
+    a.nchunks = p.nchunks;
+    a.tickets = reinterpret_cast<int*>(workspace);
+    a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
+    dim3 grid(a.nchunks, B, p.groups);
+    if (act == LF_ACT_SQUARE)
+        o_dtype == LF_BF16 ? launch_rowsums<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums)
+                           : launch_rowsums<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums);
+    else
+        o_dtype == LF_BF16 ? launch_rowsums<LSQ_ACT_RUNTIME, true>(p.nl, grid, stream, a, rowsums)
+                           : launch_rowsums<LSQ_ACT_RUNTIME, false>(p.nl, grid, stream, a, rowsums);
+    return check_launch();
+}
+
+extern "C" int lf_lsq_grid_grad(const float* rowsums, const float* yrow, const double* beta, const double* zinv,
+                                const double* gbeta, int B, int L, int H, int order, int mask_rows, double* g_rowp,
+                                lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(rowsums && yrow && beta && zinv && gbeta && g_rowp);
+    LF_REQUIRE(B > 0 && L > 0 && H > 0 && order >= 0 && order <= LF_MAX_ORDER && mask_rows >= 0 && mask_rows <= H);
+    lf_launch(lsq_grid_grad_kernel, (H + LSQ_GG_THREADS - 1) / LSQ_GG_THREADS, LSQ_GG_THREADS, 0, stream, rowsums, yrow,
+              beta, zinv, gbeta, B, L, H, order, mask_rows, g_rowp);
     return check_launch();
 }
 

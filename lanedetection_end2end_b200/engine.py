@@ -367,6 +367,8 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     if not e2e and L != 4:
         raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
                          "loader's 4 line flags over %d lane maps" % L)
+    if getattr(criterion, "learn_homography", False):
+        criterion.bind(model)
     dev = next(model.parameters()).device
     model.train()
     meters = DeviceMeters(("loss", "rmse"), dev)

@@ -50,6 +50,11 @@ class Projections:
         self._crit = backprojection_loss(options)      # owns Y56, y', M^-1 (the same constants, BP/Loss_crit.py:166-188)
         self.M, self.M_inv = self._crit.M, self._crit.M_inv
 
+    def bind(self, model):
+        """Project with ``model``'s learned warp (--learn_homography), read from its last forward."""
+        self._crit.bind(model)
+        return self
+
     def compute_all(self, betas):
         """betas: sequence of L tensors [B, order+1, 1] (Net.forward's beta0..3, None entries skipped) -> [B, L, 56] f64."""
         betas = [b for b in betas if b is not None]
@@ -63,6 +68,14 @@ class Projections:
         lane = torch.empty(L, dtype=torch.float64, device=dev)
         loss = torch.empty(1, dtype=torch.float64, device=dev)
         xcal = torch.empty(B, L, 56, dtype=torch.float64, device=dev)
+        warp = self._crit.warp()
+        if warp is not None:
+            g = torch.empty(L + 1, 65, dtype=torch.float64, device=dev)
+            _capi.call("lf_backproj_loss_dev", _capi.ptr(warp.yk.detach()), _capi.ptr(warp.Minv.detach()), _capi.ptr(beta),
+                       _capi.ptr(zeros), _capi.ptr(ones), B, L, n, _capi.ptr(lane), _capi.ptr(loss),
+                       _capi.ptr(torch.empty_like(beta)), _capi.ptr(xcal), _capi.ptr(g[:L]), _capi.ptr(g[L]),
+                       _capi.ptr(self._crit._fused_ticket(dev)), _capi.stream_ptr())
+            return resize_coordinates(xcal)
         host = self._crit._fused_host_constants()
         p = lambda t: ctypes.c_void_p(t.data_ptr())
         _capi.call("lf_backproj_loss", host[0].ctypes.data, host[1].ctypes.data, host[2].ctypes.data, p(beta), p(zeros), p(ones),
@@ -255,6 +268,8 @@ def test_model(loader, model, criterion, criterion_seg, criterion_line_class, cr
     dev = next(model.parameters()).device
     scorer = _scorer_for(os.path.join(args.test_dir, "test_label.json"), dev)
     params = Projections(args)
+    if getattr(args, "learn_homography", False):
+        params.bind(model)
 
     def post(out):
         horizon_pred = torch.sigmoid(out[7]).sum(dim=1)
@@ -323,6 +338,8 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
     if not e2e and L != 4:
         raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
                          "loader's 4 line flags over %d lane maps" % L)
+    if getattr(criterion, "learn_homography", False):
+        criterion.bind(model)
     dev = next(model.parameters()).device
     meters = DeviceMeters(("loss", "acc_hor", "acc_line", "rmse"), dev)
     status = BatchStatus(len(loader), dev)

@@ -79,7 +79,9 @@ class LsqFunction(torch.autograd.Function):
     """beta, masked = LSQ(o).  o: [B,L,H,W] f32/bf16 raw (or pre-activated) maps."""
 
     @staticmethod
-    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out):
+    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out, rowp=None):
+        # rowp: a learned warp's (alpha, gamma, y') per row (homography.WarpTables.rowp); the forward then also keeps the
+        # row sums and the backward returns dL/drowp
         _capi.require_cuda(o)
         if order < 0 or order > _capi.MAX_ORDER:
             raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(order))
@@ -96,19 +98,30 @@ class LsqFunction(torch.autograd.Function):
         nbytes = h.lf_lsq_workspace_bytes(B, L, H, W, order)
         ws = _workspace(dev, nbytes)
         esz = o.element_size()
-        with torch.cuda.device(dev):
-            _capi.call("lf_lsq_fwd", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab), _capi.ptr(tables.ytab),
-                       _capi.ptr(tables.yrow), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
-                       _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status),
-                       _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
-                       nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
+        rowsums = None
+        if rowp is not None and ctx.needs_input_grad[-1]:
+            rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _capi.call("lf_lsq_fwd_rowsums", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.yrow), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                           _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status), _capi.ptr(rowsums),
+                           _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
+                           nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
+        else:
+            # the fixed warp, or a learned warp without a gradient (validation, test scoring): no row sums
+            with torch.cuda.device(dev):
+                _capi.call("lf_lsq_fwd", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab), _capi.ptr(tables.ytab),
+                           _capi.ptr(tables.yrow), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                           _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status),
+                           _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
+                           nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
         if status_out is None:
             # same implicit sync + RuntimeError as torch.inverse in the reference
             # (BP/Networks/LSQ_layer.py:114, caught at BP/main.py:289-292)
             st = int(status.item())
             if st:
                 raise RuntimeError(status_message(st))
-        ctx.save_for_backward(o, beta, zinv)
+        ctx.save_for_backward(o, beta, zinv, rowsums)
         ctx.tables = tables
         ctx.cfg = (order, mask_rows, act)
         if masked is not None:
@@ -118,7 +131,7 @@ class LsqFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gbeta, _gmasked):
-        o, beta, zinv = ctx.saved_tensors
+        o, beta, zinv, rowsums = ctx.saved_tensors
         order, mask_rows, act = ctx.cfg
         t = ctx.tables
         B, L, H, W = o.shape
@@ -129,7 +142,12 @@ class LsqFunction(torch.autograd.Function):
                        _capi.ptr(t.yrow), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
                        _capi.ptr(gbeta), _capi.ptr(d_o), _capi.stream_ptr(),
                        nbytes=2 * B * L * H * W * o.element_size())
-        return d_o, None, None, None, None, None, None, None, None
+        g_rowp = None
+        if rowsums is not None:
+            g_rowp = torch.empty(H, 3, dtype=torch.float64, device=o.device)
+            _capi.call("lf_lsq_grid_grad", _capi.ptr(rowsums), _capi.ptr(t.yrow), _capi.ptr(beta), _capi.ptr(zinv),
+                       _capi.ptr(gbeta), B, L, H, order, mask_rows, _capi.ptr(g_rowp), _capi.stream_ptr())
+        return d_o, None, None, None, None, None, None, None, None, g_rowp
 
 
 def lsq(o, grid, order, const=255.0, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False,
@@ -142,3 +160,13 @@ def lsq(o, grid, order, const=255.0, mask_rows=0, act="none", reg_ls=0.0, use_ch
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
     return LsqFunction.apply(o, tables, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked,
                              status_out)
+
+
+def lsq_warp(o, warp, order, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False, want_masked=False, status_out=None):
+    """``lsq`` on a learned warp's tables (homography.WarpTables): beta has a gradient with respect to ``warp.rowp``
+    as well as ``o``."""
+    if act not in _capi.ACT_IDS:
+        raise NotImplementedError("Activation type: {} is not implemented".format(act))
+    solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
+    return LsqFunction.apply(o, warp, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked, status_out,
+                             warp.rowp)
