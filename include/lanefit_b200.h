@@ -570,6 +570,15 @@ int lf_ce2d_fwd(const float* x, const long long* target, const float* weight, in
                 double* loss, lf_stream_t stream);
 int lf_ce2d_bwd(const float* x, const long long* target, const float* weight, int B, int C, int H, int W, const double* sums,
                 const double* gout, float* dx, lf_stream_t stream);
+/* Confusion counts of a segmentation output (the proxy branch's validation metrics): logits [B][C][H][W] float, target
+ * [B][H][W] int64; for every pixel with 0 <= target < C, counts[target * C + pred] += 1, pred the segmentation branch's
+ * argmax (the first maximum wins; a NaN logit in class c >= 1 never wins; a NaN in class 0 keeps class 0, since no
+ * comparison with it succeeds).  counts [C*C] int64 is zeroed by the caller and accumulated; exact and independent of
+ * the launch order.  status: NULL, or a device int whose nonzero value makes the launch count nothing (the LSQ status
+ * word of a skipped batch).  Capturable, never synchronises.  2 <= C <= 8 and positive sizes, else
+ * LF_ERR_INVALID_ARGUMENT. */
+int lf_seg_confusion(const float* logits, const long long* target, int B, int C, int H, int W, const int* status,
+                     long long* counts, lf_stream_t stream);
 
 /* Loader image path on the GPU (csrc/input_pipe.cu; replaces BP/Dataloader/Load_Data_new.py:127-131,166-167,178-181):
  * frames uint8 [N][Hin][Win][3] (decoded RGB) -> rows [crop_y0, crop_y0+crop_rows) -> PIL-BILINEAR resize to [Ho][Wo]

@@ -85,6 +85,51 @@ class CrossEntropyLoss2d(nn.Module):
         return _CE2dFunction.apply(output, target.long(), None if w is None else w.float().contiguous())
 
 
+def seg_proxy_loss(loss_fit, criterion_seg, output_seg, gt, weight):
+    """The --seg_proxy joint loss: (loss_fit + weight * ce, ce) with ce = criterion_seg(output_seg, gt), the sum formed in
+    float64 in that order, so an eager loop and a graph replay form the same bits.  ``loss_fit`` is the end-to-end loss
+    (with --clas, ``loss * weight_fit + (line + horizon) * weight_class``).  Targets outside [0, L] add to neither the
+    loss nor the weight sum (lf_ce2d); the reference's nn.CrossEntropyLoss would device-assert on them."""
+    ce = criterion_seg(output_seg, gt)
+    return loss_fit.double() + weight * ce.double(), ce
+
+
+def seg_confusion(logits, target, counts, status=None):
+    """counts[t * C + pred] += 1 over the pixels of ``logits`` [B, C, H, W] float32 whose ``target`` [B, H, W] int64 t is
+    in [0, C); pred is the segmentation branch's argmax (the first maximum wins).  ``counts`` [C * C] int64 is
+    accumulated; a nonzero ``status`` (device int32, the LSQ status word) makes the launch count nothing.  One
+    capturable launch of lf_seg_confusion (csrc/seg.cu), no synchronisation."""
+    _capi.require_cuda(logits, target, counts, status)
+    if logits.dtype != torch.float32 or target.dtype != torch.int64 or counts.dtype != torch.int64:
+        raise ValueError("seg_confusion takes float32 logits, int64 target and int64 counts, got %s, %s, %s"
+                         % (logits.dtype, target.dtype, counts.dtype))
+    if target.dim() == 4:                           # the loader hands [B,1,H,W]
+        target = target[:, 0]
+    B, C, H, W = logits.shape
+    if tuple(target.shape) != (B, H, W) or counts.numel() != C * C or not counts.is_contiguous():
+        raise ValueError("seg_confusion: target %s and counts of %d for logits %s" % (tuple(target.shape), counts.numel(),
+                                                                                      tuple(logits.shape)))
+    if status is not None and status.dtype != torch.int32:
+        raise ValueError("seg_confusion: the status word is int32, got %s" % status.dtype)
+    logits, target = logits.contiguous(), target.contiguous()
+    _capi.call("lf_seg_confusion", _capi.ptr(logits), _capi.ptr(target), B, C, H, W, _capi.ptr(status), _capi.ptr(counts),
+               _capi.stream_ptr(), nbytes=4 * logits.numel() + 8 * target.numel())
+    return counts
+
+
+def seg_metrics_from_confusion(counts):
+    """Pixel accuracy, per-class IoU n_cc / (row_c + col_c - n_cc) (NaN where the denominator is 0) and their mean over
+    the classes with a nonzero denominator, from a [C, C] (target, prediction) count matrix on the host."""
+    n = torch.as_tensor(counts, dtype=torch.int64).cpu()
+    diag, rows, cols = n.diagonal(), n.sum(1), n.sum(0)
+    total = int(n.sum())
+    den = rows + cols - diag
+    iou = [float(d) / float(u) if u else float("nan") for d, u in zip(diag.tolist(), den.tolist())]
+    seen = [v for v, u in zip(iou, den.tolist()) if u]
+    return {"pixel_acc": float(diag.sum()) / total if total else float("nan"), "iou": iou,
+            "miou": sum(seen) / len(seen) if seen else float("nan"), "confusion": n.tolist()}
+
+
 def _design(y, order):
     return torch.stack([y ** k for k in range(order, 0, -1)] + [torch.ones_like(y)], 1)
 

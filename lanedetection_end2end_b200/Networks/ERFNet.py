@@ -251,12 +251,15 @@ class Decoder(nn.Module):
 
 class Net(nn.Module):
     """ERFNet.  forward(input, flag, only_encode=False) -> (encoder_output, decoder_output, output_seg)
-    (reference :164-176; the BEV variant returns the first two only, see ERFNet_bev)."""
+    (reference :164-176; the BEV variant returns the first two only, see ERFNet_bev).
+    ``do_segmentation=True`` builds the decoder's second branch (``decoder.layers1``: the decoder's six stages and a
+    16 -> out_channels + 1 head on the shared encoder output), whose logits are then ``output_seg``; without it
+    ``output_seg`` is the encoder output, as in the reference, which never passes the flag."""
 
-    def __init__(self, layers=18, in_channels=1, out_channels=1, pretrained=False, pool=False):
+    def __init__(self, layers=18, in_channels=1, out_channels=1, pretrained=False, pool=False, do_segmentation=False):
         super().__init__()
         self.encoder = Encoder(in_channels, out_channels)
-        self.decoder = Decoder(out_channels, pretrained)
+        self.decoder = Decoder(out_channels, pretrained, do_segmentation=do_segmentation)
 
     def forward(self, input, flag, only_encode=False):
         global _PENDING_COUNTERS

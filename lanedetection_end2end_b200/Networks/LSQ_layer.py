@@ -188,9 +188,21 @@ class Net(nn.Module):
         M, _ = get_homography(resize, args.no_mapping)
         M = torch.from_numpy(M).unsqueeze_(0).expand([args.batch_size, 3, 3]).float()
 
+        # --seg_proxy: the decoder's second branch (net.decoder.layers1, the reference's dormant `do_segmentation`
+        # decoder) on the shared encoder, trained with a cross-entropy proxy term next to the fit (engine.train_epoch);
+        # its logits [B, L + 1, H, W] are output_seg.  A checkpoint without the branch loads with strict=False, the
+        # branch then keeps its define_init_weights start.
+        self.seg_proxy = bool(getattr(args, "seg_proxy", False))
+        if self.seg_proxy and not args.end_to_end:
+            raise ValueError("--seg_proxy needs --end_to_end True: the segmentation branch already trains the decoder "
+                             "output with cross-entropy")
+        if self.seg_proxy and args.pretrained:
+            raise ValueError("--seg_proxy cannot be combined with --pretrained: its phases change the trained parameter "
+                             "sets")
         out_channels = args.nclasses + int(not args.end_to_end)
+        kw = {"do_segmentation": True} if self.seg_proxy else {}
         self.net = define_model(mod=args.mod, layers=args.layers, in_channels=args.channels_in,
-                                out_channels=out_channels, pretrained=args.pretrained, pool=args.pool)
+                                out_channels=out_channels, pretrained=args.pretrained, pool=args.pool, **kw)
         self.activation = activation_layer(args.activation_layer, args.no_cuda)
         self.grid = ProjectiveGridGenerator(size, M, args.no_cuda)
         self.ls_layer = Weighted_least_squares(size, args.nclasses, args.order, args.no_cuda,

@@ -87,6 +87,8 @@ _FLAGS = [
     ("--end_to_end", _B(True)),
     ("--no_mapping", _B(False)),
     ("--learn_homography", _B(False)),
+    ("--seg_proxy", _B(False)),
+    ("--weight_seg_proxy", dict(type=float, default=1.0)),
     ("--gamma", dict(type=float, default=0.0)),
     ("--clas", _B(False)),
     ("--cudnn", _B(True)),

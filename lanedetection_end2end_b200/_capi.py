@@ -247,6 +247,7 @@ _NET_PROTOS = {
     "lf_ce2d_blocks": (_i, [_i, _i, _i]),
     "lf_ce2d_fwd": (_i, [_p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p]),
     "lf_ce2d_bwd": (_i, [_p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "lf_seg_confusion": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p]),
     "lf_frame_preprocess": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p]),
     "lf_linear_chunks": (_i, [_i]),
     "lf_rowmean_fwd": (_i, [_p, _i, _i, _i, _i, _p, _p]),

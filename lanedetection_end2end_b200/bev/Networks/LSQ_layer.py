@@ -73,6 +73,8 @@ class Net(nn.Module):
     def __init__(self, args):
         super().__init__()
         from . import define_model
+        if getattr(args, "seg_proxy", False):
+            raise ValueError("--seg_proxy is not supported by the bird's-eye-view Net: its ERFNet has no second decoder")
         resize = args.resize
         size, M, _ = Init_Projective_transform(args.nclasses, args.batch_size, args.resize)
         self.M = M

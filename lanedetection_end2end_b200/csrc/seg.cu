@@ -132,6 +132,38 @@ __global__ void ce2d_finalize_kernel(const double* __restrict__ partial, int nbl
     }
 }
 
+// Confusion counts of the proxy segmentation branch (validation metrics): counts[t * C + pred] += 1 for every pixel whose
+// target t is in [0, C); pred is seg_argmax's winner.  Each CTA counts into a shared-memory histogram (lanes of a warp
+// that hit the same bin add once, through their leader), then adds each nonzero bin to `counts` with one 64-bit integer
+// atomic: the result is exact and independent of the order.  A nonzero *status (the LSQ status word of the batch)
+// makes the launch count nothing.  The loop's trip count is uniform over the CTA, so every lane reaches __match_any_sync.
+__global__ void __launch_bounds__(SEG_THREADS) seg_confusion_kernel(const float* __restrict__ x, const long long* __restrict__ target,
+                                                                    int B, int C, long long HW, const int* __restrict__ status,
+                                                                    unsigned long long* __restrict__ counts) {
+    pdl_entry();
+    if (status && *status) return;
+    __shared__ unsigned long long hist[SEG_MAXC * SEG_MAXC];
+    for (int k = threadIdx.x; k < C * C; k += blockDim.x) hist[k] = 0ull;
+    __syncthreads();
+    const long long total = (long long)B * HW;
+    for (long long base = (long long)blockIdx.x * blockDim.x; base < total; base += (long long)gridDim.x * blockDim.x) {
+        const long long i = base + threadIdx.x;
+        int bin = -1;
+        if (i < total) {
+            const long long t = target[i];
+            if (t >= 0 && t < C) {
+                const long long b = i / HW, p = i - b * HW;
+                bin = (int)t * C + seg_argmax(x + (size_t)b * C * HW + p, C, HW);
+            }
+        }
+        const unsigned same = __match_any_sync(0xffffffffu, bin);
+        if (bin >= 0 && (threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&hist[bin], (unsigned long long)__popc(same));
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < C * C; k += blockDim.x)
+        if (hist[k]) atomicAdd(counts + k, hist[k]);
+}
+
 static int seg_blocks(long long total) {
     const long long b = (total + SEG_THREADS - 1) / SEG_THREADS;
     const long long cap = (long long)device_sms() * 8;
@@ -177,5 +209,16 @@ extern "C" int lf_ce2d_bwd(const float* x, const long long* target, const float*
     LF_REQUIRE(x && target && sums && dx && B >= 1 && C >= 1 && C <= SEG_MAXC && H >= 1 && W >= 1);
     const long long HW = (long long)H * W;
     lf_launch(ce2d_kernel<true>, seg_blocks(B * HW), SEG_THREADS, 0, stream, x, target, weight, B, C, HW, (double*)nullptr, sums, gout, dx);
+    return check_launch();
+}
+
+// counts [C*C] int64, zeroed by the caller and accumulated over launches; status NULL or the batch's status word
+extern "C" int lf_seg_confusion(const float* logits, const long long* target, int B, int C, int H, int W, const int* status,
+                                long long* counts, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(logits && target && counts && B >= 1 && C >= 2 && C <= SEG_MAXC && H >= 1 && W >= 1);
+    const long long HW = (long long)H * W;
+    lf_launch(seg_confusion_kernel, seg_blocks(B * HW), SEG_THREADS, 0, stream, logits, target, B, C, HW, status,
+              reinterpret_cast<unsigned long long*>(counts));
     return check_launch();
 }

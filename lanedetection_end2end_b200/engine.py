@@ -317,7 +317,8 @@ def _keeping_batchnorm_stats(model, build):
     return out
 
 
-def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch):
+def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch,
+                seg_metrics=None):
     """One training epoch of the reference's main.py loop (BP/main.py:225-359), each batch one replay of a
     GraphedTrainStep that holds the forward, the loss, the backward, the fused optimizer's update and the meter updates.
     Returns (losses.avg, rmse_metric.avg) -- rmse_metric is updated with --end_to_end False only, as in the reference.
@@ -348,9 +349,14 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     save_freq is not drawn.  Every other epoch follows ``args.end_to_end``, which the caller's get_flags(epoch) sets:
     the segmentation branch through output_conv2, or end to end through output_conv and the heads, whose optimizer
     state starts at step 1 while output_conv2 keeps its state.  --clas with --end_to_end False raises ValueError outside
-    the skip epochs (main.py:320-325 would call the line criterion on None)."""
+    the skip epochs (main.py:320-325 would call the line criterion on None).
+
+    A model built with --seg_proxy (``model.seg_proxy``) trains its second decoder in the same step: the loss is
+    Loss_crit.seg_proxy_loss, ``L_fit + weight_seg_proxy * criterion_seg(output_seg, gt)`` in float64, L_fit the loss
+    above; losses.avg is that total.  The proxy term has a device meter of its own; pass a dict as ``seg_metrics`` to
+    receive its average under "ce"."""
     from .optim import FusedOptimizer
-    from .Loss_crit import fused_backprojection_loss
+    from .Loss_crit import fused_backprojection_loss, seg_proxy_loss
     from .Networks import utils as nutils
     if not isinstance(optimizer, FusedOptimizer):
         raise TypeError("train_epoch runs the update in the graph: it needs an optim.FusedOptimizer "
@@ -371,7 +377,8 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
         criterion.bind(model)
     dev = next(model.parameters()).device
     model.train()
-    meters = DeviceMeters(("loss", "rmse"), dev)
+    proxy = bool(getattr(model, "seg_proxy", False))
+    meters = DeviceMeters(("loss", "rmse") + (("seg_proxy",) if proxy else ()), dev)
     status = BatchStatus(len(loader), dev)
     static = {}
 
@@ -386,6 +393,8 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
             loss_horizon = criterion_horizon(out[7], static["gt_horizon"]).double()
             loss_line = criterion_line_class(out[6], static["gt_line"]).double()
             loss = loss * args.weight_fit + (loss_line + loss_horizon) * args.weight_class
+        if proxy:
+            loss, static["seg_proxy"] = seg_proxy_loss(loss, criterion_seg, out[8], static["gt"], args.weight_seg_proxy)
         return loss
 
     def post(out, loss):
@@ -396,6 +405,8 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
         if not e2e:
             meters.update("rmse", static["rmse"], ok, n)
         meters.update("loss", loss, ok, n)
+        if proxy:
+            meters.update("seg_proxy", static["seg_proxy"], ok, n)
         status.record(model.lsq_status)
         return out[4]
 
@@ -450,6 +461,8 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
         return 0, 0
     m = meters.read()
     status.print_skipped(labels)
+    if proxy and seg_metrics is not None:
+        seg_metrics["ce"] = m["seg_proxy"][1]
     return m["loss"][1], m["rmse"][1]
 
 

@@ -26,10 +26,10 @@ import torch
 
 if __package__:
     from . import _capi
-    from .Loss_crit import backprojection_loss
+    from .Loss_crit import backprojection_loss, seg_confusion, seg_metrics_from_confusion
 else:                                   # imported top-level next to the reference's main.py / test.py
     import _capi
-    from Loss_crit import backprojection_loss
+    from Loss_crit import backprojection_loss, seg_confusion, seg_metrics_from_confusion
 
 TUSIMPLE_SAMPLES = 56                   # h_samples 160..710 step 10: what Projections predicts
 TUSIMPLE_LANES = 4                      # predicted lanes of the 4-lane --clas model
@@ -312,7 +312,8 @@ def test_model(loader, model, criterion, criterion_seg, criterion_line_class, cr
     return acc_seg[0]
 
 
-def validate(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0):
+def validate(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0,
+             seg_metrics=None):
     """The reference's validation pass (BP/main.py:419-526), same return value: (losses.avg, acc_hor_tot.avg,
     acc_line_tot.avg, rmse_metric_valid.avg).  ``args`` is main.py's global args, passed in.
 
@@ -325,7 +326,13 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
     pass.  A batch shorter than the first (a loader that keeps its last batch) is replayed by a second graph of its size,
     so its losses are the ones main.py computes on it.  The host synchronises only at the print_freq lines, at
     save_weightmap('valid', ...) every 25 batches (called with the static outputs) and at the end.  The --clas BCE losses
-    main.py adds after losses.update change nothing it returns and are not computed."""
+    main.py adds after losses.update change nothing it returns and are not computed.
+
+    A model built with --seg_proxy (``model.seg_proxy``) also scores its proxy segmentation branch in each replay, guarded
+    like the meters: criterion_seg(output_seg, gt) into a device meter and Loss_crit.seg_confusion into the pass's
+    [L+1, L+1] (target, prediction) count matrix.  At the end of the pass one more line is printed (proxy cross-entropy,
+    pixel accuracy, per-class IoU and mIoU over the classes with a nonzero denominator) and a dict passed as
+    ``seg_metrics`` receives "ce", "pixel_acc", "iou", "miou" and "confusion".  The returned tuple is unchanged."""
     if __package__:
         from .engine import GraphedInference, DeviceMeters, BatchStatus, lane_losses, _reporting
         from .Networks import utils as nutils
@@ -341,9 +348,11 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
     if getattr(criterion, "learn_homography", False):
         criterion.bind(model)
     dev = next(model.parameters()).device
-    meters = DeviceMeters(("loss", "acc_hor", "acc_line", "rmse"), dev)
+    proxy = bool(getattr(model, "seg_proxy", False))
+    meters = DeviceMeters(("loss", "acc_hor", "acc_line", "rmse") + (("seg_proxy",) if proxy else ()), dev)
     status = BatchStatus(len(loader), dev)
     graphs = {}                     # rows -> (GraphedInference, static batch tensors)
+    counts = torch.zeros((L + 1) ** 2, dtype=torch.int64, device=dev) if proxy else None
 
     def build(batch):
         st = {k: v.to(dev, non_blocking=True).clone() for k, v in batch.items()}
@@ -357,12 +366,17 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
             else:
                 loss = criterion_seg(out[5], st["gt"])
                 loss_metric, x_cal = lane_losses(criterion, out, lanes, vp, L)
+            if proxy:
+                ce = criterion_seg(out[8], st["gt"])
             if not torch.cuda.is_current_stream_capturing():
                 return x_cal                 # warm-up passes: no meter or log entry
             ok = model.lsq_status.reshape(()).eq(0)
             if not e2e:
                 meters.update("rmse", loss_metric, ok, n)
             meters.update("loss", loss, ok, n)
+            if proxy:
+                meters.update("seg_proxy", ce, ok, n)
+                seg_confusion(out[8], st["gt"], counts, model.lsq_status)
             if args.clas:
                 horizon_pred = torch.round(torch.nn.Sigmoid()(out[7]))
                 acc = torch.eq(horizon_pred, st["gt_horizon"])
@@ -420,6 +434,13 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
         model.defer_status_check = deferred
     m = meters.read()
     status.print_skipped(labels)
+    if proxy:
+        seg = seg_metrics_from_confusion(counts.view(L + 1, L + 1))
+        seg["ce"] = m["seg_proxy"][1]
+        print("===> Proxy segmentation on validation set: ENTROPY {:.8}  pixel acc {:.8}  IoU [{}]  mIoU {:.8}".format(
+            seg["ce"], seg["pixel_acc"], ", ".join("{:.6}".format(v) for v in seg["iou"]), seg["miou"]))
+        if seg_metrics is not None:
+            seg_metrics.update(seg)
     if args.evaluate:
         crit_string = "TOT LOSS" if args.clas else ("MSE" if args.loss_policy == "backproject" and e2e else
                                                     "AREA**2" if args.loss_policy == "area" and e2e else "ENTROPY")
