@@ -11,8 +11,9 @@
 // __host__ __device__: `lf_backproj_loss_host` runs the same code on the CPU so the CPU test suite can pin the math
 // against the oracle (a test hook -- nothing in the product calls it).
 //
-// STATUS: validated on CPU only (round 1 ran out of GPU budget); the module path keeps the torch implementation
-// unless LANEFIT_FUSED_LOSS=1.
+// This is the training loss of every back-projection step (Loss_crit.fused_backprojection_loss, which
+// engine.GraphedTrainStep and engine.train_epoch call); tests/test_net_gpu.py checks it on the GPU against the
+// per-lane calls of Loss_crit.backprojection_loss.
 #include "lf_common.cuh"
 
 namespace lf {

@@ -10,15 +10,9 @@ the LSQ status word are static outputs the caller reads when it wants to (no syn
 The graph only contains our C-ABI kernels, a handful of tiny float64 torch ops of the loss, torch's
 graph-safe Philox draws for the Dropout2d masks, and (optionally) the NCCL all-reduce.
 """
-import os
 import time
 
 import torch
-
-# lf_backproj_loss: one launch for the loss of all lanes + its gradient instead of ~40 tiny float64 torch launches.
-# GPU-validated (tests/test_net_gpu.py::test_fused_backprojection_loss_kernel): on by default;
-# LANEFIT_FUSED_LOSS=0 falls back to the torch ops of Loss_crit.backprojection_loss.forward_lanes.
-FUSED_LOSS = os.environ.get("LANEFIT_FUSED_LOSS", "1") != "0"
 
 
 def model_forward(model, x, gt_line, end_to_end):
@@ -46,9 +40,10 @@ class GraphedTrainStep:
     hyperparameters first if a param_groups value changed (schedulers work without a recapture).
 
     ``gt_line``: optional example [B, 4] tensor, cloned into a static buffer ``self.gt_line`` that the forward reads (the
-    segmentation branch's substitution, end_to_end=False); default a host tensor of zeros.  ``loss_fn``: optional
-    callable(forward 9-tuple) -> scalar loss that replaces the lane criterion and ``extra_loss``.  ``post``: optional
-    callable(forward 9-tuple, detached loss) run at the end of every step, after the update (its return value is
+    segmentation branch's substitution, end_to_end=False); default a host tensor of zeros.  The loss is
+    Loss_crit.fused_backprojection_loss of ``criterion`` (a Loss_crit.backprojection_loss) over the ``nclasses`` lanes,
+    plus ``extra_loss``; ``loss_fn``: optional callable(forward 9-tuple) -> scalar loss that replaces both.  ``post``:
+    optional callable(forward 9-tuple, detached loss) run at the end of every step, after the update (its return value is
     ``self.post_out``); the warm-up steps run it too.
 
     ``early_return=True``: the forward is ``model(x, gt_line, end_to_end, early_return=True)``, the decoder output alone
@@ -125,19 +120,11 @@ class GraphedTrainStep:
             scale = lane_valid_scale(self.valid, self.L)
         if self.loss_fn is not None:
             loss = self.loss_fn(out)
-        elif FUSED_LOSS and hasattr(self.crit, "_fused_host_constants"):
+        else:
             from .Loss_crit import fused_backprojection_loss
             loss, _ = fused_backprojection_loss(self.crit, out[:self.L], self.xgt, self.valid, lane_scale=scale)
-        elif hasattr(self.crit, "forward_lanes"):
-            loss, _ = self.crit.forward_lanes(out[:self.L], self.xgt, self.valid, lane_scale=scale)    # all lanes in one pass
-        else:
-            loss = 0
-            for l in range(self.L):
-                ll, _ = self.crit(out[l], self.xgt[:, l], self.valid[:, l])
-                loss = loss + ll
-            loss = loss / self.L
-        if self.extra_loss is not None and self.loss_fn is None:
-            loss = loss + self.extra_loss(out)
+            if self.extra_loss is not None:
+                loss = loss + self.extra_loss(out)
         loss.backward()
         if self.reducer is not None:
             self.reducer()
@@ -317,6 +304,150 @@ def _keeping_batchnorm_stats(model, build):
     return out
 
 
+def _device_copies(tensors, casts, dev):
+    """Static device buffers for a batch: clones of ``tensors`` (name -> tensor), then ``casts`` (name -> dtype)."""
+    st = {k: v.to(dev, non_blocking=True).clone() for k, v in tensors.items()}
+    st.update({k: st[k].to(dtype) for k, dtype in casts.items()})
+    return st
+
+
+def _train_replays(loader, model, optimizer, static, fields, casts, post, report=None, print_freq=0, save_freq=0,
+                   gt_line=False, early_return=False, **step_kw):
+    """The loop of the graphed training epochs: each batch one replay of a GraphedTrainStep over the FusedOptimizer
+    ``optimizer``.  Returns the step, None when the loader yields no batch.
+
+    ``fields(batch)`` names the loader tuple's tensors that become static device buffers: ``static`` receives the first
+    batch's copies (_device_copies with ``casts``), later batches are copied into them, and every batch must have the
+    first one's size.  ``static["input"]`` (with ``gt_line=True`` also ``static["gt_line"]``, which the forward then
+    reads) is the step's own buffer.  ``step_kw`` (loss_fn, end_to_end) and ``early_return`` go to the GraphedTrainStep;
+    the loss reads its batch through loss_fn.  ``post(out, loss)`` runs in the captured step only, not in the warm-up
+    steps; after it the step's LSQ status word is logged (not with ``early_return``, which has no least-squares layer),
+    and the reference's line for each skipped batch is printed at the end.  ``report(i, printing, saving, batch,
+    post_out, (batch time, its average))`` runs at the print_freq / save_freq points of a batch that was not skipped:
+    the only host synchronisations before the end."""
+    dev = next(model.parameters()).device
+    model.train()
+    status = None if early_return else BatchStatus(len(loader), dev)
+
+    def captured_post(out, loss):
+        if not torch.cuda.is_current_stream_capturing():
+            return None                      # warm-up steps: no meter or log entry
+        ret = post(out, loss)
+        if status is not None:
+            status.record(model.lsq_status)
+        return ret
+
+    step, labels = None, []
+    bt_sum, bt_n, end = 0.0, 0, time.time()
+    deferred = model.defer_status_check
+    try:
+        for i, batch in enumerate(loader):
+            tensors = fields(batch)
+            if step is None:
+                static.update(_device_copies(tensors, casts, dev))
+                none = torch.empty(0, device=dev)
+                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
+                    model, None, 0, static["input"], none, none, optimizer=optimizer,
+                    gt_line=static["gt_line"] if gt_line else None, post=captured_post, early_return=early_return,
+                    **step_kw))
+                static["input"] = step.x              # the step's own copies are what its forward reads
+                if gt_line:
+                    static["gt_line"] = step.gt_line
+            else:
+                if batch[0].shape[0] != step.x.shape[0]:
+                    raise ValueError("batch of %d images after a first batch of %d: a training epoch replays one batch "
+                                     "size" % (batch[0].shape[0], step.x.shape[0]))
+                for k, v in tensors.items():
+                    static[k].copy_(v, non_blocking=True)
+            if status is not None:
+                status.check(i)
+            labels.append(batch[3])
+            step()
+            now = time.time()
+            bt_val, end = now - end, now
+            bt_sum, bt_n = bt_sum + bt_val, bt_n + 1
+            printing, saving = _reporting(i, print_freq), _reporting(i, save_freq)
+            # a skipped batch reports nothing, as main.py's `continue`
+            if (printing or saving) and not int(status.log[i]):
+                report(i, printing, saving, batch, step.post_out, (bt_val, bt_sum / bt_n))
+    finally:
+        model.defer_status_check = deferred
+    if status is not None:
+        status.print_skipped(labels)
+    return step
+
+
+def _valid_replays(loader, model, fields, casts, post, report, print_freq, gt_line=False, end_to_end=True):
+    """The loop of the graphed validation passes: each batch one replay of a GraphedInference, with one graph and one
+    set of static buffers per batch size (a batch shorter than the first gets its own; a larger one raises ValueError).
+
+    ``fields`` and ``casts`` as in _train_replays, per graph; with ``gt_line=True`` the forward reads the graph's
+    ``st["gt_line"]``.  ``post(out, st)`` is the graph's post on its static batch ``st``; after it the captured pass
+    logs and zeroes the LSQ status word, and the reference's line for each skipped batch is printed at the end.
+    ``report(i, printing, saving, batch, graph, st)`` runs at the print_freq / 25 points of a batch that was not
+    skipped: the only host synchronisations before the end."""
+    dev = next(model.parameters()).device
+    status = BatchStatus(len(loader), dev)
+    graphs = {}                     # rows -> (GraphedInference, static batch tensors)
+
+    def build(tensors):
+        st = _device_copies(tensors, casts, dev)
+
+        def captured_post(out):
+            ret = post(out, st)
+            if torch.cuda.is_current_stream_capturing():
+                status.record(model.lsq_status)
+                model.lsq_status.zero_()
+            return ret
+
+        g = GraphedInference(model, st["input"], post=captured_post, gt_line=st["gt_line"] if gt_line else None,
+                             end_to_end=end_to_end)
+        st["input"] = g.x
+        if gt_line:
+            st["gt_line"] = g.gt_line        # the forward's substitution and the accuracies read one buffer
+        model.lsq_status.zero_()
+        return g, st
+
+    first, labels = None, []
+    deferred = model.defer_status_check
+    try:
+        with torch.no_grad():
+            for i, batch in enumerate(loader):
+                tensors, n = fields(batch), batch[0].shape[0]
+                status.check(i)
+                if first is None:
+                    first = n
+                elif n > first:
+                    raise ValueError("batch of %d images after a first batch of %d" % (n, first))
+                if n in graphs:
+                    g, st = graphs[n]
+                    for k, v in tensors.items():
+                        st[k].copy_(v, non_blocking=True)
+                else:
+                    g, st = graphs[n] = build(tensors)
+                labels.append(batch[3])
+                g.graph.replay()
+                printing, saving = _reporting(i, print_freq), _reporting(i, 25)
+                # a skipped batch reports nothing, as main.py's `continue`
+                if (printing or saving) and not int(status.log[i]):
+                    report(i, printing, saving, batch, g, st)
+    finally:
+        model.defer_status_check = deferred
+    status.print_skipped(labels)
+
+
+def check_bp_args(args, criterion, model):
+    """The settings train_epoch and inference.validate run: ValueError naming the first one they do not.  A criterion
+    built with --learn_homography is bound to ``model``'s learned warp."""
+    if args.clas and not args.end_to_end:
+        raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
+    if not args.end_to_end and args.nclasses != 4:
+        raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
+                         "loader's 4 line flags over %d lane maps" % args.nclasses)
+    if getattr(criterion, "learn_homography", False):
+        criterion.bind(model)
+
+
 def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch,
                 seg_metrics=None):
     """One training epoch of the reference's main.py loop (BP/main.py:225-359), each batch one replay of a
@@ -366,20 +497,11 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
                          "the switch to end-to-end change the parameter set.  Build the optimizer with "
                          "define_optim(..., fused=True, per_param_step=True)")
     if args.pretrained and epoch < args.pretrain_epochs and epoch < args.skip_epochs:
-        return _train_skip_epoch(loader, model, optimizer, criterion_seg, args)
-    if args.clas and not args.end_to_end:
-        raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
+        return _train_skip_epoch(loader, model, optimizer, criterion_seg)
+    check_bp_args(args, criterion, model)
     e2e, L = bool(args.end_to_end), args.nclasses
-    if not e2e and L != 4:
-        raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
-                         "loader's 4 line flags over %d lane maps" % L)
-    if getattr(criterion, "learn_homography", False):
-        criterion.bind(model)
-    dev = next(model.parameters()).device
-    model.train()
     proxy = bool(getattr(model, "seg_proxy", False))
-    meters = DeviceMeters(("loss", "rmse") + (("seg_proxy",) if proxy else ()), dev)
-    status = BatchStatus(len(loader), dev)
+    meters = DeviceMeters(("loss", "rmse") + (("seg_proxy",) if proxy else ()), next(model.parameters()).device)
     static = {}
 
     def loss_fn(out):
@@ -398,8 +520,6 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
         return loss
 
     def post(out, loss):
-        if not torch.cuda.is_current_stream_capturing():
-            return None                      # warm-up steps: no meter or log entry
         ok = model.lsq_status.reshape(()).eq(0)
         n = static["input"].shape[0]
         if not e2e:
@@ -407,102 +527,48 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
         meters.update("loss", loss, ok, n)
         if proxy:
             meters.update("seg_proxy", static["seg_proxy"], ok, n)
-        status.record(model.lsq_status)
         return out[4]
 
-    step, labels = None, []
-    bt_sum, bt_n, end = 0.0, 0, time.time()
-    deferred = model.defer_status_check
-    try:
-        for i, (input, gt, lanes, idx, gt_line, gt_horizon, valid_points) in enumerate(loader):
-            batch = {"input": input, "gt": gt.squeeze(1), "lanes": lanes, "gt_line": gt_line, "gt_horizon": gt_horizon,
-                     "valid": valid_points}
-            if step is None:
-                for k, v in batch.items():
-                    static[k] = v.to(dev, non_blocking=True).clone()
-                static["input"] = static["input"].float()
-                static["gt"] = static["gt"].long()
-                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
-                    model, criterion, L, static["input"], static["lanes"], static["valid"], optimizer=optimizer,
-                    gt_line=None if e2e else static["gt_line"], end_to_end=e2e, loss_fn=loss_fn, post=post))
-                static["input"] = step.x              # the step's own copies are what its forward reads
-                if not e2e:
-                    static["gt_line"] = step.gt_line
-            else:
-                if input.shape[0] != step.x.shape[0]:
-                    raise ValueError("batch of %d images after a first batch of %d: train_epoch replays one batch size"
-                                     % (input.shape[0], step.x.shape[0]))
-                for k, v in batch.items():
-                    static[k].copy_(v, non_blocking=True)
-            status.check(i)
-            labels.append(idx)
-            step()
-            now = time.time()
-            bt_val, end = now - end, now
-            bt_sum, bt_n = bt_sum + bt_val, bt_n + 1
-            if not (_reporting(i, args.print_freq) or _reporting(i, args.save_freq)) or int(status.log[i]):
-                continue                             # a skipped batch reports nothing, as main.py's `continue`
+    def report(i, printing, saving, batch, masked, bt):
+        if printing:
             m = meters.read()
-            if _reporting(i, args.print_freq):
-                print('Epoch: [{0}][{1}/{2}]\t'
-                      'Time {3:.3f} ({4:.3f})\t'
-                      'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
-                      'rmse_metric {rmse[0]:.8f} ({rmse[1]:.8f})'.format(
-                          epoch + 1, i + 1, len(loader), bt_val, bt_sum / bt_n, loss=m["loss"], rmse=m["rmse"]))
-            if _reporting(i, args.save_freq):
-                lanes = static["lanes"]
-                nutils.save_weightmap('train', step.post_out, *static["x_cal"],
-                                      lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :], lanes[:, 3, :], static["gt"], 0, i,
-                                      static["input"], args.no_ortho, args.resize, args.save_path, args.nclasses,
-                                      args.no_mapping)
-    finally:
-        model.defer_status_check = deferred
-    if step is None:
+            print('Epoch: [{0}][{1}/{2}]\t'
+                  'Time {3:.3f} ({4:.3f})\t'
+                  'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                  'rmse_metric {rmse[0]:.8f} ({rmse[1]:.8f})'.format(
+                      epoch + 1, i + 1, len(loader), bt[0], bt[1], loss=m["loss"], rmse=m["rmse"]))
+        if saving:
+            lanes = static["lanes"]
+            nutils.save_weightmap('train', masked, *static["x_cal"], lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :],
+                                  lanes[:, 3, :], static["gt"], 0, i, static["input"], args.no_ortho, args.resize,
+                                  args.save_path, args.nclasses, args.no_mapping)
+
+    fields = lambda b: {"input": b[0], "gt": b[1].squeeze(1), "lanes": b[2], "gt_line": b[4], "gt_horizon": b[5],
+                        "valid": b[6]}
+    casts = {"input": torch.float32, "gt": torch.int64}
+    if _train_replays(loader, model, optimizer, static, fields, casts, post, report, args.print_freq, args.save_freq,
+                      gt_line=not e2e, loss_fn=loss_fn, end_to_end=e2e) is None:
         return 0, 0
     m = meters.read()
-    status.print_skipped(labels)
     if proxy and seg_metrics is not None:
         seg_metrics["ce"] = m["seg_proxy"][1]
     return m["loss"][1], m["rmse"][1]
 
 
-def _train_skip_epoch(loader, model, optimizer, criterion_seg, args):
+def _train_skip_epoch(loader, model, optimizer, criterion_seg):
     """A skip epoch of --pretrained (BP/main.py:255-282) as graph replays: the decoder output through output_conv2, the
     segmentation loss and the unguarded update; returns (losses_skip.avg, 0.0)."""
     dev = next(model.parameters()).device
-    model.train()
     meters = DeviceMeters(("loss_skip",), dev)
     always = torch.ones((), dtype=torch.bool, device=dev)
     static = {}
 
     def post(out, loss):
-        if torch.cuda.is_current_stream_capturing():          # warm-up steps: no meter entry
-            meters.update("loss_skip", loss, always, static["input"].shape[0])
-        return None
+        meters.update("loss_skip", loss, always, static["input"].shape[0])
 
-    step = None
-    deferred = model.defer_status_check
-    try:
-        for i, (input, gt, lanes, idx, gt_line, gt_horizon, valid_points) in enumerate(loader):
-            if step is None:
-                static["input"] = input.to(dev, non_blocking=True).float()
-                static["gt"] = gt.squeeze(1).to(dev, non_blocking=True).long().clone()
-                none = torch.empty(0, device=dev)     # the loss reads gt through loss_fn: no lane-sample inputs
-                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
-                    model, None, args.nclasses, static["input"], none, none, optimizer=optimizer,
-                    end_to_end=False, loss_fn=lambda out: criterion_seg(out, static["gt"]), post=post,
-                    early_return=True))
-                static["input"] = step.x              # the step's own copy is what its forward reads
-            else:
-                if input.shape[0] != step.x.shape[0]:
-                    raise ValueError("batch of %d images after a first batch of %d: train_epoch replays one batch size"
-                                     % (input.shape[0], step.x.shape[0]))
-                static["input"].copy_(input, non_blocking=True)
-                static["gt"].copy_(gt.squeeze(1), non_blocking=True)
-            step()
-    finally:
-        model.defer_status_check = deferred
-    if step is None:
+    if _train_replays(loader, model, optimizer, static, lambda b: {"input": b[0], "gt": b[1].squeeze(1)},
+                      {"input": torch.float32, "gt": torch.int64}, post, early_return=True, end_to_end=False,
+                      loss_fn=lambda out: criterion_seg(out, static["gt"])) is None:
         return 0, 0
     return meters.read()["loss_skip"][1], 0.0
 
@@ -554,10 +620,7 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
                         "(define_optim(..., fused=True)), got %s" % type(optimizer).__name__)
     check_bev_args(args)
     e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
-    dev = next(model.parameters()).device
-    model.train()
-    meters = DeviceMeters(("loss", "area", "exact"), dev)
-    status = BatchStatus(len(loader), dev)
+    meters = DeviceMeters(("loss", "area", "exact"), next(model.parameters()).device)
     static = {}
 
     def loss_fn(out):
@@ -569,65 +632,31 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
         return criterion_seg(out[6], static["gt"])
 
     def post(out, loss):
-        if not torch.cuda.is_current_stream_capturing():
-            return None                      # warm-up steps: no meter or log entry
         ok = model.lsq_status.reshape(()).eq(0)
         n = static["input"].shape[0]
         if not e2e:
             meters.update("area", static["area"], ok, n)
         meters.update("loss", loss, ok, n)
         meters.update("exact", static["exact"], ok, n)
-        status.record(model.lsq_status)
         return out
 
-    step, labels, M_inv = None, [], None
-    bt_sum, bt_n, end = 0.0, 0, time.time()
-    deferred = model.defer_status_check
-    try:
-        for i, (input, gt, params, idx, gt_line, gt_horizon) in enumerate(loader):
-            batch = {"input": input, "gt": gt, "params": params}
-            if step is None:
-                for k, v in batch.items():
-                    static[k] = v.to(dev, non_blocking=True).clone()
-                static["input"] = static["input"].float()
-                # the BEV loss reads its batch through loss_fn: the step's lane-sample inputs stay empty
-                none = torch.empty(0, device=dev)
-                step = _keeping_batchnorm_stats(model, lambda: GraphedTrainStep(
-                    model, criterion, L, static["input"], none, none, optimizer=optimizer, end_to_end=e2e,
-                    loss_fn=loss_fn, post=post))
-                static["input"] = step.x              # the step's own copy is what its forward reads
-            else:
-                if input.shape[0] != step.x.shape[0]:
-                    raise ValueError("batch of %d images after a first batch of %d: train_epoch_bev replays one batch "
-                                     "size" % (input.shape[0], step.x.shape[0]))
-                for k, v in batch.items():
-                    static[k].copy_(v, non_blocking=True)
-            status.check(i)
-            labels.append(idx)
-            step()
-            now = time.time()
-            bt_val, end = now - end, now
-            bt_sum, bt_n = bt_sum + bt_val, bt_n + 1
-            if not (_reporting(i, args.print_freq) or _reporting(i, args.save_freq)) or int(status.log[i]):
-                continue                             # a skipped batch reports nothing, as main.py's `continue`
-            if _reporting(i, args.print_freq):
-                m = meters.read()
-                print('Epoch: [{0}][{1}/{2}]\t'
-                      'Time {3:.3f} ({4:.3f})\t'
-                      'Loss {loss[0]:.8f} ({loss[1]:.8f})'.format(
-                          epoch + 1, i + 1, len(loader), bt_val, bt_sum / bt_n, loss=m["loss"]))
-            if _reporting(i, args.save_freq):
-                if M_inv is None:
-                    from .Dataloader.Load_Data_new import get_homography
-                    M_inv = get_homography(args.resize)
-                out, p = step.post_out, static["params"]
-                nutils.save_weightmap('train', out[5], M_inv, out[4], *out[:4], p[:, 0, :], p[:, 1, :], p[:, 2, :],
-                                      p[:, 3, :], gt_line, static["gt"], 0, i, static["input"], args.no_ortho, args.resize,
-                                      args.save_path)
-    finally:
-        model.defer_status_check = deferred
-    if step is None:
+    def report(i, printing, saving, batch, out, bt):
+        if printing:
+            m = meters.read()
+            print('Epoch: [{0}][{1}/{2}]\t'
+                  'Time {3:.3f} ({4:.3f})\t'
+                  'Loss {loss[0]:.8f} ({loss[1]:.8f})'.format(
+                      epoch + 1, i + 1, len(loader), bt[0], bt[1], loss=m["loss"]))
+        if saving:
+            from .Dataloader.Load_Data_new import get_homography
+            p = static["params"]
+            nutils.save_weightmap('train', out[5], get_homography(args.resize), out[4], *out[:4], p[:, 0, :], p[:, 1, :],
+                                  p[:, 2, :], p[:, 3, :], batch[4], static["gt"], 0, i, static["input"], args.no_ortho,
+                                  args.resize, args.save_path)
+
+    fields = lambda b: {"input": b[0], "gt": b[1], "params": b[2]}
+    if _train_replays(loader, model, optimizer, static, fields, {"input": torch.float32}, post, report, args.print_freq,
+                      args.save_freq, loss_fn=loss_fn, end_to_end=e2e) is None:
         return 0, 0, 0
     m = meters.read()
-    status.print_skipped(labels)
     return m["loss"][1], m["area"][1], m["exact"][1]

@@ -334,106 +334,65 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
     pixel accuracy, per-class IoU and mIoU over the classes with a nonzero denominator) and a dict passed as
     ``seg_metrics`` receives "ce", "pixel_acc", "iou", "miou" and "confusion".  The returned tuple is unchanged."""
     if __package__:
-        from .engine import GraphedInference, DeviceMeters, BatchStatus, lane_losses, _reporting
+        from .engine import DeviceMeters, lane_losses, check_bp_args, _valid_replays
         from .Networks import utils as nutils
     else:
-        from engine import GraphedInference, DeviceMeters, BatchStatus, lane_losses, _reporting
+        from engine import DeviceMeters, lane_losses, check_bp_args, _valid_replays
         from Networks import utils as nutils
-    if args.clas and not args.end_to_end:
-        raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
+    check_bp_args(args, criterion, model)
     e2e, L = bool(args.end_to_end), args.nclasses
-    if not e2e and L != 4:
-        raise ValueError("--end_to_end False needs 4 lanes: the reference's gt_line substitution does not broadcast the "
-                         "loader's 4 line flags over %d lane maps" % L)
-    if getattr(criterion, "learn_homography", False):
-        criterion.bind(model)
     dev = next(model.parameters()).device
     proxy = bool(getattr(model, "seg_proxy", False))
     meters = DeviceMeters(("loss", "acc_hor", "acc_line", "rmse") + (("seg_proxy",) if proxy else ()), dev)
-    status = BatchStatus(len(loader), dev)
-    graphs = {}                     # rows -> (GraphedInference, static batch tensors)
     counts = torch.zeros((L + 1) ** 2, dtype=torch.int64, device=dev) if proxy else None
 
-    def build(batch):
-        st = {k: v.to(dev, non_blocking=True).clone() for k, v in batch.items()}
-        st["input"], st["gt"] = st["input"].float(), st["gt"].long()
+    def post(out, st):
         n = st["input"].shape[0]
-
-        def post(out):
-            lanes, vp = st["lanes"], st["valid"]
-            if e2e:
-                loss, x_cal = lane_losses(criterion, out, lanes, vp, L)
-            else:
-                loss = criterion_seg(out[5], st["gt"])
-                loss_metric, x_cal = lane_losses(criterion, out, lanes, vp, L)
-            if proxy:
-                ce = criterion_seg(out[8], st["gt"])
-            if not torch.cuda.is_current_stream_capturing():
-                return x_cal                 # warm-up passes: no meter or log entry
-            ok = model.lsq_status.reshape(()).eq(0)
-            if not e2e:
-                meters.update("rmse", loss_metric, ok, n)
-            meters.update("loss", loss, ok, n)
-            if proxy:
-                meters.update("seg_proxy", ce, ok, n)
-                seg_confusion(out[8], st["gt"], counts, model.lsq_status)
-            if args.clas:
-                horizon_pred = torch.round(torch.nn.Sigmoid()(out[7]))
-                acc = torch.eq(horizon_pred, st["gt_horizon"])
-                acc_hor = torch.sum(acc).float() / (args.resize * args.val_batch_size)
-                meters.update("acc_hor", acc_hor, ok)
-                line_pred = torch.round(torch.nn.Sigmoid()(out[6]))
-                acc = torch.eq(line_pred, st["gt_line"])
-                acc_line = torch.sum(acc).float() / (args.nclasses * args.val_batch_size)
-                meters.update("acc_line", acc_line, ok)
-            status.record(model.lsq_status)
-            model.lsq_status.zero_()
-            return x_cal
-
-        g = GraphedInference(model, st["input"], post=post, gt_line=None if e2e else st["gt_line"], end_to_end=e2e)
-        st["input"] = g.x
+        lanes, vp = st["lanes"], st["valid"]
+        if e2e:
+            loss, x_cal = lane_losses(criterion, out, lanes, vp, L)
+        else:
+            loss = criterion_seg(out[5], st["gt"])
+            loss_metric, x_cal = lane_losses(criterion, out, lanes, vp, L)
+        if proxy:
+            ce = criterion_seg(out[8], st["gt"])
+        if not torch.cuda.is_current_stream_capturing():
+            return x_cal                 # warm-up passes: no meter entry
+        ok = model.lsq_status.reshape(()).eq(0)
         if not e2e:
-            st["gt_line"] = g.gt_line        # the forward's substitution and the accuracies read one buffer
-        model.lsq_status.zero_()
-        return g, st
+            meters.update("rmse", loss_metric, ok, n)
+        meters.update("loss", loss, ok, n)
+        if proxy:
+            meters.update("seg_proxy", ce, ok, n)
+            seg_confusion(out[8], st["gt"], counts, model.lsq_status)
+        if args.clas:
+            horizon_pred = torch.round(torch.nn.Sigmoid()(out[7]))
+            acc = torch.eq(horizon_pred, st["gt_horizon"])
+            acc_hor = torch.sum(acc).float() / (args.resize * args.val_batch_size)
+            meters.update("acc_hor", acc_hor, ok)
+            line_pred = torch.round(torch.nn.Sigmoid()(out[6]))
+            acc = torch.eq(line_pred, st["gt_line"])
+            acc_line = torch.sum(acc).float() / (args.nclasses * args.val_batch_size)
+            meters.update("acc_line", acc_line, ok)
+        return x_cal
 
-    deferred = model.defer_status_check
-    first, labels = None, []
-    try:
-        with torch.no_grad():
-            for i, (input, gt, lanes, idx, gt_line, gt_horizon, index, valid_points) in enumerate(loader):
-                batch = {"input": input, "gt": gt.squeeze(1), "lanes": lanes, "gt_line": gt_line, "gt_horizon": gt_horizon,
-                         "valid": valid_points}
-                n = input.shape[0]
-                status.check(i)
-                if first is None:
-                    first = n
-                elif n > first:
-                    raise ValueError("batch of %d images after a first batch of %d" % (n, first))
-                if n in graphs:
-                    g, st = graphs[n]
-                    for k, v in batch.items():
-                        st[k].copy_(v, non_blocking=True)
-                else:
-                    g, st = graphs[n] = build(batch)
-                labels.append(idx)
-                g.graph.replay()
-                if not (_reporting(i, args.print_freq) or _reporting(i, 25)) or int(status.log[i]):
-                    continue                     # a skipped batch reports nothing, as main.py's `continue`
-                if _reporting(i, args.print_freq):
-                    m = meters.read()
-                    print('Test: [{0}/{1}]\t'
-                          'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
-                          'rmse {rmse[0]:.8f} ({rmse[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], rmse=m["rmse"]))
-                if _reporting(i, 25):
-                    lanes = st["lanes"]
-                    nutils.save_weightmap('valid', g.out[4], *g.post_out, lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :],
-                                          lanes[:, 3, :], st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
-                                          args.save_path, args.nclasses, args.no_mapping)
-    finally:
-        model.defer_status_check = deferred
+    def report(i, printing, saving, batch, g, st):
+        if printing:
+            m = meters.read()
+            print('Test: [{0}/{1}]\t'
+                  'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                  'rmse {rmse[0]:.8f} ({rmse[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], rmse=m["rmse"]))
+        if saving:
+            lanes = st["lanes"]
+            nutils.save_weightmap('valid', g.out[4], *g.post_out, lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :],
+                                  lanes[:, 3, :], st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
+                                  args.save_path, args.nclasses, args.no_mapping)
+
+    fields = lambda b: {"input": b[0], "gt": b[1].squeeze(1), "lanes": b[2], "gt_line": b[4], "gt_horizon": b[5],
+                        "valid": b[7]}
+    _valid_replays(loader, model, fields, {"input": torch.float32, "gt": torch.int64}, post, report, args.print_freq,
+                   gt_line=not e2e, end_to_end=e2e)
     m = meters.read()
-    status.print_skipped(labels)
     if proxy:
         seg = seg_metrics_from_confusion(counts.view(L + 1, L + 1))
         seg["ce"] = m["seg_proxy"][1]
@@ -464,83 +423,48 @@ def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, 
     the first is replayed by a second graph of its size.  The host synchronises only at the print_freq lines, at
     save_weightmap('valid', ...) every 25 batches and at the end."""
     if __package__:
-        from .engine import GraphedInference, DeviceMeters, BatchStatus, _reporting, check_bev_args
+        from .engine import DeviceMeters, check_bev_args, _valid_replays
         from .Loss_crit import fused_area_loss
         from .Networks import utils as nutils
     else:
-        from engine import GraphedInference, DeviceMeters, BatchStatus, _reporting, check_bev_args
+        from engine import DeviceMeters, check_bev_args, _valid_replays
         from Loss_crit import fused_area_loss
         from Networks import utils as nutils
     check_bev_args(args)
     e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
-    dev = next(model.parameters()).device
-    meters = DeviceMeters(("loss", "area", "exact"), dev)
-    status = BatchStatus(len(loader), dev)
-    graphs = {}                     # rows -> (GraphedInference, static batch tensors)
+    meters = DeviceMeters(("loss", "area", "exact"), next(model.parameters()).device)
 
-    def build(batch):
-        st = {k: v.to(dev, non_blocking=True).clone() for k, v in batch.items()}
-        st["input"] = st["input"].float()
+    def post(out, st):
         n = st["input"].shape[0]
+        if e2e:
+            loss, exact = fused_area_loss(out[:L], st["params"], wf, exact=True)
+        else:
+            loss = criterion_seg(out[6], st["gt"])
+            area, exact = fused_area_loss(out[:2], st["params"], wf, exact=True)
+        if not torch.cuda.is_current_stream_capturing():
+            return None                  # warm-up passes: no meter entry
+        ok = model.lsq_status.reshape(()).eq(0)
+        if not e2e:
+            meters.update("area", area, ok, n)
+        meters.update("exact", exact, ok, n)
+        meters.update("loss", loss, ok, n)
+        return None
 
-        def post(out):
-            if e2e:
-                loss, exact = fused_area_loss(out[:L], st["params"], wf, exact=True)
-            else:
-                loss = criterion_seg(out[6], st["gt"])
-                area, exact = fused_area_loss(out[:2], st["params"], wf, exact=True)
-            if not torch.cuda.is_current_stream_capturing():
-                return None                  # warm-up passes: no meter or log entry
-            ok = model.lsq_status.reshape(()).eq(0)
-            if not e2e:
-                meters.update("area", area, ok, n)
-            meters.update("exact", exact, ok, n)
-            meters.update("loss", loss, ok, n)
-            status.record(model.lsq_status)
-            model.lsq_status.zero_()
-            return None
+    def report(i, printing, saving, batch, g, st):
+        if printing:
+            m = meters.read()
+            print('Test: [{0}/{1}]\t'
+                  'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
+                  'Area {area[0]:.8f} ({area[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], area=m["area"]))
+        if saving:
+            out, p = g.out, st["params"]
+            nutils.save_weightmap('valid', out[5], M_inv, out[4], *out[:4], p[:, 0, :], p[:, 1, :], p[:, 2, :],
+                                  p[:, 3, :], batch[4], st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
+                                  args.save_path)
 
-        g = GraphedInference(model, st["input"], post=post, end_to_end=e2e)
-        st["input"] = g.x
-        model.lsq_status.zero_()
-        return g, st
-
-    deferred = model.defer_status_check
-    first, labels = None, []
-    try:
-        with torch.no_grad():
-            for i, (input, gt, params, idx, gt_line, gt_horizon, index) in enumerate(loader):
-                batch = {"input": input, "gt": gt, "params": params}
-                n = input.shape[0]
-                status.check(i)
-                if first is None:
-                    first = n
-                elif n > first:
-                    raise ValueError("batch of %d images after a first batch of %d" % (n, first))
-                if n in graphs:
-                    g, st = graphs[n]
-                    for k, v in batch.items():
-                        st[k].copy_(v, non_blocking=True)
-                else:
-                    g, st = graphs[n] = build(batch)
-                labels.append(idx)
-                g.graph.replay()
-                if not (_reporting(i, args.print_freq) or _reporting(i, 25)) or int(status.log[i]):
-                    continue                     # a skipped batch reports nothing, as main.py's `continue`
-                if _reporting(i, args.print_freq):
-                    m = meters.read()
-                    print('Test: [{0}/{1}]\t'
-                          'Loss {loss[0]:.8f} ({loss[1]:.8f})\t'
-                          'Area {area[0]:.8f} ({area[1]:.8f})'.format(i + 1, len(loader), loss=m["loss"], area=m["area"]))
-                if _reporting(i, 25):
-                    out, p = g.out, st["params"]
-                    nutils.save_weightmap('valid', out[5], M_inv, out[4], *out[:4], p[:, 0, :], p[:, 1, :], p[:, 2, :],
-                                          p[:, 3, :], gt_line, st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
-                                          args.save_path)
-    finally:
-        model.defer_status_check = deferred
+    _valid_replays(loader, model, lambda b: {"input": b[0], "gt": b[1], "params": b[2]}, {"input": torch.float32}, post,
+                   report, args.print_freq, end_to_end=e2e)
     m = meters.read()
-    status.print_skipped(labels)
     if args.evaluate:
         crit_string = "AREA**2" if e2e else "ENTROPY"
         print("===> Average {}-loss on validation set is {:.8}".format(crit_string, m["loss"][1]))

@@ -80,6 +80,25 @@ def test_a_later_batch_larger_than_the_first_raises(monkeypatch):
     assert model.defer_status_check is False
 
 
+@pytest.mark.parametrize("loop", ["validate_bev", "skip_epoch"])
+def test_other_loops_refuse_a_later_batch_of_another_size(monkeypatch, loop):
+    """validate_bev refuses a larger later batch; the --pretrained skip epoch (epoch 0 < skip_epochs) any other size."""
+    monkeypatch.setattr(engine, "GraphedInference", _Graphed)
+    monkeypatch.setattr(engine, "GraphedTrainStep", _GraphedStep)
+    model = _Model()
+    if loop == "validate_bev":
+        with pytest.raises(ValueError, match="batch of 3 images after a first batch of 2"):
+            inference.validate_bev([_batch(2), _batch(3)], model, None, None, None, None, None,
+                                   _args("--nclasses", "2", "--order", "2", "--loss_policy", "area"))
+    else:
+        opt = FusedOptimizer(model.parameters(), "adam", 1e-3, 0, per_param_step=True)
+        for n in (1, 3):
+            with pytest.raises(ValueError, match="batch of %d images after a first batch of 2" % n):
+                engine.train_epoch([_batch(2), _batch(n)], model, opt, None, None, None, None,
+                                   _args("--pretrained", "True"), 0)
+    assert model.defer_status_check is False
+
+
 def test_seg_lane_maps_line_prototype_matches_header():
     hdr = open(os.path.join(ROOT, "include", "lanefit_b200.h")).read()
     for name in ("lf_seg_lane_maps", "lf_seg_lane_maps_line"):
