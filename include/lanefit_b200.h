@@ -699,6 +699,24 @@ size_t lf_jpeg_workspace_bytes(LfJpegImage* images, int N, size_t* coef_bytes);
 int lf_jpeg_decode(const void* blob, int N, int W, int H, unsigned char* out, int* status, void* coef, size_t coef_bytes,
                    void* workspace, size_t workspace_bytes, lf_stream_t stream);
 
+/* Baseline JPEG encode (csrc/jpeg_enc.cu): a batch of N same-size frames, uint8 RGB [N][H][W][3] (ncomp 3) or grayscale
+ * [N][H][W] (ncomp 1) -> one JPEG file per frame, byte-identical to Pillow's
+ * Image.fromarray(a).save(buf, "JPEG", quality=q, subsampling=s) (libjpeg-turbo: fixed-point YCbCr, h2v2 downsampling,
+ * ISLOW forward DCT, its reciprocal quantisation, standard Huffman tables, no restart markers).
+ *   sampling: 2 = 4:2:0 (Pillow's default), 0 = 4:4:4.  A grayscale file codes the same bytes either way; Pillow's header
+ *   records 2x2 for its component under 4:2:0, and so does this one.  W, H in 1..65535.
+ *   qtables: HOST uint16 [ncomp == 3 ? 2 : 1][64], natural order, each entry 1..255 (lf_jpeg_quality_tables fills them).
+ *   out: device bytes, image n's file at out + n * out_cap; out_cap >= lf_jpeg_encode_bound(W, H, ncomp, sampling).
+ *   out_len: device int64 [N], each file's length.  workspace: lf_jpeg_encode_workspace_bytes(N, W, H, ncomp, sampling).
+ * Four launches (block transform, bit-offset scan, bit packing, byte stuffing); never synchronises, graph-capturable.
+ * Calls sharing `workspace` must be ordered by the caller.  Bad shapes, sampling, tables or capacity return
+ * LF_ERR_INVALID_ARGUMENT. */
+int lf_jpeg_quality_tables(int quality, int ncomp, unsigned short* qtables);  /* HOST: jpeg_set_quality(q, TRUE), q 1..100 */
+long long lf_jpeg_encode_bound(int W, int H, int ncomp, int sampling);        /* HOST: worst-case file bytes, 0 = invalid */
+size_t lf_jpeg_encode_workspace_bytes(int N, int W, int H, int ncomp, int sampling);   /* HOST: 0 = invalid */
+int lf_jpeg_encode(const unsigned char* frames, int N, int W, int H, int ncomp, int sampling, const unsigned short* qtables,
+                   unsigned char* out, long long out_cap, long long* out_len, void* workspace, lf_stream_t stream);
+
 /* PNG decode of label maps (csrc/png.cu; replaces Image.open(f).convert('P') of BP/Dataloader/Load_Data_new.py:120-121):
  * a batch of same-size non-interlaced PNGs, 8-bit grayscale or 1/2/4/8-bit palette -> uint8 [N][H][W] holding the gray
  * values or palette indices, bit-identical to Pillow.  The chunks are walked on the host (lanedetection_end2end_b200/png.py),
@@ -749,6 +767,16 @@ int lf_label_preprocess(const unsigned char* maps, int N, int Hin, int Win, int 
 int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* horizon_pred, int B, int P, int S, const int* gt_x,
                       const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes, double* per_image,
                       lf_stream_t stream);
+
+/* The predicted points drawn onto the test frames (csrc/tusimple.cu; the cv2.circle loop of BP/test.py:115-119):
+ * frames uint8 [N][H][W][3] in place; lanes [N][L][S] int32 (-2 = no point) at rows h_samples [N][S] int32; colors: HOST
+ * uint8 [L][3], the colour of each lane.  Every point is stamped with cv2.circle(img, (x, y), radius, color, thickness=-1)'s
+ * pixels (LINE_8, shift 0; the stamp's spans are computed on the host), clipped at the frame borders; where stamps overlap
+ * the pixel takes the colour of the last one in the reference's order (lane by lane, point by point).  One launch. */
+#define LF_DRAW_MAX_LANES 8
+#define LF_DRAW_MAX_RADIUS 16
+int lf_draw_lane_points(unsigned char* frames, int N, int H, int W, const int* lanes, int L, int S, const int* h_samples,
+                        const unsigned char* colors, int radius, lf_stream_t stream);
 
 /* The TuSimple loader's device cache (csrc/loader.cu; Dataloader/Load_Data_new.py of this package, replacing the per-sample
  * work of BP/Dataloader/Load_Data_new.py:110-197 after decoding).  A cache is two slot-addressed uint8 buffers of resized,

@@ -169,6 +169,7 @@ class LfPngImage(ctypes.Structure):
 
 TUSIMPLE_MAX_GT = 8
 TUSIMPLE_MAX_S = 64
+DRAW_MAX_LANES, DRAW_MAX_RADIUS = 8, 16
 LOADER_LANES, LOADER_POINTS = 4, 56
 LOADER_BEV_COEFFS = 3
 
@@ -183,6 +184,11 @@ _NET_PROTOS = {
     "lf_label_preprocess": (_i, [_p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _p, _p]),
     "lf_jpeg_workspace_bytes": (_c_size_t, [_p, _i, _p]),
     "lf_jpeg_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p, _c_size_t, _p]),
+    "lf_jpeg_quality_tables": (_i, [_i, _i, _p]),
+    "lf_jpeg_encode_bound": (_ll, [_i, _i, _i, _i]),
+    "lf_jpeg_encode_workspace_bytes": (_c_size_t, [_i, _i, _i, _i, _i]),
+    "lf_jpeg_encode": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _ll, _p, _p, _p]),
+    "lf_draw_lane_points": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _i, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
     "lf_optim_step_pp": (_i, [_i, _p, _p, _i, _ll, _p, _p, _i, _p, _p, _p, _p]),
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i, _i]),

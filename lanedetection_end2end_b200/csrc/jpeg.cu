@@ -31,33 +31,7 @@ __constant__ unsigned char c_natural[80] = {
     6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31,
     39, 46, 53, 60, 61, 54, 47, 55, 62, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63, 63};
 
-// ---- CTA-wide scans (blockDim.x == JT) --------------------------------------------------------------------------------
-__device__ unsigned long long cta_excl_sum(unsigned long long v, unsigned long long* sh, unsigned long long& total) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned long long x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sh[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        unsigned long long t = sh[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, t, o);
-            if (lane >= o) t += y;
-        }
-        sh[lane] = t;
-    }
-    __syncthreads();
-    const unsigned long long pre = (w ? sh[w - 1] : 0ull) + x - v;
-    total = sh[31];
-    __syncthreads();
-    return pre;
-}
-
+// ---- CTA-wide scans (blockDim.x == JT; cta_excl_sum is in lf_common.cuh) ----------------------------------------------
 // segmented sum: (f, v) with f = "a segment starts inside"; returns the carry into this thread (sum since the last start)
 __device__ __forceinline__ void seg_comb(int& f, int& v, int pf, int pv) {
     if (!f) v += pv;

@@ -117,6 +117,34 @@ __device__ __forceinline__ f32x2_t f2_fma(f32x2_t a, f32x2_t b, f32x2_t c) {
     return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
+// Exclusive sum over a CTA of exactly 1024 threads (32 warps); *total receives the CTA's sum.  sh: 32 entries of shared
+// memory.  Ends with a barrier, so sh can be reused at once.
+__device__ inline unsigned long long cta_excl_sum(unsigned long long v, unsigned long long* sh, unsigned long long& total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    unsigned long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) sh[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        unsigned long long t = sh[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, t, o);
+            if (lane >= o) t += y;
+        }
+        sh[lane] = t;
+    }
+    __syncthreads();
+    const unsigned long long pre = (w ? sh[w - 1] : 0ull) + x - v;
+    total = sh[31];
+    __syncthreads();
+    return pre;
+}
+
 // streaming 128-bit load (read once, do not pollute L1)
 __device__ __forceinline__ float4 ld_stream_f4(const float4* p) {
     float4 r;

@@ -12,6 +12,13 @@
 // divisions, so the result equals LaneEval's bit for bit.  One CTA per launch, one warp per image: a latency-bound launch.
 // The batch covers file rows pos .. pos + B - 1; rows >= N are not scored, and the launch advances *pos by B so a
 // captured graph can be replayed once per batch.
+//
+// lf_draw_lane_points stamps the predicted points onto the test frames as BP/test.py:115-119 does with cv2.circle(...,
+// thickness=-1): one CTA per frame; each (point, stamp pixel) pair writes its lane's colour unless a later point in the
+// drawing order (lane by lane, point by point) also covers the pixel, so every pixel is written at most once and the last
+// stamp wins without ordering the writes.
+#include <climits>
+
 #include "lf_common.cuh"
 
 namespace lf {
@@ -105,9 +112,83 @@ __global__ void __launch_bounds__(TS_WARPS * 32) tusimple_score_kernel(
     if (threadIdx.x == 0) *pos = (int)(p0 + B);
 }
 
+struct DrawParams {
+    int hw[LF_DRAW_MAX_RADIUS + 1];              // stamp half-width on rows 0..radius from the centre
+    unsigned char rgb[LF_DRAW_MAX_LANES][3];
+};
+
+constexpr int DRAW_OFF = INT_MIN;                // no point, or a point whose stamp misses the frame
+
+__global__ void __launch_bounds__(256) draw_lane_points_kernel(uint8_t* __restrict__ frames, int H, int W, const int* __restrict__ lanes,
+                                                               int L, int S, const int* __restrict__ h_samples, int R,
+                                                               const __grid_constant__ DrawParams D) {
+    pdl_entry();
+    __shared__ int s_x[LF_DRAW_MAX_LANES * LF_TUSIMPLE_MAX_S], s_y[LF_DRAW_MAX_LANES * LF_TUSIMPLE_MAX_S];
+    const int n = blockIdx.x, np = L * S;
+    for (int p = threadIdx.x; p < np; p += blockDim.x) {
+        const int x = lanes[(size_t)n * np + p], y = h_samples[(size_t)n * S + p % S];
+        const bool off = x == -2 || x < -R || x >= W + R || y < -R || y >= H + R;
+        s_x[p] = off ? DRAW_OFF : x;
+        s_y[p] = y;
+    }
+    __syncthreads();
+    const int side = 2 * R + 1, box = side * side;
+    uint8_t* img = frames + (size_t)n * H * W * 3;
+    for (int it = threadIdx.x; it < np * box; it += blockDim.x) {
+        const int p = it / box, j = it - p * box;
+        if (s_x[p] == DRAW_OFF) continue;
+        const int dy = j / side - R, dx = j % side - R;
+        if (abs(dx) > D.hw[abs(dy)]) continue;
+        const int px = s_x[p] + dx, py = s_y[p] + dy;
+        if (px < 0 || px >= W || py < 0 || py >= H) continue;
+        bool later = false;
+        for (int q = p + 1; q < np && !later; ++q) {
+            const int ey = py - s_y[q];
+            later = s_x[q] != DRAW_OFF && abs(ey) <= R && abs(px - s_x[q]) <= D.hw[abs(ey)];
+        }
+        if (later) continue;
+        uint8_t* o = img + ((size_t)py * W + px) * 3;
+        const unsigned char* c = D.rgb[p / S];
+        o[0] = c[0];
+        o[1] = c[1];
+        o[2] = c[2];
+    }
+}
+
 }  // namespace lf
 
 using namespace lf;
+
+// Half-widths of cv2's filled integer circle (drawing.cpp Circle with fill, LINE_8, shift 0): the midpoint loop emits
+// spans on rows cy -+ dy (x within dx) and cy -+ dx (x within dy); the stamp is their union.
+static void circle_halfwidths(int R, int* hw) {
+    for (int i = 0; i <= R; ++i) hw[i] = -1;
+    int err = 0, dx = R, dy = 0, plus = 1, minus = (R << 1) - 1;
+    while (dx >= dy) {
+        hw[dy] = hw[dy] > dx ? hw[dy] : dx;
+        hw[dx] = hw[dx] > dy ? hw[dx] : dy;
+        ++dy;
+        err += plus;
+        plus += 2;
+        const int mask = (err <= 0) - 1;
+        err -= minus & mask;
+        dx += mask;
+        minus -= mask & 2;
+    }
+}
+
+extern "C" int lf_draw_lane_points(unsigned char* frames, int N, int H, int W, const int* lanes, int L, int S, const int* h_samples,
+                                   const unsigned char* colors, int radius, lf_stream_t stream_) {
+    LF_REQUIRE(frames && lanes && h_samples && colors && N >= 1 && H >= 1 && W >= 1);
+    LF_REQUIRE(L >= 1 && L <= LF_DRAW_MAX_LANES && S >= 1 && S <= LF_TUSIMPLE_MAX_S && radius >= 0 && radius <= LF_DRAW_MAX_RADIUS);
+    DrawParams D;
+    circle_halfwidths(radius, D.hw);
+    for (int l = 0; l < L; ++l)
+        for (int k = 0; k < 3; ++k) D.rgb[l][k] = colors[l * 3 + k];
+    lf_launch(draw_lane_points_kernel, dim3(N), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream_), frames, H, W, lanes, L, S,
+              h_samples, radius, D);
+    return check_launch();
+}
 
 extern "C" int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* horizon_pred, int B, int P, int S,
                                  const int* gt_x, const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes,

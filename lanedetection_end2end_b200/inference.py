@@ -10,6 +10,8 @@ curve coefficients after ``model(input, ...)``.
   TuSimpleScorer             BP/test.py:66-99 + eval_lane.py:27-95  gating and LaneEval scoring on the GPU, one launch
                                                  (lf_tusimple_score, csrc/tusimple.cu) per batch
   test_model                 BP/test.py:23-129   the per-epoch test-set evaluation, one CUDA-graph replay per batch
+  draw_lane_points           BP/test.py:115-119  the predicted points stamped onto frames as cv2.circle(..., thickness=-1)
+  render_testset             BP/test.py:111-121  decode, stamp and re-encode the test frames on the GPU, one file per row
   validate / validate_bev    BP/main.py:419-526, BEV/main.py:362-501  validation passes, one CUDA-graph replay per batch
 
 ``Projections.compute_coordinates`` keeps the reference's name, argument and result ([B, order+1, 1] float64 -> [B, 56]
@@ -34,6 +36,7 @@ else:                                   # imported top-level next to the referen
 TUSIMPLE_SAMPLES = 56                   # h_samples 160..710 step 10: what Projections predicts
 TUSIMPLE_LANES = 4                      # predicted lanes of the 4-lane --clas model
 PIXEL_THRESH = 20                       # LaneEval.pixel_thresh (pt_thresh 0.85 lives in the kernel)
+COLORMAP = [(255, 0, 0), (0, 255, 0), (255, 255, 0), (0, 0, 255), (0, 128, 128)]   # BP/test.py:31, colour of lane i
 
 
 def resize_coordinates(array):
@@ -246,9 +249,11 @@ def _scorer_for(gt_file, device):
     return hit[1]
 
 
-def test_model(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0):
+def test_model(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0,
+               render_dir=None):
     """The reference's per-epoch test-set evaluation (BP/test.py:23-129), same signature and return value (the TuSimple
-    accuracy).  Reads args.test_dir/test_label.json, writes args.save_path/test_set_predictions.json.
+    accuracy).  Reads args.test_dir/test_label.json, writes args.save_path/test_set_predictions.json.  With ``render_dir``
+    set, the predicted lanes are then drawn onto the test frames into render_dir/{row}.jpg (render_testset).
 
     Each batch is one CUDA-graph replay of the eval forward, the heads' post-processing (the reference's torch ops),
     Projections.compute_all and TuSimpleScorer.score; the host only copies the batch into the static input (a shorter last
@@ -309,7 +314,111 @@ def test_model(loader, model, criterion, criterion_seg, criterion_line_class, cr
     acc_seg = scorer.result()
     print(acc_seg)
     print("===> Average ACC on TESTSET is {:.8} in {:.6}s for a batch".format(acc_seg[0], start.elapsed_time(end) / 1e3 / batches))
+    if render_dir is not None:
+        render_testset(scorer.lanes, scorer.rows, args.test_dir, render_dir)
     return acc_seg[0]
+
+
+def draw_lane_points(frames, lanes, h_samples, colors=None, radius=3):
+    """Stamp every point of ``lanes`` onto ``frames`` in place, as the reference's drawing loop does
+    (BP/test.py:115-119: cv2.circle(img, (x, y), radius, colormap[lane], thickness=-1) lane by lane, point by point; the
+    last stamp wins where they overlap).  frames uint8 [N,H,W,3], lanes int32 [N,L,S] (-2 = no point), h_samples int32
+    [N,S] (the row of each sample), colors L RGB triples (default COLORMAP).  One launch of lf_draw_lane_points."""
+    N, L, S = lanes.shape
+    colors = COLORMAP[:L] if colors is None else colors
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3 or frames.shape[0] != N:
+        raise ValueError("frames must be uint8 [%d,H,W,3], got %s %s" % (N, frames.dtype, tuple(frames.shape)))
+    if lanes.dtype != torch.int32 or h_samples.dtype != torch.int32 or tuple(h_samples.shape) != (N, S):
+        raise ValueError("lanes must be int32 [N,L,S] and h_samples int32 [N,S], got %s %s and %s %s"
+                         % (lanes.dtype, tuple(lanes.shape), h_samples.dtype, tuple(h_samples.shape)))
+    if len(colors) != L or L > _capi.DRAW_MAX_LANES:
+        raise ValueError("%d lanes need %d colours (at most %d lanes), got %d" % (L, L, _capi.DRAW_MAX_LANES, len(colors)))
+    if not 0 <= radius <= _capi.DRAW_MAX_RADIUS:
+        raise ValueError("radius must be in 0..%d, got %r" % (_capi.DRAW_MAX_RADIUS, radius))
+    _capi.require_cuda(frames, lanes, h_samples)
+    if not frames.is_contiguous():
+        raise ValueError("frames are drawn in place and must be contiguous")
+    rgb = np.ascontiguousarray(np.asarray(colors, np.uint8).reshape(L, 3))
+    lanes, h_samples = lanes.contiguous(), h_samples.contiguous()
+    _capi.call("lf_draw_lane_points", _capi.ptr(frames), N, frames.shape[1], frames.shape[2], _capi.ptr(lanes), L, S,
+               _capi.ptr(h_samples), rgb.ctypes.data, int(radius), _capi.stream_ptr())
+    return frames
+
+
+def render_testset(lanes, rows, test_dir, out_dir, batch_size=32):
+    """The overlay of the reference's --draw_testset (BP/test.py:111-121) on the GPU: for row i, the frame
+    test_dir/rows[i]['raw_file'] decoded (jpeg.JpegDecoder, as Image.open(f).convert('RGB')), lanes[i] stamped at
+    rows[i]['h_samples'] in COLORMAP's colours with radius 3, encoded as Pillow's img.save(path) would (jpeg.JpegEncoder:
+    quality 75, 4:2:0) and written to out_dir/{i}.jpg; i is the reference's im_id.  ``lanes`` is TuSimpleScorer.lanes after a
+    pass ([N, L, S] int32 on the device) and ``rows`` its ground-truth rows.  A frame the decoder refuses raises ValueError
+    naming the file; there is no CPU fallback.  The reference's weight-map image {im_id}_vis.jpg is not written: the
+    reference cannot save it (Pillow has no JPEG writer for its float image).  Returns the paths written."""
+    if __package__:
+        from .jpeg import JpegDecoder, JpegEncoder
+    else:
+        from jpeg import JpegDecoder, JpegEncoder
+    N, L, S = lanes.shape
+    if len(rows) != N:
+        raise ValueError("%d rows for %d lane sets" % (len(rows), N))
+    _capi.require_cuda(lanes)
+    dev = lanes.device
+    lanes = lanes.to(torch.int32)
+    dec, enc = JpegDecoder(dev), JpegEncoder(dev)
+    os.makedirs(out_dir, exist_ok=True)
+    written = []
+    for b0 in range(0, N, batch_size):
+        idx = range(b0, min(N, b0 + batch_size))
+        paths = [os.path.join(test_dir, rows[i]["raw_file"]) for i in idx]
+        datas = []
+        for p in paths:
+            with open(p, "rb") as f:
+                datas.append(f.read())
+        try:
+            frames = dec(datas)
+        except ValueError as e:
+            raise ValueError("%s: %s" % (_refused_frame(dec, paths, datas, False) or ", ".join(paths), e)) from None
+        for i, p in zip(idx, paths):
+            if len(rows[i]["h_samples"]) != S:
+                raise ValueError("%s: %d h_samples for %d lane samples" % (p, len(rows[i]["h_samples"]), S))
+        h = torch.tensor([rows[i]["h_samples"] for i in idx], dtype=torch.int32).to(dev, non_blocking=True)
+        draw_lane_points(frames, lanes[b0:b0 + len(idx)], h)
+        files = enc(frames)
+        try:
+            dec.check()
+        except ValueError as e:
+            raise ValueError("%s: %s" % (_refused_frame(JpegDecoder(dev), paths, datas, True) or ", ".join(paths), e)) from None
+        for i, data in zip(idx, files):
+            path = os.path.join(out_dir, "{}.jpg".format(i))
+            with open(path, "wb") as f:
+                f.write(data)
+            written.append(path)
+    return written
+
+
+def _refused_frame(dec, paths, datas, frames_ok):
+    """The first file of a refused batch that the decoder refuses on its own: its headers (frames_ok False: parsing or a
+    size that differs from the batch's first), or its entropy-coded data (frames_ok True: one decode and check per file)."""
+    if __package__:
+        from .jpeg import parse
+    else:
+        from jpeg import parse
+    size = None
+    for p, d in zip(paths, datas):
+        if not frames_ok:
+            try:
+                h = parse(d)
+            except ValueError:
+                return p
+            if size is not None and (h.width, h.height) != size:
+                return p
+            size = size or (h.width, h.height)
+            continue
+        dec([d])
+        try:
+            dec.check()
+        except ValueError:
+            return p
+    return None
 
 
 def validate(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch=0,

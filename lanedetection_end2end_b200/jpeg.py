@@ -13,7 +13,9 @@ naming the feature.  There is no CPU fallback.
 
 Host work per image is a walk over the markers (no per-byte Python loop: finding the end of the entropy-coded segment is
 one regular-expression search, unstuffing and restart markers are handled on the device).  The frames belong to the
-stream current at the call; a consumer on another stream waits for that stream and calls frames.record_stream(...)."""
+stream current at the call; a consumer on another stream waits for that stream and calls frames.record_stream(...).
+
+JpegEncoder is the other direction (csrc/jpeg_enc.cu): frames -> files byte-identical to Pillow's baseline encoder."""
 import functools
 import re
 
@@ -364,3 +366,85 @@ class JpegDecoder:
             self._last = torch.cuda.Event()
             self._last.record(stream)
             raise ValueError("corrupt JPEG data: entropy-coded segment truncated or invalid (status 0x%x)" % s)
+
+
+_SAMPLING_IDS = {"4:2:0": 2, "4:4:4": 0}
+
+
+class JpegEncoder:
+    """Batch baseline JPEG encoder on one device (csrc/jpeg_enc.cu): uint8 [N,H,W,3] RGB or [N,H,W] grayscale frames ->
+    one file per frame, byte-identical to Image.fromarray(frame).save(buf, "JPEG", quality=quality,
+    subsampling=subsampling) of Pillow.  quality 1..100 (libjpeg's scaling of the Annex K tables, forced baseline);
+    subsampling "4:2:0" (Pillow's default) or "4:4:4".  Standard Huffman tables, no restart markers.
+
+        enc = JpegEncoder("cuda", quality=75)
+        files = enc(frames)                               # list of bytes; one synchronisation to read the lengths
+        buf, offsets, lengths = enc.encode_async(frames)  # device tensors: file n is buf[offsets[n]:offsets[n] + lengths[n]]
+
+    Calls are ordered among themselves (they share the workspace); the outputs belong to the stream current at the call.
+    encode_async can be captured into a CUDA graph once the workspace for its shape exists (one eager call first)."""
+
+    def __init__(self, device="cuda", quality=75, subsampling="4:2:0"):
+        import torch
+        if subsampling not in _SAMPLING_IDS:
+            raise ValueError("subsampling must be one of %s, got %r" % (sorted(_SAMPLING_IDS), subsampling))
+        if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
+            raise ValueError("quality must be an integer in 1..100, got %r" % (quality,))
+        self.device = torch.device(device)
+        self.quality, self.subsampling = int(quality), subsampling
+        self._qt = {}
+        for ncomp in (1, 3):
+            qt = np.zeros((2, 64), np.uint16)
+            _capi.check(_capi.lib().lf_jpeg_quality_tables(self.quality, ncomp, qt.ctypes.data), "lf_jpeg_quality_tables")
+            self._qt[ncomp] = qt
+        self._ws = None
+        self._last = None
+
+    def encode_async(self, frames):
+        """frames: uint8 CUDA tensor [N,H,W,3] or [N,H,W] -> (buffer uint8, offsets int64 [N], lengths int64 [N]), all on
+        the device; no synchronisation."""
+        import torch
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or frames.dim() not in (3, 4) or \
+                (frames.dim() == 4 and frames.shape[3] != 3) or frames.shape[0] < 1:
+            raise ValueError("frames must be a uint8 tensor [N,H,W,3] or [N,H,W], got %s %s"
+                             % (getattr(frames, "dtype", type(frames)), tuple(getattr(frames, "shape", ()))))
+        _capi.require_cuda(frames)
+        N, H, W = (int(v) for v in frames.shape[:3])
+        ncomp = 3 if frames.dim() == 4 else 1
+        sampling = _SAMPLING_IDS[self.subsampling]
+        lib = _capi.lib()
+        cap = lib.lf_jpeg_encode_bound(W, H, ncomp, sampling)
+        wsb = lib.lf_jpeg_encode_workspace_bytes(N, W, H, ncomp, sampling)
+        if cap <= 0 or wsb == 0:
+            raise ValueError("cannot encode %dx%d frames (JPEG sizes are 1..65535)" % (W, H))
+        frames = frames.contiguous()
+        stream = torch.cuda.current_stream(self.device)
+        capturing = torch.cuda.is_current_stream_capturing()      # a graph orders its own replays
+        if self._last is not None and not capturing:
+            stream.wait_event(self._last)
+        if self._ws is None or self._ws.numel() < wsb:
+            self._ws = torch.empty(wsb, dtype=torch.uint8, device=self.device)
+        if not capturing:
+            self._ws.record_stream(stream)
+        buf = torch.empty(N * cap, dtype=torch.uint8, device=self.device)
+        lengths = torch.empty(N, dtype=torch.int64, device=self.device)
+        _capi.call("lf_jpeg_encode", _capi.ptr(frames), N, W, H, ncomp, sampling, self._qt[ncomp].ctypes.data, _capi.ptr(buf), cap,
+                   _capi.ptr(lengths), _capi.ptr(self._ws), _capi.stream_ptr(), nbytes=frames.numel())
+        if not capturing:
+            self._last = torch.cuda.Event()
+            self._last.record(stream)
+        offsets = torch.arange(N, dtype=torch.int64, device=self.device) * cap
+        return buf, offsets, lengths
+
+    def __call__(self, frames):
+        """frames -> list of N JPEG files (bytes)."""
+        import torch
+        buf, offsets, lengths = self.encode_async(frames)
+        lens = lengths.cpu().tolist()                     # the one synchronisation
+        cap = int(buf.numel()) // len(lens)
+        packed = torch.cat([buf[n * cap:n * cap + l] for n, l in enumerate(lens)]).cpu().numpy()
+        out, o = [], 0
+        for l in lens:
+            out.append(packed[o:o + l].tobytes())
+            o += l
+        return out
