@@ -768,6 +768,27 @@ int lf_tusimple_score(const double* x_cal, const float* line_pred, const int* ho
                       const int* gt_lanes, const double* thresh, int N, int G, int* pos, int* lanes, double* per_image,
                       lf_stream_t stream);
 
+/* The bird's-eye-view validation score of one batch (csrc/tusimple.cu; write_lsq_results(..., all_branches_ready=False,
+ * horizon_on=False) of BEV/Dataloader/Load_Data_new.py:335-410 and LaneEval.bench of BEV/eval_lane.py, as
+ * BEV/main.py:445-488 run them): one launch, no host synchronisation, graph-capturable.
+ *   beta [B][4][3] f32: each image's fitted coefficients (a, b, c) per lane; rows [B] int64: each image's validation row;
+ *   status: device int32, the batch's LSQ status word; pos: device int64, the visit slot of image 0 (image b's results go
+ *   to slot *pos + b; slots >= V are not written; *pos is not changed).  warp: HOST [18] f64, M then M^-1 row-major (cv2's
+ *   getPerspectiveTransform of the normalised trapezoid, as write_lsq_results builds them); no_ortho != 0 samples the
+ *   curve in the image plane instead.
+ *   Ground-truth table of the validation file (N rows, table width G lanes, 4 <= G <= LF_TUSIMPLE_MAX_GT; every row has at
+ *   least 4 lanes): gt_S [N] samples per row (<= LF_TUSIMPLE_MAX_S), h_samples [N][LF_TUSIMPLE_MAX_S] int32, gt_x
+ *   [N][G][LF_TUSIMPLE_MAX_S] int32, gt_lanes [N], thresh [N][G] f64 (LaneEval.get_angle's threshold of each lane).
+ *   Per visit slot (V slots): lanes [V][4][LF_TUSIMPLE_MAX_S] int64: the sampled columns write_lsq_results writes
+ *   (np.int_(np.round(x * 1279)), -2 outside a lane's labelled rows, every float64 step in the host formula's order without
+ *   FMA contraction; NaN and values beyond int64 give INT64_MIN as numpy does on x86-64); per_row [V][3] f64:
+ *   LaneEval.bench's (accuracy, fp, fn) of the slot's row, bit-identical; scored [V] int32: 1 when the status word was 0,
+ *   else 0. */
+int lf_bev_lane_score(const float* beta, const long long* rows, const int* status, const long long* pos, int B, int no_ortho,
+                      const double* warp, const int* gt_S, const int* h_samples, const int* gt_x, const int* gt_lanes,
+                      const double* thresh, int N, int G, long long V, long long* lanes, double* per_row, int* scored,
+                      lf_stream_t stream);
+
 /* The predicted points drawn onto the test frames (csrc/tusimple.cu; the cv2.circle loop of BP/test.py:115-119):
  * frames uint8 [N][H][W][3] in place; lanes [N][L][S] int32 (-2 = no point) at rows h_samples [N][S] int32; colors: HOST
  * uint8 [L][3], the colour of each lane.  Every point is stamped with cv2.circle(img, (x, y), radius, color, thickness=-1)'s

@@ -151,7 +151,8 @@ class Classification(nn.Module):
         else:
             self.fully_connected_horizon = nn.Linear(64 * rows, resize)
 
-    def forward(self, x):
+    def stages(self, x):
+        """The four conv -> BatchNorm -> ReLU stages on the encoder map x: NHWC [B, rows, cols, 64]."""
         _heads, _net = submodule("ops_heads"), _ops_net
         from .ERFNet import _track
         h = _net.as_nhwc(x)
@@ -161,6 +162,11 @@ class Classification(nn.Module):
         for conv, bn in ((self.conv1, self.conv1_bn), (self.conv2, self.conv2_bn),
                          (self.conv3, self.conv3_bn), (self.conv4, self.conv4_bn)):
             h = _heads.conv_bn_relu(h, conv, bn, self.training, _track)
+        return h
+
+    def forward(self, x):
+        _heads = submodule("ops_heads")
+        h = self.stages(x)
         if self.class_type == "line":
             f = _heads.MaxPool2FlatFunction.apply(h)
             f = _heads.LinearFunction.apply(f, self.fully_connected1.weight, self.fully_connected1.bias, True)

@@ -179,6 +179,7 @@ _NET_PROTOS = {
     "lf_loader_label_rows": (_i, [_p, _i, _i, _i, _p, _p, _p, _p]),
     "lf_loader_assemble_bev": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "lf_tusimple_score": (_i, [_p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p]),
+    "lf_bev_lane_score": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _ll, _p, _p, _p, _p]),
     "lf_png_workspace_bytes": (_c_size_t, [_p, _i]),
     "lf_png_decode": (_i, [_p, _i, _i, _i, _p, _p, _p, _c_size_t, _p]),
     "lf_label_preprocess": (_i, [_p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _p, _p]),

@@ -4,7 +4,8 @@ Differences from the BP variant (all served by the same fused kernel, csrc/lsq.c
   * normalised image coordinates in [0,1) and a fixed normalised homography (reference :17-32, :66-87);
     the grid is rebuilt by ``project_layer(M)`` every forward (:324);
   * ``y = 1 - y'`` (:109), orders 0..2 only (:110-118), beta returned as float32 (:167);
-  * ``Net.forward(input, end_to_end)`` -> (beta0, beta1, beta2, beta3, masked, M, output, line, horizon) (:326).
+  * ``Net.forward(input, end_to_end)`` -> (beta0, beta1, beta2, beta3, masked, M, output, line, horizon) (:326); with
+    --clas the end-to-end forward runs the line-type head (line [B, 3, 4], its own tail) and the horizon head.
 """
 from math import ceil
 
@@ -64,7 +65,31 @@ class Weighted_least_squares(_L.Weighted_least_squares):
         return self._split(beta)
 
 
-Classification = _L.Classification
+class Classification(_L.Classification):
+    """Line-type / horizon heads of the BEV variant (reference :170-228), on the library's kernels like the BP class whose
+    conv / BatchNorm / pooling stages and horizon head they share.  The line head differs: after fully_connected1
+    (32768 -> 128, ReLU) come four Linear(128, 3), fully_connected_line1..4, concatenated to class logits [B, 3, 4]
+    (3 line types for each of the 4 lanes).  Their weights run stacked as one [12, 128] linear layer: every output is
+    computed independently, so one lf_linear_fwd launch gives the four heads' values."""
+
+    def __init__(self, class_type, size, channels_in, resize):
+        super().__init__(class_type, size, channels_in, resize)
+        if class_type == "line":
+            del self.fully_connected_line1
+            self.fully_connected_line1 = nn.Linear(128, 3)
+            self.fully_connected_line2 = nn.Linear(128, 3)
+            self.fully_connected_line3 = nn.Linear(128, 3)
+            self.fully_connected_line4 = nn.Linear(128, 3)
+
+    def forward(self, x):
+        if self.class_type != "line":
+            return super().forward(x)
+        _heads = _L.submodule("ops_heads")
+        f = _heads.MaxPool2FlatFunction.apply(self.stages(x))
+        f = _heads.LinearFunction.apply(f, self.fully_connected1.weight, self.fully_connected1.bias, True)
+        fcs = (self.fully_connected_line1, self.fully_connected_line2, self.fully_connected_line3, self.fully_connected_line4)
+        y = _heads.LinearFunction.apply(f, torch.cat([fc.weight for fc in fcs]), torch.cat([fc.bias for fc in fcs]), False)
+        return y.view(-1, 4, 3).transpose(1, 2)
 
 
 class Net(nn.Module):
@@ -91,6 +116,11 @@ class Net(nn.Module):
         self.end_to_end = args.end_to_end
         self.pretrained = args.pretrained
         self.classification_branch = args.clas
+        if self.classification_branch:
+            self.line_classification = Classification("line", size=(32, 64), channels_in=128, resize=resize)
+            self.horizon_estimation = Classification("horizon", size=(32, 64), channels_in=128, resize=resize)
+            # the heads' conv weights are re-packed by the ERFNet module's weight packer, as in the BP Net
+            self.net.__dict__["_pack_extra"] = (self.line_classification, self.horizon_estimation)
         if not args.no_cuda:
             self.M = self.M.cuda()
             self.idx_row = self.idx_row.cuda()
@@ -115,6 +145,9 @@ class Net(nn.Module):
             with torch.no_grad():
                 beta, _ = self.ls_layer.forward_all(masked, grid, status_out=status, max_order=2)
         else:
+            if self.classification_branch:
+                line = self.line_classification(shared_encoder)
+                horizon = self.horizon_estimation(shared_encoder)
             beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows, act=self.activation.kind,
                                                      want_masked=True, status_out=status, max_order=2)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)

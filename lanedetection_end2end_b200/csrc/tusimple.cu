@@ -26,6 +26,55 @@ namespace lf {
 constexpr int TS_WARPS = 8;
 constexpr int TS_MAXP = 4;      // predicted lanes (the reference's 4-lane --clas model)
 
+// LaneEval.bench of one row (eval_lane.py:27-57), called by a whole warp: one thread per (ground-truth lane, prediction)
+// pair counts the samples with |p' - g'| < thresh[g] (a negative value counts as -100; the difference and its absolute
+// value wrap as numpy's int64 do), then lane 0 forms (accuracy, fp, fn) with LaneEval's float64 operations in its order.
+// pred [P][S] (the warp's gated lanes), gx [g_n][gs] (the row's ground-truth columns, lane stride gs), th [g_n].
+template <typename T>
+__device__ void lane_eval_row(const T* pred, int P, int S, const int* __restrict__ gx, int gs, const double* __restrict__ th,
+                              int g_n, double* s_acc, int lane, double* r) {
+    const bool early = g_n + 2 < P;           // LaneEval's early return (0, 0, 1)
+    if (!early && lane < g_n * P) {
+        const int g = lane / P, p = lane - g * P;
+        const int* gl = gx + (size_t)g * gs;
+        const double t = th[g];
+        int cnt = 0;
+        for (int s = 0; s < S; ++s) {
+            const long long pv = pred[p * S + s] >= 0 ? (long long)pred[p * S + s] : -100;
+            const long long gv = gl[s] >= 0 ? gl[s] : -100;
+            const unsigned long long d = (unsigned long long)pv - (unsigned long long)gv;
+            const long long ad = (long long)((long long)d < 0 ? 0ull - d : d);
+            cnt += (double)ad < t ? 1 : 0;
+        }
+        s_acc[lane] = (double)cnt / (double)S;
+    }
+    __syncwarp();
+    if (lane == 0) {
+        if (early) {
+            r[0] = 0.0;
+            r[1] = 0.0;
+            r[2] = 1.0;
+        } else {
+            double sum = 0.0, mn = 0.0, fn = 0.0, matched = 0.0;
+            for (int g = 0; g < g_n; ++g) {
+                double m = s_acc[g * P];
+                for (int p = 1; p < P; ++p) m = s_acc[g * P + p] > m ? s_acc[g * P + p] : m;
+                if (m < 0.85) fn += 1.0;
+                else matched += 1.0;
+                sum += m;
+                mn = (g == 0 || m < mn) ? m : mn;
+            }
+            const double fp = (double)P - matched;
+            if (g_n > 4 && fn > 0.0) fn -= 1.0;
+            if (g_n > 4) sum -= mn;
+            const double den = fmax(fmin(4.0, (double)g_n), 1.0);
+            r[0] = sum / den;
+            r[1] = fp / (double)P;
+            r[2] = fn / den;
+        }
+    }
+}
+
 __global__ void __launch_bounds__(TS_WARPS * 32) tusimple_score_kernel(
     const double* __restrict__ x_cal, const float* __restrict__ line_pred, const int* __restrict__ horizon_pred, int B, int P,
     int S, const int* __restrict__ gt_x, const int* __restrict__ gt_lanes, const double* __restrict__ thresh, int N, int G,
@@ -65,51 +114,90 @@ __global__ void __launch_bounds__(TS_WARPS * 32) tusimple_score_kernel(
             s_pred[warp][i] = q;
         }
         __syncwarp();
-        // ---- LaneEval.bench: one thread per (ground-truth lane, prediction) pair
-        const int g_n = min(max(gt_lanes[row], 0), G);
-        const bool early = g_n + 2 < P;           // LaneEval's early return (0, 0, 1)
-        if (!early && lane < g_n * P) {
-            const int g = lane / P, p = lane - g * P;
-            const int* gx = gt_x + ((size_t)row * G + g) * S;
-            const double th = thresh[(size_t)row * G + g];
-            int cnt = 0;
-            for (int s = 0; s < S; ++s) {
-                const long long pv = s_pred[warp][p * S + s] >= 0 ? s_pred[warp][p * S + s] : -100;
-                const long long gv = gx[s] >= 0 ? gx[s] : -100;
-                cnt += (double)llabs(pv - gv) < th ? 1 : 0;
-            }
-            s_acc[warp][lane] = (double)cnt / (double)S;
-        }
-        __syncwarp();
-        if (lane == 0) {
-            double* r = per_image + (size_t)row * 3;
-            if (early) {
-                r[0] = 0.0;
-                r[1] = 0.0;
-                r[2] = 1.0;
-            } else {
-                double sum = 0.0, mn = 0.0, fn = 0.0, matched = 0.0;
-                for (int g = 0; g < g_n; ++g) {
-                    double m = s_acc[warp][g * P];
-                    for (int p = 1; p < P; ++p) m = s_acc[warp][g * P + p] > m ? s_acc[warp][g * P + p] : m;
-                    if (m < 0.85) fn += 1.0;
-                    else matched += 1.0;
-                    sum += m;
-                    mn = (g == 0 || m < mn) ? m : mn;
-                }
-                const double fp = (double)P - matched;
-                if (g_n > 4 && fn > 0.0) fn -= 1.0;
-                if (g_n > 4) sum -= mn;
-                const double den = fmax(fmin(4.0, (double)g_n), 1.0);
-                r[0] = sum / den;
-                r[1] = fp / (double)P;
-                r[2] = fn / den;
-            }
-        }
+        lane_eval_row(s_pred[warp], P, S, gt_x + (size_t)row * G * S, S, thresh + (size_t)row * G,
+                      min(max(gt_lanes[row], 0), G), s_acc[warp], lane, per_image + (size_t)row * 3);
         __syncwarp();
     }
     __syncthreads();
     if (threadIdx.x == 0) *pos = (int)(p0 + B);
+}
+
+struct BevWarp {
+    double m11, m12, m21, m22;                   // M: the rows that map a normalised y into the bird's-eye view
+    double i00, i01, i02, i20, i21, i22;         // M^-1: the rows that give x and the homogeneous w back in the image
+};
+
+// numpy's np.int_ of a rounded float64 on x86-64: NaN and values outside int64 become INT64_MIN
+__device__ __forceinline__ long long np_int64_rn(double v) {
+    return fabs(v) < 9223372036854775808.0 ? __double2ll_rn(v) : LLONG_MIN;
+}
+
+// The validation pass's lane sampling and score (BEV/main.py:445-488): write_lsq_results with all_branches_ready = False
+// and horizon_on = False, then LaneEval.bench, for the batch's validation rows.  One warp per image; image b's results go
+// to visit slot *pos + b (the caller advances *pos after the launch, so a captured graph can be replayed per batch).
+// Every float64 operation is the host formula's, in its order, as an explicit _rn intrinsic so that nothing contracts
+// into an FMA.
+__global__ void __launch_bounds__(TS_WARPS * 32) bev_lane_score_kernel(
+    const float* __restrict__ beta, const long long* __restrict__ rows, const int* __restrict__ status,
+    const long long* __restrict__ pos, int B, int no_ortho, const __grid_constant__ BevWarp Wp, const int* __restrict__ gt_S,
+    const int* __restrict__ h_samples, const int* __restrict__ gt_x, const int* __restrict__ gt_lanes,
+    const double* __restrict__ thresh, int N, int G, long long V, long long* __restrict__ lanes, double* __restrict__ per_row,
+    int* __restrict__ scored) {
+    pdl_entry();
+    constexpr int MS = LF_TUSIMPLE_MAX_S;
+    __shared__ long long s_pred[TS_WARPS][TS_MAXP * MS];
+    __shared__ double s_acc[TS_WARPS][LF_TUSIMPLE_MAX_GT * TS_MAXP];
+    __shared__ int s_lo[TS_WARPS][TS_MAXP], s_hi[TS_WARPS][TS_MAXP];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.x * TS_WARPS + warp;
+    if (b >= B) return;
+    const long long row = rows[b], slot = *pos + b;
+    if (row < 0 || row >= N || slot < 0 || slot >= V) return;
+    const int S = gt_S[row];
+    const int* hs = h_samples + (size_t)row * MS;
+    const int* gx = gt_x + (size_t)row * G * MS;
+    // the labelled rows of each lane: points from max(210, min y) to max y are kept; a lane without one stays -2
+    if (lane < TS_MAXP) {
+        int lo = INT_MAX, hi = INT_MIN;
+        for (int s = 0; s < S; ++s)
+            if (gx[(size_t)lane * MS + s] != -2) {
+                lo = min(lo, hs[s]);
+                hi = max(hi, hs[s]);
+            }
+        s_lo[warp][lane] = hi == INT_MIN ? 1 : max(210, lo);
+        s_hi[warp][lane] = hi == INT_MIN ? 0 : hi;
+    }
+    __syncwarp();
+    long long* out = lanes + (size_t)slot * TS_MAXP * MS;
+    for (int i = lane; i < TS_MAXP * S; i += 32) {
+        const int p = i / S, s = i - p * S;
+        const int y = hs[s];
+        long long q = -2;
+        if (s_lo[warp][p] <= y && y <= s_hi[warp][p]) {
+            const double a = beta[((size_t)b * TS_MAXP + p) * 3], bb = beta[((size_t)b * TS_MAXP + p) * 3 + 1],
+                         c = beta[((size_t)b * TS_MAXP + p) * 3 + 2];
+            const double yd = __ddiv_rn((double)(y - 80), 639.0);
+            double x;
+            if (no_ortho) {
+                const double u = __dadd_rn(1.0, -yd);
+                x = __dadd_rn(__dadd_rn(__dmul_rn(a, __dmul_rn(u, u)), __dmul_rn(bb, u)), c);
+            } else {
+                const double yp = __ddiv_rn(__dadd_rn(__dmul_rn(Wp.m11, yd), Wp.m12), __dadd_rn(__dmul_rn(Wp.m21, yd), Wp.m22));
+                const double ye = __dadd_rn(1.0, -yp);
+                const double xb = __dadd_rn(__dadd_rn(__dmul_rn(a, __dmul_rn(ye, ye)), __dmul_rn(bb, ye)), c);
+                const double tx = __dadd_rn(__dadd_rn(__dmul_rn(Wp.i00, xb), __dmul_rn(Wp.i01, yp)), Wp.i02);
+                const double tw = __dadd_rn(__dadd_rn(__dmul_rn(Wp.i20, xb), __dmul_rn(Wp.i21, yp)), Wp.i22);
+                x = __ddiv_rn(tx, tw);
+            }
+            q = np_int64_rn(__dmul_rn(x, 1279.0));
+        }
+        out[p * MS + s] = q;
+        s_pred[warp][p * S + s] = q;
+    }
+    __syncwarp();
+    lane_eval_row(s_pred[warp], TS_MAXP, S, gx, MS, thresh + (size_t)row * G, min(max(gt_lanes[row], 0), G), s_acc[warp],
+                  lane, per_row + (size_t)slot * 3);
+    if (lane == 0) scored[slot] = *status == 0 ? 1 : 0;
 }
 
 struct DrawParams {
@@ -199,5 +287,21 @@ extern "C" int lf_tusimple_score(const double* x_cal, const float* line_pred, co
     LF_REQUIRE(!line_pred || P == TS_MAXP);
     lf_launch(tusimple_score_kernel, 1, TS_WARPS * 32, 0, stream, x_cal, line_pred, horizon_pred, B, P, S, gt_x, gt_lanes, thresh,
               N, G, pos, lanes, per_image);
+    return check_launch();
+}
+
+extern "C" int lf_bev_lane_score(const float* beta, const long long* rows, const int* status, const long long* pos, int B,
+                                 int no_ortho, const double* warp, const int* gt_S, const int* h_samples, const int* gt_x,
+                                 const int* gt_lanes, const double* thresh, int N, int G, long long V, long long* lanes,
+                                 double* per_row, int* scored, lf_stream_t stream_) {
+    LF_REQUIRE(beta && rows && status && pos && warp && gt_S && h_samples && gt_x && gt_lanes && thresh && lanes && per_row &&
+               scored);
+    LF_REQUIRE(B > 0 && N > 0 && V > 0 && G >= TS_MAXP && G <= LF_TUSIMPLE_MAX_GT);
+    BevWarp Wp;
+    Wp.m11 = warp[4], Wp.m12 = warp[5], Wp.m21 = warp[7], Wp.m22 = warp[8];
+    Wp.i00 = warp[9], Wp.i01 = warp[10], Wp.i02 = warp[11], Wp.i20 = warp[15], Wp.i21 = warp[16], Wp.i22 = warp[17];
+    lf_launch(bev_lane_score_kernel, dim3((B + TS_WARPS - 1) / TS_WARPS), dim3(TS_WARPS * 32), 0,
+              reinterpret_cast<cudaStream_t>(stream_), beta, rows, status, pos, B, no_ortho, Wp, gt_S, h_samples, gt_x, gt_lanes,
+              thresh, N, G, V, lanes, per_row, scored);
     return check_launch();
 }

@@ -576,8 +576,9 @@ def _train_skip_epoch(loader, model, optimizer, criterion_seg):
 def check_bev_args(args):
     """The settings train_epoch_bev and inference.validate_bev run: ValueError naming the first one they do not."""
     from .Loss_crit import AREA_WEIGHTS
-    if args.clas:
-        raise ValueError("--clas is not supported: the bird's-eye-view Net builds no line-type or horizon heads")
+    if args.clas and (args.nclasses != 4 or not args.end_to_end):
+        raise ValueError("--clas needs 4 lanes and --end_to_end True (BEV/main.py:39-40; the heads run on the end-to-end "
+                         "branch only), got %d lanes with end_to_end %s" % (args.nclasses, bool(args.end_to_end)))
     if args.pretrained:
         raise ValueError("--pretrained is not supported: its segmentation phase and the switch to end-to-end change the "
                          "parameter set, which a FusedOptimizer refuses")
@@ -591,6 +592,13 @@ def check_bev_args(args):
     if not args.end_to_end and args.nclasses != 2:
         raise ValueError("--end_to_end False needs 2 lanes: the bird's-eye-view Net's segmentation branch fits two lane "
                          "maps")
+
+
+def clas_loss(loss, out, st, criterion_line_class, criterion_horizon, args):
+    """BEV/main.py:250-253 (and :429-431): the fit loss combined with the line-type and horizon heads' losses, float32."""
+    loss_horizon = criterion_horizon(out[8], st["gt_horizon"])
+    loss_line = criterion_line_class(out[7], st["gt_line"])
+    return loss * args.weight_fit + (loss_line + loss_horizon) * args.weight_class
 
 
 def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterion_line_class, criterion_horizon, args, epoch):
@@ -608,9 +616,12 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
     End-to-end, the loss is Loss_crit.fused_area_loss over the lanes (main.py:222-237; the 4-lane masks change nothing,
     see there): float64 terms rounded once, so it equals the reference's float32 sum to rounding.  --end_to_end False:
     criterion_seg(output, gt), and the 2-lane area without gradient as avg_area (main.py:239-244).  The exact-area metric
-    (main.py:272-280) comes from the same launch, per image bit-identical to the reference's CPU polynomial.  --clas,
-    --pretrained, loss policies other than area, orders other than 2 and other lane counts raise ValueError
-    (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch.  Dropout masks are drawn in the
+    (main.py:272-280) comes from the same launch, per image bit-identical to the reference's CPU polynomial.  With --clas
+    (4 lanes, end to end) the loss is ``loss * weight_fit + (loss_line + loss_horizon) * weight_class`` in float32, as
+    main.py:246-253 forms it before losses.update: criterion_line_class on the line head's [B, 3, 4] logits against the
+    loader's gt_line, criterion_horizon on the horizon head against gt_horizon.  --clas with other lane counts or
+    --end_to_end False, --pretrained, loss policies other than area, orders other than 2 and other lane counts raise
+    ValueError (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch.  Dropout masks are drawn in the
     graph; BatchNorm running statistics are those of the epoch's batches."""
     from .optim import FusedOptimizer
     from .Loss_crit import fused_area_loss
@@ -626,6 +637,8 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
     def loss_fn(out):
         if e2e:
             loss, static["exact"] = fused_area_loss(out[:L], static["params"], wf, exact=True)
+            if args.clas:
+                loss = clas_loss(loss, out, static, criterion_line_class, criterion_horizon, args)
             return loss
         with torch.no_grad():
             static["area"], static["exact"] = fused_area_loss(out[:2], static["params"], wf, exact=True)
@@ -654,7 +667,7 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
                                   p[:, 2, :], p[:, 3, :], batch[4], static["gt"], 0, i, static["input"], args.no_ortho,
                                   args.resize, args.save_path)
 
-    fields = lambda b: {"input": b[0], "gt": b[1], "params": b[2]}
+    fields = lambda b: {"input": b[0], "gt": b[1], "params": b[2], "gt_line": b[4], "gt_horizon": b[5]}
     if _train_replays(loader, model, optimizer, static, fields, {"input": torch.float32}, post, report, args.print_freq,
                       args.save_freq, loss_fn=loss_fn, end_to_end=e2e) is None:
         return 0, 0, 0

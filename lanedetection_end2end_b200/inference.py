@@ -237,15 +237,162 @@ class TuSimpleScorer:
         write_tusimple_predictions(json_file, self.rows, self.predictions(), 0)
 
 
-_SCORERS = {}           # (absolute path, device) -> (file stamp, TuSimpleScorer): one table build per ground-truth file
+class BevLaneScorer:
+    """The bird's-eye-view validation score on the GPU (BEV/main.py:445-488): write_lsq_results(..., all_branches_ready=False,
+    horizon_on=False) and LaneEval.bench_one_submit over the pass's validation rows.
+
+    Construction parses the validation rows (validation_set.json: a path or its parsed rows) once into ground-truth tables:
+    every row needs a unique raw_file, at most LF_TUSIMPLE_MAX_S h_samples (the TuSimple files hold 48 or 56), between 4 and
+    LF_TUSIMPLE_MAX_GT lanes of len(h_samples) int32 columns; each lane's threshold is lane_threshold's.  A pass is
+    ``begin(capacity, resize)``, one ``score`` per batch (one lf_bev_lane_score launch plus a few device copies, no
+    synchronisation, graph-capturable; the batch's results go to the next visit slots) and ``finish``: one device-to-host
+    copy, the two files written in visit order, [accuracy, fp, fn] as bench_one_submit returns them on those files."""
+
+    def __init__(self, gt_rows_or_path, device="cuda"):
+        import cv2
+        if isinstance(gt_rows_or_path, (str, bytes, os.PathLike)):
+            with open(gt_rows_or_path) as f:
+                rows = [json.loads(line) for line in f.readlines()]
+        else:
+            rows = list(gt_rows_or_path)
+        N, G, MS = len(rows), _capi.TUSIMPLE_MAX_GT, _capi.TUSIMPLE_MAX_S
+        if N == 0:
+            raise ValueError("the validation set has no rows")
+        gt_S = np.zeros(N, np.int32)
+        h_tab = np.zeros((N, MS), np.int32)
+        gt_x = np.full((N, G, MS), -2, np.int32)
+        gt_n = np.zeros(N, np.int32)
+        thresh = np.zeros((N, G), np.float64)
+        seen = set()
+        for i, row in enumerate(rows):
+            name = row.get("raw_file")
+            if name is None or "lanes" not in row or "h_samples" not in row:
+                raise ValueError("validation row %d lacks raw_file, lanes or h_samples" % i)
+            if name in seen:
+                raise ValueError("%s: duplicate raw_file in the validation set" % name)
+            seen.add(name)
+            h, lanes = row["h_samples"], row["lanes"]
+            if not 1 <= len(h) <= MS:
+                raise ValueError("%s: %d h_samples, the table holds 1 to %d" % (name, len(h), MS))
+            if not TUSIMPLE_LANES <= len(lanes) <= G:
+                raise ValueError("%s: %d lanes; write_lsq_results samples %d and the table holds %d"
+                                 % (name, len(lanes), TUSIMPLE_LANES, G))
+            h_arr = np.asarray(h)
+            if h_arr.dtype.kind not in "iu" or h_arr.min() < -2 ** 31 or h_arr.max() >= 2 ** 31:
+                raise ValueError("%s: h_samples that are not int32 rows" % name)
+            for j, lane in enumerate(lanes):
+                if len(lane) != len(h):
+                    raise ValueError("%s: lane %d has %d samples for %d h_samples" % (name, j, len(lane), len(h)))
+                arr = np.asarray(lane)
+                if arr.dtype.kind not in "iu" or arr.min() < -2 ** 31 or arr.max() >= 2 ** 31:
+                    raise ValueError("%s: lane %d holds values that are not int32 pixel columns" % (name, j))
+                gt_x[i, j, :len(h)] = arr
+                thresh[i, j] = lane_threshold(arr, h)
+            gt_S[i], gt_n[i] = len(h), len(lanes)
+            h_tab[i, :len(h)] = h_arr
+        src = np.float32([[0.45, 0.3], [0.55, 0.3], [0.1, 1], [0.9, 1]])
+        dst = np.float32([[0.45, 0.3], [0.55, 0.3], [0.45, 1], [0.55, 1]])
+        self.warp = np.ascontiguousarray(np.concatenate([cv2.getPerspectiveTransform(src, dst).reshape(-1),
+                                                         cv2.getPerspectiveTransform(dst, src).reshape(-1)]), np.float64)
+        dev = torch.device(device)
+        self.rows, self.N, self.device = rows, N, dev
+        t = lambda a: torch.from_numpy(a).to(dev)
+        self.gt_S, self.h_samples, self.gt_x, self.gt_lanes, self.thresh = t(gt_S), t(h_tab), t(gt_x), t(gt_n), t(thresh)
+        self.V = 0
+
+    def begin(self, capacity, resize):
+        """Start a pass of at most ``capacity`` visits whose horizon heads have ``resize`` rows.  One device buffer holds
+        every per-visit result, so that finish() is one copy."""
+        V, R, MS = max(1, int(capacity)), int(resize), _capi.TUSIMPLE_MAX_S
+        parts = [("per_row", torch.float64, (V, 3)), ("lanes", torch.int64, (V, TUSIMPLE_LANES, MS)),
+                 ("line_id", torch.int64, (V, TUSIMPLE_LANES)), ("row", torch.int64, (V,)), ("pos", torch.int64, (1,)),
+                 ("params", torch.float32, (V, TUSIMPLE_LANES, 3)), ("horizon", torch.float32, (V, R)),
+                 ("scored", torch.int32, (V,))]
+        sizes = [int(np.prod(shape)) * torch.empty(0, dtype=dt).element_size() for _, dt, shape in parts]
+        self._out = torch.zeros(sum(sizes), dtype=torch.uint8, device=self.device)
+        self._views = lambda buf: {name: buf[off - n:off].view(dt).view(shape) for (name, dt, shape), n, off
+                                   in zip(parts, sizes, np.cumsum(sizes).tolist())}
+        for name, t in self._views(self._out).items():
+            setattr(self, name, t)
+        self._slots = torch.arange(V, dtype=torch.int64, device=self.device)
+        self.V = V
+
+    def score(self, beta, line_id, horizon_est, rows, status, no_ortho):
+        """beta [B, 4, 3] f32 (the lanes' fitted coefficients), line_id [B, 4] int64 (argmax of the line head),
+        horizon_est [B, resize] f32 (rounded sigmoid of the horizon head), rows [B] int64 (validation rows), status: the
+        batch's LSQ status word (int32 [1]).  No synchronisation."""
+        B = beta.shape[0]
+        if tuple(beta.shape[1:]) != (TUSIMPLE_LANES, 3) or beta.dtype != torch.float32:
+            raise ValueError("beta must be float32 [B, 4, 3], got %s %s" % (beta.dtype, tuple(beta.shape)))
+        if rows.dtype != torch.int64 or tuple(rows.shape) != (B,):
+            raise ValueError("rows must be int64 [B], got %s %s" % (rows.dtype, tuple(rows.shape)))
+        _capi.require_cuda(beta, rows, status)
+        beta, rows = beta.contiguous(), rows.contiguous()
+        slots = self._slots[:B] + self.pos
+        self.params.index_copy_(0, slots, beta)
+        self.line_id.index_copy_(0, slots, line_id.to(torch.int64))
+        self.horizon.index_copy_(0, slots, horizon_est.to(torch.float32))
+        self.row.index_copy_(0, slots, rows)
+        p = _capi.ptr
+        _capi.call("lf_bev_lane_score", p(beta), p(rows), p(status), p(self.pos), B, int(bool(no_ortho)),
+                   self.warp.ctypes.data, p(self.gt_S), p(self.h_samples), p(self.gt_x), p(self.gt_lanes), p(self.thresh),
+                   self.N, _capi.TUSIMPLE_MAX_GT, self.V, p(self.lanes), p(self.per_row), p(self.scored),
+                   _capi.stream_ptr())
+        self.pos.add_(B)
+
+    def finish(self, dst_file=None, ls_file=None):
+        """[accuracy, fp, fn] of the pass's scored visits, summed in visit order as bench_one_submit sums the file
+        ``ls_file`` against ``dst_file``; those two files are written when given (BEV/main.py:456-467 and
+        write_lsq_results).  None when no visit was scored."""
+        h = self._views(self._out.cpu())
+        n = min(int(h["pos"][0]), self.V)
+        scored, rows, per_row, params, line_id, horizon, lanes = (
+            h[k][:n].tolist() for k in ("scored", "row", "per_row", "params", "line_id", "horizon", "lanes"))
+        bad = [r for r in rows if not 0 <= r < self.N]
+        if bad:
+            # the kernel leaves such a visit unscored; BEV/main.py:459 would raise at valid_set_labels[index[j]]
+            raise IndexError("validation row %d of a batch is outside the %d rows of the validation set: "
+                             "validation_set.json does not match the loader's validation split" % (bad[0], self.N))
+        dst = open(dst_file, "w") if dst_file else None
+        ls = open(ls_file, "w") if ls_file else None
+        try:
+            accuracy, fp, fn, names = 0., 0., 0., set()
+            for v in range(n):
+                if not scored[v]:
+                    continue
+                row = dict(self.rows[rows[v]])
+                row["params"], row["line_id"], row["horizon_est"] = params[v], line_id[v], horizon[v]
+                if dst:
+                    json.dump(row, dst)
+                    dst.write("\n")
+                if ls:
+                    row["run_time"] = 20
+                    row["lanes"] = [lane[:len(row["h_samples"])] for lane in lanes[v]]
+                    json.dump(row, ls)
+                    ls.write("\n")
+                a, p, f = per_row[v]
+                accuracy += a
+                fp += p
+                fn += f
+                names.add(self.rows[rows[v]]["raw_file"])
+        finally:
+            for f in (dst, ls):
+                if f:
+                    f.close()
+        if not names:
+            return None
+        return [accuracy / len(names), fp / len(names), fn / len(names)]
 
 
-def _scorer_for(gt_file, device):
+_SCORERS = {}           # (absolute path, device) -> (file stamp, scorer): one table build per ground-truth file
+
+
+def _scorer_for(gt_file, device, cls=TuSimpleScorer):
     st = os.stat(gt_file)
     key, stamp = (os.path.abspath(gt_file), str(device)), (st.st_mtime_ns, st.st_size)
     hit = _SCORERS.get(key)
-    if hit is None or hit[0] != stamp:
-        hit = _SCORERS[key] = (stamp, TuSimpleScorer(gt_file, device))
+    if hit is None or hit[0] != stamp or not isinstance(hit[1], cls):
+        hit = _SCORERS[key] = (stamp, cls(gt_file, device))
     return hit[1]
 
 
@@ -521,8 +668,8 @@ def validate(loader, model, criterion, criterion_seg, criterion_line_class, crit
 
 def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, criterion_horizon, M_inv, args, epoch=0):
     """The bird's-eye-view experiment's validation pass (Birds_Eye_View_Loss/main.py:362-501), same return value:
-    (losses.avg, avg_area.avg, avg_trapezium_rule.avg, acc_hor_tot.avg, acc_line_tot.avg), the accuracies 0 (--clas is
-    refused, engine.check_bev_args).
+    (losses.avg, avg_area.avg, avg_trapezium_rule.avg, acc_hor_tot.avg, acc_line_tot.avg), the accuracies 0 without
+    --clas.
 
     The loader yields the BEV valid loader's 7-tuples (input, gt, params, idx, gt_line, gt_horizon, index), on the device
     as bev.Dataloader.Load_Data_new gives them.  Each batch is one replay of a GraphedInference whose post= hook holds
@@ -530,26 +677,47 @@ def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, 
     criterion_seg and the 2-lane area, and the meter updates guarded by the LSQ status word: a batch with a singular system
     updates no meter, as main.py's `continue` does, and its line is printed at the end of the pass.  A batch shorter than
     the first is replayed by a second graph of its size.  The host synchronises only at the print_freq lines, at
-    save_weightmap('valid', ...) every 25 batches and at the end."""
+    save_weightmap('valid', ...) every 25 batches and at the end.
+
+    With --clas (4 lanes, end to end; engine.check_bev_args) each replay also holds main.py:417-431: the rounded-sigmoid
+    horizon accuracy over resize * batch_size and the argmax line accuracy over nclasses * batch_size (batch_size, not
+    val_batch_size, also for a short batch) into meters updated with n = 1, and the heads' losses in the loss
+    (engine.clas_loss).  It scores the set on the device (BevLaneScorer over args.save_path/validation_set.json, one table
+    build per file version): each replay samples and scores its images into the next visit slots.  At the end of the
+    pass validation_set_dst.json and ls_result.json are written to args.save_path with every image of a batch that was not
+    skipped, in visit order, and main.py's ACC_SEG line is printed with bench_one_submit's accuracy on those files.
+    main.py rewrites validation_set_dst.json for every batch, so its score covers the last batch only (NOTES.md)."""
     if __package__:
-        from .engine import DeviceMeters, check_bev_args, _valid_replays
+        from .engine import DeviceMeters, check_bev_args, clas_loss, _valid_replays
         from .Loss_crit import fused_area_loss
         from .Networks import utils as nutils
     else:
-        from engine import DeviceMeters, check_bev_args, _valid_replays
+        from engine import DeviceMeters, check_bev_args, clas_loss, _valid_replays
         from Loss_crit import fused_area_loss
         from Networks import utils as nutils
     check_bev_args(args)
-    e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
-    meters = DeviceMeters(("loss", "area", "exact"), next(model.parameters()).device)
+    e2e, L, wf, clas = bool(args.end_to_end), args.nclasses, args.weight_funct, bool(args.clas)
+    dev = next(model.parameters()).device
+    meters = DeviceMeters(("loss", "area", "exact", "acc_hor", "acc_line"), dev)
+    scorer = _scorer_for(os.path.join(args.save_path, "validation_set.json"), dev, BevLaneScorer) if clas else None
+    started = []
 
     def post(out, st):
         n = st["input"].shape[0]
+        if clas and not started:         # the first batch is the largest: every visit has a slot
+            scorer.begin(len(loader) * n, args.resize)
+            started.append(True)
         if e2e:
             loss, exact = fused_area_loss(out[:L], st["params"], wf, exact=True)
         else:
             loss = criterion_seg(out[6], st["gt"])
             area, exact = fused_area_loss(out[:2], st["params"], wf, exact=True)
+        if clas:
+            horizon_pred = torch.round(torch.nn.Sigmoid()(out[8]))
+            acc_hor = torch.sum(torch.eq(horizon_pred, st["gt_horizon"])).float() / (args.resize * args.batch_size)
+            _, line_pred = torch.max(out[7], 1)
+            acc_line = torch.sum(torch.eq(line_pred, st["gt_line"])).float() / (args.nclasses * args.batch_size)
+            loss = clas_loss(loss, out, st, criterion_line_class, criterion_horizon, args)
         if not torch.cuda.is_current_stream_capturing():
             return None                  # warm-up passes: no meter entry
         ok = model.lsq_status.reshape(()).eq(0)
@@ -557,6 +725,11 @@ def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, 
             meters.update("area", area, ok, n)
         meters.update("exact", exact, ok, n)
         meters.update("loss", loss, ok, n)
+        if clas:
+            meters.update("acc_hor", acc_hor, ok)
+            meters.update("acc_line", acc_line, ok)
+            scorer.score(torch.cat(out[:4], 2).transpose(1, 2), line_pred, horizon_pred, st["index"], model.lsq_status,
+                         args.no_ortho)
         return None
 
     def report(i, printing, saving, batch, g, st):
@@ -571,13 +744,23 @@ def validate_bev(loader, model, criterion, criterion_seg, criterion_line_class, 
                                   p[:, 3, :], batch[4], st["gt"], 0, i, st["input"], args.no_ortho, args.resize,
                                   args.save_path)
 
-    _valid_replays(loader, model, lambda b: {"input": b[0], "gt": b[1], "params": b[2]}, {"input": torch.float32}, post,
-                   report, args.print_freq, end_to_end=e2e)
+    fields = lambda b: dict({"input": b[0], "gt": b[1], "params": b[2]},
+                            **({"gt_line": b[4], "gt_horizon": b[5], "index": b[6]} if clas else {}))
+    casts = dict({"input": torch.float32}, **({"index": torch.int64} if clas else {}))
+    _valid_replays(loader, model, fields, casts, post, report, args.print_freq, end_to_end=e2e)
     m = meters.read()
+    if started:
+        acc_seg = scorer.finish(os.path.join(args.save_path, "validation_set_dst.json"),
+                                os.path.join(args.save_path, "ls_result.json"))
+        if acc_seg is not None:
+            print("===> Average ACC_SEG on val is {:.8}".format(acc_seg[0]))
     if args.evaluate:
-        crit_string = "AREA**2" if e2e else "ENTROPY"
+        crit_string = "TOT LOSS" if clas else "AREA**2" if e2e else "ENTROPY"
         print("===> Average {}-loss on validation set is {:.8}".format(crit_string, m["loss"][1]))
         print("===> Average exact area on validation set is {:.8}".format(m["exact"][1]))
         if not e2e:
             print("===> Average area**2 on validation set is {:.8}".format(m["area"][1]))
-    return m["loss"][1], m["area"][1], m["exact"][1], 0, 0
+        if clas:
+            print("===> Average HORIZON ACC on val is {:.8}".format(m["acc_hor"][1]))
+            print("===> Average LINE ACC on val is {:.8}".format(m["acc_hor"][1]))
+    return m["loss"][1], m["area"][1], m["exact"][1], m["acc_hor"][1], m["acc_line"][1]
