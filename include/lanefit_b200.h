@@ -145,6 +145,29 @@ int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab,
                const double* beta, const double* zinv, const double* gbeta,
                void* d_o, lf_stream_t stream);
 
+/* Per-pixel keep map (the reference's trapezium mask, --trapezium_mask): lf_lsq_fwd, lf_lsq_fwd_rowsums and lf_lsq_bwd
+ * with one more operand,
+ *   keep     [H,W] uint8, shared by every image and lane: where keep is 0 the activated map act(o) is replaced by
+ *            +0.0 before it is squared, so the pixel adds nothing to S_k, T_k (or the row sums), `masked` holds +0.0
+ *            there and d_o is +0.0 there (o is still read; NaN or Inf there changes no output bit).  Any nonzero
+ *            byte keeps the pixel.  Required (NULL is LF_ERR_INVALID_ARGUMENT); on the row-separable kernel it must
+ *            be 16-byte aligned like o.
+ * Rows [0, mask_rows) are handled as without the map.  The plan is lf_lsq_plan's for the same arguments: the map
+ * changes neither the kernel choice, the lanes per CTA nor the chunks.  An all-ones map gives the bits of the entry
+ * point without it for act = LF_ACT_SQUARE, for lf_lsq_bwd_keep and on the general kernel; the row-separable forward
+ * with a run-time activation may differ from them in the last bits of its fp32 row sums. */
+int lf_lsq_fwd_keep(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                    const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                    int solver, double* beta, double* zinv, float* masked, int* status, void* workspace,
+                    size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_fwd_rowsums_keep(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                            int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                            double* beta, double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                            size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_bwd_keep(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                    const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act,
+                    const double* beta, const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream);
+
 /* ========================================================================= *
  * ERFNet encoder/decoder building blocks (BP/Networks/ERFNet.py:11-176).
  * Feature maps are NHWC fp32: element (n,y,x,c) at ((n*H+y)*W+x)*cstride + coff + c.

@@ -8,6 +8,7 @@ the fused sm_90a kernels in csrc/lsq.cu through the C ABI.
   Weighted_least_squares  :72-154
   Classification          :157-207   (SURVEY.md 8f-2: on the library's kernels through ops_heads.py)
   Net                     :210-315
+  trapezium_keep          :236-246 (the column / corner masks the reference builds and leaves unused)
 """
 from math import ceil
 
@@ -78,6 +79,24 @@ def ProjectiveGridGenerator(size, theta, no_cuda):
     return g.expand(N, H * W, 2)
 
 
+def trapezium_keep(resize, zero_rows):
+    """--trapezium_mask: keep [resize, 2*resize] uint8, 0 on the rows < zero_rows, on the columns idx_col1 / idx_col2
+    and where idx_mask is nonzero, 1 elsewhere.  idx_col1 / idx_col2 / idx_mask are built with the reference
+    constructor's own expressions (BP/Networks/LSQ_layer.py:236-246, Birds_Eye_View_Loss/...:257-266), including the
+    truncation of linspace(1, 13, 14).long() to [1, 1, 2, .., 13]."""
+    n_row = 13
+    idx_col1 = torch.linspace(1, n_row, n_row + 1).long()
+    idx_col2 = torch.linspace(0, n_row, n_row + 1).long() + 2 * resize - (n_row + 1)
+    idx_mask = (np.arange(resize)[:, None] < np.arange(2 * resize) - (resize + 10)) * 1
+    idx_mask = np.flip(idx_mask, 1).copy() + idx_mask
+    keep = torch.ones(resize, 2 * resize, dtype=torch.uint8)
+    keep[:zero_rows] = 0
+    keep[:, idx_col1] = 0
+    keep[:, idx_col2] = 0
+    keep[torch.from_numpy(idx_mask) != 0] = 0
+    return keep
+
+
 class Weighted_least_squares(nn.Module):
     """beta_k = argmin sum_p (W_k,p (x_p - phi(y_p)^T beta))^2 per image and lane.
 
@@ -101,13 +120,14 @@ class Weighted_least_squares(nn.Module):
         self.y_const = y_const          # the reference hard-codes 255 (:94) whatever --resize is
         self.out_dtype = out_dtype
 
-    def forward_all(self, W, grid, mask_rows=0, act="none", want_masked=False, status_out=None, max_order=4):
+    def forward_all(self, W, grid, mask_rows=0, act="none", want_masked=False, status_out=None, max_order=4, keep=None):
+        """keep: optional bool / uint8 [H, W] map; act(W) is zeroed where it is 0 before the fit (ops_lsq.lsq)."""
         if self.order > max_order:
             raise NotImplementedError(
                 "Requested order {} for polynomial fit is not implemented".format(self.order))
         Wm = W.reshape(-1, self.nclasses, self.H, self.W)
         beta, masked = _ops.lsq(Wm, grid, self.order, self.y_const, mask_rows, act, self.reg_ls_value,
-                                self.use_cholesky, want_masked, status_out)
+                                self.use_cholesky, want_masked, status_out, keep)
         return beta, masked
 
     def _split(self, beta):
@@ -236,8 +256,13 @@ class Net(nn.Module):
                 raise ValueError("--learn_homography needs --loss_policy backproject (the loss that sees the warp), got %r"
                                  % (args.loss_policy,))
             self.homography = submodule("homography").LearnedHomography(resize, self.zero_rows)
+        # --trapezium_mask: the per-pixel keep map of the end-to-end fit (NOTES.md "Trapezium mask"); a plain attribute
+        # like idx_row, not a buffer, so checkpoints stay the reference's
+        self.keep = trapezium_keep(resize, self.zero_rows) if getattr(args, "trapezium_mask", False) else None
         if not args.no_cuda:
             self.idx_row = self.idx_row.cuda()
+            if self.keep is not None:
+                self.keep = self.keep.cuda()
         self.defer_status_check = False
         self.lsq_status = None
 
@@ -260,6 +285,9 @@ class Net(nn.Module):
         if grid.device != output.device:
             grid = self.grid = grid.to(output.device)
         grid = grid[:output.size(0)]
+        keep = self.keep
+        if keep is not None and keep.device != output.device:
+            keep = self.keep = keep.to(output.device)
 
         if not end_to_end:
             # segmentation pre-training branch (:279-293): argmax -> per-lane label maps,
@@ -291,24 +319,25 @@ class Net(nn.Module):
             if self.classification_branch:
                 line = self.line_classification(shared_encoder)
                 horizon = self.horizon_estimation(shared_encoder)
-            # activation (:295) + row mask (:301) + least squares (:314) in one launch;
+            # activation (:295) + row mask (:301) [+ the trapezium keep map] + least squares (:314) in one launch;
             # `masked` is materialised only because the API returns it (:315)
             if warp is not None:
-                beta, masked = self._lsq_warp(output, warp, self.zero_rows, self.activation.kind, True, st, status is None)
+                beta, masked = self._lsq_warp(output, warp, self.zero_rows, self.activation.kind, True, st, status is None,
+                                              keep)
             else:
                 beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows,
                                                          act=self.activation.kind, want_masked=True,
-                                                         status_out=status, max_order=3)
+                                                         status_out=status, max_order=3, keep=keep)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)
         return beta0, beta1, beta2, beta3, masked, output, line, horizon, output_seg
 
-    def _lsq_warp(self, W, warp, mask_rows, act, want_masked, status, check):
+    def _lsq_warp(self, W, warp, mask_rows, act, want_masked, status, check, keep=None):
         ls = self.ls_layer
         if ls.order > 3:
             raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(ls.order))
         Wm = W.reshape(-1, ls.nclasses, ls.H, ls.W)
         beta, masked = _ops.lsq_warp(Wm, warp, ls.order, mask_rows, act, ls.reg_ls_value, ls.use_cholesky, want_masked,
-                                     status)
+                                     status, keep)
         if check:
             # the status word holds the warp's guard as well as the solve's: one host read, as torch.inverse's raise
             st = int(status.item())

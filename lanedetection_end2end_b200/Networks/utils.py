@@ -89,6 +89,7 @@ _FLAGS = [
     ("--learn_homography", _B(False)),
     ("--seg_proxy", _B(False)),
     ("--weight_seg_proxy", dict(type=float, default=1.0)),
+    ("--trapezium_mask", _B(False)),
     ("--gamma", dict(type=float, default=0.0)),
     ("--clas", _B(False)),
     ("--cudnn", _B(True)),

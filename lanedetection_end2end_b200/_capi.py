@@ -243,6 +243,11 @@ _NET_PROTOS = {
     "lf_lsq_fwd_rowsums": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p, _p, _p,
                                 ctypes.c_size_t, _p]),
     "lf_lsq_grid_grad": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p]),
+    "lf_lsq_fwd_keep": (_i, [_p, _i, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p, _p,
+                             ctypes.c_size_t, _p]),
+    "lf_lsq_fwd_rowsums_keep": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p,
+                                     _p, _p, ctypes.c_size_t, _p]),
+    "lf_lsq_bwd_keep": (_i, [_p, _i, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
     "lf_homography_tables": (_i, [_p, _i, _i, ctypes.c_double, _p, _p, _p, _p, _p, _p, _p, _p]),
     "lf_homography_bwd": (_i, [_p, _i, _i, _p, _p, _p, _p, _p]),
     "lf_homography_host": (_i, [_p, _i, _p, _p, _p]),

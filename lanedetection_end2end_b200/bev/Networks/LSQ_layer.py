@@ -5,7 +5,8 @@ Differences from the BP variant (all served by the same fused kernel, csrc/lsq.c
     the grid is rebuilt by ``project_layer(M)`` every forward (:324);
   * ``y = 1 - y'`` (:109), orders 0..2 only (:110-118), beta returned as float32 (:167);
   * ``Net.forward(input, end_to_end)`` -> (beta0, beta1, beta2, beta3, masked, M, output, line, horizon) (:326); with
-    --clas the end-to-end forward runs the line-type head (line [B, 3, 4], its own tail) and the horizon head.
+    --clas the end-to-end forward runs the line-type head (line [B, 3, 4], its own tail) and the horizon head;
+  * --trapezium_mask: the end-to-end fit takes the BP Net's keep map (LSQ_layer.trapezium_keep).
 """
 from math import ceil
 
@@ -113,6 +114,8 @@ class Net(nn.Module):
                                                args.use_cholesky)
         self.zero_rows = ceil(resize * args.mask_percentage)
         self.idx_row = torch.linspace(0, self.zero_rows - 1, self.zero_rows).long()
+        # --trapezium_mask: the end-to-end fit's per-pixel keep map, as in the BP Net (plain attribute, not a buffer)
+        self.keep = _L.trapezium_keep(resize, self.zero_rows) if getattr(args, "trapezium_mask", False) else None
         self.end_to_end = args.end_to_end
         self.pretrained = args.pretrained
         self.classification_branch = args.clas
@@ -124,6 +127,8 @@ class Net(nn.Module):
         if not args.no_cuda:
             self.M = self.M.cuda()
             self.idx_row = self.idx_row.cuda()
+            if self.keep is not None:
+                self.keep = self.keep.cuda()
         self.defer_status_check = False
         self.lsq_status = None
 
@@ -148,7 +153,9 @@ class Net(nn.Module):
             if self.classification_branch:
                 line = self.line_classification(shared_encoder)
                 horizon = self.horizon_estimation(shared_encoder)
+            if self.keep is not None and self.keep.device != output.device:
+                self.keep = self.keep.to(output.device)
             beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows, act=self.activation.kind,
-                                                     want_masked=True, status_out=status, max_order=2)
+                                                     want_masked=True, status_out=status, max_order=2, keep=self.keep)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)
         return beta0, beta1, beta2, beta3, masked, self.M, output, line, horizon

@@ -13,6 +13,10 @@
 //    moment k"), which keeps the kernel far from the fp64 pipe limit.
 //  * x table reads (L2-resident, batch-invariant) are amortised over the lanes of an
 //    image: one CTA handles (row chunk, image, up to 4 lanes).
+//  * Per-pixel keep map (the *_keep entry points, KEEP template flag): an optional uint8 [H, W] map shared by every
+//    image and lane zeroes act(o) where it is 0, before the square -- the reference's trapezium mask.  Its 16-byte
+//    rows are read with the x table's (L2-resident); the KEEP = false instantiations compile to the same code as
+//    before the flag existed.
 //  * Cross-CTA reduction is deterministic: per-chunk partials in a workspace, the last
 //    CTA to arrive (ticket atomic) sums them in fixed order and one thread per system
 //    solves it in fp64 registers (LU with partial pivoting == torch.inverse, or
@@ -123,6 +127,30 @@ __device__ __forceinline__ void load_xv(const float* xrow, int cv, float (&x)[V]
         const float4 t = __ldg(reinterpret_cast<const float4*>(xrow) + cv * (V / 4) + q);
         x[4 * q] = t.x; x[4 * q + 1] = t.y; x[4 * q + 2] = t.z; x[4 * q + 3] = t.w;
     }
+}
+
+// keep bytes of V consecutive pixels (4 or 8 bytes, aligned with the map vector); byte e is pixel e
+template <int V>
+__device__ __forceinline__ void load_keepv(const uint8_t* krow, int cv, uint32_t (&k)[V / 4]) {
+    if constexpr (V == 8) {
+        const uint2 t = __ldg(reinterpret_cast<const uint2*>(krow) + cv);
+        k[0] = t.x;
+        k[1] = t.y;
+    } else {
+        k[0] = __ldg(reinterpret_cast<const unsigned int*>(krow) + cv);
+    }
+}
+template <int V>
+__device__ __forceinline__ bool kept(const uint32_t (&k)[V / 4], int e) {
+    return ((k[e >> 2] >> (8 * (e & 3))) & 0xffu) != 0u;
+}
+// v, or +0.0 where the pixel is masked: a bitwise AND in inline PTX, so the compiler cannot fold the mask into the
+// square and the row sums after it (whatever v holds at a masked pixel, NaN and Inf included, the result is +0.0).
+template <int V>
+__device__ __forceinline__ float keep_or_zero(const uint32_t (&k)[V / 4], int e, float v) {
+    uint32_t r;
+    asm("and.b32 %0, %1, %2;" : "=r"(r) : "r"(__float_as_uint(v)), "r"(kept<V>(k, e) ? 0xffffffffu : 0u));
+    return __uint_as_float(r);
 }
 
 template <bool BF16>
@@ -378,8 +406,10 @@ __device__ __forceinline__ int packed_holder(int i) {
 // ROWSUMS: also accumulate C_r = sum_c w c and store (A_r, B_r, C_r) of every unmasked row in rowsums [B][L][H][3] --
 // what the gradient with respect to a learned homography's tables needs (lsq_grid_grad_kernel).  `rowsums` is a kernel
 // parameter of its own, not an LsqArgs field, so the other kernels' argument block stays as it was.
-template <int ACT_T, bool BF16, int NL, bool ROWSUMS>
-__device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* rowsums) {
+// KEEP: act(o) is zeroed where keep [H][W] (uint8, a kernel parameter of its own like rowsums) is 0, so w, the
+// moments, the row sums and `masked` see a zero there.
+template <int ACT_T, bool BF16, int NL, bool ROWSUMS, bool KEEP>
+__device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* rowsums, const uint8_t* keep) {
     pdl_entry();
     __shared__ double red[LSQ_WARPS][LSQ_MAXL][LSQ_MAXNM];
     __shared__ double mom[LSQ_MAXL][LSQ_MAXNM];
@@ -437,6 +467,8 @@ __device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* row
             for (int u = 0; u < RU; ++u) {
                 float x[V];
                 load_xv<V>(a.xtab + rowoff[u], cv, x);
+                uint32_t kw[V / 4];
+                if constexpr (KEEP) load_keepv<V>(keep + rowoff[u], cv, kw);
 #pragma unroll
                 for (int l = 0; l < NL; ++l) {
                     const size_t off = map_base[l] + rowoff[u] + (size_t)V * cv;
@@ -448,6 +480,7 @@ __device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* row
 #pragma unroll
                     for (int e = 0; e < V; ++e) {
                         o[e] = act_fn<ACT_T>(o[e], a.act);
+                        if constexpr (KEEP) o[e] = keep_or_zero<V>(kw, e, o[e]);
                         const float w = o[e] * o[e];
                         sa += w;
                         sb = fmaf(w, x[e], sb);
@@ -512,12 +545,25 @@ __device__ __forceinline__ void lsq_fwd_rowsep_body(const LsqArgs& a, float* row
 
 template <int ACT_T, bool BF16, int NL>
 __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_kernel(const LsqArgs a) {
-    lsq_fwd_rowsep_body<ACT_T, BF16, NL, false>(a, nullptr);
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, false, false>(a, nullptr, nullptr);
 }
 
 template <int ACT_T, bool BF16, int NL>
 __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsums_kernel(const LsqArgs a, float* rowsums) {
-    lsq_fwd_rowsep_body<ACT_T, BF16, NL, true>(a, rowsums);
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, true, false>(a, rowsums, nullptr);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_keep_kernel(const LsqArgs a,
+                                                                                               const uint8_t* keep) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, false, true>(a, nullptr, keep);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsums_keep_kernel(const LsqArgs a,
+                                                                                                float* rowsums,
+                                                                                                const uint8_t* keep) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, true, true>(a, rowsums, keep);
 }
 
 // ---------------------------------------------------------------------------------
@@ -580,8 +626,8 @@ __global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const flo
 // Forward, general grid (y varies inside a row): per-pixel fp64 accumulation of all
 // 3d+2 moments.  grid = (nchunks, B, L), one lane per CTA.  Slow path, any W.
 // ---------------------------------------------------------------------------------
-template <int ACT_T, bool BF16>
-__global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_kernel(const LsqArgs a) {
+template <int ACT_T, bool BF16, bool KEEP>
+__device__ __forceinline__ void lsq_fwd_general_body(const LsqArgs& a, const uint8_t* keep) {
     pdl_entry();
     __shared__ double red[LSQ_WARPS][LSQ_MAXL][LSQ_MAXNM];
     __shared__ double mom[LSQ_MAXL][LSQ_MAXNM];
@@ -600,7 +646,8 @@ __global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_kernel(const LsqA
         for (size_t p = (size_t)m_begin * a.W + threadIdx.x; p < (size_t)m_end * a.W; p += LSQ_THREADS) a.masked[map_off + p] = 0.f;
     const size_t p_begin = (size_t)r_begin * a.W, p_end = (size_t)r_end * a.W;
     for (size_t p = p_begin + threadIdx.x; p < p_end; p += LSQ_THREADS) {
-        const float v = act_fn<ACT_T>(load_map1<BF16>(a.o, map_off + p), a.act);
+        float v = act_fn<ACT_T>(load_map1<BF16>(a.o, map_off + p), a.act);
+        if constexpr (KEEP) v = __ldg(keep + p) ? v : 0.f;
         if (a.masked) a.masked[map_off + p] = v;
         const double w = (double)(v * v);
         const double y = (double)__ldg(a.ytab + p);
@@ -626,6 +673,16 @@ __global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_kernel(const LsqA
     lsq_chunk_tail(a, red, mom, chunk, b, l, l, 1);
 }
 
+template <int ACT_T, bool BF16>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_kernel(const LsqArgs a) {
+    lsq_fwd_general_body<ACT_T, BF16, false>(a, nullptr);
+}
+
+template <int ACT_T, bool BF16>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_keep_kernel(const LsqArgs a, const uint8_t* keep) {
+    lsq_fwd_general_body<ACT_T, BF16, true>(a, keep);
+}
+
 // ---------------------------------------------------------------------------------
 // Backward.  d_o = m * a'(o) * 2 a(o) * (x - phi^T beta) * (phi^T z),  z = Z^-1 g.
 // ---------------------------------------------------------------------------------
@@ -646,8 +703,8 @@ __device__ __forceinline__ void lsq_bwd_load_coeffs(const LsqArgs& a, int b, int
     __syncthreads();
 }
 
-template <int ACT_T, bool BF16, int NL>
-__global__ void __launch_bounds__(LSQ_THREADS, 4) lsq_bwd_rowsep_kernel(const LsqArgs a) {
+template <int ACT_T, bool BF16, int NL, bool KEEP>
+__device__ __forceinline__ void lsq_bwd_rowsep_body(const LsqArgs& a, const uint8_t* keep) {
     pdl_entry();
     __shared__ double bs[LSQ_MAXL][LF_MAX_ORDER + 1], zs[LSQ_MAXL][LF_MAX_ORDER + 1];
     const int chunk = blockIdx.x, b = blockIdx.y, lg = blockIdx.z;
@@ -692,6 +749,8 @@ __global__ void __launch_bounds__(LSQ_THREADS, 4) lsq_bwd_rowsep_kernel(const Ls
         for (int cv = lane; cv < WV; cv += 32) {
             float x[V];
             load_xv<V>(a.xtab + rowoff, cv, x);
+            uint32_t kw[V / 4];
+            if constexpr (KEEP) load_keepv<V>(keep + rowoff, cv, kw);
 #pragma unroll
             for (int l = 0; l < NL; ++l) {
                 // unconditional load from a clamped lane (see the forward kernel); only the store is predicated
@@ -713,14 +772,29 @@ __global__ void __launch_bounds__(LSQ_THREADS, 4) lsq_bwd_rowsep_kernel(const Ls
                     for (int e = 0; e < V; ++e)
                         g[e] = dact_times_act<ACT_T>(o[e], a.act) * (((x[e] - qh[l]) - ql[l]) * sf[l]);
                 }
+                if constexpr (KEEP) {
+#pragma unroll
+                    for (int e = 0; e < V; ++e) g[e] = kept<V>(kw, e) ? g[e] : 0.f;
+                }
                 if (l < nl) store_mapv<BF16>(a.d_o, off, g);
             }
         }
     }
 }
 
-template <int ACT_T, bool BF16>
-__global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_kernel(const LsqArgs a) {
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_kernel(const LsqArgs a) {
+    lsq_bwd_rowsep_body<ACT_T, BF16, NL, false>(a, nullptr);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_keep_kernel(const LsqArgs a,
+                                                                                               const uint8_t* keep) {
+    lsq_bwd_rowsep_body<ACT_T, BF16, NL, true>(a, keep);
+}
+
+template <int ACT_T, bool BF16, bool KEEP>
+__device__ __forceinline__ void lsq_bwd_general_body(const LsqArgs& a, const uint8_t* keep) {
     pdl_entry();
     __shared__ double bs[LSQ_MAXL][LF_MAX_ORDER + 1], zs[LSQ_MAXL][LF_MAX_ORDER + 1];
     const int chunk = blockIdx.x, b = blockIdx.y, l = blockIdx.z;
@@ -740,9 +814,20 @@ __global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_kernel(const LsqA
             q = fma(q, y, bs[0][i]);
             s = fma(s, y, zs[0][i]);
         }
-        const float g = (float)((double)dact_times_act<ACT_T>(o, a.act) * ((double)__ldg(a.xtab + p) - q) * s);
+        float g = (float)((double)dact_times_act<ACT_T>(o, a.act) * ((double)__ldg(a.xtab + p) - q) * s);
+        if constexpr (KEEP) g = __ldg(keep + p) ? g : 0.f;
         store_map1<BF16>(a.d_o, map_off + p, g);
     }
+}
+
+template <int ACT_T, bool BF16>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_kernel(const LsqArgs a) {
+    lsq_bwd_general_body<ACT_T, BF16, false>(a, nullptr);
+}
+
+template <int ACT_T, bool BF16>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_keep_kernel(const LsqArgs a, const uint8_t* keep) {
+    lsq_bwd_general_body<ACT_T, BF16, true>(a, keep);
 }
 
 // Chunks per system (image x lane group).  Every chunk gets an equal share of the unmasked rows (and of the masked
@@ -837,58 +922,59 @@ extern "C" size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order) 
     return LSQ_TICKET_BYTES + (size_t)B * L * nchunks * (3 * order + 2) * sizeof(double);
 }
 
-#define LSQ_DISPATCH(KERNEL, grid, args)                                                   \
-    do {                                                                                   \
-        if (args.act == LF_ACT_SQUARE) {                                                   \
-            if (o_dtype == LF_BF16)                                                        \
-                lf_launch(KERNEL<LF_ACT_SQUARE, true>, grid, LSQ_THREADS, 0, stream, args);       \
-            else                                                                           \
-                lf_launch(KERNEL<LF_ACT_SQUARE, false>, grid, LSQ_THREADS, 0, stream, args);      \
-        } else {                                                                           \
-            if (o_dtype == LF_BF16)                                                        \
-                lf_launch(KERNEL<LSQ_ACT_RUNTIME, true>, grid, LSQ_THREADS, 0, stream, args);     \
-            else                                                                           \
-                lf_launch(KERNEL<LSQ_ACT_RUNTIME, false>, grid, LSQ_THREADS, 0, stream, args);    \
-        }                                                                                  \
+// Launch KERNEL<activation template, bf16 map[, NL]> with the kernel arguments that follow `grid` (LsqArgs `a` first).
+#define LSQ_DISPATCH(KERNEL, grid, ...)                                                            \
+    do {                                                                                           \
+        if (a.act == LF_ACT_SQUARE) {                                                              \
+            if (o_dtype == LF_BF16)                                                                \
+                lf_launch(KERNEL<LF_ACT_SQUARE, true>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);    \
+            else                                                                                   \
+                lf_launch(KERNEL<LF_ACT_SQUARE, false>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);   \
+        } else {                                                                                   \
+            if (o_dtype == LF_BF16)                                                                \
+                lf_launch(KERNEL<LSQ_ACT_RUNTIME, true>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);  \
+            else                                                                                   \
+                lf_launch(KERNEL<LSQ_ACT_RUNTIME, false>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__); \
+        }                                                                                          \
     } while (0)
 
-#define LSQ_DISPATCH_NL2(KERNEL, NL, grid, args)                                               \
-    do {                                                                                       \
-        if (args.act == LF_ACT_SQUARE) {                                                       \
-            if (o_dtype == LF_BF16)                                                            \
-                lf_launch(KERNEL<LF_ACT_SQUARE, true, NL>, grid, LSQ_THREADS, 0, stream, args);       \
-            else                                                                               \
-                lf_launch(KERNEL<LF_ACT_SQUARE, false, NL>, grid, LSQ_THREADS, 0, stream, args);      \
-        } else {                                                                               \
-            if (o_dtype == LF_BF16)                                                            \
-                lf_launch(KERNEL<LSQ_ACT_RUNTIME, true, NL>, grid, LSQ_THREADS, 0, stream, args);     \
-            else                                                                               \
-                lf_launch(KERNEL<LSQ_ACT_RUNTIME, false, NL>, grid, LSQ_THREADS, 0, stream, args);    \
-        }                                                                                      \
+#define LSQ_DISPATCH_NL2(KERNEL, NL, grid, ...)                                                        \
+    do {                                                                                               \
+        if (a.act == LF_ACT_SQUARE) {                                                                  \
+            if (o_dtype == LF_BF16)                                                                    \
+                lf_launch(KERNEL<LF_ACT_SQUARE, true, NL>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);    \
+            else                                                                                       \
+                lf_launch(KERNEL<LF_ACT_SQUARE, false, NL>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);   \
+        } else {                                                                                       \
+            if (o_dtype == LF_BF16)                                                                    \
+                lf_launch(KERNEL<LSQ_ACT_RUNTIME, true, NL>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__);  \
+            else                                                                                       \
+                lf_launch(KERNEL<LSQ_ACT_RUNTIME, false, NL>, grid, LSQ_THREADS, 0, stream, __VA_ARGS__); \
+        }                                                                                              \
     } while (0)
 
-#define LSQ_DISPATCH_NL(KERNEL, nlg, grid, args)                       \
-    do {                                                               \
-        switch (nlg) {                                                 \
-            case 1: LSQ_DISPATCH_NL2(KERNEL, 1, grid, args); break;    \
-            case 2: LSQ_DISPATCH_NL2(KERNEL, 2, grid, args); break;    \
-            case 3: LSQ_DISPATCH_NL2(KERNEL, 3, grid, args); break;    \
-            default: LSQ_DISPATCH_NL2(KERNEL, 4, grid, args); break;   \
-        }                                                              \
+#define LSQ_DISPATCH_NL(KERNEL, nlg, grid, ...)                               \
+    do {                                                                      \
+        switch (nlg) {                                                        \
+            case 1: LSQ_DISPATCH_NL2(KERNEL, 1, grid, __VA_ARGS__); break;    \
+            case 2: LSQ_DISPATCH_NL2(KERNEL, 2, grid, __VA_ARGS__); break;    \
+            case 3: LSQ_DISPATCH_NL2(KERNEL, 3, grid, __VA_ARGS__); break;    \
+            default: LSQ_DISPATCH_NL2(KERNEL, 4, grid, __VA_ARGS__); break;   \
+        }                                                                     \
     } while (0)
 
-extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
-                          int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
-                          double* beta, double* zinv, float* masked, int* status, void* workspace,
-                          size_t workspace_bytes, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// lf_lsq_fwd and lf_lsq_fwd_keep (keep = NULL: the KEEP = false kernels, exactly as before the keep map existed)
+static int lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                   const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                   int solver, double* beta, double* zinv, float* masked, int* status, void* workspace,
+                   size_t workspace_bytes, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && status && workspace);
     LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
     LsqPlan p{};
     const int rc = lsq_plan(0, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
     if (rc != LF_OK) return rc;
     if (workspace_bytes < lf_lsq_workspace_bytes(B, L, H, W, order)) return LF_ERR_WORKSPACE_TOO_SMALL;
-    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked));
+    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked) && aligned16(keep));
     LsqArgs a{};
     a.o = o; a.xtab = xtab; a.ytab = ytab; a.yrow = yrow;
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
@@ -898,37 +984,68 @@ extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const f
     a.tickets = reinterpret_cast<int*>(workspace);
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
     dim3 grid(a.nchunks, B, p.groups);
-    if (p.rowsep)
-        LSQ_DISPATCH_NL(lsq_fwd_rowsep_kernel, p.nl, grid, a);
-    else
-        LSQ_DISPATCH(lsq_fwd_general_kernel, grid, a);
+    if (p.rowsep) {
+        if (keep)
+            LSQ_DISPATCH_NL(lsq_fwd_rowsep_keep_kernel, p.nl, grid, a, keep);
+        else
+            LSQ_DISPATCH_NL(lsq_fwd_rowsep_kernel, p.nl, grid, a);
+    } else {
+        if (keep)
+            LSQ_DISPATCH(lsq_fwd_general_keep_kernel, grid, a, keep);
+        else
+            LSQ_DISPATCH(lsq_fwd_general_kernel, grid, a);
+    }
     return check_launch();
 }
 
+extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
+                          int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                          double* beta, double* zinv, float* masked, int* status, void* workspace,
+                          size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                   masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_keep(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                               const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act,
+                               double reg_ls, int solver, double* beta, double* zinv, float* masked, int* status,
+                               void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                   masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+template <int ACT_T, bool BF16, int NL>
+static void launch_rowsums_nl(dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums, const uint8_t* keep) {
+    if (keep)
+        lf_launch(lsq_fwd_rowsums_keep_kernel<ACT_T, BF16, NL>, grid, LSQ_THREADS, 0, stream, a, rowsums, keep);
+    else
+        lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, NL>, grid, LSQ_THREADS, 0, stream, a, rowsums);
+}
+
 template <int ACT_T, bool BF16>
-static void launch_rowsums(int nl, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums) {
+static void launch_rowsums(int nl, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums, const uint8_t* keep) {
     switch (nl) {
-        case 1: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 1>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
-        case 2: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 2>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
-        case 3: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 3>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
-        default: lf_launch(lsq_fwd_rowsums_kernel<ACT_T, BF16, 4>, grid, LSQ_THREADS, 0, stream, a, rowsums); break;
+        case 1: launch_rowsums_nl<ACT_T, BF16, 1>(grid, stream, a, rowsums, keep); break;
+        case 2: launch_rowsums_nl<ACT_T, BF16, 2>(grid, stream, a, rowsums, keep); break;
+        case 3: launch_rowsums_nl<ACT_T, BF16, 3>(grid, stream, a, rowsums, keep); break;
+        default: launch_rowsums_nl<ACT_T, BF16, 4>(grid, stream, a, rowsums, keep); break;
     }
 }
 
 // lf_lsq_fwd on the row-separable kernel that also stores the row sums: same arguments and plan, yrow required,
-// rowsums [B][L][H][3] float32 (rows >= mask_rows written).
-extern "C" int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L, int H,
-                                  int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
-                                  double* zinv, float* masked, int* status, float* rowsums, void* workspace,
-                                  size_t workspace_bytes, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// rowsums [B][L][H][3] float32 (rows >= mask_rows written).  keep as in lsq_fwd.
+static int lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
+                           int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                           double* beta, double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                           size_t workspace_bytes, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && yrow && beta && zinv && status && rowsums && workspace);
     LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
     LsqPlan p{};
     const int rc = lsq_plan(0, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
     if (rc != LF_OK) return rc;
     if (workspace_bytes < lf_lsq_workspace_bytes(B, L, H, W, order)) return LF_ERR_WORKSPACE_TOO_SMALL;
-    LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked));
+    LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked) && aligned16(keep));
     LsqArgs a{};
     a.o = o; a.xtab = xtab; a.yrow = yrow;
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
@@ -938,12 +1055,30 @@ extern "C" int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab,
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
     dim3 grid(a.nchunks, B, p.groups);
     if (act == LF_ACT_SQUARE)
-        o_dtype == LF_BF16 ? launch_rowsums<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums)
-                           : launch_rowsums<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums);
+        o_dtype == LF_BF16 ? launch_rowsums<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums, keep)
+                           : launch_rowsums<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums, keep);
     else
-        o_dtype == LF_BF16 ? launch_rowsums<LSQ_ACT_RUNTIME, true>(p.nl, grid, stream, a, rowsums)
-                           : launch_rowsums<LSQ_ACT_RUNTIME, false>(p.nl, grid, stream, a, rowsums);
+        o_dtype == LF_BF16 ? launch_rowsums<LSQ_ACT_RUNTIME, true>(p.nl, grid, stream, a, rowsums, keep)
+                           : launch_rowsums<LSQ_ACT_RUNTIME, false>(p.nl, grid, stream, a, rowsums, keep);
     return check_launch();
+}
+
+extern "C" int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L, int H,
+                                  int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
+                                  double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                                  size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, nullptr, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                           masked, status, rowsums, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_rowsums_keep(const void* o, int o_dtype, const float* xtab, const float* yrow,
+                                       const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows,
+                                       int act, double reg_ls, int solver, double* beta, double* zinv, float* masked,
+                                       int* status, float* rowsums, void* workspace, size_t workspace_bytes,
+                                       lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, keep, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                           masked, status, rowsums, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int lf_lsq_grid_grad(const float* rowsums, const float* yrow, const double* beta, const double* zinv,
@@ -957,15 +1092,15 @@ extern "C" int lf_lsq_grid_grad(const float* rowsums, const float* yrow, const d
     return check_launch();
 }
 
-extern "C" int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
-                          int L, int H, int W, int order, int mask_rows, int act, const double* beta,
-                          const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// lf_lsq_bwd and lf_lsq_bwd_keep (keep = NULL: the KEEP = false kernels)
+static int lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                   const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act, const double* beta,
+                   const double* zinv, const double* gbeta, void* d_o, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && gbeta && d_o);
     LsqPlan p{};
     const int rc = lsq_plan(1, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
     if (rc != LF_OK) return rc;
-    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(d_o));
+    if (p.rowsep) LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(d_o) && aligned16(keep));
     LsqArgs a{};
     a.o = o; a.xtab = xtab; a.ytab = ytab; a.yrow = yrow;
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act;
@@ -973,9 +1108,32 @@ extern "C" int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const f
     a.nchunks = p.nchunks;
     a.rows_per_cta = 0;
     dim3 grid(a.nchunks, B, p.groups);
-    if (p.rowsep)
-        LSQ_DISPATCH_NL(lsq_bwd_rowsep_kernel, p.nl, grid, a);
-    else
-        LSQ_DISPATCH(lsq_bwd_general_kernel, grid, a);
+    if (p.rowsep) {
+        if (keep)
+            LSQ_DISPATCH_NL(lsq_bwd_rowsep_keep_kernel, p.nl, grid, a, keep);
+        else
+            LSQ_DISPATCH_NL(lsq_bwd_rowsep_kernel, p.nl, grid, a);
+    } else {
+        if (keep)
+            LSQ_DISPATCH(lsq_bwd_general_keep_kernel, grid, a, keep);
+        else
+            LSQ_DISPATCH(lsq_bwd_general_kernel, grid, a);
+    }
     return check_launch();
+}
+
+extern "C" int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
+                          int L, int H, int W, int order, int mask_rows, int act, const double* beta,
+                          const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                   reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_bwd_keep(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                               const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act,
+                               const double* beta, const double* zinv, const double* gbeta, void* d_o,
+                               lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                   reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -1,6 +1,6 @@
 """Host side of the fused weighted least-squares layer: grid tables, workspace
 and the ``torch.autograd.Function`` that calls ``lf_lsq_fwd`` / ``lf_lsq_bwd``
-(include/lanefit_b200.h).  Torch is plumbing here (device memory, streams,
+(include/lanefit_b200.h), or their ``*_keep`` variants when a per-pixel keep map is given.  Torch is plumbing here (device memory, streams,
 autograd graph); all arithmetic on the maps happens in csrc/lsq.cu.
 """
 import torch
@@ -64,6 +64,22 @@ def _workspace(device, nbytes):
     return ws
 
 
+def keep_map(keep, H, W, device):
+    """A per-pixel keep map as the ``*_keep`` kernels read it: uint8 [H, W], contiguous, on ``device``; any nonzero
+    byte keeps the pixel.  Accepts a bool or uint8 [H, W] tensor on that device (a bool map is viewed, not copied);
+    None stays None (no map: the plain entry points)."""
+    if keep is None:
+        return None
+    if not isinstance(keep, torch.Tensor) or keep.dtype not in (torch.bool, torch.uint8) or tuple(keep.shape) != (H, W):
+        raise ValueError("keep must be a bool or uint8 tensor of shape [%d, %d]; got %s" % (
+            H, W, "%s %s" % (tuple(keep.shape), keep.dtype) if isinstance(keep, torch.Tensor) else type(keep).__name__))
+    if keep.device != torch.device(device):
+        raise ValueError("keep is on %s but the maps are on %s" % (keep.device, device))
+    if keep.dtype == torch.bool:
+        keep = keep.view(torch.uint8)
+    return keep.contiguous()
+
+
 def status_message(st):
     parts = []
     if st & _capi.STATUS_SINGULAR:
@@ -79,9 +95,9 @@ class LsqFunction(torch.autograd.Function):
     """beta, masked = LSQ(o).  o: [B,L,H,W] f32/bf16 raw (or pre-activated) maps."""
 
     @staticmethod
-    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out, rowp=None):
+    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out, rowp=None, keep=None):
         # rowp: a learned warp's (alpha, gamma, y') per row (homography.WarpTables.rowp); the forward then also keeps the
-        # row sums and the backward returns dL/drowp
+        # row sums and the backward returns dL/drowp.  keep: uint8 [H, W] from keep_map, or None
         _capi.require_cuda(o)
         if order < 0 or order > _capi.MAX_ORDER:
             raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(order))
@@ -99,19 +115,22 @@ class LsqFunction(torch.autograd.Function):
         ws = _workspace(dev, nbytes)
         esz = o.element_size()
         rowsums = None
-        if rowp is not None and ctx.needs_input_grad[-1]:
+        # with a keep map the *_keep entry points take it right after the tables
+        kp = () if keep is None else (_capi.ptr(keep),)
+        sfx = "" if keep is None else "_keep"
+        if rowp is not None and ctx.needs_input_grad[9]:
             rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
-                _capi.call("lf_lsq_fwd_rowsums", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
-                           _capi.ptr(tables.yrow), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                _capi.call("lf_lsq_fwd_rowsums" + sfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.yrow), *kp, B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
                            _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status), _capi.ptr(rowsums),
                            _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
                            nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
         else:
             # the fixed warp, or a learned warp without a gradient (validation, test scoring): no row sums
             with torch.cuda.device(dev):
-                _capi.call("lf_lsq_fwd", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab), _capi.ptr(tables.ytab),
-                           _capi.ptr(tables.yrow), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                _capi.call("lf_lsq_fwd" + sfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.ytab), _capi.ptr(tables.yrow), *kp, B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
                            _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status),
                            _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
                            nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
@@ -121,7 +140,7 @@ class LsqFunction(torch.autograd.Function):
             st = int(status.item())
             if st:
                 raise RuntimeError(status_message(st))
-        ctx.save_for_backward(o, beta, zinv, rowsums)
+        ctx.save_for_backward(o, beta, zinv, rowsums, keep)
         ctx.tables = tables
         ctx.cfg = (order, mask_rows, act)
         if masked is not None:
@@ -131,15 +150,16 @@ class LsqFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gbeta, _gmasked):
-        o, beta, zinv, rowsums = ctx.saved_tensors
+        o, beta, zinv, rowsums, keep = ctx.saved_tensors
         order, mask_rows, act = ctx.cfg
         t = ctx.tables
         B, L, H, W = o.shape
         gbeta = gbeta.to(torch.float64).contiguous()
         d_o = torch.empty_like(o)
         with torch.cuda.device(o.device):
-            _capi.call("lf_lsq_bwd", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(t.xtab), _capi.ptr(t.ytab),
-                       _capi.ptr(t.yrow), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
+            _capi.call("lf_lsq_bwd" + ("" if keep is None else "_keep"), _capi.ptr(o), _capi.dtype_id(o),
+                       _capi.ptr(t.xtab), _capi.ptr(t.ytab), _capi.ptr(t.yrow),
+                       *(() if keep is None else (_capi.ptr(keep),)), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
                        _capi.ptr(gbeta), _capi.ptr(d_o), _capi.stream_ptr(),
                        nbytes=2 * B * L * H * W * o.element_size())
         g_rowp = None
@@ -147,26 +167,28 @@ class LsqFunction(torch.autograd.Function):
             g_rowp = torch.empty(H, 3, dtype=torch.float64, device=o.device)
             _capi.call("lf_lsq_grid_grad", _capi.ptr(rowsums), _capi.ptr(t.yrow), _capi.ptr(beta), _capi.ptr(zinv),
                        _capi.ptr(gbeta), B, L, H, order, mask_rows, _capi.ptr(g_rowp), _capi.stream_ptr())
-        return d_o, None, None, None, None, None, None, None, None, g_rowp
+        return d_o, None, None, None, None, None, None, None, None, g_rowp, None
 
 
 def lsq(o, grid, order, const=255.0, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False,
-        want_masked=False, status_out=None):
-    """Functional entry: returns (beta [B,L,order+1] f64, masked or None)."""
+        want_masked=False, status_out=None, keep=None):
+    """Functional entry: returns (beta [B,L,order+1] f64, masked or None).  keep: optional bool / uint8 [H, W] map
+    shared by every image and lane; act(o) is zeroed where it is 0 (masked holds the zeros, d_o is 0 there)."""
     B, L, H, W = o.shape
     tables = grid_tables(grid, H, W, const)
     if act not in _capi.ACT_IDS:
         raise NotImplementedError("Activation type: {} is not implemented".format(act))
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
     return LsqFunction.apply(o, tables, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked,
-                             status_out)
+                             status_out, None, keep_map(keep, H, W, o.device))
 
 
-def lsq_warp(o, warp, order, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False, want_masked=False, status_out=None):
+def lsq_warp(o, warp, order, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False, want_masked=False, status_out=None,
+             keep=None):
     """``lsq`` on a learned warp's tables (homography.WarpTables): beta has a gradient with respect to ``warp.rowp``
-    as well as ``o``."""
+    as well as ``o``; the row sums behind it cover the kept pixels only."""
     if act not in _capi.ACT_IDS:
         raise NotImplementedError("Activation type: {} is not implemented".format(act))
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
     return LsqFunction.apply(o, warp, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked, status_out,
-                             warp.rowp)
+                             warp.rowp, keep_map(keep, o.shape[2], o.shape[3], o.device))
