@@ -542,6 +542,50 @@ int lf_homography_host(const float* theta, int resize, double* Mpair, double* ro
 int lf_homography_bwd_host(const float* theta, int resize, int mask_rows, const double* g_rowp, const double* g_minv,
                            const double* g_yk, double* g_theta);
 
+/* Predicted bird's-eye-view homography (csrc/homography.cu, --predict_homography): one warp per image from z [B][3]
+ * float32, the output of the spatial-transformer branch.  delta = tanh(z) / 16 (f64) moves get_homography(resize)'s
+ * DESTINATION corners: the left column by delta_0 * 2*resize, the right column by delta_1 * 2*resize, the top row by
+ * delta_2 * resize; source corners and the bottom row stay fixed, so every warp is row-preserving (closed form).
+ * lf_predicted_homography_tables: delta [B][3], M / Minv [B][9], rowp [B][resize][3], yk [B][56] (f64), xtab
+ * [B][resize][2*resize], yrow [B][resize] (f32), each image's slice as lf_homography_tables computes it; the guard of
+ * lf_homography_tables on every image, OR-ed once into *status.  lf_predicted_homography_bwd: g_z [B][3] f32 from dL/drowp
+ * [B][resize][3], dL/dMinv [B][9], dL/dyk [B][56] (f64, each may be NULL), forward-mode dual numbers through tanh / 16,
+ * one fixed-order tree per image.  All DEVICE.  Test hooks on host arrays for one image: _host takes delta [3] (f64)
+ * directly and returns Mpair [18] (M, Minv), rowp [resize][3] and yk [56] when not NULL; _bwd_host returns g_z [3] f64. */
+int lf_predicted_homography_tables(const float* z, int B, int resize, int mask_rows, double y_const, double* delta,
+                                   double* M, double* Minv, double* rowp, float* xtab, float* yrow, double* yk,
+                                   int* status, lf_stream_t stream);
+int lf_predicted_homography_bwd(const float* z, int B, int resize, int mask_rows, const double* g_rowp,
+                                const double* g_minv, const double* g_yk, float* g_z, lf_stream_t stream);
+int lf_predicted_homography_host(const double* delta, int resize, double* Mpair, double* rowp, double* yk);
+int lf_predicted_homography_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
+                                     const double* g_minv, const double* g_yk, double* g_z);
+
+/* Per-image least-squares tables (a predicted homography): xtab [B][H][W] and yrow [B][H], image b fitted on its own
+ * slice, on the row-separable plan only (LF_ERR_INVALID_ARGUMENT when lf_lsq_plan would not pick it).
+ * lf_lsq_fwd_per_image: lf_lsq_fwd (rowsums = NULL) or lf_lsq_fwd_rowsums (rowsums [B][L][H][3]); keep as the *_keep
+ * entry points, or NULL for none.  lf_lsq_bwd_per_image: lf_lsq_bwd / lf_lsq_bwd_keep likewise.  Each image's outputs
+ * are a single-image call's bits on that image's tables.  lf_lsq_grid_grad_per_image: g_rowp [B][H][3], image b's
+ * lf_lsq_grid_grad summed over its own lanes only.  All DEVICE. */
+int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
+                         int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
+                         double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                         size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_bwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
+                         int L, int H, int W, int order, int mask_rows, int act, const double* beta, const double* zinv,
+                         const double* gbeta, void* d_o, lf_stream_t stream);
+int lf_lsq_grid_grad_per_image(const float* rowsums, const float* yrow, const double* beta, const double* zinv,
+                               const double* gbeta, int B, int L, int H, int order, int mask_rows, double* g_rowp,
+                               lf_stream_t stream);
+
+/* lf_backproj_loss_dev with one warp per image: yk [B][56], Minv [B][9]; g_const [B][65] holds each image's gradient
+ * (dloss/dMinv, then dloss/dyk); scratch: lf_backproj_loss_per_image_scratch(B, L) doubles.  With every image given
+ * the same warp, loss, dbeta and xcal are lf_backproj_loss_dev's bits.  All DEVICE. */
+size_t lf_backproj_loss_per_image_scratch(int B, int L);
+int lf_backproj_loss_per_image(const double* yk, const double* Minv, const double* beta, const double* x_gt,
+                               const double* valid, int B, int L, int n, double* lane_loss, double* loss, double* dbeta,
+                               double* xcal, double* scratch, double* g_const, unsigned int* ticket, lf_stream_t stream);
+
 
 /* Area loss of the bird's-eye-view experiment over all lanes, its gradient and the exact-area metric in one launch
  * (csrc/loss.cu; replaces Birds_Eye_View_Loss/Loss_crit.py:98-134 summed over the lanes as BEV/main.py:223,237 does, and

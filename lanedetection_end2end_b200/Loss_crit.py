@@ -152,8 +152,9 @@ class backprojection_loss(nn.Module):
         self.y_prime = (self.M[1, 1] * y_d + self.M[1, 2]) / (self.M[2, 1] * y_d + self.M[2, 2])
         self.Y = _design(255 - self.y_prime, options.order)            # [56, order+1]  (:176-188)
         self._dev = None
-        # --learn_homography: the warp is the model's (bind), read every call from its last forward
-        self.learn_homography = bool(getattr(options, "learn_homography", False))
+        # --learn_homography / --predict_homography: the warp is the model's (bind), read every call from its last forward
+        self.learn_homography = bool(getattr(options, "learn_homography", False)
+                                     or getattr(options, "predict_homography", False))
         self.__dict__["_warp"] = None
 
     def bind(self, model):
@@ -162,7 +163,10 @@ class backprojection_loss(nn.Module):
         until it is bound, so it never silently uses the fixed warp."""
         warp = getattr(model, "homography", None)
         if warp is None:
-            raise ValueError("bind() needs a model built with --learn_homography (it has no learned warp)")
+            warp = getattr(model, "DLT", None)         # --predict_homography: one warp per image
+        if warp is None:
+            raise ValueError("bind() needs a model built with --learn_homography or --predict_homography (it has no "
+                             "learned warp)")
         self.__dict__["_warp"] = warp
         return self
 
@@ -180,6 +184,11 @@ class backprojection_loss(nn.Module):
     def _warp_constants(self, device):
         """(M^-1 [3,3], Y [56, n], c_num, c_den) of the bound warp, differentiable (the torch path of forward*)."""
         w = self.warp()
+        if w.per_image:
+            # one warp per image: Mi [B, 3, 3], Y [B, 56, n], c_num / c_den [B, 56]
+            Mi, yp = w.Minv.view(-1, 3, 3), w.yk
+            Y = torch.stack([_design(255 - y, self.Y.shape[1] - 1) for y in yp.unbind(0)])
+            return Mi, Y, Mi[:, 0, 1, None] * yp + Mi[:, 0, 2, None], Mi[:, 2, 1, None] * yp + Mi[:, 2, 2, None]
         Mi, yp = w.Minv.view(3, 3), w.yk
         Y = _design(255 - yp, self.Y.shape[1] - 1)
         return Mi, Y, Mi[0, 1] * yp + Mi[0, 2], Mi[2, 1] * yp + Mi[2, 2]
@@ -207,8 +216,13 @@ class backprojection_loss(nn.Module):
             Mi, Y, c_num, c_den = self._warp_constants(betas[0].device)
         else:
             Mi, Y, c_num, c_den = self.M_inv, self.Y, self._c_num, self._c_den
-        x_prime = p @ Y.t()                                                         # [B, L, 56]
-        x_cal = (Mi[0, 0] * x_prime + c_num) / (Mi[2, 0] * x_prime + c_den)
+        if Mi.dim() == 3:                                                           # one warp per image
+            x_prime = p @ Y.transpose(1, 2)                                         # [B, L, 56]
+            x_cal = (Mi[:, 0, 0, None, None] * x_prime + c_num[:, None]) / (Mi[:, 2, 0, None, None] * x_prime
+                                                                              + c_den[:, None])
+        else:
+            x_prime = p @ Y.t()                                                     # [B, L, 56]
+            x_cal = (Mi[0, 0] * x_prime + c_num) / (Mi[2, 0] * x_prime + c_den)
         v = valid_samples[:, :L]
         x_err = (x_gt[:, :L] - x_cal) * v
         nvalid = v.sum(dim=(0, 2))                                                  # per lane, like the per-lane calls
@@ -247,9 +261,14 @@ class backprojection_loss(nn.Module):
             Mi, Y, c_num, c_den = self._warp_constants(params.device)
         else:
             Mi, Y, c_num, c_den = self.M_inv, self.Y, self._c_num, self._c_den
-        x_prime = p @ Y.t()                                             # [B,56]   (:205)
-        num = Mi[0, 0] * x_prime + c_num                                # M^-1 [x', y', 1]^T  (:208-210)
-        den = Mi[2, 0] * x_prime + c_den
+        if Mi.dim() == 3:                                               # one warp per image
+            x_prime = (Y @ p.unsqueeze(-1)).squeeze(-1)                 # [B,56]
+            num = Mi[:, 0, 0, None] * x_prime + c_num
+            den = Mi[:, 2, 0, None] * x_prime + c_den
+        else:
+            x_prime = p @ Y.t()                                         # [B,56]   (:205)
+            num = Mi[0, 0] * x_prime + c_num                            # M^-1 [x', y', 1]^T  (:208-210)
+            den = Mi[2, 0] * x_prime + c_den
         x_cal = num / den
         x_err = (x_gt - x_cal) * valid_samples                          # (:214)
         nvalid = valid_samples.sum()
@@ -327,6 +346,41 @@ class _FusedBackprojLossWarp(torch.autograd.Function):
         return dbeta * g, None, None, g_const[:9] * g, g_const[9:] * g, None, None
 
 
+class _FusedBackprojLossPerImage(torch.autograd.Function):
+    """_FusedBackprojLossWarp with one warp per image (lf_backproj_loss_per_image): Minv [B, 9], yk [B, 56], and their
+    gradients per image."""
+
+    @staticmethod
+    def forward(ctx, beta, x_gt, valid, Minv, yk, crit, lane_scale=None):
+        B, L, n = beta.shape
+        dev = beta.device
+        lane = torch.empty(L, dtype=torch.float64, device=dev)
+        loss = torch.empty(1, dtype=torch.float64, device=dev)
+        dbeta = torch.empty_like(beta)
+        xcal = torch.empty(B, L, 56, dtype=torch.float64, device=dev)
+        nscr = int(_capi.lib().lf_backproj_loss_per_image_scratch(B, L))
+        scratch = torch.empty(nscr, dtype=torch.float64, device=dev)
+        g_const = torch.empty(B, 65, dtype=torch.float64, device=dev)
+        p = _capi.ptr
+        _capi.call("lf_backproj_loss_per_image", p(yk.detach().contiguous()), p(Minv.detach().contiguous()), p(beta),
+                   p(x_gt), p(valid), B, L, n, p(lane), p(loss), p(dbeta), p(xcal), p(scratch), p(g_const),
+                   p(crit._fused_ticket(dev)), _capi.stream_ptr())
+        if lane_scale is not None:      # the kernel's outputs are linear in per-lane factors
+            ls = lane_scale.to(torch.float64)
+            loss = (lane * ls).mean().reshape(1)
+            dbeta = dbeta * ls.view(1, L, 1)
+            g_part = scratch[nscr - L * B * 65:].view(L, B, 65)          # the per-lane gradients, after the constants
+            g_const = (g_part * ls.view(L, 1, 1)).sum(0)
+        ctx.save_for_backward(dbeta, g_const)
+        ctx.mark_non_differentiable(xcal)
+        return loss.reshape(()), xcal
+
+    @staticmethod
+    def backward(ctx, g, _g_xcal):
+        dbeta, g_const = ctx.saved_tensors
+        return dbeta * g, None, None, g_const[:, :9] * g, g_const[:, 9:] * g, None, None
+
+
 def fused_backprojection_loss(crit, betas, x_gt, valid, lane_scale=None):
     """``mean_l crit(betas[l], x_gt[:, l], valid[:, l])[0]`` (what BP/main.py:297-305 computes) in one launch.
     betas: sequence of L tensors [B, order+1, 1] float64 (Net.forward's beta0..3); x_gt, valid: [B, >=L, 56] float64.
@@ -334,6 +388,9 @@ def fused_backprojection_loss(crit, betas, x_gt, valid, lane_scale=None):
     L = len(betas)
     beta = torch.stack([b.reshape(b.shape[0], -1) for b in betas], 1).double().contiguous()      # [B, L, n]
     warp = crit.warp() if hasattr(crit, "warp") else None
+    if warp is not None and warp.per_image:
+        return _FusedBackprojLossPerImage.apply(beta, x_gt[:, :L].double().contiguous(), valid[:, :L].double().contiguous(),
+                                                warp.Minv, warp.yk, crit, lane_scale)
     if warp is not None:
         return _FusedBackprojLossWarp.apply(beta, x_gt[:, :L].double().contiguous(), valid[:, :L].double().contiguous(),
                                             warp.Minv, warp.yk, crit, lane_scale)

@@ -256,6 +256,28 @@ class Net(nn.Module):
                 raise ValueError("--learn_homography needs --loss_policy backproject (the loss that sees the warp), got %r"
                                  % (args.loss_policy,))
             self.homography = submodule("homography").LearnedHomography(resize, self.zero_rows)
+        # --predict_homography: one warp per image from the spatial-transformer branch on the encoder map (the
+        # reference's DLT module, state_dict keys DLT.spatial_trans.*); a checkpoint without the branch loads with
+        # strict=False and starts from the fixed warp (fully_connected2 = 0)
+        self.predict_homography = bool(getattr(args, "predict_homography", False))
+        if self.predict_homography:
+            if self.learn_homography:
+                raise ValueError("--predict_homography cannot be combined with --learn_homography: pick one warp model")
+            if args.no_mapping:
+                raise ValueError("--predict_homography predicts the bird's-eye-view warp; it cannot be combined with "
+                                 "--no_mapping")
+            if getattr(args, "loss_policy", "backproject") != "backproject":
+                raise ValueError("--predict_homography needs --loss_policy backproject (the loss that sees the warp), got "
+                                 "%r" % (args.loss_policy,))
+            if not args.end_to_end or args.pretrained:
+                raise ValueError("--predict_homography needs --end_to_end True and no --pretrained: the branch is trained "
+                                 "by the fit's loss only")
+            if resize % 4:
+                # the per-image least-squares kernels are the row-separable ones only, whose 16-byte loads need
+                # 2 * resize to be a multiple of 8 (bf16 maps)
+                raise ValueError("--predict_homography needs --resize a multiple of 4, got %d" % resize)
+            self.DLT = submodule("homography").PredictedHomography(resize, self.zero_rows, size=(32, 64), channels_in=128)
+            self.net.__dict__["_pack_extra"] = tuple(self.net.__dict__.get("_pack_extra", ())) + (self.DLT,)
         # --trapezium_mask: the per-pixel keep map of the end-to-end fit (NOTES.md "Trapezium mask"); a plain attribute
         # like idx_row, not a buffer, so checkpoints stay the reference's
         self.keep = trapezium_keep(resize, self.zero_rows) if getattr(args, "trapezium_mask", False) else None
@@ -281,6 +303,9 @@ class Net(nn.Module):
         if self.learn_homography:
             st = status if status is not None else torch.zeros(1, dtype=torch.int32, device=output.device)
             warp = self.homography(st)
+        elif self.predict_homography:
+            st = status if status is not None else torch.zeros(1, dtype=torch.int32, device=output.device)
+            warp = self.DLT(shared_encoder, st)
         grid = self.grid
         if grid.device != output.device:
             grid = self.grid = grid.to(output.device)

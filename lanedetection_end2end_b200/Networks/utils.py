@@ -87,6 +87,7 @@ _FLAGS = [
     ("--end_to_end", _B(True)),
     ("--no_mapping", _B(False)),
     ("--learn_homography", _B(False)),
+    ("--predict_homography", _B(False)),
     ("--seg_proxy", _B(False)),
     ("--weight_seg_proxy", dict(type=float, default=1.0)),
     ("--trapezium_mask", _B(False)),
@@ -247,7 +248,12 @@ def _init_module(m, conv_init):
     """One rule for every scheme (BP/Networks/utils.py:498-559): Conv*/Linear weights by
     ``conv_init``, their biases zero; BatchNorm2d weight ~ N(1, 0.02), bias 0."""
     name = m.__class__.__name__
-    if "Conv" in name or "Linear" in name or name in ("DownConv", "FactorisedConv"):
+    if getattr(m, "zero_init", False):
+        # the predicted homography's last layer (homography.SpatialTransformer.fully_connected2) stays at zero so that a
+        # new model starts from the fixed warp; the reference's kaiming init would re-draw it
+        m.weight.data.zero_()
+        m.bias.data.zero_()
+    elif "Conv" in name or "Linear" in name or name in ("DownConv", "FactorisedConv"):
         w = getattr(m, "weight", None)
         if w is not None:
             conv_init(w.data)

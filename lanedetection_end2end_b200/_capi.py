@@ -252,6 +252,16 @@ _NET_PROTOS = {
     "lf_homography_bwd": (_i, [_p, _i, _i, _p, _p, _p, _p, _p]),
     "lf_homography_host": (_i, [_p, _i, _p, _p, _p]),
     "lf_homography_bwd_host": (_i, [_p, _i, _i, _p, _p, _p, _p]),
+    "lf_predicted_homography_tables": (_i, [_p, _i, _i, _i, ctypes.c_double, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_predicted_homography_bwd": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "lf_predicted_homography_host": (_i, [_p, _i, _p, _p, _p]),
+    "lf_predicted_homography_bwd_host": (_i, [_p, _i, _i, _p, _p, _p, _p]),
+    "lf_lsq_fwd_per_image": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p, _p,
+                                  _p, ctypes.c_size_t, _p]),
+    "lf_lsq_bwd_per_image": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "lf_lsq_grid_grad_per_image": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p]),
+    "lf_backproj_loss_per_image_scratch": (ctypes.c_size_t, [_i, _i]),
+    "lf_backproj_loss_per_image": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "lf_area_loss": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
     "lf_area_loss_host": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p]),
     "lf_seg_lane_maps": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p]),

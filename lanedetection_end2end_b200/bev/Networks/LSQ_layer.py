@@ -101,6 +101,9 @@ class Net(nn.Module):
         from . import define_model
         if getattr(args, "seg_proxy", False):
             raise ValueError("--seg_proxy is not supported by the bird's-eye-view Net: its ERFNet has no second decoder")
+        if getattr(args, "predict_homography", False):
+            raise ValueError("--predict_homography applies to the back-projection Net: the bird's-eye-view labels are "
+                             "coefficients in the fixed warp's coordinates, which a per-image warp would move")
         resize = args.resize
         size, M, _ = Init_Projective_transform(args.nclasses, args.batch_size, args.resize)
         self.M = M

@@ -171,28 +171,30 @@ __global__ void __launch_bounds__(HG_THREADS) homography_tables_kernel(const flo
     }
 }
 
-// One thread's share of dL/dtheta: rows t, t + T, ... (unmasked rows only), sample t < 56, and M^-1 on thread 0.
-__host__ __device__ inline void homography_bwd_partial(const Dual<HG_NT>* m, int t, int nthreads, int R, int mask_rows,
+// One thread's share of dL/dtheta (N tangents): rows t, t + T, ... (unmasked rows only), sample t < 56, and M^-1 on
+// thread 0.
+template <int N>
+__host__ __device__ inline void homography_bwd_partial(const Dual<N>* m, int t, int nthreads, int R, int mask_rows,
                                                        const double* g_rowp, const double* g_minv, const double* g_yk,
                                                        double* acc) {
-    for (int j = 0; j < HG_NT; ++j) acc[j] = 0.0;
+    for (int j = 0; j < N; ++j) acc[j] = 0.0;
     if (g_rowp)
         for (int v = mask_rows + t; v < R; v += nthreads) {
-            Dual<HG_NT> p[3];
+            Dual<N> p[3];
             row_params(m, (double)v, p);
             for (int k = 0; k < 3; ++k) {
                 const double g = g_rowp[(size_t)v * 3 + k];
-                for (int j = 0; j < HG_NT; ++j) acc[j] += g * p[k].d[j];
+                for (int j = 0; j < N; ++j) acc[j] += g * p[k].d[j];
             }
         }
     if (g_yk && t < HG_SAMPLES) {
-        const Dual<HG_NT> y(sample_row(t));
-        const Dual<HG_NT> q = (m[4] * y + m[5]) / (m[7] * y + m[8]);
-        for (int j = 0; j < HG_NT; ++j) acc[j] += g_yk[t] * q.d[j];
+        const Dual<N> y(sample_row(t));
+        const Dual<N> q = (m[4] * y + m[5]) / (m[7] * y + m[8]);
+        for (int j = 0; j < N; ++j) acc[j] += g_yk[t] * q.d[j];
     }
     if (g_minv && t == 0)
         for (int i = 0; i < 9; ++i)
-            for (int j = 0; j < HG_NT; ++j) acc[j] += g_minv[i] * m[9 + i].d[j];
+            for (int j = 0; j < N; ++j) acc[j] += g_minv[i] * m[9 + i].d[j];
 }
 
 __global__ void __launch_bounds__(HG_BWD_THREADS) homography_bwd_kernel(const float* __restrict__ theta, int R, int mask_rows,
@@ -208,7 +210,7 @@ __global__ void __launch_bounds__(HG_BWD_THREADS) homography_bwd_kernel(const fl
     Dual<HG_NT> m[18];
     warp_pair_dual(th, R, m);
     double acc[HG_NT];
-    homography_bwd_partial(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp, g_minv, g_yk, acc);
+    homography_bwd_partial<HG_NT>(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp, g_minv, g_yk, acc);
     for (int j = 0; j < HG_NT; ++j) red[j][t] = acc[j];
     __syncthreads();
     for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1) {   // fixed tree
@@ -217,6 +219,120 @@ __global__ void __launch_bounds__(HG_BWD_THREADS) homography_bwd_kernel(const fl
         __syncthreads();
     }
     if (t < HG_NT) g_theta[t] = (float)red[t][0];
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Predicted homography (--predict_homography, DESIGN.md "Predicted homography"): one warp per image from the branch's
+// output z [B][3], the reference DLT's parametrisation on get_homography(resize)'s corners.  delta = tanh(z) / 16 moves
+// the DESTINATION corners -- the left column by delta_0 * 2R, the right column by delta_1 * 2R, the top row by
+// delta_2 * R -- while the source corners and the bottom row stay fixed, so both warps stay row-preserving and the
+// closed form above applies (no 6x6 solve).
+constexpr int PH_NZ = 3;
+
+template <class T>
+__host__ __device__ inline void predicted_pair(const T* delta, int R, T* m) {
+    const double w = 2.0 * R;
+    const float zero5[HG_NT] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    T sx[4], dx[4], yt, yb, Yt, Yb;
+    warp_corners<T>(zero5, R, sx, yt, yb, dx, Yt, Yb);
+    dx[0] = dx[0] + delta[0] * T(w);
+    dx[2] = dx[2] + delta[0] * T(w);
+    dx[1] = dx[1] + delta[1] * T(w);
+    dx[3] = dx[3] + delta[1] * T(w);
+    Yt = Yt + delta[2] * T((double)R);
+    row_preserving<T>(sx, yt, yb, dx, Yt, Yb, m);
+    row_preserving<T>(dx, Yt, Yb, sx, yt, yb, m + 9);
+}
+
+// delta_j = tanh(z_j) / 16 in fp64, with tangent j seeded as d delta_j / d z_j = (1 - tanh^2) / 16
+__host__ __device__ inline void predicted_delta(const float* z, double* delta, Dual<PH_NZ>* dd) {
+    for (int j = 0; j < PH_NZ; ++j) {
+        const double t = tanh((double)z[j]);
+        delta[j] = t / 16.0;
+        if (dd) {
+            dd[j] = Dual<PH_NZ>(delta[j]);
+            dd[j].d[j] = (1.0 - t * t) / 16.0;
+        }
+    }
+}
+
+// grid (R, B): image b's row v, as homography_tables_kernel on image b's warp.  Per-image outputs are contiguous slices:
+// delta [B][3], M / Minv [B][9], rowp [B][R][3], xtab [B][R][2R], yrow [B][R], yk [B][56].
+__global__ void __launch_bounds__(HG_THREADS) predicted_tables_kernel(const float* __restrict__ z, int R, int mask_rows,
+                                                                       double y_const, double* __restrict__ delta,
+                                                                       double* __restrict__ M, double* __restrict__ Minv,
+                                                                       double* __restrict__ rowp, float* __restrict__ xtab,
+                                                                       float* __restrict__ yrow, double* __restrict__ yk,
+                                                                       int* __restrict__ status) {
+    pdl_entry();
+    const int v = blockIdx.x, b = blockIdx.y, t = threadIdx.x, W = 2 * R;
+    float zb[PH_NZ];
+    for (int j = 0; j < PH_NZ; ++j) zb[j] = z[(size_t)b * PH_NZ + j];
+    double dl[PH_NZ];
+    predicted_delta(zb, dl, nullptr);
+    double m[18];
+    predicted_pair<double>(dl, R, m);
+    double p[3];
+    row_params<double>(m, (double)v, p);
+    const bool guarded = v >= mask_rows;
+    bool bad = false;
+    float* xrow = xtab + ((size_t)b * R + v) * W;
+    for (int u = t; u < W; u += HG_THREADS) {
+        const float x = (float)(p[0] * u + p[1]);
+        xrow[u] = x;
+        bad |= !isfinite(x);
+    }
+    if (t == 0) {
+        const double den = (m[7] * v + m[8]) * (m[7] * (R - 1) + m[8]);
+        const float y = (float)(y_const - p[2]);
+        double* rp = rowp + ((size_t)b * R + v) * 3;
+        rp[0] = p[0];
+        rp[1] = p[1];
+        rp[2] = p[2];
+        yrow[(size_t)b * R + v] = y;
+        bad |= !(den > 0.0) || !isfinite(p[0]) || !isfinite(p[1]) || !isfinite(y);
+    }
+    // any image's unmasked row at or above its vanishing line: the whole batch is skipped like a singular system
+    if (guarded && bad) atomicOr(status, LF_STATUS_NONFINITE);
+    if (v == 0) {
+        if (t < PH_NZ) delta[(size_t)b * PH_NZ + t] = dl[t];
+        if (t < 9) M[(size_t)b * 9 + t] = m[t];
+        if (t >= 9 && t < 18) Minv[(size_t)b * 9 + t - 9] = m[t];
+        if (t < HG_SAMPLES) {
+            const double y = sample_row(t);
+            yk[(size_t)b * HG_SAMPLES + t] = (m[4] * y + m[5]) / (m[7] * y + m[8]);
+        }
+    }
+}
+
+// grid B: dL/dz of image b from its dL/drowp [R][3], dL/dMinv [9], dL/dyk [56]; the fixed tree of homography_bwd_kernel
+__global__ void __launch_bounds__(HG_BWD_THREADS) predicted_bwd_kernel(const float* __restrict__ z, int R, int mask_rows,
+                                                                        const double* __restrict__ g_rowp,
+                                                                        const double* __restrict__ g_minv,
+                                                                        const double* __restrict__ g_yk,
+                                                                        float* __restrict__ g_z) {
+    pdl_entry();
+    __shared__ double red[PH_NZ][HG_BWD_THREADS];
+    const int t = threadIdx.x, b = blockIdx.x;
+    float zb[PH_NZ];
+    for (int j = 0; j < PH_NZ; ++j) zb[j] = z[(size_t)b * PH_NZ + j];
+    double dl[PH_NZ];
+    Dual<PH_NZ> dd[PH_NZ];
+    predicted_delta(zb, dl, dd);
+    Dual<PH_NZ> m[18];
+    predicted_pair<Dual<PH_NZ>>(dd, R, m);
+    double acc[PH_NZ];
+    homography_bwd_partial<PH_NZ>(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp ? g_rowp + (size_t)b * R * 3 : nullptr,
+                                  g_minv ? g_minv + (size_t)b * 9 : nullptr,
+                                  g_yk ? g_yk + (size_t)b * HG_SAMPLES : nullptr, acc);
+    for (int j = 0; j < PH_NZ; ++j) red[j][t] = acc[j];
+    __syncthreads();
+    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1) {
+        if (t < w)
+            for (int j = 0; j < PH_NZ; ++j) red[j][t] += red[j][t + w];
+        __syncthreads();
+    }
+    if (t < PH_NZ) g_z[(size_t)b * PH_NZ + t] = (float)red[t][0];
 }
 
 }  // namespace lf
@@ -267,12 +383,71 @@ extern "C" int lf_homography_bwd_host(const float* theta, int resize, int mask_r
     double red[HG_NT][HG_BWD_THREADS];
     for (int t = 0; t < HG_BWD_THREADS; ++t) {
         double acc[HG_NT];
-        homography_bwd_partial(m, t, HG_BWD_THREADS, resize, mask_rows, g_rowp, g_minv, g_yk, acc);
+        homography_bwd_partial<HG_NT>(m, t, HG_BWD_THREADS, resize, mask_rows, g_rowp, g_minv, g_yk, acc);
         for (int j = 0; j < HG_NT; ++j) red[j][t] = acc[j];
     }
     for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1)
         for (int t = 0; t < w; ++t)
             for (int j = 0; j < HG_NT; ++j) red[j][t] += red[j][t + w];
     for (int j = 0; j < HG_NT; ++j) g_theta[j] = red[j][0];
+    return LF_OK;
+}
+
+// z [B][3] f32 -> delta [B][3], M [B][9], Minv [B][9], rowp [B][R][3], yk [B][56] (f64), xtab [B][R][2R], yrow [B][R]
+// (f32); status as lf_homography_tables, OR-ed once for the batch -- all DEVICE.
+extern "C" int lf_predicted_homography_tables(const float* z, int B, int resize, int mask_rows, double y_const,
+                                              double* delta, double* M, double* Minv, double* rowp, float* xtab,
+                                              float* yrow, double* yk, int* status, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(z && delta && M && Minv && rowp && xtab && yrow && yk && status);
+    LF_REQUIRE(B > 0 && B <= 65535 && resize >= 2 && resize <= 65535 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(predicted_tables_kernel, dim3(resize, B), HG_THREADS, 0, stream, z, resize, mask_rows, y_const, delta, M,
+              Minv, rowp, xtab, yrow, yk, status);
+    return check_launch();
+}
+
+// dL/dz [B][3] f32 from dL/drowp [B][R][3], dL/dMinv [B][9], dL/dyk [B][56] (each f64, may be NULL) -- DEVICE.
+extern "C" int lf_predicted_homography_bwd(const float* z, int B, int resize, int mask_rows, const double* g_rowp,
+                                           const double* g_minv, const double* g_yk, float* g_z, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(z && g_z && B > 0 && resize >= 2 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(predicted_bwd_kernel, B, HG_BWD_THREADS, 0, stream, z, resize, mask_rows, g_rowp, g_minv, g_yk, g_z);
+    return check_launch();
+}
+
+// TEST HOOKS (host arrays, one image; never called by the package).  lf_predicted_homography_host: Mpair [18] (M, M^-1)
+// of delta [3] given directly (inside the tanh box [-1/16, 1/16]^3), rowp [R][3] and yk [56] when not NULL.
+// lf_predicted_homography_bwd_host: dL/dz [3] (f64) of z [3], the kernel's partials and tree.
+extern "C" int lf_predicted_homography_host(const double* delta, int resize, double* Mpair, double* rowp, double* yk) {
+    if (!(delta && Mpair && resize >= 2)) return LF_ERR_INVALID_ARGUMENT;
+    predicted_pair<double>(delta, resize, Mpair);
+    if (rowp)
+        for (int v = 0; v < resize; ++v) row_params<double>(Mpair, (double)v, rowp + (size_t)v * 3);
+    if (yk)
+        for (int s = 0; s < HG_SAMPLES; ++s) {
+            const double y = sample_row(s);
+            yk[s] = (Mpair[4] * y + Mpair[5]) / (Mpair[7] * y + Mpair[8]);
+        }
+    return LF_OK;
+}
+
+extern "C" int lf_predicted_homography_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
+                                                const double* g_minv, const double* g_yk, double* g_z) {
+    if (!(z && g_z && resize >= 2 && mask_rows >= 0 && mask_rows <= resize)) return LF_ERR_INVALID_ARGUMENT;
+    double dl[PH_NZ];
+    Dual<PH_NZ> dd[PH_NZ];
+    predicted_delta(z, dl, dd);
+    Dual<PH_NZ> m[18];
+    predicted_pair<Dual<PH_NZ>>(dd, resize, m);
+    double red[PH_NZ][HG_BWD_THREADS];
+    for (int t = 0; t < HG_BWD_THREADS; ++t) {
+        double acc[PH_NZ];
+        homography_bwd_partial<PH_NZ>(m, t, HG_BWD_THREADS, resize, mask_rows, g_rowp, g_minv, g_yk, acc);
+        for (int j = 0; j < PH_NZ; ++j) red[j][t] = acc[j];
+    }
+    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1)
+        for (int t = 0; t < w; ++t)
+            for (int j = 0; j < PH_NZ; ++j) red[j][t] += red[j][t + w];
+    for (int j = 0; j < PH_NZ; ++j) g_z[j] = red[j][0];
     return LF_OK;
 }

@@ -335,6 +335,111 @@ __global__ void __launch_bounds__(BP_THREADS) backproj_loss_dev_kernel(const dou
     }
 }
 
+
+// The same loss with one warp per image (a predicted homography, --predict_homography): yk [B][56], Minv [B][9].  Each
+// lane CTA first builds the B images' constants into its own slice of `consts` (global scratch, [L][B]); passes 1 and 2
+// then run backproj_loss_dev_kernel's thread assignment and per-point code on image b's constants, so with every image
+// given the same warp the loss, dbeta and xcal are that kernel's bits.  Pass 3 keeps the constants' gradient per image:
+// g_part [L][B][65], and the last CTA sums it over the lanes in lane order into g_const [B][65].
+__global__ void __launch_bounds__(BP_THREADS) backproj_loss_pi_kernel(const double* __restrict__ yk,
+                                                                       const double* __restrict__ Minv,
+                                                                       const double* __restrict__ beta,
+                                                                       const double* __restrict__ x_gt,
+                                                                       const double* __restrict__ valid, int B, int L, int n,
+                                                                       double* __restrict__ lane_loss,
+                                                                       double* __restrict__ dbeta, double* __restrict__ xcal,
+                                                                       BpConst* __restrict__ consts,
+                                                                       double* __restrict__ g_part, unsigned int* ticket,
+                                                                       double* __restrict__ loss, double* __restrict__ g_const) {
+    pdl_entry();
+    __shared__ double red_sq[BP_THREADS], red_nv[BP_THREADS];
+    __shared__ double gm[9][BP_S];
+    __shared__ double s_scale;
+    const int l = blockIdx.x;
+    const int tid = threadIdx.x;
+    BpConst* cs = consts + (size_t)l * B;
+    for (int i = tid; i < B * BP_S; i += BP_THREADS) {
+        const int b = i / BP_S, s = i - b * BP_S;
+        bp_const_row(yk + (size_t)b * BP_S, Minv + (size_t)b * 9, n, s, cs + b);
+    }
+    __syncthreads();
+    double sq = 0.0, nv = 0.0;
+    for (int i = tid; i < B * BP_S; i += BP_THREADS) {
+        const int b = i / BP_S, s = i - b * BP_S;
+        const size_t o = ((size_t)b * L + l) * BP_S + s;
+        double xc, q, dq;
+        bp_point(cs[b], beta + ((size_t)b * L + l) * n, n, s, x_gt[o], valid[o], &xc, &q, &dq);
+        if (xcal) xcal[o] = xc;
+        sq += q;
+        nv += valid[o];
+    }
+    red_sq[tid] = sq;
+    red_nv[tid] = nv;
+    __syncthreads();
+    for (int w = BP_THREADS / 2; w > 0; w >>= 1) {
+        if (tid < w) {
+            red_sq[tid] += red_sq[tid + w];
+            red_nv[tid] += red_nv[tid + w];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const double denom = red_nv[0] == 0.0 ? 1.0 : red_nv[0];
+        lane_loss[l] = red_sq[0] / denom;
+        s_scale = 1.0 / (denom * (double)L);
+    }
+    __syncthreads();
+    const double scale = s_scale;
+    for (int i = tid; i < B * n; i += BP_THREADS) {
+        const int b = i / n, k = i - b * n;
+        const double* bt = beta + ((size_t)b * L + l) * n;
+        double g = 0.0;
+        for (int s = 0; s < BP_S; ++s) {
+            const size_t o = ((size_t)b * L + l) * BP_S + s;
+            double xc, q, dq;
+            bp_point(cs[b], bt, n, s, x_gt[o], valid[o], &xc, &q, &dq);
+            g += dq * cs[b].Y[s][k];
+        }
+        dbeta[((size_t)b * L + l) * n + k] = g * scale;
+    }
+    // pass 3, image by image: dloss/dy'_s on thread s, dloss/dM^-1 summed over the samples in order
+    for (int b = 0; b < B; ++b) {
+        double* gp = g_part + ((size_t)l * B + b) * BP_NG;
+        if (tid < BP_S) {
+            double gmi[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+            const size_t o = ((size_t)b * L + l) * BP_S + tid;
+            const double gy = bp_point_const_grad(cs[b], beta + ((size_t)b * L + l) * n, n, tid, x_gt[o], valid[o], gmi);
+            gp[9 + tid] = gy * scale;
+            for (int i = 0; i < 9; ++i) gm[i][tid] = gmi[i];
+        }
+        __syncthreads();
+        if (tid < 9) {
+            double g = 0.0;
+            for (int s = 0; s < BP_S; ++s) g += gm[tid][s];
+            gp[tid] = g * scale;
+        }
+        __syncthreads();
+    }
+    __threadfence();
+    __syncthreads();
+    __shared__ bool last;
+    if (tid == 0) last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    for (int i = tid; i < B * BP_NG; i += BP_THREADS) {
+        double g = 0.0;
+        for (int j = 0; j < L; ++j) g += __ldcg(g_part + (size_t)j * B * BP_NG + i);
+        g_const[i] = g;
+    }
+    if (tid == 0) {
+        double tot = 0.0;
+        for (int j = 0; j < L; ++j) tot += __ldcg(lane_loss + j);
+        *loss = tot / (double)L;
+        *ticket = 0u;
+    }
+}
+
 }  // namespace lf
 
 // yk [56], Minv [9]: DEVICE constants; beta, x_gt, valid, lane_loss, loss, dbeta, xcal (or NULL), ticket as
@@ -347,6 +452,29 @@ extern "C" int lf_backproj_loss_dev(const double* yk, const double* Minv, const 
     LF_REQUIRE(B > 0 && L > 0 && L <= 65535 && n >= 1 && n <= BP_MAXN);
     lf_launch(backproj_loss_dev_kernel, L, BP_THREADS, 0, stream, yk, Minv, beta, x_gt, valid, B, L, n, lane_loss, dbeta, xcal,
               g_part, ticket, loss, g_const);
+    return check_launch();
+}
+
+// Scratch doubles lf_backproj_loss_per_image needs for B images and L lanes: the per-lane constants and gradients.
+extern "C" size_t lf_backproj_loss_per_image_scratch(int B, int L) {
+    if (B <= 0 || L <= 0) return 0;
+    return (size_t)L * B * (sizeof(BpConst) / sizeof(double) + BP_NG);
+}
+
+// lf_backproj_loss_dev with one warp per image: yk [B][56], Minv [B][9]; g_const [B][65] = each image's dloss/dM^-1 (9)
+// then dloss/dy'_k (56); scratch: lf_backproj_loss_per_image_scratch(B, L) doubles -- all DEVICE.
+extern "C" int lf_backproj_loss_per_image(const double* yk, const double* Minv, const double* beta, const double* x_gt,
+                                          const double* valid, int B, int L, int n, double* lane_loss, double* loss,
+                                          double* dbeta, double* xcal, double* scratch, double* g_const,
+                                          unsigned int* ticket, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(yk && Minv && beta && x_gt && valid && lane_loss && loss && dbeta && scratch && g_const && ticket);
+    LF_REQUIRE(B > 0 && L > 0 && L <= 65535 && n >= 1 && n <= BP_MAXN);
+    LF_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 7) == 0);
+    BpConst* consts = reinterpret_cast<BpConst*>(scratch);
+    double* g_part = scratch + (size_t)L * B * (sizeof(BpConst) / sizeof(double));
+    lf_launch(backproj_loss_pi_kernel, L, BP_THREADS, 0, stream, yk, Minv, beta, x_gt, valid, B, L, n, lane_loss, dbeta,
+              xcal, consts, g_part, ticket, loss, g_const);
     return check_launch();
 }
 

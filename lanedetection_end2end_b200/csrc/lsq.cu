@@ -566,6 +566,24 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
     lsq_fwd_rowsep_body<ACT_T, BF16, NL, true, true>(a, rowsums, keep);
 }
 
+// Per-image tables (a predicted homography, lf_lsq_fwd_per_image / lf_lsq_bwd_per_image): a.xtab is [B][H][W] and
+// a.yrow [B][H]; the CTAs of image b run the shared-table body on b's slice, so the arithmetic is the shared-table
+// kernel's and the existing kernels are untouched.
+__device__ __forceinline__ LsqArgs lsq_image_args(const LsqArgs& a, int b) {
+    LsqArgs ai = a;
+    ai.xtab = a.xtab + (size_t)b * a.H * a.W;
+    ai.yrow = a.yrow + (size_t)b * a.H;
+    return ai;
+}
+
+// ROWSUMS / KEEP as above; rowsums and keep may be unused
+template <int ACT_T, bool BF16, int NL, bool ROWSUMS, bool KEEP>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_pi_kernel(const LsqArgs a,
+                                                                                             float* rowsums,
+                                                                                             const uint8_t* keep) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, ROWSUMS, KEEP>(lsq_image_args(a, blockIdx.y), rowsums, keep);
+}
+
 // ---------------------------------------------------------------------------------
 // Gradient of the loss with respect to the row-separable tables x_{r,c} = alpha_r c + gamma_r, y_r = const - y'_r,
 // from the forward's row sums (DESIGN.md "Learned homography"), summed over images and lanes in a fixed order:
@@ -575,16 +593,11 @@ __global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rows
 // ---------------------------------------------------------------------------------
 constexpr int LSQ_GG_THREADS = 128;
 
-__global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const float* __restrict__ rowsums,
-                                                                        const float* __restrict__ yrow,
-                                                                        const double* __restrict__ beta,
-                                                                        const double* __restrict__ zinv,
-                                                                        const double* __restrict__ gbeta, int B, int L,
-                                                                        int H, int order, int mask_rows,
-                                                                        double* __restrict__ g_rowp) {
-    pdl_entry();
-    const int r = blockIdx.x * LSQ_GG_THREADS + threadIdx.x;
-    if (r >= H) return;
+// row r of g_rowp, summed over the systems bl0 .. bl0 + nbl - 1 in order
+__device__ __forceinline__ void lsq_grid_grad_row(const float* __restrict__ rowsums, const float* __restrict__ yrow,
+                                                  const double* __restrict__ beta, const double* __restrict__ zinv,
+                                                  const double* __restrict__ gbeta, int bl0, int nbl, int H, int order,
+                                                  int mask_rows, int r, double* __restrict__ g_rowp) {
     const int n = order + 1;
     double ga = 0.0, gg = 0.0, gy = 0.0;
     if (r >= mask_rows) {
@@ -597,7 +610,7 @@ __global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const flo
             pwm = pwm * y + pw;
             pw *= y;
         }
-        for (int bl = 0; bl < B * L; ++bl) {
+        for (int bl = bl0; bl < bl0 + nbl; ++bl) {
             const double* bt = beta + (size_t)bl * n;
             const double* zi = zinv + (size_t)bl * n * n;
             const double* g = gbeta + (size_t)bl * n;
@@ -620,6 +633,35 @@ __global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const flo
     g_rowp[(size_t)r * 3 + 0] = ga;
     g_rowp[(size_t)r * 3 + 1] = gg;
     g_rowp[(size_t)r * 3 + 2] = -gy;
+}
+
+__global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_kernel(const float* __restrict__ rowsums,
+                                                                        const float* __restrict__ yrow,
+                                                                        const double* __restrict__ beta,
+                                                                        const double* __restrict__ zinv,
+                                                                        const double* __restrict__ gbeta, int B, int L,
+                                                                        int H, int order, int mask_rows,
+                                                                        double* __restrict__ g_rowp) {
+    pdl_entry();
+    const int r = blockIdx.x * LSQ_GG_THREADS + threadIdx.x;
+    if (r >= H) return;
+    lsq_grid_grad_row(rowsums, yrow, beta, zinv, gbeta, 0, B * L, H, order, mask_rows, r, g_rowp);
+}
+
+// per-image tables: grid (rows, B), image b's g_rowp [H][3] summed over its lanes only, from its yrow [H]
+__global__ void __launch_bounds__(LSQ_GG_THREADS) lsq_grid_grad_pi_kernel(const float* __restrict__ rowsums,
+                                                                           const float* __restrict__ yrow,
+                                                                           const double* __restrict__ beta,
+                                                                           const double* __restrict__ zinv,
+                                                                           const double* __restrict__ gbeta, int L, int H,
+                                                                           int order, int mask_rows,
+                                                                           double* __restrict__ g_rowp) {
+    pdl_entry();
+    const int r = blockIdx.x * LSQ_GG_THREADS + threadIdx.x, b = blockIdx.y;
+    if (r >= H) return;
+    // image b's systems are bl = b L .. b L + L - 1; rowsums is indexed by bl, so only yrow and g_rowp move
+    lsq_grid_grad_row(rowsums, yrow + (size_t)b * H, beta, zinv, gbeta, b * L, L, H, order, mask_rows, r,
+                      g_rowp + (size_t)b * H * 3);
 }
 
 // ---------------------------------------------------------------------------------
@@ -791,6 +833,19 @@ template <int ACT_T, bool BF16, int NL>
 __global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_keep_kernel(const LsqArgs a,
                                                                                                const uint8_t* keep) {
     lsq_bwd_rowsep_body<ACT_T, BF16, NL, true>(a, keep);
+}
+
+// per-image tables (lf_lsq_bwd_per_image)
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_pi_kernel(const LsqArgs a,
+                                                                                             const uint8_t* keep) {
+    lsq_bwd_rowsep_body<ACT_T, BF16, NL, false>(lsq_image_args(a, blockIdx.y), keep);
+}
+
+template <int ACT_T, bool BF16, int NL>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_pi_keep_kernel(const LsqArgs a,
+                                                                                                  const uint8_t* keep) {
+    lsq_bwd_rowsep_body<ACT_T, BF16, NL, true>(lsq_image_args(a, blockIdx.y), keep);
 }
 
 template <int ACT_T, bool BF16, bool KEEP>
@@ -1136,4 +1191,102 @@ extern "C" int lf_lsq_bwd_keep(const void* o, int o_dtype, const float* xtab, co
     LF_REQUIRE(keep);
     return lsq_bwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
                    reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Per-image tables (a predicted homography, --predict_homography): xtab [B][H][W] and yrow [B][H], image b fitted on its
+// own slice, on the row-separable kernels only (yrow is required and W must suit the 16-byte loads).  Same plan, checks,
+// workspace and outputs as the shared-table entry points; rowsums (NULL: none, as lf_lsq_fwd) and keep (NULL: no map)
+// select the instantiation, exactly as lf_lsq_fwd_rowsums / the *_keep entry points do.
+template <int ACT_T, bool BF16, int NL>
+static void launch_fwd_pi_nl(dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums, const uint8_t* keep) {
+    if (rowsums) {
+        if (keep)
+            lf_launch(lsq_fwd_rowsep_pi_kernel<ACT_T, BF16, NL, true, true>, grid, LSQ_THREADS, 0, stream, a, rowsums, keep);
+        else
+            lf_launch(lsq_fwd_rowsep_pi_kernel<ACT_T, BF16, NL, true, false>, grid, LSQ_THREADS, 0, stream, a, rowsums, keep);
+    } else {
+        if (keep)
+            lf_launch(lsq_fwd_rowsep_pi_kernel<ACT_T, BF16, NL, false, true>, grid, LSQ_THREADS, 0, stream, a, rowsums, keep);
+        else
+            lf_launch(lsq_fwd_rowsep_pi_kernel<ACT_T, BF16, NL, false, false>, grid, LSQ_THREADS, 0, stream, a, rowsums, keep);
+    }
+}
+
+template <int ACT_T, bool BF16>
+static void launch_fwd_pi(int nl, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums, const uint8_t* keep) {
+    switch (nl) {
+        case 1: launch_fwd_pi_nl<ACT_T, BF16, 1>(grid, stream, a, rowsums, keep); break;
+        case 2: launch_fwd_pi_nl<ACT_T, BF16, 2>(grid, stream, a, rowsums, keep); break;
+        case 3: launch_fwd_pi_nl<ACT_T, BF16, 3>(grid, stream, a, rowsums, keep); break;
+        default: launch_fwd_pi_nl<ACT_T, BF16, 4>(grid, stream, a, rowsums, keep); break;
+    }
+}
+
+extern "C" int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                                    int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                                    int solver, double* beta, double* zinv, float* masked, int* status, float* rowsums,
+                                    void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(o && xtab && yrow && beta && zinv && status && workspace);
+    LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
+    LsqPlan p{};
+    const int rc = lsq_plan(0, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    if (!p.rowsep) return LF_ERR_INVALID_ARGUMENT;
+    if (workspace_bytes < lf_lsq_workspace_bytes(B, L, H, W, order)) return LF_ERR_WORKSPACE_TOO_SMALL;
+    LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(masked) && aligned16(keep));
+    LsqArgs a{};
+    a.o = o; a.xtab = xtab; a.yrow = yrow;
+    a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
+    a.reg_ls = reg_ls; a.beta = beta; a.zinv = zinv; a.masked = masked; a.status = status;
+    a.nchunks = p.nchunks;
+    a.tickets = reinterpret_cast<int*>(workspace);
+    a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
+    dim3 grid(a.nchunks, B, p.groups);
+    if (act == LF_ACT_SQUARE)
+        o_dtype == LF_BF16 ? launch_fwd_pi<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums, keep)
+                           : launch_fwd_pi<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums, keep);
+    else
+        o_dtype == LF_BF16 ? launch_fwd_pi<LSQ_ACT_RUNTIME, true>(p.nl, grid, stream, a, rowsums, keep)
+                           : launch_fwd_pi<LSQ_ACT_RUNTIME, false>(p.nl, grid, stream, a, rowsums, keep);
+    return check_launch();
+}
+
+extern "C" int lf_lsq_bwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                                    int B, int L, int H, int W, int order, int mask_rows, int act, const double* beta,
+                                    const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(o && xtab && yrow && beta && zinv && gbeta && d_o);
+    LsqPlan p{};
+    const int rc = lsq_plan(1, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
+    if (rc != LF_OK) return rc;
+    if (!p.rowsep) return LF_ERR_INVALID_ARGUMENT;
+    LF_REQUIRE(aligned16(o) && aligned16(xtab) && aligned16(d_o) && aligned16(keep));
+    LsqArgs a{};
+    a.o = o; a.xtab = xtab; a.yrow = yrow;
+    a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act;
+    a.beta = const_cast<double*>(beta); a.zinv = const_cast<double*>(zinv); a.gbeta = gbeta; a.d_o = d_o;
+    a.nchunks = p.nchunks;
+    a.rows_per_cta = 0;
+    dim3 grid(a.nchunks, B, p.groups);
+    if (keep)
+        LSQ_DISPATCH_NL(lsq_bwd_rowsep_pi_keep_kernel, p.nl, grid, a, keep);
+    else
+        LSQ_DISPATCH_NL(lsq_bwd_rowsep_pi_kernel, p.nl, grid, a, keep);
+    return check_launch();
+}
+
+// g_rowp [B][H][3] f64: image b's table gradient, summed over its lanes (rowsums, beta, zinv, gbeta as lf_lsq_grid_grad,
+// yrow [B][H]) -- DEVICE.
+extern "C" int lf_lsq_grid_grad_per_image(const float* rowsums, const float* yrow, const double* beta, const double* zinv,
+                                          const double* gbeta, int B, int L, int H, int order, int mask_rows,
+                                          double* g_rowp, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(rowsums && yrow && beta && zinv && gbeta && g_rowp);
+    LF_REQUIRE(B > 0 && B <= 65535 && L > 0 && H > 0 && order >= 0 && order <= LF_MAX_ORDER && mask_rows >= 0 &&
+               mask_rows <= H);
+    lf_launch(lsq_grid_grad_pi_kernel, dim3((H + LSQ_GG_THREADS - 1) / LSQ_GG_THREADS, B), LSQ_GG_THREADS, 0, stream,
+              rowsums, yrow, beta, zinv, gbeta, L, H, order, mask_rows, g_rowp);
+    return check_launch();
 }

@@ -1,4 +1,7 @@
-"""Learned bird's-eye-view homography (``--learn_homography``): the warp of ``get_homography(resize)`` with its source
+"""Learned bird's-eye-view homography (``--learn_homography``) and the predicted per-image homography
+(``--predict_homography``, ``PredictedHomography`` below).
+
+``--learn_homography``: the warp of ``get_homography(resize)`` with its source
 corners shifted by a learnable ``offsets`` [5] (float32, initialised to zero), so that the back-projection ``Net`` can
 fine-tune the fixed transformation together with the network.
 
@@ -26,9 +29,13 @@ class WarpTables:
     ytab = None
     rowsep = True
 
-    def __init__(self, rowp, Minv, yk, M, xtab, yrow, H, W):
+    def __init__(self, rowp, Minv, yk, M, xtab, yrow, H, W, delta=None):
         self.rowp, self.Minv, self.yk, self.M = rowp, Minv, yk, M
         self.xtab, self.yrow, self.H, self.W = xtab, yrow, H, W
+        # per image (PredictedHomography): every field gains a leading batch dimension -- rowp [B, R, 3], Minv / M
+        # [B, 9], yk [B, 56], xtab [B, R*2R], yrow [B, R] -- and delta [B, 3] holds tanh(z) / 16
+        self.delta = delta
+        self.per_image = delta is not None
 
 
 class _WarpFunction(torch.autograd.Function):
@@ -92,4 +99,118 @@ def warp_host(theta, resize):
     yk = np.zeros(N_SAMPLES)
     _capi.check(_capi.lib().lf_homography_host(th.ctypes.data, resize, Mpair.ctypes.data, rowp.ctypes.data, yk.ctypes.data),
                 "lf_homography_host")
+    return Mpair[:9].reshape(3, 3), Mpair[9:].reshape(3, 3), rowp, yk
+
+
+class _PredictedWarpFunction(torch.autograd.Function):
+
+    @staticmethod
+    def forward(ctx, z, resize, mask_rows, y_const, status):
+        _capi.require_cuda(z, status)
+        z = z.detach().float().contiguous()
+        B, dev = z.shape[0], z.device
+        R, W = resize, 2 * resize
+        f64 = dict(dtype=torch.float64, device=dev)
+        delta = torch.empty(B, 3, **f64)
+        M = torch.empty(B, 9, **f64)
+        Minv = torch.empty(B, 9, **f64)
+        rowp = torch.empty(B, R, 3, **f64)
+        yk = torch.empty(B, N_SAMPLES, **f64)
+        xtab = torch.empty(B, R * W, dtype=torch.float32, device=dev)
+        yrow = torch.empty(B, R, dtype=torch.float32, device=dev)
+        p = _capi.ptr
+        _capi.call("lf_predicted_homography_tables", p(z), B, R, mask_rows, float(y_const), p(delta), p(M), p(Minv), p(rowp),
+                   p(xtab), p(yrow), p(yk), p(status), _capi.stream_ptr(), nbytes=4 * B * R * W)
+        ctx.save_for_backward(z)
+        ctx.cfg = (R, mask_rows)
+        ctx.mark_non_differentiable(M, xtab, yrow, delta)
+        return rowp, Minv, yk, M, xtab, yrow, delta
+
+    @staticmethod
+    def backward(ctx, g_rowp, g_minv, g_yk, _gm, _gx, _gy, _gd):
+        (z,) = ctx.saved_tensors
+        R, mask_rows = ctx.cfg
+        prep = lambda g: None if g is None else g.to(torch.float64).contiguous()
+        g_z = torch.empty_like(z)
+        _capi.call("lf_predicted_homography_bwd", _capi.ptr(z), z.shape[0], R, mask_rows, _capi.ptr(prep(g_rowp)),
+                   _capi.ptr(prep(g_minv)), _capi.ptr(prep(g_yk)), _capi.ptr(g_z), _capi.stream_ptr())
+        return g_z, None, None, None, None
+
+
+class SpatialTransformer(nn.Module):
+    """The reference's ``Spatial_transformer_net`` (Backprojection_Loss/Networks/Least_squares_net.py) on the encoder
+    map [B, 128, rows, cols]: conv 1x1 / 3x3 / 3x3 with BatchNorm + ReLU, max-pool 2x2, conv 3x3 + BatchNorm + ReLU,
+    Linear + ReLU, Linear(128, 3) -> z [B, 3].  The modules only hold the parameters under the reference's names; forward
+    runs on the library's kernels as the Classification heads do (ops_heads).  As in the reference, ``conv5`` is built and
+    never used (it receives no gradient) and ``conv4_bn`` is registered once, where its first assignment put it.
+    ``fully_connected2`` starts at zero (``zero_init``: define_init_weights leaves it there), so a new model starts from
+    the fixed warp."""
+
+    def __init__(self, size, channels_in):
+        super().__init__()
+        self.conv1 = nn.Conv2d(channels_in, 128, 1)
+        self.conv1_bn = nn.BatchNorm2d(128)
+        self.conv2 = nn.Conv2d(128, 128, 3, padding=1)
+        self.conv2_bn = nn.BatchNorm2d(128)
+        self.conv3 = nn.Conv2d(128, 64, 3, padding=1)
+        self.conv3_bn = nn.BatchNorm2d(64)
+        self.conv4 = nn.Conv2d(64, 64, 3, padding=1)
+        self.conv4_bn = nn.BatchNorm2d(64)
+        rows, cols = size
+        self.size = (rows, cols)
+        self.maxpool = nn.MaxPool2d((2, 2), stride=2)
+        self.conv5 = nn.Conv2d(64, 64, 3, padding=1)
+        self.fully_connected1 = nn.Linear(64 * rows * cols // 4, 128)
+        self.fully_connected2 = nn.Linear(128, 3)
+        self.fully_connected2.zero_init = True
+        with torch.no_grad():
+            self.fully_connected2.weight.zero_()
+            self.fully_connected2.bias.zero_()
+
+    def forward(self, x):
+        from . import ops_heads, ops_net
+        from .Networks.ERFNet import _track
+        h = ops_net.as_nhwc(x)
+        _capi.require_cuda(h)
+        if tuple(h.shape[1:3]) != self.size:
+            raise ValueError("spatial transformer built for a %dx%d encoder map, got %dx%d" % (self.size + tuple(h.shape[1:3])))
+        for conv, bn in ((self.conv1, self.conv1_bn), (self.conv2, self.conv2_bn), (self.conv3, self.conv3_bn)):
+            h = ops_heads.conv_bn_relu(h, conv, bn, self.training, _track)
+        h = ops_heads.MaxPool2Function.apply(h)
+        h = ops_heads.conv_bn_relu(h, self.conv4, self.conv4_bn, self.training, _track)
+        f = ops_heads.NchwFlatFunction.apply(h)
+        f = ops_heads.LinearFunction.apply(f, self.fully_connected1.weight, self.fully_connected1.bias, True)
+        return ops_heads.LinearFunction.apply(f, self.fully_connected2.weight, self.fully_connected2.bias, False)
+
+
+class PredictedHomography(nn.Module):
+    """``--predict_homography``: the reference's ``DLT`` module -- the spatial-transformer branch (``spatial_trans``)
+    and one row-preserving warp per image built on the device from its output z (lf_predicted_homography_tables).
+    ``forward(encoder_map, status)`` keeps the batched WarpTables as ``self.current`` for the loss bound to the model
+    and returns it; ORs LF_STATUS_NONFINITE into ``status`` when any image's unmasked row reaches its vanishing line."""
+
+    def __init__(self, resize, mask_rows, size=(32, 64), channels_in=128, y_const=255.0):
+        super().__init__()
+        self.resize, self.mask_rows, self.y_const = resize, mask_rows, y_const
+        self.spatial_trans = SpatialTransformer(size, channels_in)
+        self.current = None
+
+    def forward(self, encoder_map, status):
+        z = self.spatial_trans(encoder_map)
+        rowp, Minv, yk, M, xtab, yrow, delta = _PredictedWarpFunction.apply(z, self.resize, self.mask_rows, self.y_const,
+                                                                            status)
+        self.current = WarpTables(rowp, Minv, yk, M, xtab, yrow, self.resize, 2 * self.resize, delta=delta)
+        return self.current
+
+
+def predicted_warp_host(delta, resize):
+    """(M [3,3], M^-1 [3,3], rowp [R,3], yk [56]) of one image's delta [3] (inside [-1/16, 1/16]^3) as float64 numpy
+    arrays, by the kernel's own closed form on the host (lf_predicted_homography_host)."""
+    import numpy as np
+    d = np.ascontiguousarray(np.asarray(delta, dtype=np.float64).reshape(3))
+    Mpair = np.zeros(18)
+    rowp = np.zeros((resize, 3))
+    yk = np.zeros(N_SAMPLES)
+    _capi.check(_capi.lib().lf_predicted_homography_host(d.ctypes.data, resize, Mpair.ctypes.data, rowp.ctypes.data,
+                                                           yk.ctypes.data), "lf_predicted_homography_host")
     return Mpair[:9].reshape(3, 3), Mpair[9:].reshape(3, 3), rowp, yk

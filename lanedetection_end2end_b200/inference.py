@@ -54,7 +54,8 @@ class Projections:
         self.M, self.M_inv = self._crit.M, self._crit.M_inv
 
     def bind(self, model):
-        """Project with ``model``'s learned warp (--learn_homography), read from its last forward."""
+        """Project with ``model``'s learned warp (--learn_homography) or its per-image warps (--predict_homography), read
+        from its last forward."""
         self._crit.bind(model)
         return self
 
@@ -72,6 +73,14 @@ class Projections:
         loss = torch.empty(1, dtype=torch.float64, device=dev)
         xcal = torch.empty(B, L, 56, dtype=torch.float64, device=dev)
         warp = self._crit.warp()
+        if warp is not None and warp.per_image:
+            scratch = torch.empty(int(_capi.lib().lf_backproj_loss_per_image_scratch(B, L)), dtype=torch.float64, device=dev)
+            _capi.call("lf_backproj_loss_per_image", _capi.ptr(warp.yk.detach()), _capi.ptr(warp.Minv.detach()),
+                       _capi.ptr(beta), _capi.ptr(zeros), _capi.ptr(ones), B, L, n, _capi.ptr(lane), _capi.ptr(loss),
+                       _capi.ptr(torch.empty_like(beta)), _capi.ptr(xcal), _capi.ptr(scratch),
+                       _capi.ptr(torch.empty(B, 65, dtype=torch.float64, device=dev)),
+                       _capi.ptr(self._crit._fused_ticket(dev)), _capi.stream_ptr())
+            return resize_coordinates(xcal)
         if warp is not None:
             g = torch.empty(L + 1, 65, dtype=torch.float64, device=dev)
             _capi.call("lf_backproj_loss_dev", _capi.ptr(warp.yk.detach()), _capi.ptr(warp.Minv.detach()), _capi.ptr(beta),
@@ -420,7 +429,7 @@ def test_model(loader, model, criterion, criterion_seg, criterion_line_class, cr
     dev = next(model.parameters()).device
     scorer = _scorer_for(os.path.join(args.test_dir, "test_label.json"), dev)
     params = Projections(args)
-    if getattr(args, "learn_homography", False):
+    if getattr(args, "learn_homography", False) or getattr(args, "predict_homography", False):
         params.bind(model)
 
     def post(out):

@@ -150,6 +150,45 @@ class MaxPool2FlatFunction(torch.autograd.Function):
         return dx
 
 
+class MaxPool2Function(torch.autograd.Function):
+    """MaxPool2d(2, 2) on NHWC, NHWC out: [B, H/2, W/2, C] (the spatial-transformer branch pools between two convs)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        N, H, W, C = x.shape
+        p = torch.empty(N, H // 2, W // 2, C, dtype=torch.float32, device=x.device)
+        _capi.call("lf_maxpool2_fwd", ptr(x), N, H, W, C, C, ptr(p), C, 0, o._stream())
+        ctx.save_for_backward(x)
+        return p
+
+    @staticmethod
+    def backward(ctx, dp):
+        x, = ctx.saved_tensors
+        N, H, W, C = x.shape
+        dx = torch.empty_like(x)
+        _capi.call("lf_maxpool2_bwd", ptr(x), N, H, W, C, C, ptr(dp.contiguous()), C, 0, ptr(dx), C, 0, o._stream())
+        return dx
+
+
+class NchwFlatFunction(torch.autograd.Function):
+    """NHWC [B, H, W, C] flattened in the reference's NCHW order, x.view(B, -1) on NCHW: [B, C*H*W]."""
+
+    @staticmethod
+    def forward(ctx, x):
+        N, H, W, C = x.shape
+        flat = torch.empty(N, C * H * W, dtype=torch.float32, device=x.device)
+        _capi.call("lf_nhwc_to_nchw", ptr(x.contiguous()), N, H, W, C, ptr(flat), o._stream())
+        ctx.shape = (N, H, W, C)
+        return flat
+
+    @staticmethod
+    def backward(ctx, dflat):
+        N, H, W, C = ctx.shape
+        dx = torch.empty(N, H, W, C, dtype=torch.float32, device=dflat.device)
+        _capi.call("lf_nchw_to_nhwc", ptr(dflat.contiguous()), N, C, H, W, ptr(dx), o._stream())
+        return dx
+
+
 class RowMeanFlatFunction(torch.autograd.Function):
     """AvgPool2d((1, W)) on NHWC, flattened in NCHW order: [B, C*H] (reference :184,201-202)."""
 

@@ -118,7 +118,18 @@ class LsqFunction(torch.autograd.Function):
         # with a keep map the *_keep entry points take it right after the tables
         kp = () if keep is None else (_capi.ptr(keep),)
         sfx = "" if keep is None else "_keep"
-        if rowp is not None and ctx.needs_input_grad[9]:
+        per_image = getattr(tables, "per_image", False)
+        if per_image:
+            # a predicted homography: image b's tables are xtab[b] / yrow[b]; row sums only when rowp needs a gradient
+            if rowp is not None and ctx.needs_input_grad[9]:
+                rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _capi.call("lf_lsq_fwd_per_image", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.yrow), _capi.ptr(keep), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                           _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status), _capi.ptr(rowsums),
+                           _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
+                           nbytes=B * L * H * W * (esz + (4 if want_masked else 0)) + 4 * B * H * W)
+        elif rowp is not None and ctx.needs_input_grad[9]:
             rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
                 _capi.call("lf_lsq_fwd_rowsums" + sfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
@@ -156,6 +167,19 @@ class LsqFunction(torch.autograd.Function):
         B, L, H, W = o.shape
         gbeta = gbeta.to(torch.float64).contiguous()
         d_o = torch.empty_like(o)
+        if getattr(t, "per_image", False):
+            with torch.cuda.device(o.device):
+                _capi.call("lf_lsq_bwd_per_image", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(t.xtab), _capi.ptr(t.yrow),
+                           _capi.ptr(keep), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
+                           _capi.ptr(gbeta), _capi.ptr(d_o), _capi.stream_ptr(),
+                           nbytes=2 * B * L * H * W * o.element_size() + 4 * B * H * W)
+                g_rowp = None
+                if rowsums is not None:
+                    g_rowp = torch.empty(B, H, 3, dtype=torch.float64, device=o.device)
+                    _capi.call("lf_lsq_grid_grad_per_image", _capi.ptr(rowsums), _capi.ptr(t.yrow), _capi.ptr(beta),
+                               _capi.ptr(zinv), _capi.ptr(gbeta), B, L, H, order, mask_rows, _capi.ptr(g_rowp),
+                               _capi.stream_ptr())
+            return d_o, None, None, None, None, None, None, None, None, g_rowp, None
         with torch.cuda.device(o.device):
             _capi.call("lf_lsq_bwd" + ("" if keep is None else "_keep"), _capi.ptr(o), _capi.dtype_id(o),
                        _capi.ptr(t.xtab), _capi.ptr(t.ytab), _capi.ptr(t.yrow),
@@ -186,7 +210,10 @@ def lsq(o, grid, order, const=255.0, mask_rows=0, act="none", reg_ls=0.0, use_ch
 def lsq_warp(o, warp, order, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False, want_masked=False, status_out=None,
              keep=None):
     """``lsq`` on a learned warp's tables (homography.WarpTables): beta has a gradient with respect to ``warp.rowp``
-    as well as ``o``; the row sums behind it cover the kept pixels only."""
+    as well as ``o``; the row sums behind it cover the kept pixels only.  A per-image warp (``warp.per_image``, a
+    predicted homography) fits image b on its own tables and gives rowp [B, R, 3] its per-image gradient."""
+    if getattr(warp, "per_image", False) and warp.xtab.shape[0] != o.shape[0]:
+        raise ValueError("per-image warp tables for %d images, maps for %d" % (warp.xtab.shape[0], o.shape[0]))
     if act not in _capi.ACT_IDS:
         raise NotImplementedError("Activation type: {} is not implemented".format(act))
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
