@@ -561,6 +561,26 @@ int lf_predicted_homography_host(const double* delta, int resize, double* Mpair,
 int lf_predicted_homography_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
                                      const double* g_minv, const double* g_yk, double* g_z);
 
+/* The same per-image warp in the source-corner parametrisation (--predict_homography_corners source): z [B][5] float32,
+ * theta = tanh(z) / 64 rounded to float32 is lf_homography_tables' theta for each image (source corners moved,
+ * destination corners and bottom row fixed).  lf_predicted_homography_source_tables: theta [B][5] f32 and the tables of
+ * lf_predicted_homography_tables, image b's slice bit for bit lf_homography_tables(theta_b); the same guard.
+ * lf_predicted_homography_source_bwd: g_z [B][5] f32 and, when g_theta is not NULL, g_theta [B][5] f64 = dL/dtheta_b as
+ * lf_homography_bwd's tree sums it for one warp, from dL/drowp [B][resize][3], dL/dMinv [B][9], dL/dyk [B][56] (f64,
+ * each may be NULL); g_z = g_theta (1 - tanh^2 z) / 64.  All DEVICE.  Test hooks on host arrays for one image:
+ * _source_host takes z [5] and returns theta [5] (when not NULL), then as lf_homography_host; _source_bwd_host returns
+ * g_z [5] and g_theta [5] (when not NULL) in f64. */
+int lf_predicted_homography_source_tables(const float* z, int B, int resize, int mask_rows, double y_const, float* theta,
+                                          double* M, double* Minv, double* rowp, float* xtab, float* yrow, double* yk,
+                                          int* status, lf_stream_t stream);
+int lf_predicted_homography_source_bwd(const float* z, int B, int resize, int mask_rows, const double* g_rowp,
+                                       const double* g_minv, const double* g_yk, float* g_z, double* g_theta,
+                                       lf_stream_t stream);
+int lf_predicted_homography_source_host(const float* z, int resize, float* theta, double* Mpair, double* rowp,
+                                        double* yk);
+int lf_predicted_homography_source_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
+                                            const double* g_minv, const double* g_yk, double* g_z, double* g_theta);
+
 /* Per-image least-squares tables (a predicted homography): xtab [B][H][W] and yrow [B][H], image b fitted on its own
  * slice, on the row-separable plan only (LF_ERR_INVALID_ARGUMENT when lf_lsq_plan would not pick it).
  * lf_lsq_fwd_per_image: lf_lsq_fwd (rowsums = NULL) or lf_lsq_fwd_rowsums (rowsums [B][L][H][3]); keep as the *_keep

@@ -260,6 +260,12 @@ class Net(nn.Module):
         # reference's DLT module, state_dict keys DLT.spatial_trans.*); a checkpoint without the branch loads with
         # strict=False and starts from the fixed warp (fully_connected2 = 0)
         self.predict_homography = bool(getattr(args, "predict_homography", False))
+        # --predict_homography_corners source: the branch predicts --learn_homography's five source-corner offsets per
+        # image (the reference's destination corners give the loss nothing to learn from: NOTES.md); a destination-mode
+        # checkpoint loads with DLT.spatial_trans.fully_connected2.* dropped and strict=False
+        corners = getattr(args, "predict_homography_corners", "destination")
+        if corners != "destination" and not self.predict_homography:
+            raise ValueError("--predict_homography_corners %s needs --predict_homography True" % corners)
         if self.predict_homography:
             if self.learn_homography:
                 raise ValueError("--predict_homography cannot be combined with --learn_homography: pick one warp model")
@@ -276,7 +282,8 @@ class Net(nn.Module):
                 # the per-image least-squares kernels are the row-separable ones only, whose 16-byte loads need
                 # 2 * resize to be a multiple of 8 (bf16 maps)
                 raise ValueError("--predict_homography needs --resize a multiple of 4, got %d" % resize)
-            self.DLT = submodule("homography").PredictedHomography(resize, self.zero_rows, size=(32, 64), channels_in=128)
+            self.DLT = submodule("homography").PredictedHomography(resize, self.zero_rows, size=(32, 64), channels_in=128,
+                                                                   corners=corners)
             self.net.__dict__["_pack_extra"] = tuple(self.net.__dict__.get("_pack_extra", ())) + (self.DLT,)
         # --trapezium_mask: the per-pixel keep map of the end-to-end fit (NOTES.md "Trapezium mask"); a plain attribute
         # like idx_row, not a buffer, so checkpoints stay the reference's

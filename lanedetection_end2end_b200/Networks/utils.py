@@ -88,6 +88,7 @@ _FLAGS = [
     ("--no_mapping", _B(False)),
     ("--learn_homography", _B(False)),
     ("--predict_homography", _B(False)),
+    ("--predict_homography_corners", dict(type=str, default="destination", choices=["destination", "source"])),
     ("--seg_proxy", _B(False)),
     ("--weight_seg_proxy", dict(type=float, default=1.0)),
     ("--trapezium_mask", _B(False)),

@@ -256,6 +256,10 @@ _NET_PROTOS = {
     "lf_predicted_homography_bwd": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p]),
     "lf_predicted_homography_host": (_i, [_p, _i, _p, _p, _p]),
     "lf_predicted_homography_bwd_host": (_i, [_p, _i, _i, _p, _p, _p, _p]),
+    "lf_predicted_homography_source_tables": (_i, [_p, _i, _i, _i, ctypes.c_double, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "lf_predicted_homography_source_bwd": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
+    "lf_predicted_homography_source_host": (_i, [_p, _i, _p, _p, _p, _p]),
+    "lf_predicted_homography_source_bwd_host": (_i, [_p, _i, _i, _p, _p, _p, _p, _p]),
     "lf_lsq_fwd_per_image": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, ctypes.c_double, _i, _p, _p, _p, _p, _p,
                                   _p, ctypes.c_size_t, _p]),
     "lf_lsq_bwd_per_image": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),

@@ -101,7 +101,8 @@ class Net(nn.Module):
         from . import define_model
         if getattr(args, "seg_proxy", False):
             raise ValueError("--seg_proxy is not supported by the bird's-eye-view Net: its ERFNet has no second decoder")
-        if getattr(args, "predict_homography", False):
+        if getattr(args, "predict_homography", False) or getattr(args, "predict_homography_corners",
+                                                                 "destination") != "destination":
             raise ValueError("--predict_homography applies to the back-projection Net: the bird's-eye-view labels are "
                              "coefficients in the fixed warp's coordinates, which a per-image warp would move")
         resize = args.resize

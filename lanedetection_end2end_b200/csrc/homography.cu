@@ -223,10 +223,16 @@ __global__ void __launch_bounds__(HG_BWD_THREADS) homography_bwd_kernel(const fl
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Predicted homography (--predict_homography, DESIGN.md "Predicted homography"): one warp per image from the branch's
-// output z [B][3], the reference DLT's parametrisation on get_homography(resize)'s corners.  delta = tanh(z) / 16 moves
-// the DESTINATION corners -- the left column by delta_0 * 2R, the right column by delta_1 * 2R, the top row by
-// delta_2 * R -- while the source corners and the bottom row stay fixed, so both warps stay row-preserving and the
-// closed form above applies (no 6x6 solve).
+// output z [B][NZ], in one of two parametrisations of get_homography(resize)'s corners (--predict_homography_corners).
+// Both keep the corner rows level, so both warps stay row-preserving and the closed form above applies (no 6x6 or 8x8
+// solve).
+//
+//   destination (the reference DLT's): delta = tanh(z) / 16 [3] moves the DESTINATION corners -- the left column by
+//     delta_0 * 2R, the right column by delta_1 * 2R, the top row by delta_2 * R -- with the source corners and the bottom
+//     row fixed.  Any two such warps differ by an affine change of the bird's-eye-view coordinates, which the fit and
+//     the back-projection undo: the loss does not see this warp (NOTES.md).
+//   source (--learn_homography's, per image): theta = tanh(z) / 64 [5], rounded to float32, moves the SOURCE corners as
+//     warp_corners does; each image's tables are lf_homography_tables(theta_b).
 constexpr int PH_NZ = 3;
 
 template <class T>
@@ -256,22 +262,66 @@ __host__ __device__ inline void predicted_delta(const float* z, double* delta, D
     }
 }
 
+// The parametrisations as policies of the kernels and host hooks below.  NZ: entries of z per image; Param: the type of
+// the per-image parameters the tables kernel writes (delta f64, theta f32); warp(): those parameters and the pair
+// (M, M^-1); warp_dual(): the pair on dual numbers; dz(): dL/dz_j from the tree's sum of tangent j.
+struct DestinationCorners {
+    static constexpr int NZ = PH_NZ;
+    using Param = double;
+    __host__ __device__ static void warp(const float* z, int R, double* delta, double* m) {
+        predicted_delta(z, delta, nullptr);
+        predicted_pair<double>(delta, R, m);
+    }
+    // tangent j is d/dz_j (seeded in predicted_delta), so the sum is dL/dz_j
+    __host__ __device__ static void warp_dual(const float* z, int R, Dual<NZ>* m) {
+        double dl[NZ];
+        Dual<NZ> dd[NZ];
+        predicted_delta(z, dl, dd);
+        predicted_pair<Dual<NZ>>(dd, R, m);
+    }
+    __host__ __device__ static double dz(const float*, int, double g) { return g; }
+};
+
+struct SourceCorners {
+    static constexpr int NZ = HG_NT;
+    using Param = float;
+    // theta_j = tanh(z_j) / 64 rounded to float32: the theta of --learn_homography, so warp_pair gives its bits
+    __host__ __device__ static void theta_of(const float* z, float* theta) {
+        for (int j = 0; j < NZ; ++j) theta[j] = (float)(tanh((double)z[j]) / 64.0);
+    }
+    __host__ __device__ static void warp(const float* z, int R, float* theta, double* m) {
+        theta_of(z, theta);
+        warp_pair<double>(theta, R, m);
+    }
+    // tangent j is d/dtheta_j (warp_pair_dual's seeds 2R, R): the tree reduces dL/dtheta_b exactly as
+    // homography_bwd_kernel reduces dL/dtheta, and dz() applies d theta_j / d z_j = (1 - tanh^2 z_j) / 64 once, after it
+    __host__ __device__ static void warp_dual(const float* z, int R, Dual<NZ>* m) {
+        float th[NZ];
+        theta_of(z, th);
+        warp_pair_dual(th, R, m);
+    }
+    __host__ __device__ static double dz(const float* z, int j, double g) {
+        const double t = tanh((double)z[j]);
+        return g * ((1.0 - t * t) / 64.0);
+    }
+};
+
 // grid (R, B): image b's row v, as homography_tables_kernel on image b's warp.  Per-image outputs are contiguous slices:
-// delta [B][3], M / Minv [B][9], rowp [B][R][3], xtab [B][R][2R], yrow [B][R], yk [B][56].
+// param [B][NZ], M / Minv [B][9], rowp [B][R][3], xtab [B][R][2R], yrow [B][R], yk [B][56].
+template <class P>
 __global__ void __launch_bounds__(HG_THREADS) predicted_tables_kernel(const float* __restrict__ z, int R, int mask_rows,
-                                                                       double y_const, double* __restrict__ delta,
+                                                                       double y_const, typename P::Param* __restrict__ param,
                                                                        double* __restrict__ M, double* __restrict__ Minv,
                                                                        double* __restrict__ rowp, float* __restrict__ xtab,
                                                                        float* __restrict__ yrow, double* __restrict__ yk,
                                                                        int* __restrict__ status) {
     pdl_entry();
     const int v = blockIdx.x, b = blockIdx.y, t = threadIdx.x, W = 2 * R;
-    float zb[PH_NZ];
-    for (int j = 0; j < PH_NZ; ++j) zb[j] = z[(size_t)b * PH_NZ + j];
-    double dl[PH_NZ];
-    predicted_delta(zb, dl, nullptr);
+    float zb[P::NZ];
+    for (int j = 0; j < P::NZ; ++j) zb[j] = z[(size_t)b * P::NZ + j];
+    typename P::Param q[P::NZ];
     double m[18];
-    predicted_pair<double>(dl, R, m);
+    P::warp(zb, R, q, m);
     double p[3];
     row_params<double>(m, (double)v, p);
     const bool guarded = v >= mask_rows;
@@ -295,7 +345,7 @@ __global__ void __launch_bounds__(HG_THREADS) predicted_tables_kernel(const floa
     // any image's unmasked row at or above its vanishing line: the whole batch is skipped like a singular system
     if (guarded && bad) atomicOr(status, LF_STATUS_NONFINITE);
     if (v == 0) {
-        if (t < PH_NZ) delta[(size_t)b * PH_NZ + t] = dl[t];
+        if (t < P::NZ) param[(size_t)b * P::NZ + t] = q[t];
         if (t < 9) M[(size_t)b * 9 + t] = m[t];
         if (t >= 9 && t < 18) Minv[(size_t)b * 9 + t - 9] = m[t];
         if (t < HG_SAMPLES) {
@@ -305,34 +355,57 @@ __global__ void __launch_bounds__(HG_THREADS) predicted_tables_kernel(const floa
     }
 }
 
-// grid B: dL/dz of image b from its dL/drowp [R][3], dL/dMinv [9], dL/dyk [56]; the fixed tree of homography_bwd_kernel
+// grid B: dL/dz of image b from its dL/drowp [R][3], dL/dMinv [9], dL/dyk [56]; the fixed tree of homography_bwd_kernel.
+// g_sum [B][NZ] (f64, may be NULL): the tree's sums themselves (source corners: dL/dtheta_b).
+template <class P>
 __global__ void __launch_bounds__(HG_BWD_THREADS) predicted_bwd_kernel(const float* __restrict__ z, int R, int mask_rows,
                                                                         const double* __restrict__ g_rowp,
                                                                         const double* __restrict__ g_minv,
                                                                         const double* __restrict__ g_yk,
-                                                                        float* __restrict__ g_z) {
+                                                                        float* __restrict__ g_z, double* __restrict__ g_sum) {
     pdl_entry();
-    __shared__ double red[PH_NZ][HG_BWD_THREADS];
+    __shared__ double red[P::NZ][HG_BWD_THREADS];
     const int t = threadIdx.x, b = blockIdx.x;
-    float zb[PH_NZ];
-    for (int j = 0; j < PH_NZ; ++j) zb[j] = z[(size_t)b * PH_NZ + j];
-    double dl[PH_NZ];
-    Dual<PH_NZ> dd[PH_NZ];
-    predicted_delta(zb, dl, dd);
-    Dual<PH_NZ> m[18];
-    predicted_pair<Dual<PH_NZ>>(dd, R, m);
-    double acc[PH_NZ];
-    homography_bwd_partial<PH_NZ>(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp ? g_rowp + (size_t)b * R * 3 : nullptr,
+    float zb[P::NZ];
+    for (int j = 0; j < P::NZ; ++j) zb[j] = z[(size_t)b * P::NZ + j];
+    Dual<P::NZ> m[18];
+    P::warp_dual(zb, R, m);
+    double acc[P::NZ];
+    homography_bwd_partial<P::NZ>(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp ? g_rowp + (size_t)b * R * 3 : nullptr,
                                   g_minv ? g_minv + (size_t)b * 9 : nullptr,
                                   g_yk ? g_yk + (size_t)b * HG_SAMPLES : nullptr, acc);
-    for (int j = 0; j < PH_NZ; ++j) red[j][t] = acc[j];
+    for (int j = 0; j < P::NZ; ++j) red[j][t] = acc[j];
     __syncthreads();
     for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1) {
         if (t < w)
-            for (int j = 0; j < PH_NZ; ++j) red[j][t] += red[j][t + w];
+            for (int j = 0; j < P::NZ; ++j) red[j][t] += red[j][t + w];
         __syncthreads();
     }
-    if (t < PH_NZ) g_z[(size_t)b * PH_NZ + t] = (float)red[t][0];
+    if (t < P::NZ) {
+        g_z[(size_t)b * P::NZ + t] = (float)P::dz(zb, t, red[t][0]);
+        if (g_sum) g_sum[(size_t)b * P::NZ + t] = red[t][0];
+    }
+}
+
+// the same on the host for one image (the test hooks): the kernel's partials and tree
+template <class P>
+static void predicted_bwd_host(const float* z, int R, int mask_rows, const double* g_rowp, const double* g_minv,
+                               const double* g_yk, double* g_z, double* g_sum) {
+    Dual<P::NZ> m[18];
+    P::warp_dual(z, R, m);
+    double red[P::NZ][HG_BWD_THREADS];
+    for (int t = 0; t < HG_BWD_THREADS; ++t) {
+        double acc[P::NZ];
+        homography_bwd_partial<P::NZ>(m, t, HG_BWD_THREADS, R, mask_rows, g_rowp, g_minv, g_yk, acc);
+        for (int j = 0; j < P::NZ; ++j) red[j][t] = acc[j];
+    }
+    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1)
+        for (int t = 0; t < w; ++t)
+            for (int j = 0; j < P::NZ; ++j) red[j][t] += red[j][t + w];
+    for (int j = 0; j < P::NZ; ++j) {
+        g_z[j] = P::dz(z, j, red[j][0]);
+        if (g_sum) g_sum[j] = red[j][0];
+    }
 }
 
 }  // namespace lf
@@ -393,26 +466,57 @@ extern "C" int lf_homography_bwd_host(const float* theta, int resize, int mask_r
     return LF_OK;
 }
 
+template <class P>
+static int predicted_tables_run(const float* z, int B, int resize, int mask_rows, double y_const,
+                                typename P::Param* param, double* M, double* Minv, double* rowp, float* xtab, float* yrow,
+                                double* yk, int* status, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(z && param && M && Minv && rowp && xtab && yrow && yk && status);
+    LF_REQUIRE(B > 0 && B <= 65535 && resize >= 2 && resize <= 65535 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(predicted_tables_kernel<P>, dim3(resize, B), HG_THREADS, 0, stream, z, resize, mask_rows, y_const, param, M,
+              Minv, rowp, xtab, yrow, yk, status);
+    return check_launch();
+}
+
+template <class P>
+static int predicted_bwd_run(const float* z, int B, int resize, int mask_rows, const double* g_rowp, const double* g_minv,
+                             const double* g_yk, float* g_z, double* g_sum, lf_stream_t stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    LF_REQUIRE(z && g_z && B > 0 && resize >= 2 && mask_rows >= 0 && mask_rows <= resize);
+    lf_launch(predicted_bwd_kernel<P>, B, HG_BWD_THREADS, 0, stream, z, resize, mask_rows, g_rowp, g_minv, g_yk, g_z, g_sum);
+    return check_launch();
+}
+
 // z [B][3] f32 -> delta [B][3], M [B][9], Minv [B][9], rowp [B][R][3], yk [B][56] (f64), xtab [B][R][2R], yrow [B][R]
 // (f32); status as lf_homography_tables, OR-ed once for the batch -- all DEVICE.
 extern "C" int lf_predicted_homography_tables(const float* z, int B, int resize, int mask_rows, double y_const,
                                               double* delta, double* M, double* Minv, double* rowp, float* xtab,
                                               float* yrow, double* yk, int* status, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    LF_REQUIRE(z && delta && M && Minv && rowp && xtab && yrow && yk && status);
-    LF_REQUIRE(B > 0 && B <= 65535 && resize >= 2 && resize <= 65535 && mask_rows >= 0 && mask_rows <= resize);
-    lf_launch(predicted_tables_kernel, dim3(resize, B), HG_THREADS, 0, stream, z, resize, mask_rows, y_const, delta, M,
-              Minv, rowp, xtab, yrow, yk, status);
-    return check_launch();
+    return predicted_tables_run<DestinationCorners>(z, B, resize, mask_rows, y_const, delta, M, Minv, rowp, xtab, yrow, yk,
+                                                    status, stream_);
 }
 
 // dL/dz [B][3] f32 from dL/drowp [B][R][3], dL/dMinv [B][9], dL/dyk [B][56] (each f64, may be NULL) -- DEVICE.
 extern "C" int lf_predicted_homography_bwd(const float* z, int B, int resize, int mask_rows, const double* g_rowp,
                                            const double* g_minv, const double* g_yk, float* g_z, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    LF_REQUIRE(z && g_z && B > 0 && resize >= 2 && mask_rows >= 0 && mask_rows <= resize);
-    lf_launch(predicted_bwd_kernel, B, HG_BWD_THREADS, 0, stream, z, resize, mask_rows, g_rowp, g_minv, g_yk, g_z);
-    return check_launch();
+    return predicted_bwd_run<DestinationCorners>(z, B, resize, mask_rows, g_rowp, g_minv, g_yk, g_z, nullptr, stream_);
+}
+
+// The source-corner parametrisation: z [B][5] f32 -> theta [B][5] f32 (tanh(z) / 64 rounded), and the tables of
+// lf_predicted_homography_tables, image b's bit for bit lf_homography_tables(theta_b) -- all DEVICE.
+extern "C" int lf_predicted_homography_source_tables(const float* z, int B, int resize, int mask_rows, double y_const,
+                                                     float* theta, double* M, double* Minv, double* rowp, float* xtab,
+                                                     float* yrow, double* yk, int* status, lf_stream_t stream_) {
+    return predicted_tables_run<SourceCorners>(z, B, resize, mask_rows, y_const, theta, M, Minv, rowp, xtab, yrow, yk,
+                                               status, stream_);
+}
+
+// dL/dz [B][5] f32 and, when g_theta is not NULL, dL/dtheta [B][5] f64 (image b's as lf_homography_bwd reduces it) from
+// dL/drowp [B][R][3], dL/dMinv [B][9], dL/dyk [B][56] (each f64, may be NULL) -- DEVICE.
+extern "C" int lf_predicted_homography_source_bwd(const float* z, int B, int resize, int mask_rows, const double* g_rowp,
+                                                  const double* g_minv, const double* g_yk, float* g_z, double* g_theta,
+                                                  lf_stream_t stream_) {
+    return predicted_bwd_run<SourceCorners>(z, B, resize, mask_rows, g_rowp, g_minv, g_yk, g_z, g_theta, stream_);
 }
 
 // TEST HOOKS (host arrays, one image; never called by the package).  lf_predicted_homography_host: Mpair [18] (M, M^-1)
@@ -434,20 +538,27 @@ extern "C" int lf_predicted_homography_host(const double* delta, int resize, dou
 extern "C" int lf_predicted_homography_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
                                                 const double* g_minv, const double* g_yk, double* g_z) {
     if (!(z && g_z && resize >= 2 && mask_rows >= 0 && mask_rows <= resize)) return LF_ERR_INVALID_ARGUMENT;
-    double dl[PH_NZ];
-    Dual<PH_NZ> dd[PH_NZ];
-    predicted_delta(z, dl, dd);
-    Dual<PH_NZ> m[18];
-    predicted_pair<Dual<PH_NZ>>(dd, resize, m);
-    double red[PH_NZ][HG_BWD_THREADS];
-    for (int t = 0; t < HG_BWD_THREADS; ++t) {
-        double acc[PH_NZ];
-        homography_bwd_partial<PH_NZ>(m, t, HG_BWD_THREADS, resize, mask_rows, g_rowp, g_minv, g_yk, acc);
-        for (int j = 0; j < PH_NZ; ++j) red[j][t] = acc[j];
-    }
-    for (int w = HG_BWD_THREADS / 2; w > 0; w >>= 1)
-        for (int t = 0; t < w; ++t)
-            for (int j = 0; j < PH_NZ; ++j) red[j][t] += red[j][t + w];
-    for (int j = 0; j < PH_NZ; ++j) g_z[j] = red[j][0];
+    predicted_bwd_host<DestinationCorners>(z, resize, mask_rows, g_rowp, g_minv, g_yk, g_z, nullptr);
+    return LF_OK;
+}
+
+// lf_predicted_homography_source_host: theta [5] (when not NULL) and Mpair [18] of z [5], then as lf_homography_host.
+// lf_predicted_homography_source_bwd_host: dL/dz [5] and, when not NULL, dL/dtheta [5] (f64), the kernel's partials
+// and tree.
+extern "C" int lf_predicted_homography_source_host(const float* z, int resize, float* theta, double* Mpair, double* rowp,
+                                                   double* yk) {
+    if (!(z && Mpair && resize >= 2)) return LF_ERR_INVALID_ARGUMENT;
+    float th[HG_NT];
+    SourceCorners::theta_of(z, th);
+    if (theta)
+        for (int j = 0; j < HG_NT; ++j) theta[j] = th[j];
+    return lf_homography_host(th, resize, Mpair, rowp, yk);
+}
+
+extern "C" int lf_predicted_homography_source_bwd_host(const float* z, int resize, int mask_rows, const double* g_rowp,
+                                                       const double* g_minv, const double* g_yk, double* g_z,
+                                                       double* g_theta) {
+    if (!(z && g_z && resize >= 2 && mask_rows >= 0 && mask_rows <= resize)) return LF_ERR_INVALID_ARGUMENT;
+    predicted_bwd_host<SourceCorners>(z, resize, mask_rows, g_rowp, g_minv, g_yk, g_z, g_theta);
     return LF_OK;
 }

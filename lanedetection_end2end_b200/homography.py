@@ -33,7 +33,8 @@ class WarpTables:
         self.rowp, self.Minv, self.yk, self.M = rowp, Minv, yk, M
         self.xtab, self.yrow, self.H, self.W = xtab, yrow, H, W
         # per image (PredictedHomography): every field gains a leading batch dimension -- rowp [B, R, 3], Minv / M
-        # [B, 9], yk [B, 56], xtab [B, R*2R], yrow [B, R] -- and delta [B, 3] holds tanh(z) / 16
+        # [B, 9], yk [B, 56], xtab [B, R*2R], yrow [B, R] -- and delta holds the per-image parameters: [B, 3] f64
+        # tanh(z) / 16 for the destination corners, [B, 5] f32 theta = tanh(z) / 64 for the source corners
         self.delta = delta
         self.per_image = delta is not None
 
@@ -102,51 +103,88 @@ def warp_host(theta, resize):
     return Mpair[:9].reshape(3, 3), Mpair[9:].reshape(3, 3), rowp, yk
 
 
+# the two parametrisations of the branch's output z (--predict_homography_corners): entries of z per image, dtype of
+# the per-image parameters the tables entry point writes (delta / theta), and the tables and backward entry points
+CORNERS = {"destination": (3, torch.float64, "lf_predicted_homography_tables", "lf_predicted_homography_bwd"),
+           "source": (5, torch.float32, "lf_predicted_homography_source_tables", "lf_predicted_homography_source_bwd")}
+
+
+def _predicted_forward(ctx, corners, z, resize, mask_rows, y_const, status):
+    _capi.require_cuda(z, status)
+    nz, param_dtype, tables, _ = CORNERS[corners]
+    z = z.detach().float().contiguous()
+    B, dev = z.shape[0], z.device
+    if tuple(z.shape) != (B, nz):
+        raise ValueError("%s corners need z [B, %d], got %s" % (corners, nz, tuple(z.shape)))
+    R, W = resize, 2 * resize
+    f64 = dict(dtype=torch.float64, device=dev)
+    param = torch.empty(B, nz, dtype=param_dtype, device=dev)
+    M = torch.empty(B, 9, **f64)
+    Minv = torch.empty(B, 9, **f64)
+    rowp = torch.empty(B, R, 3, **f64)
+    yk = torch.empty(B, N_SAMPLES, **f64)
+    xtab = torch.empty(B, R * W, dtype=torch.float32, device=dev)
+    yrow = torch.empty(B, R, dtype=torch.float32, device=dev)
+    p = _capi.ptr
+    _capi.call(tables, p(z), B, R, mask_rows, float(y_const), p(param), p(M), p(Minv), p(rowp), p(xtab), p(yrow), p(yk),
+               p(status), _capi.stream_ptr(), nbytes=4 * B * R * W)
+    ctx.save_for_backward(z)
+    ctx.cfg = (corners, R, mask_rows)
+    ctx.mark_non_differentiable(M, xtab, yrow, param)
+    return rowp, Minv, yk, M, xtab, yrow, param
+
+
+def _predicted_backward(ctx, g_rowp, g_minv, g_yk):
+    (z,) = ctx.saved_tensors
+    corners, R, mask_rows = ctx.cfg
+    bwd = CORNERS[corners][3]
+    prep = lambda g: None if g is None else g.to(torch.float64).contiguous()
+    g_z = torch.empty_like(z)
+    extra = (None,) if corners == "source" else ()         # dL/dtheta in f64: not needed here
+    _capi.call(bwd, _capi.ptr(z), z.shape[0], R, mask_rows, _capi.ptr(prep(g_rowp)), _capi.ptr(prep(g_minv)),
+               _capi.ptr(prep(g_yk)), _capi.ptr(g_z), *extra, _capi.stream_ptr())
+    return g_z, None, None, None, None
+
+
 class _PredictedWarpFunction(torch.autograd.Function):
+    """z [B, 3] -> the destination-corner warps: (rowp, Minv, yk, M, xtab, yrow, delta [B, 3] f64)."""
 
     @staticmethod
     def forward(ctx, z, resize, mask_rows, y_const, status):
-        _capi.require_cuda(z, status)
-        z = z.detach().float().contiguous()
-        B, dev = z.shape[0], z.device
-        R, W = resize, 2 * resize
-        f64 = dict(dtype=torch.float64, device=dev)
-        delta = torch.empty(B, 3, **f64)
-        M = torch.empty(B, 9, **f64)
-        Minv = torch.empty(B, 9, **f64)
-        rowp = torch.empty(B, R, 3, **f64)
-        yk = torch.empty(B, N_SAMPLES, **f64)
-        xtab = torch.empty(B, R * W, dtype=torch.float32, device=dev)
-        yrow = torch.empty(B, R, dtype=torch.float32, device=dev)
-        p = _capi.ptr
-        _capi.call("lf_predicted_homography_tables", p(z), B, R, mask_rows, float(y_const), p(delta), p(M), p(Minv), p(rowp),
-                   p(xtab), p(yrow), p(yk), p(status), _capi.stream_ptr(), nbytes=4 * B * R * W)
-        ctx.save_for_backward(z)
-        ctx.cfg = (R, mask_rows)
-        ctx.mark_non_differentiable(M, xtab, yrow, delta)
-        return rowp, Minv, yk, M, xtab, yrow, delta
+        return _predicted_forward(ctx, "destination", z, resize, mask_rows, y_const, status)
 
     @staticmethod
     def backward(ctx, g_rowp, g_minv, g_yk, _gm, _gx, _gy, _gd):
-        (z,) = ctx.saved_tensors
-        R, mask_rows = ctx.cfg
-        prep = lambda g: None if g is None else g.to(torch.float64).contiguous()
-        g_z = torch.empty_like(z)
-        _capi.call("lf_predicted_homography_bwd", _capi.ptr(z), z.shape[0], R, mask_rows, _capi.ptr(prep(g_rowp)),
-                   _capi.ptr(prep(g_minv)), _capi.ptr(prep(g_yk)), _capi.ptr(g_z), _capi.stream_ptr())
-        return g_z, None, None, None, None
+        return _predicted_backward(ctx, g_rowp, g_minv, g_yk)
+
+
+class _PredictedSourceWarpFunction(torch.autograd.Function):
+    """z [B, 5] -> the source-corner warps: (rowp, Minv, yk, M, xtab, yrow, theta [B, 5] f32), image b's tables those of
+    --learn_homography's warp at theta_b = tanh(z_b) / 64."""
+
+    @staticmethod
+    def forward(ctx, z, resize, mask_rows, y_const, status):
+        return _predicted_forward(ctx, "source", z, resize, mask_rows, y_const, status)
+
+    @staticmethod
+    def backward(ctx, g_rowp, g_minv, g_yk, _gm, _gx, _gy, _gt):
+        return _predicted_backward(ctx, g_rowp, g_minv, g_yk)
+
+
+_PREDICTED_FUNCTIONS = {"destination": _PredictedWarpFunction, "source": _PredictedSourceWarpFunction}
 
 
 class SpatialTransformer(nn.Module):
     """The reference's ``Spatial_transformer_net`` (Backprojection_Loss/Networks/Least_squares_net.py) on the encoder
     map [B, 128, rows, cols]: conv 1x1 / 3x3 / 3x3 with BatchNorm + ReLU, max-pool 2x2, conv 3x3 + BatchNorm + ReLU,
-    Linear + ReLU, Linear(128, 3) -> z [B, 3].  The modules only hold the parameters under the reference's names; forward
-    runs on the library's kernels as the Classification heads do (ops_heads).  As in the reference, ``conv5`` is built and
-    never used (it receives no gradient) and ``conv4_bn`` is registered once, where its first assignment put it.
+    Linear + ReLU, Linear(128, nz) -> z [B, nz] (nz = 3, the reference's; 5 for the source corners).  The modules only
+    hold the parameters under the reference's names; forward runs on the library's kernels as the Classification heads
+    do (ops_heads).  As in the reference, ``conv5`` is built and never used (it receives no gradient) and ``conv4_bn`` is
+    registered once, where its first assignment put it.
     ``fully_connected2`` starts at zero (``zero_init``: define_init_weights leaves it there), so a new model starts from
     the fixed warp."""
 
-    def __init__(self, size, channels_in):
+    def __init__(self, size, channels_in, nz=3):
         super().__init__()
         self.conv1 = nn.Conv2d(channels_in, 128, 1)
         self.conv1_bn = nn.BatchNorm2d(128)
@@ -161,7 +199,7 @@ class SpatialTransformer(nn.Module):
         self.maxpool = nn.MaxPool2d((2, 2), stride=2)
         self.conv5 = nn.Conv2d(64, 64, 3, padding=1)
         self.fully_connected1 = nn.Linear(64 * rows * cols // 4, 128)
-        self.fully_connected2 = nn.Linear(128, 3)
+        self.fully_connected2 = nn.Linear(128, nz)
         self.fully_connected2.zero_init = True
         with torch.no_grad():
             self.fully_connected2.weight.zero_()
@@ -185,21 +223,27 @@ class SpatialTransformer(nn.Module):
 
 class PredictedHomography(nn.Module):
     """``--predict_homography``: the reference's ``DLT`` module -- the spatial-transformer branch (``spatial_trans``)
-    and one row-preserving warp per image built on the device from its output z (lf_predicted_homography_tables).
-    ``forward(encoder_map, status)`` keeps the batched WarpTables as ``self.current`` for the loss bound to the model
-    and returns it; ORs LF_STATUS_NONFINITE into ``status`` when any image's unmasked row reaches its vanishing line."""
+    and one row-preserving warp per image built on the device from its output z.  ``corners`` picks the parametrisation
+    (``--predict_homography_corners``): ``"destination"``, the reference's (z [B, 3], delta = tanh(z) / 16 moves the
+    destination corners; lf_predicted_homography_tables), or ``"source"`` (z [B, 5], theta = tanh(z) / 64 moves the
+    source corners as ``LearnedHomography.offsets`` does; lf_predicted_homography_source_tables).  Only the source
+    corners change what the loss sees (NOTES.md "Predicted homography").  ``forward(encoder_map, status)`` keeps the
+    batched WarpTables (``delta`` holding delta or theta) as ``self.current`` for the loss bound to the model and
+    returns it; ORs LF_STATUS_NONFINITE into ``status`` when any image's unmasked row reaches its vanishing line."""
 
-    def __init__(self, resize, mask_rows, size=(32, 64), channels_in=128, y_const=255.0):
+    def __init__(self, resize, mask_rows, size=(32, 64), channels_in=128, y_const=255.0, corners="destination"):
         super().__init__()
-        self.resize, self.mask_rows, self.y_const = resize, mask_rows, y_const
-        self.spatial_trans = SpatialTransformer(size, channels_in)
+        if corners not in CORNERS:
+            raise ValueError("corners must be one of %s, got %r" % (sorted(CORNERS), corners))
+        self.resize, self.mask_rows, self.y_const, self.corners = resize, mask_rows, y_const, corners
+        self.spatial_trans = SpatialTransformer(size, channels_in, nz=CORNERS[corners][0])
         self.current = None
 
     def forward(self, encoder_map, status):
         z = self.spatial_trans(encoder_map)
-        rowp, Minv, yk, M, xtab, yrow, delta = _PredictedWarpFunction.apply(z, self.resize, self.mask_rows, self.y_const,
-                                                                            status)
-        self.current = WarpTables(rowp, Minv, yk, M, xtab, yrow, self.resize, 2 * self.resize, delta=delta)
+        rowp, Minv, yk, M, xtab, yrow, param = _PREDICTED_FUNCTIONS[self.corners].apply(z, self.resize, self.mask_rows,
+                                                                                       self.y_const, status)
+        self.current = WarpTables(rowp, Minv, yk, M, xtab, yrow, self.resize, 2 * self.resize, delta=param)
         return self.current
 
 
@@ -214,3 +258,18 @@ def predicted_warp_host(delta, resize):
     _capi.check(_capi.lib().lf_predicted_homography_host(d.ctypes.data, resize, Mpair.ctypes.data, rowp.ctypes.data,
                                                            yk.ctypes.data), "lf_predicted_homography_host")
     return Mpair[:9].reshape(3, 3), Mpair[9:].reshape(3, 3), rowp, yk
+
+
+def predicted_source_warp_host(z, resize):
+    """(theta [5] f32, M [3,3], M^-1 [3,3], rowp [R,3], yk [56]) of one image's z [5] in the source-corner
+    parametrisation, as numpy arrays, by the kernel's own code on the host (lf_predicted_homography_source_host)."""
+    import numpy as np
+    zz = np.ascontiguousarray(np.asarray(z, dtype=np.float32).reshape(5))
+    theta = np.zeros(5, np.float32)
+    Mpair = np.zeros(18)
+    rowp = np.zeros((resize, 3))
+    yk = np.zeros(N_SAMPLES)
+    _capi.check(_capi.lib().lf_predicted_homography_source_host(zz.ctypes.data, resize, theta.ctypes.data, Mpair.ctypes.data,
+                                                                  rowp.ctypes.data, yk.ctypes.data),
+                "lf_predicted_homography_source_host")
+    return theta, Mpair[:9].reshape(3, 3), Mpair[9:].reshape(3, 3), rowp, yk

@@ -1,9 +1,13 @@
 """What --predict_homography costs: train.sh's graphed training step (4 lanes, order 3, --clas 1, batch 32, resize 256,
 fused Adam in the graph) and the graphed eval forward (GraphedInference) with and without the flag, in the tf32x3 and
 bf16 convolution modes; the per-launch time of each new kernel; the peak memory of each arm.  Writes
-profiles/h100/bench_predict_homography.json (or --out).
+profiles/h100/bench_predict_homography.json (or --out).  ``--corners source`` times the source-corner
+parametrisation (--predict_homography_corners source) instead: the fixed warp, the destination corners and the source
+corners side by side, and the tables kernel and its backward in both parametrisations; it writes
+profiles/h100/bench_predict_homography_source.json.
 
-    python tools/bench_predict_homography.py [--out PATH] [--rounds 3] [--steps 30] [--launches 200]
+    python tools/bench_predict_homography.py [--corners destination|source] [--out PATH] [--rounds 3] [--steps 30]
+                                             [--launches 200]
 
 Step: engine.GraphedTrainStep over the model, the fused back-projection loss and FusedOptimizer("adam"), on synthetic
 device-resident inputs; eval: one GraphedInference replay.  CUDA events around --steps replays after a warm-up; every arm
@@ -27,14 +31,15 @@ from bench_homography import BATCH, LANES, ORDER, RESIZE, gpu_info, time_events 
 MASK_ROWS = 52          # ceil(256 * 0.2), train.sh's --mask_percentage 0.2
 
 
-def make_args(predict):
+def make_args(predict, corners="destination"):
     from lanedetection_end2end_b200.Networks.utils import define_args
     return define_args().parse_args(["--image_dir", ".", "--gt_dir", ".", "--loss_policy", "backproject", "--batch_size",
                                      str(BATCH), "--resize", str(RESIZE), "--nclasses", str(LANES), "--order", str(ORDER),
-                                     "--clas", "True", "--mask_percentage", "0.2", "--predict_homography", str(predict)])
+                                     "--clas", "True", "--mask_percentage", "0.2", "--predict_homography", str(predict),
+                                     "--predict_homography_corners", corners])
 
 
-def make_step(predict, mode):
+def make_step(predict, mode, corners="destination"):
     import torch
     from lanedetection_end2end_b200 import ops_net
     from lanedetection_end2end_b200.engine import GraphedTrainStep
@@ -42,7 +47,7 @@ def make_step(predict, mode):
     from lanedetection_end2end_b200.Networks.LSQ_layer import Net
     from lanedetection_end2end_b200.optim import FusedOptimizer
     ops_net.set_conv_mode(mode)
-    args = make_args(predict)
+    args = make_args(predict, corners)
     torch.manual_seed(0)
     model = Net(args).cuda()
     opt = FusedOptimizer([p for p in model.parameters() if p.requires_grad], "adam", lr=1e-4)
@@ -61,14 +66,14 @@ def make_step(predict, mode):
     return run
 
 
-def make_eval(predict, mode):
+def make_eval(predict, mode, corners="destination"):
     import torch
     from lanedetection_end2end_b200 import ops_net
     from lanedetection_end2end_b200.engine import GraphedInference
     from lanedetection_end2end_b200.Networks.LSQ_layer import Net
     ops_net.set_conv_mode(mode)
     torch.manual_seed(0)
-    model = Net(make_args(predict)).cuda().eval()
+    model = Net(make_args(predict, corners)).cuda().eval()
     x = torch.rand(BATCH, 3, RESIZE, 2 * RESIZE, device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
     g = GraphedInference(model, x)
 
@@ -133,6 +138,33 @@ def kernel_arms():
     }
 
 
+def source_kernel_arms():
+    """The tables kernel and its backward of both parametrisations on the train.sh shapes, distinct per-image warps."""
+    import torch
+    from lanedetection_end2end_b200 import _capi
+    B, H = BATCH, RESIZE
+    g = torch.Generator(device="cuda").manual_seed(2)
+    f64 = dict(dtype=torch.float64, device="cuda")
+    M, Minv = torch.empty(B, 9, **f64), torch.empty(B, 9, **f64)
+    rowp, yk = torch.empty(B, H, 3, **f64), torch.empty(B, 56, **f64)
+    xtab, yrow = torch.empty(B, H * 2 * H, device="cuda"), torch.empty(B, H, device="cuda")
+    st = torch.zeros(1, dtype=torch.int32, device="cuda")
+    g_rowp = torch.randn(B, H, 3, generator=g, **f64)
+    g_minv, g_yk = torch.randn(B, 9, generator=g, **f64), torch.randn(B, 56, generator=g, **f64)
+    p = _capi.ptr
+    arms = {}
+    for name, nz, pdt, extra in (("lf_predicted_homography", 3, torch.float64, ()),
+                                 ("lf_predicted_homography_source", 5, torch.float32, (None,))):
+        z = torch.randn(B, nz, device="cuda", generator=g) * 0.5
+        prm, g_z = torch.empty(B, nz, dtype=pdt, device="cuda"), torch.empty(B, nz, device="cuda")
+        arms[name + "_tables"] = (lambda name=name, z=z, prm=prm: _capi.call(
+            name + "_tables", p(z), B, H, MASK_ROWS, 255.0, p(prm), p(M), p(Minv), p(rowp), p(xtab), p(yrow), p(yk), p(st),
+            _capi.stream_ptr()))
+        arms[name + "_bwd"] = (lambda name=name, z=z, g_z=g_z, extra=extra: _capi.call(
+            name + "_bwd", p(z), B, H, MASK_ROWS, p(g_rowp), p(g_minv), p(g_yk), p(g_z), *extra, _capi.stream_ptr()))
+    return arms
+
+
 def measured(build):
     """(callable, peak MB allocated while building it and running it three times, above the allocation before)."""
     import torch
@@ -148,31 +180,40 @@ def measured(build):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100", "bench_predict_homography.json"))
+    ap.add_argument("--corners", choices=["destination", "source"], default="destination")
+    ap.add_argument("--out", default=None)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--launches", type=int, default=200)
     a = ap.parse_args()
+    if a.out is None:
+        a.out = os.path.join(ROOT, "profiles", "h100", "bench_predict_homography%s.json"
+                             % ("_source" if a.corners == "source" else ""))
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_predict_homography.py needs a GPU")
     from lanedetection_end2end_b200 import ops_net
     default_mode = ops_net.CONV_MODE
     arms, peak = {}, {}
+    if a.corners == "source":
+        # (label, --predict_homography, --predict_homography_corners): each arm next to the others every round
+        variants = (("fixed", False, "destination"), ("destination", True, "destination"), ("source", True, "source"))
+    else:
+        variants = (("fixed", False, "destination"), ("predict", True, "destination"))
     for mode in ("tf32x3", "bf16"):
-        for predict in (False, True):
-            k = "%s/%s" % (mode, "predict" if predict else "fixed")
-            arms["step/" + k], peak["step/" + k] = measured(lambda: make_step(predict, mode))
-    for predict in (False, True):
-        k = "eval/tf32x3/%s" % ("predict" if predict else "fixed")
-        arms[k], peak[k] = measured(lambda: make_eval(predict, "tf32x3"))
+        for label, predict, corners in variants:
+            k = "%s/%s" % (mode, label)
+            arms["step/" + k], peak["step/" + k] = measured(lambda: make_step(predict, mode, corners))
+    for label, predict, corners in variants:
+        k = "eval/tf32x3/%s" % label
+        arms[k], peak[k] = measured(lambda: make_eval(predict, "tf32x3", corners))
     ops_net.set_conv_mode(default_mode)
-    kern = kernel_arms()
+    kern = source_kernel_arms() if a.corners == "source" else kernel_arms()
     for f in list(arms.values()) + list(kern.values()):
         time_events(f, 3)
     rec = {"arm_ms": {k: [] for k in arms}, "kernel_ms": {k: [] for k in kern}}
     for _ in range(a.rounds):
-        for k, f in arms.items():             # each arm next to its partner (fixed, then predict), every round
+        for k, f in arms.items():             # each arm next to its partners (fixed first), every round
             rec["arm_ms"][k].append(time_events(f, a.steps))
         for k, f in kern.items():
             rec["kernel_ms"][k].append(time_events(f, a.launches))
