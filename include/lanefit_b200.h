@@ -745,6 +745,45 @@ int lf_optim_step_pp(int algo, const LfOptimSegPP* segs, const int* slots, int n
                      const LfOptimHyper* hyper, long long* steps, int nparams, void* scalars, long long* skipped,
                      const int* status, lf_stream_t stream);
 
+/* Gradient clipping by the global L2 norm, torch.nn.utils.clip_grad_norm_(params, max_norm) before the update, inside the
+ * captured step.  `clip` is a DEVICE LfGradClip, zeroed once before first use, then max_norm set (> 0, finite; a
+ * replay reads its current value, so a new threshold needs no recapture).
+ * lf_grad_norm (lf_grad_norm_pp over an LfOptimSegPP table): one launch over the rows' gradients, chunked as the update
+ *   chunks them.  Each fp32 element is squared exactly in fp64 and summed in fp64, one partial per chunk into
+ *   `workspace` (DEVICE, lf_grad_norm_workspace_bytes(nchunks) bytes, 8-byte aligned); the last CTA (ticket, left at
+ *   zero) sums the partials in a fixed order.  Every order is set by the table alone, so the result is bit-identical
+ *   from run to run and does not depend on the grid size or on a gradient's alignment.  It writes
+ *     total_norm = fp32(sqrt(sum)), the sqrt in fp64 and rounded once;
+ *     clip_coef  = min(fl(fl(1 / fl(total_norm + fl(1e-6))) * max_norm), 1) in fp32, torch's op order (`max_norm /
+ *                  (total_norm + 1e-6)` is reciprocal() * max_norm), a NaN kept as torch.clamp keeps it;
+ *     nonfinite  = 1 exactly when some element is NaN or +-Inf, else 0.  The squares are non-negative and fp64 cannot
+ *                  overflow on their sum (each is below 2^256), so the sum is non-finite only through such an element.
+ *   The norm is more exact than torch's fp32 per-tensor norms and may differ from them in the last bits.
+ * lf_optim_step_clip / lf_optim_step_pp_clip: the update of lf_optim_step / lf_optim_step_pp with every gradient element
+ *   first multiplied by clip_coef (one fp32 rounding, torch's _foreach_mul_(grads, clip_coef)), then the same
+ *   arithmetic.  The gradients themselves are not rewritten.  The launch is skipped -- no parameter, state tensor or step
+ *   count changes -- when the status word is nonzero or `nonfinite` is set; each skipped launch increments the skipped
+ *   count, and one skipped by `nonfinite` alone (status NULL or zero) also increments clip->nonfinite_skipped.
+ * Never synchronise; graph-capturable.  Calls sharing `clip` or `workspace` must be ordered by the caller. */
+typedef struct LfGradClip {
+    float max_norm;                 /* in */
+    float total_norm;               /* out of the norm launch */
+    float clip_coef;                /* out of the norm launch */
+    int nonfinite;                  /* out of the norm launch */
+    long long nonfinite_skipped;    /* updates skipped by `nonfinite` alone */
+    unsigned long long ticket;
+} LfGradClip;
+size_t lf_grad_norm_workspace_bytes(long long nchunks);     /* HOST; 0 for nchunks <= 0 */
+int lf_grad_norm(const LfOptimSeg* segs, int nsegs, long long nchunks, LfGradClip* clip, void* workspace,
+                 size_t workspace_bytes, lf_stream_t stream);
+int lf_grad_norm_pp(const LfOptimSegPP* segs, int nsegs, long long nchunks, LfGradClip* clip, void* workspace,
+                    size_t workspace_bytes, lf_stream_t stream);
+int lf_optim_step_clip(int algo, const LfOptimSeg* segs, int nsegs, long long nchunks, const LfOptimHyper* hyper,
+                       LfOptimState* state, const int* status, LfGradClip* clip, lf_stream_t stream);
+int lf_optim_step_pp_clip(int algo, const LfOptimSegPP* segs, const int* slots, int nsegs, long long nchunks,
+                          const LfOptimHyper* hyper, long long* steps, int nparams, void* scalars, long long* skipped,
+                          const int* status, LfGradClip* clip, lf_stream_t stream);
+
 /* Baseline JPEG decode (csrc/jpeg.cu; replaces Image.open(f).convert('RGB') of BP/Dataloader/Load_Data_new.py:118-119):
  * a batch of same-size baseline (SOF0 / 8-bit SOF1, Huffman) single-scan JPEGs, YCbCr 4:4:4 / 4:2:2 / 4:2:0 or grayscale,
  * with or without restart markers -> uint8 RGB [N][H][W][3], bit-identical to Pillow (libjpeg-turbo: ISLOW IDCT, fancy

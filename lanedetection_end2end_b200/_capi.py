@@ -140,6 +140,11 @@ class LfOptimSegPP(ctypes.Structure):
     _fields_ = [("seg", LfOptimSeg), ("slot", _i), ("reserved", _i)]
 
 
+class LfGradClip(ctypes.Structure):
+    _fields_ = [("max_norm", _c_float), ("total_norm", _c_float), ("clip_coef", _c_float), ("nonfinite", _i),
+                ("nonfinite_skipped", _ll), ("ticket", ctypes.c_ulonglong)]
+
+
 STATUS_JPEG_CORRUPT = 8
 JPEG_PIECE_BYTES = 128
 JPEG_MAX_BPM = 6
@@ -192,6 +197,11 @@ _NET_PROTOS = {
     "lf_draw_lane_points": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _i, _p]),
     "lf_optim_step": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p]),
     "lf_optim_step_pp": (_i, [_i, _p, _p, _i, _ll, _p, _p, _i, _p, _p, _p, _p]),
+    "lf_grad_norm_workspace_bytes": (_c_size_t, [_ll]),
+    "lf_grad_norm": (_i, [_p, _i, _ll, _p, _p, _c_size_t, _p]),
+    "lf_grad_norm_pp": (_i, [_p, _i, _ll, _p, _p, _c_size_t, _p]),
+    "lf_optim_step_clip": (_i, [_i, _p, _i, _ll, _p, _p, _p, _p, _p]),
+    "lf_optim_step_pp_clip": (_i, [_i, _p, _p, _i, _ll, _p, _p, _i, _p, _p, _p, _p, _p]),
     "lf_wgrad_tcg_ctas": (_i, [_i, _i, _i, _i, _i, _i, _i]),
     "lf_wgrad_tcg": (_i, [ctypes.POINTER(LfWgradTcgArgs), _p]),
     "lf_reduce_multi": (_i, [ctypes.POINTER(LfReduceJob), _i, _p]),

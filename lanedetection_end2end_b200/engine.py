@@ -37,7 +37,9 @@ class GraphedTrainStep:
     system changes no parameter or optimizer state, with no host synchronisation.  With a reducer the guard reads the
     word's maximum over the ranks (one all-reduce of one element, ddp.any_rank_nonzero), so every rank skips or updates
     together and the replicas stay identical.  Each call writes the optimizer's
-    hyperparameters first if a param_groups value changed (schedulers work without a recapture).
+    hyperparameters first if a param_groups value changed (schedulers work without a recapture).  An optimizer with
+    ``max_grad_norm`` takes the gradients' norm after the reducer, so under data parallelism every rank clips by the same
+    coefficient and a non-finite gradient skips every rank's update.
 
     ``gt_line``: optional example [B, 4] tensor, cloned into a static buffer ``self.gt_line`` that the forward reads (the
     segmentation branch's substitution, end_to_end=False); default a host tensor of zeros.  The loss is
@@ -324,10 +326,13 @@ def _train_replays(loader, model, optimizer, static, fields, casts, post, report
     steps; after it the step's LSQ status word is logged (not with ``early_return``, which has no least-squares layer),
     and the reference's line for each skipped batch is printed at the end.  ``report(i, printing, saving, batch,
     post_out, (batch time, its average))`` runs at the print_freq / save_freq points of a batch that was not skipped:
-    the only host synchronisations before the end."""
+    the only host synchronisations before the end.  With gradient clipping on (``optimizer.max_grad_norm``), one line at
+    the end reports the updates that a non-finite gradient skipped during the epoch, if any."""
     dev = next(model.parameters()).device
     model.train()
     status = None if early_return else BatchStatus(len(loader), dev)
+    # a device copy of LfGradClip.nonfinite_skipped: reading the count here would add a synchronisation
+    nonfinite0 = None if optimizer.max_grad_norm is None else optimizer._clip[2].clone()
 
     def captured_post(out, loss):
         if not torch.cuda.is_current_stream_capturing():
@@ -374,6 +379,10 @@ def _train_replays(loader, model, optimizer, static, fields, casts, post, report
         model.defer_status_check = deferred
     if status is not None:
         status.print_skipped(labels)
+    if nonfinite0 is not None:
+        n = int((optimizer._clip[2] - nonfinite0).item())
+        if n:
+            print("%d of %d updates skipped: non-finite gradients" % (n, len(labels)))
     return step
 
 
@@ -467,8 +476,10 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     (bce_line.double() + bce_horizon.double()) * weight_class``.  --end_to_end False: criterion_seg(output, gt), with the
     least-squares fit and the rmse metric computed without gradient (main.py:306-318).  clip_grad_norm is accepted and does
     nothing: main.py:334-335 clips the gradients of the previous batch before zero_grad() discards them, so it never changes
-    an update.  Dropout masks are drawn in the graph from torch's graph-safe Philox offsets; they do not repeat an eager
-    run's masks.  BatchNorm running statistics are those of the epoch's batches (the capture's warm-up steps leave them as
+    an update.  Clipping is asked for on the optimizer instead (define_optim(..., fused=True, max_grad_norm=...)): the
+    update then scales the gradients by torch's clip_grad_norm_ coefficient, and an update that a non-finite gradient
+    skipped is reported in one line at the end of the epoch.  Dropout masks are drawn in the graph from torch's
+    graph-safe Philox offsets; they do not repeat an eager run's masks.  BatchNorm running statistics are those of the epoch's batches (the capture's warm-up steps leave them as
     they were).
 
     --pretrained needs a FusedOptimizer built with per_param_step=True (define_optim(..., fused=True,
@@ -621,7 +632,8 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
     main.py:246-253 forms it before losses.update: criterion_line_class on the line head's [B, 3, 4] logits against the
     loader's gt_line, criterion_horizon on the horizon head against gt_horizon.  --clas with other lane counts or
     --end_to_end False, --pretrained, loss policies other than area, orders other than 2 and other lane counts raise
-    ValueError (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch.  Dropout masks are drawn in the
+    ValueError (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch; clipping is asked
+    for on the optimizer (max_grad_norm), as there.  Dropout masks are drawn in the
     graph; BatchNorm running statistics are those of the epoch's batches."""
     from .optim import FusedOptimizer
     from .Loss_crit import fused_area_loss

@@ -13,8 +13,14 @@ for a batch with a singular system, as the reference's skip of that batch does (
 parameters with a gradient must not change.  ``per_param_step=True`` keeps one device count per parameter
 (lf_optim_step_pp), as torch.optim does: the set may change between updates, which a --pretrained run does by
 construction (its segmentation epochs train ``output_conv2``, its end-to-end epochs ``output_conv`` and the heads).
+
+``max_grad_norm`` clips the gradients by their global L2 norm inside the same captured update, as
+``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)`` followed by ``step()`` would (csrc/optim.cu: lf_grad_norm, then
+lf_optim_step_clip / lf_optim_step_pp_clip), and skips the update of a batch whose gradients hold a NaN or an Inf.
 """
 import ctypes
+import math
+import numbers
 
 import torch
 
@@ -33,8 +39,20 @@ STATE_KEYS = {"adam": ("exp_avg", "exp_avg_sq"), "sgd": ("momentum_buffer",), "r
 _UNSUPPORTED = ("amsgrad", "nesterov", "centered", "maximize")
 
 
+def _checked_max_norm(v):
+    """None, or ``v`` as a float that is positive and finite in fp32 (the kernel reads it as fp32); else ValueError."""
+    if v is None:
+        return None
+    if isinstance(v, numbers.Real) and not isinstance(v, bool):
+        f32 = torch.tensor(float(v), dtype=torch.float32).item()
+        if 0 < f32 < math.inf:
+            return float(v)
+    raise ValueError("FusedOptimizer max_grad_norm must be None or a positive finite float, got %r" % (v,))
+
+
 class FusedOptimizer(torch.optim.Optimizer):
-    """``FusedOptimizer(params, kind, lr, weight_decay, per_param_step=False)`` with kind in {"adam", "sgd", "rmsprop"}:
+    """``FusedOptimizer(params, kind, lr, weight_decay, per_param_step=False, max_grad_norm=None)`` with kind in
+    {"adam", "sgd", "rmsprop"}:
     the arguments and semantics of ``define_optim(kind, params, lr, weight_decay)`` (SGD and RMSprop with momentum 0.9),
     one parameter group.
 
@@ -46,9 +64,22 @@ class FusedOptimizer(torch.optim.Optimizer):
     the set may change between updates outside CUDA graph capture (the segment table is rebuilt; a graph captured
     earlier keeps its own table), a parameter without a gradient keeps its state and its count, and checkpoints may hold
     differing steps and parameters without state.  In this mode ``step_count`` is the largest per-parameter count, i.e.
-    the updates of the parameters that took part in the most of them."""
+    the updates of the parameters that took part in the most of them.
 
-    def __init__(self, params, kind="adam", lr=1e-3, weight_decay=0, per_param_step=False):
+    ``max_grad_norm``: None (no clipping), or a positive finite float: each update first computes the total L2 norm of
+    the gradients it applies and scales every gradient element by ``min(max_grad_norm / (norm + 1e-6), 1)``, torch's
+    ``clip_grad_norm_`` coefficient in torch's fp32 arithmetic, in both step modes.  It differs from ``clip_grad_norm_``
+    in three ways: the norm is accumulated in fp64 (more exact than torch's fp32 per-tensor norms, so it may differ from
+    theirs in the last bits); ``p.grad`` keeps the backward's values, the scaling happens inside the update; and a
+    gradient holding a NaN or an Inf skips the update -- no parameter, state tensor or step count changes, and both
+    ``skipped`` and ``nonfinite_skipped`` count it -- where torch would write NaN into the parameters.  Assigning
+    ``opt.max_grad_norm`` takes effect at the next ``step()`` or graph replay (sync_hyperparameters), without a
+    recapture.  ``grad_norm`` is the last clipped update's norm as a 0-dim fp32 device tensor (no synchronisation).
+    The reference's ``--clip_grad_norm`` flag is a different thing and still clips nothing (engine.train_epoch).
+    Under data parallelism the update runs after the gradient all-reduce, so every rank computes the same norm and
+    coefficient and skips together."""
+
+    def __init__(self, params, kind="adam", lr=1e-3, weight_decay=0, per_param_step=False, max_grad_norm=None):
         if kind not in _KINDS:
             raise ValueError("FusedOptimizer kind %r: expected one of %s" % (kind, sorted(_KINDS)))
         if not isinstance(per_param_step, bool):
@@ -56,6 +87,7 @@ class FusedOptimizer(torch.optim.Optimizer):
         cls, extra, self.algo = _KINDS[kind]
         self.kind = kind
         self.per_param_step = per_param_step
+        self._max_grad_norm = _checked_max_norm(max_grad_norm)
         # torch's own constructor validates the arguments and gives the exact defaults (= param_groups keys) of this version
         defaults = dict(cls([torch.zeros(1)], lr=lr, weight_decay=weight_decay, **extra).defaults)
         super().__init__(params, defaults)
@@ -68,6 +100,9 @@ class FusedOptimizer(torch.optim.Optimizer):
         self._counters = torch.zeros(3, dtype=torch.int64, device=dev)    # LfOptimState: step, skipped, ticket
         # per_param_step: the count of parameter i (its slot) whatever tables are built over it
         self._steps = torch.zeros(len(plist), dtype=torch.int64, device=dev) if per_param_step else None
+        # LfGradClip: max_norm, total_norm, clip_coef (fp32), nonfinite (int32); nonfinite_skipped, ticket (int64)
+        self._clip = torch.zeros(4, dtype=torch.int64, device=dev)
+        self._clip_host = None
         self._hyper_host = None
         self._table_key = None
         self._captured_tables = []
@@ -96,13 +131,30 @@ class FusedOptimizer(torch.optim.Optimizer):
             return (lr, 0.0, 0.0, 0.0, wd, float(g["momentum"]))
         return (lr, 0.0, float(g["alpha"]), float(g["eps"]), wd, float(g["momentum"]))
 
+    @property
+    def max_grad_norm(self):
+        return self._max_grad_norm
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, v):
+        v = _checked_max_norm(v)
+        if (v is None) != (self._max_grad_norm is None) and self._captured_tables:
+            raise ValueError("FusedOptimizer: a captured graph holds this optimizer's update %s clipping; assigning "
+                             "max_grad_norm can change the threshold but cannot turn clipping %s"
+                             % (("without", "on") if v is not None else ("with", "off")))
+        self._max_grad_norm = v
+
     def sync_hyperparameters(self):
-        """Write the device hyperparameter block if a ``param_groups`` value changed on the host (a scheduler's lr).
-        Not during capture: a replay reads whatever the block holds then."""
+        """Write the device hyperparameter block if a ``param_groups`` value changed on the host (a scheduler's lr), and
+        the clip threshold if ``max_grad_norm`` changed.  Not during capture: a replay reads whatever the block holds
+        then."""
         vals = self._hyper_values(self.param_groups[0])
         if vals != self._hyper_host:
             self._hyper.copy_(torch.tensor(vals, dtype=torch.float64))
             self._hyper_host = vals
+        if self._max_grad_norm is not None and self._max_grad_norm != self._clip_host:
+            self._clip.view(torch.float32)[:1].copy_(torch.tensor([self._max_grad_norm], dtype=torch.float32))
+            self._clip_host = self._max_grad_norm
 
     # -- segment table --------------------------------------------------------------------------------------------------
     def grad_params(self):
@@ -145,23 +197,33 @@ class FusedOptimizer(torch.optim.Optimizer):
             self._slots = (ctypes.c_int * len(rows))(*[r[6] for r in rows])
             self._scalars = torch.empty(len(rows) * _capi.OPTIM_PP_SCALAR_BYTES // 8, dtype=torch.int64,
                                         device=self._hyper.device)
+        # the norm launch's per-chunk partials (allocated here, outside any capture, whether or not clipping is on)
+        ws = _capi.lib().lf_grad_norm_workspace_bytes(chunk)
+        self._norm_ws = torch.empty(-(-ws // 8), dtype=torch.float64, device=self._hyper.device)
         self._table_key = key
 
     def launch(self, status=None):
         """The update over the prepared table on the current stream (capturable); ``status``: optional device int32 word,
-        nonzero = skip this update."""
+        nonzero = skip this update.  With ``max_grad_norm`` set, the norm launch comes first and the update reads its
+        coefficient and its non-finite flag."""
         per_elem = 20 if self.kind == "sgd" else 28
         if torch.cuda.is_current_stream_capturing() and not any(t[0] is self._table for t in self._captured_tables):
             # a replay reads them by address for as long as this object lives
-            self._captured_tables.append((self._table, self._scalars if self.per_param_step else None))
+            self._captured_tables.append((self._table, self._scalars if self.per_param_step else None, self._norm_ws))
+        clip = () if self._max_grad_norm is None else (ptr(self._clip),)
+        suffix = "" if self._max_grad_norm is None else "_clip"
+        if clip:
+            _capi.call("lf_grad_norm_pp" if self.per_param_step else "lf_grad_norm", ptr(self._table), self._nsegs,
+                       self._nchunks, ptr(self._clip), ptr(self._norm_ws), self._norm_ws.numel() * 8, _capi.stream_ptr(),
+                       nbytes=4 * self._nelem)
         if self.per_param_step:
             skipped = ctypes.c_void_p(self._counters.data_ptr() + self._counters.element_size())    # LfOptimState.skipped
-            _capi.call("lf_optim_step_pp", self.algo, ptr(self._table), self._slots, self._nsegs, self._nchunks,
+            _capi.call("lf_optim_step_pp" + suffix, self.algo, ptr(self._table), self._slots, self._nsegs, self._nchunks,
                        ptr(self._hyper), ptr(self._steps), self._steps.numel(), ptr(self._scalars), skipped, ptr(status),
-                       _capi.stream_ptr(), nbytes=per_elem * self._nelem)
+                       *clip, _capi.stream_ptr(), nbytes=per_elem * self._nelem)
         else:
-            _capi.call("lf_optim_step", self.algo, ptr(self._table), self._nsegs, self._nchunks, ptr(self._hyper),
-                       ptr(self._counters), ptr(status), _capi.stream_ptr(), nbytes=per_elem * self._nelem)
+            _capi.call("lf_optim_step" + suffix, self.algo, ptr(self._table), self._nsegs, self._nchunks, ptr(self._hyper),
+                       ptr(self._counters), ptr(status), *clip, _capi.stream_ptr(), nbytes=per_elem * self._nelem)
         self._started = True
 
     @torch.no_grad()
@@ -199,6 +261,18 @@ class FusedOptimizer(torch.optim.Optimizer):
     @property
     def skipped(self):
         return int(self._counters[1].item())
+
+    @property
+    def nonfinite_skipped(self):
+        """Updates skipped because a gradient held a NaN or an Inf (with max_grad_norm set; also counted in
+        ``skipped``).  One synchronisation."""
+        return int(self._clip[2].item())
+
+    @property
+    def grad_norm(self):
+        """The last clipped update's total gradient norm: a 0-dim fp32 view of device memory that the next clipped
+        update overwrites (0 before the first), read without a synchronisation."""
+        return self._clip.view(torch.float32)[1]
 
     # -- checkpoints in torch.optim's format ----------------------------------------------------------------------------
     def state_dict(self):
