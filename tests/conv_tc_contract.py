@@ -1,12 +1,16 @@
-"""The contract of the 3-tap tensor-core convolution (lf_conv1d_tc, lf_conv1d_tc_x3, lf_conv1d_tc_bf16 in
-csrc/conv_tc.cu) restated in fp64, and the per-entry gate its results are held to.
+"""The contract of the 3-tap tensor-core convolution (lf_conv1d_tc, lf_conv1d_tc_x3, lf_conv1d_tc_bf16,
+lf_conv1d_tc_fp8 in csrc/conv_tc.cu) restated in fp64, and the per-entry gate its results are held to.
 
 * Operands, bit for bit as the kernel feeds the tensor core (quantisers from tcg_contract.py):
     - TF32: activations tf32_rna (the kernel rounds each slab in shared memory); the weights are read from `wpack` as
       their fp32 bits, which wgmma .tf32 truncates (tf32_trunc; the ties class of the GPU tests pins it);
     - 3xTF32: the activations split hi = tf32_rna(a), lo = tf32_rna(a - hi); the weights pre-split by the packer
       (ops_net.split_tf32); the products hi*hi + hi*lo + lo*hi, lo*lo dropped;
-    - BF16: bf16_rne on both operands (a bf16 `in` is already exact).
+    - BF16: bf16_rne on both operands (a bf16 `in` is already exact);
+    - FP8: a_q = e4m3_rne_satfinite(fl32(x * fl32(448 / x_amax[n]))) per image n (0 where x_amax[n] = 0); the weights
+      are the e4m3 bytes of `wpack` as given (pack_weights quantises each output channel co with w_scale[co]).  The
+      exact sums are dequantised with dq[n, co] = fl32(fl32(x_amax[n] / 448) * w_scale[co]), the factor the kernel
+      forms: ref = dq * sum a_q w_q, S = dq * sum |a_q w_q|.
 * The reference: out[n,y,x,co] = sum_t sum_ci a_q[n, (y,x) + tap_t, ci] * w_q[co, t*C + ci] and S = sum |a_q w_q| per
   entry, in fp64 (products of quantised operands are exact there), zero outside the image.  Taps are any three (dy, dx):
   {-d, 0, +d} for the forward, {+d, 0, -d} for the input gradient, anything on the per-tap plan.
@@ -16,8 +20,11 @@ csrc/conv_tc.cu) restated in fp64, and the per-entry gate its results are held t
   so the gate needs no special case where a pre-ReLU value is within it of zero.
 * The gate: |got - ref| <= (c_tc + steps * 2^-23) * S' per entry, S' = S + |bias| + |add_src|, steps = 3 * C / 32 (one
   rounded FADD per tap and 32-channel chunk: each is summed from zero on the tensor core and added to the running fp32
-  sum), + 1 for the 3xTF32 acs + acc, + 1 per epilogue add.  c_tc covers the tensor core's in-instruction accumulation
-  (and for 3xTF32 the correction terms, which it accumulates over all taps and chunks).
+  sum), + 1 for the 3xTF32 acs + acc or the FP8 dequantising multiply, + 1 per epilogue add.  c_tc covers the tensor
+  core's in-instruction accumulation (and for 3xTF32 the correction terms, which it accumulates over all taps and
+  chunks).
+* FP8 out_amax: out_amax[n] is exactly the max |stored value| of image n (of the bf16 values for a bf16 `out`); an
+  image whose stored outputs are all zero leaves its zero-initialised entry untouched.
 * Per-CTA partials: row r of colsum_partial / stats_partial is the sum over the tiles m = r, r + m_ctas, ... of the
   kernel's stored (fp32) output: the sum, and the sum of squares or (affine mask) of out * x.  Each thread of the
   epilogue adds 8 rows per tile in one fp32 chain, and the 16 chains of a column are combined in fp64: chains of
@@ -25,16 +32,27 @@ csrc/conv_tc.cu) restated in fp64, and the per-entry gate its results are held t
 """
 import torch
 
-from tcg_contract import (C_TC_CEILING, LF_BF16, LF_F32, TC_BF16, TC_TF32, TC_X3, ULP, bf16_rna, bf16_rne,  # noqa: F401
-                          gate_excess, rel_err, split_tf32, tc_usage, tf32_rna, tf32_rne, tf32_trunc, with_low_bits)
+from oracle import fp8_oracle
+from tcg_contract import (C_TC_CEILING as _TCG_CEILING, LF_BF16, LF_F32, TC_BF16, TC_TF32, TC_X3, ULP,  # noqa: F401
+                          bf16_rna, bf16_rne, gate_excess, rel_err, split_tf32, tc_usage, tf32_rna, tf32_rne, tf32_trunc,
+                          with_low_bits)
 
+TC_FP8 = 3                                 # lf_conv1d_tc_plan's precision of lf_conv1d_tc_fp8
 KCH = 32                                   # channels per chunk (one 128-byte swizzle row of fp32)
 TILE = 128                                 # pixels per tile
-# c_tc per precision (0 = TF32, 1 = 3xTF32, 2 = BF16).  Ceilings as for the tcg kernels (tcg_contract.C_TC_CEILING): well
-# below the half-step of the operand rounding, so that the rounding mutations keep breaking the gate.
-C_TC = {TC_TF32: 2.0 ** -21, TC_X3: 2.0 ** -21, TC_BF16: 2.0 ** -21}
-PREC_NAMES = {TC_TF32: "tf32", TC_X3: "tf32x3", TC_BF16: "bf16"}
-ENTRIES = {TC_TF32: "lf_conv1d_tc", TC_X3: "lf_conv1d_tc_x3", TC_BF16: "lf_conv1d_tc_bf16"}
+E4M3_MIN_NORMAL = 2.0 ** -6
+# c_tc per precision (0 = TF32, 1 = 3xTF32, 2 = BF16, 3 = FP8).  Ceilings as for the tcg kernels
+# (tcg_contract.C_TC_CEILING): well below the half-step of the operand rounding, so that the rounding mutations keep
+# breaking the gate.  FP8: the H100's e4m3 wgmma sums the 32 products of one k32 step with fewer mantissa bits than fp32,
+# aligned to the group's largest product.  Measured on an H100 80GB HBM3 (700 W): about 2^-15.4 of the sum of |products|
+# on Gaussian activations, but up to 2^-10.1 over the FP8 cases of tests/test_conv_tc_contract_gpu.py, from the
+# heavy-tailed ones, where one product dominates each group and the other 31 lose their low bits against it (the same
+# error with activations that are e4m3 values already, x_amax = 448 and inv = 1: none of it is quantisation).  2^-9
+# keeps 2.1x headroom over that; the ceiling 2^-8 stays 8x below e4m3's smallest relative half-step (2^-5).
+C_TC = {TC_TF32: 2.0 ** -21, TC_X3: 2.0 ** -21, TC_BF16: 2.0 ** -21, TC_FP8: 2.0 ** -9}
+C_TC_CEILING = {**_TCG_CEILING, TC_FP8: 2.0 ** -8}
+PREC_NAMES = {TC_TF32: "tf32", TC_X3: "tf32x3", TC_BF16: "bf16", TC_FP8: "fp8"}
+ENTRIES = {TC_TF32: "lf_conv1d_tc", TC_X3: "lf_conv1d_tc_x3", TC_BF16: "lf_conv1d_tc_bf16", TC_FP8: "lf_conv1d_tc_fp8"}
 
 
 def tap_list(vertical, dil, transposed=False):
@@ -46,10 +64,43 @@ def tap_list(vertical, dil, transposed=False):
 # ---------------------------------------------------------------------------------------------------------------------
 # operands
 # ---------------------------------------------------------------------------------------------------------------------
-def act_terms(x, prec, rounding=None):
+def e4m3_rne(v):
+    """cvt.rn.satfinite.e4m3x2.f32: round fp32 to e4m3 (nearest even, subnormals kept), saturated to +-448; as fp32."""
+    return fp8_oracle.e4m3(v)
+
+
+def e4m3_ftz(v):
+    """e4m3 rounding with the subnormal results flushed to zero (NOT what the kernel does: a sensitivity check)."""
+    q = e4m3_rne(v)
+    return torch.where(q.abs() < E4M3_MIN_NORMAL, torch.zeros_like(q), q)
+
+
+def e4m3_rtz(v):
+    """e4m3 rounding toward zero (NOT what the kernel does: a sensitivity check): the nearest value, one code lower in
+    magnitude wherever that rounded away from zero."""
+    q = e4m3_rne(v)
+    b = q.to(torch.float8_e4m3fn).view(torch.uint8)
+    down = (b.to(torch.int16) - 1).clamp_min(0).to(torch.uint8).view(torch.float8_e4m3fn).float()
+    return torch.where((q.abs() > v.abs()) & (q != 0), down, q)
+
+
+def fp8_inv(x_amax):
+    """[N] fp32: 448 / x_amax[n], IEEE division as the kernel's __fdiv_rn, 0 where x_amax[n] = 0."""
+    return fp8_oracle.inverse_scale(x_amax.float())
+
+
+def fp8_dq(x_amax, w_scale):
+    """[N, C] fp32: the dequantisation factors fl32(fl32(x_amax[n] / 448) * w_scale[co])."""
+    return fp8_oracle.scale(x_amax.float()).view(-1, 1) * w_scale.float().view(1, -1)
+
+
+def act_terms(x, prec, rounding=None, x_amax=None):
     """The activation operand(s) the tensor core multiplies, fp64: [a_q] or, for 3xTF32, [a_hi, a_lo].
-    rounding: override the kernel's rounding (the sensitivity checks)."""
+    rounding: override the kernel's rounding (the sensitivity checks).  FP8: x_amax [N] is the per-image scale."""
     x = x.float()
+    if prec == TC_FP8:
+        v = x * fp8_inv(x_amax).view(-1, 1, 1, 1)          # one fp32 multiply, rounded to nearest
+        return [(rounding or e4m3_rne)(v).double()]
     if prec == TC_X3:
         hi = (rounding or tf32_rna)(x)
         return [hi.double(), tf32_rna(x - hi).double()]
@@ -65,11 +116,23 @@ def weight_terms(wpack, prec, rounding=None):
         return [wpack[0].double(), wpack[1].double()]
     if prec == TC_BF16:
         return [wpack.double()]
+    if prec == TC_FP8:
+        return [wpack.view(torch.float8_e4m3fn).double()]
     return [(rounding or tf32_trunc)(wpack).double()]
 
 
+def fp8_weight_scale(w):
+    """[C] fp32 w_scale of the FP8 operand of the [C][3C] slot matrix w: max |w[co]| / 448."""
+    return fp8_oracle.scale(w.float().abs().amax(1))
+
+
 def pack_weights(w, prec):
-    """The packed operand ([C][3C] fp32) in the form the entry point takes."""
+    """The packed operand ([C][3C] fp32) in the form the entry point takes.  FP8: [C][3C] uint8 holding the e4m3 bytes
+    of w[co] * (448 / max |w[co]|), each output channel quantised on its own (its w_scale: fp8_weight_scale)."""
+    if prec == TC_FP8:
+        wf = w.float()
+        q = e4m3_rne(wf * fp8_oracle.inverse_scale(wf.abs().amax(1)).view(-1, 1))
+        return q.to(torch.float8_e4m3fn).view(torch.uint8).contiguous()
     if prec == TC_X3:
         hi, lo = split_tf32(w)
         return torch.stack([hi, lo]).contiguous()
@@ -111,12 +174,19 @@ def _tap_operand(a, t, taps, C, mut):
     return s.reshape(-1, C)
 
 
-def conv_fp64(x, wpack, prec, taps, a_round=None, w_round=None, **mut):
-    """(ref, S) [N*H*W, C] in fp64 of the bare convolution (no epilogue), from the quantised operands.
+def conv_fp64(x, wpack, prec, taps, a_round=None, w_round=None, scales=None, **mut):
+    """(ref, S) [N*H*W, C] in fp64 of the bare convolution (no epilogue), from the quantised operands; FP8: dequantised,
+    scales = (x_amax [N], w_scale [C]).
     Mutations (sensitivity checks): shift_tap = t; drop_chunk = (t, cb); halo_zero = (t, TA, vertical);
-    drop_lo_hi (3xTF32: a_lo * w_hi dropped); a_round / w_round: other operand roundings."""
+    drop_lo_hi (3xTF32: a_lo * w_hi dropped); a_round / w_round: other operand roundings; next_image_scale (FP8: image n
+    quantised and dequantised with image n+1's x_amax, the last with image 0's)."""
     N, H, W, C = x.shape
-    A = act_terms(x, prec, a_round)
+    x_amax = None
+    if prec == TC_FP8:
+        x_amax, w_scale = scales
+        if mut.get("next_image_scale"):
+            x_amax = x_amax.roll(-1)
+    A = act_terms(x, prec, a_round, x_amax)
     Wt = weight_terms(wpack, prec, w_round)
     if prec == TC_X3:
         pairs = [(0, 0), (0, 1)] + ([] if mut.get("drop_lo_hi") else [(1, 0)])
@@ -130,7 +200,20 @@ def conv_fp64(x, wpack, prec, taps, a_round=None, w_round=None, **mut):
             w = Wt[j][:, t * C:(t + 1) * C]
             ref += views[i] @ w.t()
             S += views[i].abs() @ w.abs().t()
+    if prec == TC_FP8:
+        dq = per_pixel(fp8_dq(x_amax, w_scale).double(), H * W)
+        ref, S = ref * dq, S * dq
     return ref, S
+
+
+def per_pixel(t, pixels_per_image):
+    """[N, ...] -> [N * pixels_per_image, ...]: each image's row repeated for its pixels (NHW order)."""
+    return t.repeat_interleave(pixels_per_image, 0)
+
+
+def image_amax(out, N):
+    """[N] fp32: the per-image max |stored value| FP8 reduces into out_amax (0 for an all-zero image)."""
+    return out.float().abs().reshape(N, -1).amax(1)
 
 
 def epilogue(z, S, bias=None, relu=0, mask_src=None, mask_affine=None, add_src=None, add_mask=None):
@@ -159,9 +242,9 @@ def epilogue(z, S, bias=None, relu=0, mask_src=None, mask_affine=None, add_src=N
 
 
 def steps(C, prec, adds):
-    """Rounded fp32 adds per output entry beyond the tensor core's own: one per tap and chunk, the 3xTF32 acs + acc,
-    and the epilogue's adds."""
-    return 3 * C // KCH + (1 if prec == TC_X3 else 0) + adds
+    """Rounded fp32 operations per output entry beyond the tensor core's own: one add per tap and chunk, the 3xTF32
+    acs + acc or the FP8 dequantising multiply, and the epilogue's adds."""
+    return 3 * C // KCH + (1 if prec in (TC_X3, TC_FP8) else 0) + adds
 
 
 def excess(got, ref, S, nsteps, prec, c_tc=None):
@@ -205,13 +288,15 @@ def partial_steps(N, H, W, plan):
 # ---------------------------------------------------------------------------------------------------------------------
 # a kernel-faithful fp32 emulation (the CPU tests hold it to the gate)
 # ---------------------------------------------------------------------------------------------------------------------
-def emulate(x, wpack, prec, taps, plan, bias=None, relu=0, mask_src=None, mask_affine=None, add_src=None, add_mask=None):
+def emulate(x, wpack, prec, taps, plan, bias=None, relu=0, mask_src=None, mask_affine=None, add_src=None, add_mask=None,
+            scales=None):
     """(out [P, C] fp32, colsum [m_ctas, C] fp32, stats [m_ctas, 2, C] fp64) as the kernel forms them: each tap and
     32-channel chunk summed from zero (here exactly, then rounded to fp32), added to the fp32 sum with a rounded add;
-    3xTF32's correction terms summed apart and added last; the epilogue in fp32; the partials as fp32 chains of 8 rows
-    per tile, the 16 chains of a column combined in fp64."""
+    3xTF32's correction terms summed apart and added last; FP8's sum times its fp32 dequantisation factor, rounded; the
+    epilogue in fp32; the partials as fp32 chains of 8 rows per tile, the 16 chains of a column combined in fp64 (FP8
+    takes no partials: its out_amax is image_amax(out))."""
     N, H, W, C = x.shape
-    A = act_terms(x, prec)
+    A = act_terms(x, prec, x_amax=scales[0] if prec == TC_FP8 else None)
     Wt = weight_terms(wpack, prec)
     P = N * H * W
     acc = torch.zeros(P, C, dtype=torch.float32, device=x.device)
@@ -225,6 +310,8 @@ def emulate(x, wpack, prec, taps, plan, bias=None, relu=0, mask_src=None, mask_a
             if prec == TC_X3:
                 small += views[0] @ wcols[1].t() + views[1] @ wcols[0].t()
     o = small.float() + acc if prec == TC_X3 else acc
+    if prec == TC_FP8:
+        o = o * per_pixel(fp8_dq(*scales), H * W)
     if bias is not None:
         o = o + bias.float().view(1, C)
     if relu & 1:
@@ -276,7 +363,7 @@ def query_plan(prec, in_dtype, N, H, W, C, taps):
 def plan_key(prec, in_dtype, C, plan):
     """The kernel instantiation and shared-memory plan a launch reached: (C, precision, bf16 input, resident weights,
     slab, 3xTF32 lo plan, single stage).  lo plan: "2" / "1" buffers after the ring, "stg" over the staging tile,
-    "stg+" over it and reaching back before it; "-" for TF32 / BF16."""
+    "stg+" over it and reaching back before it; "-" for TF32 / BF16 / FP8."""
     lo = "-"
     if prec == TC_X3:
         lo = ("stg+" if plan["lo_bytes"] else "stg") if plan["lo_stg"] else str(plan["n_lo"])
@@ -326,6 +413,17 @@ COVERAGE = [
     ((TC_X3, False, 64, 32, 40, False, 4, 2), (64, "tf32x3", False, True, True, "stg", False)),
     ((TC_X3, False, 64, 32, 40, False, 6, 2), (64, "tf32x3", False, True, True, "stg+", False)),
     ((TC_X3, False, 64, 32, 40, False, 7, 2), (64, "tf32x3", False, True, True, "stg+", True)),
+    ((TC_FP8, False, 128, 40, 160, True, 17, 2), (128, "fp8", False, False, True, "-", False)),
+    ((TC_FP8, False, 128, 32, 256, True, 80, 2), (128, "fp8", False, False, True, "-", True)),
+    ((TC_FP8, False, 128, 32, 4, True, 1, 2), (128, "fp8", False, True, False, "-", False)),
+    ((TC_FP8, False, 128, 32, 64, True, 1, 2), (128, "fp8", False, True, True, "-", False)),
+    ((TC_FP8, True, 128, 32, 64, False, 4, 1), (128, "fp8", True, True, False, "-", False)),
+    ((TC_FP8, True, 128, 40, 80, True, 2, 2), (128, "fp8", True, True, True, "-", False)),
+    ((TC_FP8, False, 64, 32, 256, True, 80, 2), (64, "fp8", False, False, True, "-", True)),
+    ((TC_FP8, False, 64, 64, 128, False, 1, 1), (64, "fp8", False, True, False, "-", False)),
+    ((TC_FP8, False, 64, 64, 128, True, 1, 2), (64, "fp8", False, True, True, "-", False)),
+    ((TC_FP8, True, 64, 32, 4, True, 1, 2), (64, "fp8", True, True, False, "-", False)),
+    ((TC_FP8, True, 64, 32, 32, True, 1, 2), (64, "fp8", True, True, True, "-", False)),
 ]
 
 
@@ -344,8 +442,8 @@ def universe_keys():
     found = {}
     for variant in (2, 1):
         def scan():
-            for prec in (TC_TF32, TC_X3, TC_BF16):
-                for abf in ((False, True) if prec == TC_BF16 else (False,)):
+            for prec in (TC_TF32, TC_X3, TC_BF16, TC_FP8):
+                for abf in ((False, True) if prec in (TC_BF16, TC_FP8) else (False,)):
                     for C in (64, 128):
                         for H in UNIVERSE_EXTENTS:
                             for W in UNIVERSE_EXTENTS:

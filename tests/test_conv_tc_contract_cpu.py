@@ -1,9 +1,13 @@
 """The fp64 contract of the 3-tap tensor-core convolution (tests/conv_tc_contract.py) checked without a GPU:
   * the restatement agrees with torch's float64 conv2d / conv_transpose2d for both tap orders, and with explicit shifted
-    sums for any three taps, and its epilogue with the formulas of include/lanefit_b200.h;
+    sums for any three taps, and its epilogue with the formulas of include/lanefit_b200.h; the FP8 restatement agrees with
+    conv2d of the separately quantised operands, dequantised per image and output channel, and its e4m3 quantiser
+    rounds to nearest even, keeps subnormals and saturates at 448;
   * a kernel-faithful fp32 emulation passes the gate at every precision, its per-CTA partials included;
   * each seeded bug fails the gate: a tap shifted by one pixel, a dropped chunk, a halo row read as zero, RNE instead of
     RNA, a dropped a_lo * w_hi, rounded instead of truncated weights on the ties class, a tile-to-CTA map shifted by one;
+    for FP8 also image n quantised and dequantised with image n+1's scale, flushed e4m3 subnormals and round-toward-zero
+    on e4m3 midpoints;
   * lf_conv1d_tc_plan reports every planner outcome the coverage table of the GPU tests claims, and that table reaches
     every outcome the planner produces over a wide range of shapes;
   * every argument check of the three entry points (and of the plan query) refuses with LF_ERR_INVALID_ARGUMENT before
@@ -36,6 +40,29 @@ def _x(N, H, W, C, seed, cls="randn"):
         x = cc.with_low_bits(x.abs() + 2.0 ** -20, 0x8000, 16)
         w = cc.bf16_rne(w.abs())
     return x, w, g
+
+
+def e4m3_midpoints(shape, generator, device=None):
+    """Non-negative values exactly half way between two adjacent e4m3 values (subnormal and normal, below 448)."""
+    codes = torch.randint(0, 0x7e, shape, generator=generator, device=device, dtype=torch.int16)   # 0x7e = 448
+    lo = codes.to(torch.uint8).view(torch.float8_e4m3fn).float()
+    hi = (codes + 1).to(torch.uint8).view(torch.float8_e4m3fn).float()
+    return (lo + hi) / 2
+
+
+def _x_fp8(N, H, W, C, seed, cls="randn"):
+    """FP8 operands: activations with per-image scales 10^-3 .. 10^3, or (subnormal) one outlier per image that puts most
+    quantised activations among the e4m3 subnormals, or (ties) e4m3 midpoints under x_amax = 448 (inv = 1 exactly);
+    -> (x, w, x_amax, generator)"""
+    x, w, g = _x(N, H, W, C, seed)
+    if cls == "ties":
+        x = e4m3_midpoints((N, H, W, C), g)
+        return x, w.abs(), torch.full((N,), 448.0), g
+    x = x * (10.0 ** torch.linspace(-3, 3, N)).view(-1, 1, 1, 1)[torch.randperm(N, generator=g)]
+    if cls == "subnormal":
+        big = x.abs().flatten(1).amax(1) * 2.0 ** 14
+        x.view(N, -1)[:, 7] = big
+    return x, w, x.abs().flatten(1).amax(1), g
 
 
 def _plan(N, H, W, C, taps, prec=cc.TC_TF32):
@@ -97,6 +124,58 @@ def test_reference_any_three_taps_and_x3_terms():
     whi, wlo = wp[0].double(), wp[1].double()
     full = _plain(hi + lo, whi + wlo, taps)
     assert torch.allclose(r3, full - _plain(lo, wlo, taps), rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("N,H,W,C,vertical,dil", SMALL)
+@pytest.mark.parametrize("transposed", [False, True])
+def test_fp8_reference_matches_torch_conv_of_quantised_operands(N, H, W, C, vertical, dil, transposed):
+    """FP8: the restatement is float64 conv2d / conv_transpose2d of the activations quantised per image and the weights
+    quantised per output channel (oracle/fp8_oracle.py), times the fp32 factors (x_amax[n] / 448) * w_scale[co]; an
+    all-zero image and an all-zero output channel give exactly 0."""
+    from oracle import fp8_oracle as fo
+    x, w, x_amax, _ = _x_fp8(N, H, W, C, dil + 3 * transposed)
+    x[N // 2] = 0
+    x_amax[N // 2] = 0
+    w[5] = 0
+    wp, sw = cc.pack_weights(w, cc.TC_FP8), cc.fp8_weight_scale(w)
+    ref, S = cc.conv_fp64(x, wp, cc.TC_FP8, cc.tap_list(vertical, dil, transposed), scales=(x_amax, sw))
+    w4 = _w4(w, C, vertical)
+    qw, sw4 = fo.quantize_weight(w4)
+    assert torch.equal(sw4, sw) and torch.equal(_w4(cc.weight_terms(wp, cc.TC_FP8)[0].float(), C, vertical), qw)
+    qx = fo.quantize_act(_nchw(x), x_amax).double()
+    pad, dl = ((dil, 0), (dil, 1)) if vertical else ((0, dil), (1, dil))
+    if transposed:
+        t = F.conv_transpose2d(qx, qw.double().transpose(0, 1), padding=pad, dilation=dl)
+    else:
+        t = F.conv2d(qx, qw.double(), padding=pad, dilation=dl)
+    dq = (fo.scale(x_amax).view(-1, 1, 1, 1) * sw.view(1, -1, 1, 1)).double()
+    want = (t * dq).permute(0, 2, 3, 1).reshape(-1, C)
+    assert torch.allclose(ref, want, rtol=0, atol=1e-12 * float(S.max()))
+    assert bool((S >= ref.abs() - 1e-12 * float(S.max())).all())
+    zero = ref.view(N, H, W, C)
+    assert not bool(zero[N // 2].any()) and not bool(zero[..., 5].any())
+
+
+def test_e4m3_quantiser_is_round_to_nearest_even_satfinite():
+    """e4m3_rne (cvt.rn.satfinite.e4m3x2.f32) on every code: itself; half way between two codes, the even one (also
+    between the subnormals and across the normal boundary); just off half way, the nearer one; beyond 448, 448.  And the
+    two sensitivity roundings differ from it where they should."""
+    codes = torch.arange(0, 0x7f, dtype=torch.int16)                     # 0 .. 448 (0x7f is NaN)
+    v = codes.to(torch.uint8).view(torch.float8_e4m3fn).float()
+    assert v[1] == 2.0 ** -9 and v[8] == 2.0 ** -6 and v[-1] == 448.0
+    for s in (1.0, -1.0):
+        assert torch.equal(cc.e4m3_rne(s * v), s * v)
+        mid = s * (v[:-1] + v[1:]) / 2
+        even = torch.where(codes[:-1] % 2 == 0, v[:-1], v[1:])
+        assert torch.equal(cc.e4m3_rne(mid), s * even)
+        up = torch.nextafter(mid, torch.full_like(mid, s * 1e9))
+        assert torch.equal(cc.e4m3_rne(up), s * v[1:])
+        assert torch.equal(cc.e4m3_rne(torch.nextafter(mid, torch.zeros_like(mid))), s * v[:-1])
+        assert torch.equal(cc.e4m3_rtz(mid), s * v[:-1])
+        big = torch.tensor([448.5, 464.0, 480.0, 1e6, float("inf")]) * s
+        assert torch.equal(cc.e4m3_rne(big), torch.full_like(big, 448.0 * s))
+    sub = v[1:8]
+    assert torch.equal(cc.e4m3_ftz(sub), torch.zeros_like(sub)) and torch.equal(cc.e4m3_ftz(v[8:]), v[8:])
 
 
 def _plain(a, w, taps):
@@ -199,7 +278,47 @@ def test_emulation_passes_and_seeded_bugs_fail(prec, si):
             assert cc.excess(cc.partial_fp64(vals, (rows + 1) % 3, 3), pref, pS, psteps, prec, c_tc=0.0) > 1.0
 
 
-@pytest.mark.parametrize("prec,cls", [(cc.TC_TF32, "ties"), (cc.TC_TF32, "ties_w"), (cc.TC_BF16, "ties_bf16")])
+FP8_EPI = [s for s in EPI if "affine" not in s]          # lf_conv1d_tc_fp8 takes no affine mask (nor partials)
+
+
+@pytest.mark.parametrize("cls", ["randn", "subnormal", "ties"])
+@pytest.mark.parametrize("si", range(len(SMALL)))
+def test_fp8_emulation_passes_and_seeded_bugs_fail(si, cls):
+    """the FP8 emulation passes the gate and its out_amax is the per-image max; a shifted tap, a dropped chunk, a halo row
+    read as zero, the next image's scale, flushed subnormals (subnormal class) and round-toward-zero (ties class) fail"""
+    N, H, W, C, vertical, dil = SMALL[si]
+    N = max(N, 3)                                        # images with different scales
+    for transposed in (False, True):
+        taps = cc.tap_list(vertical, dil, transposed)
+        pl = _plan(N, H, W, C, taps, cc.TC_FP8)
+        x, w, x_amax, g = _x_fp8(N, H, W, C, 10 * si + transposed, cls)
+        wp, sw = cc.pack_weights(w, cc.TC_FP8), cc.fp8_weight_scale(w)
+        kw = _epi_tensors(FP8_EPI[(si + 2 * transposed) % len(FP8_EPI)], N, H, W, C, g)
+        out, _, _ = cc.emulate(x, wp, cc.TC_FP8, taps, pl, scales=(x_amax, sw), **kw)
+        z, S = cc.conv_fp64(x, wp, cc.TC_FP8, taps, scales=(x_amax, sw))
+        ref, Sp, adds = cc.epilogue(z, S, **kw)
+        nsteps = cc.steps(C, cc.TC_FP8, adds)
+        assert cc.excess(out, ref, Sp, nsteps, cc.TC_FP8) <= 1.0
+        am = cc.image_amax(out, N)
+        assert torch.equal(am, out.abs().view(N, -1).amax(1)) and len(set(am.tolist())) == N
+
+        def fails(**m):
+            r = cc.epilogue(cc.conv_fp64(x, wp, cc.TC_FP8, taps, scales=(x_amax, sw), **m)[0], S, **kw)[0]
+            return cc.excess(r, ref, Sp, nsteps, cc.TC_FP8) > 1.0
+        assert fails(shift_tap=1), "a tap shifted by one pixel"
+        assert fails(drop_chunk=(1, C // cc.KCH - 1)), "a dropped chunk"
+        t_neg = 0 if (taps[0][0] if vertical else taps[0][1]) < 0 else 2
+        if (H if vertical else W) > pl["TA"] and dil < (H if vertical else W):
+            assert fails(halo_zero=(t_neg, pl["TA"], pl["vertical"])), "a halo row read as zero"
+        if cls == "ties":
+            assert fails(a_round=cc.e4m3_rtz), "round toward zero"
+        else:
+            assert fails(next_image_scale=True), "image n with image n+1's scale"
+        if cls == "subnormal":
+            assert fails(a_round=cc.e4m3_ftz), "flushed e4m3 subnormals"
+
+
+@pytest.mark.parametrize("prec,cls",[(cc.TC_TF32, "ties"), (cc.TC_TF32, "ties_w"), (cc.TC_BF16, "ties_bf16")])
 def test_rounding_mutations_fail_on_ties(prec, cls):
     """on ties the kernel's rounding passes and every other rounding fails: RNE for the TF32 activations' RNA, RNA for the
     bf16 RNE, rounding (either way) for the truncated TF32 weights"""

@@ -430,6 +430,11 @@ def test_net_misc_refuses_bad_arguments():
     assert h.lf_nhwc_to_nchw(P_, 70000, 4, 4, 4, P_, None) == -1
     assert h.lf_pack_gather(None, 1, 1, None) == -1 and h.lf_pack_gather(P_, 0, 1, None) == -1
     assert h.lf_pack_gather(P_, 1, 0, None) == -1 and h.lf_pack_gather(P_, 70000, 1, None) == -1
+    # lf_amax_per_image: 8 elements per step (per_image % 8), one grid row per image (N <= 65535), fp32 / bf16 only
+    for a in ((None, 0, 8, 1, P_), (P_, 0, 8, 1, None), (P_, 0, 12, 1, P_), (P_, 1, 4, 1, P_), (P_, 0, 0, 1, P_),
+              (P_, 0, -8, 1, P_), (P_, 0, 8, 0, P_), (P_, 0, 8, -1, P_), (P_, 0, 8, 65536, P_), (P_, 2, 8, 1, P_),
+              (P_, -1, 8, 1, P_)):
+        assert h.lf_amax_per_image(*a, None) == -1, a
 
 
 # ---------------------------------------------------------------------------------------------------------------------

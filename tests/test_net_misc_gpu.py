@@ -397,3 +397,55 @@ def test_pack_gather(blocks_per_job):
     hi = fc.pack_gather(src, torch.arange(5000, device=DEV, dtype=torch.int32) | fc.PACK_TF32_HI)
     lo = fc.pack_gather(src, torch.arange(5000, device=DEV, dtype=torch.int32) | fc.PACK_TF32_LO)
     assert bool(((hi.double() + lo.double() - src.double()).abs() <= 2.0 ** -22 * src.double().abs()).all())
+
+
+# =====================================================================================================================
+# per-image max |x| (the activation scale of an fp8 convolution whose input is not an fp8 convolution's output)
+# =====================================================================================================================
+AMAX_GUARD = 2.0 ** -149     # atomicMax on the float bits only raises an entry: any stray maximum overwrites this
+
+
+def _amax_input(N, per_image, g):
+    """[N, per_image] fp32: images at scales 10^-3 .. 10^3 with -0.0 entries; the only image of N = 1 and image 1 of
+    N >= 4 hold only subnormals (of fp32 and of bf16) and -0.0, image 2 a +inf, image N // 2 only zeros (half of them
+    -0.0); the last image's maximum is its last element, negative"""
+    x = _randn((N, per_image), g) * (10.0 ** torch.linspace(-3, 3, N, device=DEV)).view(-1, 1)
+    sub = 1 if N >= 4 else 0 if N == 1 else None
+    if sub is not None:
+        x[sub] = _randn((per_image,), g).clamp(-3.9, 3.9) * 2.0 ** -128
+    x[:, 1::5] = -0.0
+    if N >= 4:
+        x[2, per_image // 3] = float("inf")
+        x[N // 2] = 0.0
+        x[N // 2, ::2] = -0.0
+    x[-1, -1] = -2 * x[-1].abs().max()
+    return x
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16], ids=["f32", "bf16"])
+@pytest.mark.parametrize("N,per_image", [(1, 8), (7, 8), ("many", 8), (1, 2048 * 3 + 8), (7, 2048 * 5 + 8),
+                                         ("many", 2048 + 8), (1, 4 * 1024 * 1024 + 8), (7, 4 * 1024 * 1024)])
+def test_amax_per_image_exact(N, per_image, dtype):
+    """lf_amax_per_image == x.abs().flatten(1).amax(1) exactly: one element per image, a tail past a multiple of the
+    8 x 256 elements a CTA covers per step, several CTAs per image (4M elements), and more images than 4 x the SM count
+    (one CTA each); -0.0, fp32 subnormals, +inf and an all-zero image (which keeps its 0)"""
+    c = _capi()
+    if N == "many":
+        N = 4 * torch.cuda.get_device_properties(0).multi_processor_count + 5
+    x = _amax_input(N, per_image, _gen(N + per_image)).to(dtype)
+    want = x.float().abs().flatten(1).amax(1)
+    buf = torch.full((2 * GUARD + N,), AMAX_GUARD, device=DEV)
+    buf[GUARD:GUARD + N] = 0
+    c.call("lf_amax_per_image", _p(x), c.dtype_id(x), per_image, N, _p(buf[GUARD:]), _st())
+    torch.cuda.synchronize()
+    assert bool((buf[:GUARD] == AMAX_GUARD).all()) and bool((buf[GUARD + N:] == AMAX_GUARD).all()), "wrote outside amax"
+    got = buf[GUARD:GUARD + N]
+    assert torch.equal(got, want), (got.tolist()[:8], want.tolist()[:8])
+    if N >= 4:
+        assert got[N // 2] == 0 and got[2] == float("inf") and 0 < float(got[1]) < 2.0 ** -126
+    if N == 1:
+        assert 0 < float(got[0]) < 2.0 ** -125
+    # amax[n] = max(amax[n], ...): a second pass over the same input changes nothing
+    c.call("lf_amax_per_image", _p(x), c.dtype_id(x), per_image, N, _p(buf[GUARD:]), _st())
+    torch.cuda.synchronize()
+    assert torch.equal(buf[GUARD:GUARD + N], want)
