@@ -598,6 +598,47 @@ int lf_lsq_grid_grad_per_image(const float* rowsums, const float* yrow, const do
                                const double* gbeta, int B, int L, int H, int order, int mask_rows, double* g_rowp,
                                lf_stream_t stream);
 
+/* Prefix fits (a lane curriculum, --lane_curriculum): the forward and backward entry points above with one more
+ * argument, Lmap, the maps' channel count, right after L, the number of lanes fitted (L <= Lmap <= 65535, else
+ * LF_ERR_INVALID_ARGUMENT).  o is [B,Lmap,H,W]; lanes [0, L) are fitted and lanes [L, Lmap) are never read, solved or
+ * OR-ed into status.  beta, zinv, rowsums and the workspace are sized by L, as for the plain entry point with L lanes.
+ *   masked  [B,L,H,W] or NULL (compact, as the plain entry point's with L lanes);
+ *   d_o     [B,Lmap,H,W]: lanes [0, L) as the plain backward writes them, lanes [L, Lmap) +0.0, written by the same
+ *           launch (no separate memset).
+ * Plan, checks, alignment and bits are those of the plain entry point on a contiguous copy of o[:, :L]; with
+ * Lmap = L each is the plain entry point.  Lmap > L runs kernels of its own, so the plain entry points' kernels are
+ * those of a build without prefix fits.  All DEVICE. */
+int lf_lsq_fwd_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B, int L,
+                     int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
+                     double* zinv, float* masked, int* status, void* workspace, size_t workspace_bytes,
+                     lf_stream_t stream);
+int lf_lsq_fwd_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                          const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act,
+                          double reg_ls, int solver, double* beta, double* zinv, float* masked, int* status,
+                          void* workspace, size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_fwd_rowsums_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L, int Lmap,
+                             int H, int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
+                             double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                             size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_fwd_rowsums_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                                  int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                                  int solver, double* beta, double* zinv, float* masked, int* status, float* rowsums,
+                                  void* workspace, size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_bwd_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B, int L,
+                     int Lmap, int H, int W, int order, int mask_rows, int act, const double* beta, const double* zinv,
+                     const double* gbeta, void* d_o, lf_stream_t stream);
+int lf_lsq_bwd_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                          const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act,
+                          const double* beta, const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream);
+int lf_lsq_fwd_per_image_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                               int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                               int solver, double* beta, double* zinv, float* masked, int* status, float* rowsums,
+                               void* workspace, size_t workspace_bytes, lf_stream_t stream);
+int lf_lsq_bwd_per_image_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                               int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act,
+                               const double* beta, const double* zinv, const double* gbeta, void* d_o,
+                               lf_stream_t stream);
+
 /* lf_backproj_loss_dev with one warp per image: yk [B][56], Minv [B][9]; g_const [B][65] holds each image's gradient
  * (dloss/dMinv, then dloss/dyk); scratch: lf_backproj_loss_per_image_scratch(B, L) doubles.  With every image given
  * the same warp, loss, dbeta and xcal are lf_backproj_loss_dev's bits.  All DEVICE. */

@@ -120,22 +120,25 @@ class Weighted_least_squares(nn.Module):
         self.y_const = y_const          # the reference hard-codes 255 (:94) whatever --resize is
         self.out_dtype = out_dtype
 
-    def forward_all(self, W, grid, mask_rows=0, act="none", want_masked=False, status_out=None, max_order=4, keep=None):
-        """keep: optional bool / uint8 [H, W] map; act(W) is zeroed where it is 0 before the fit (ops_lsq.lsq)."""
+    def forward_all(self, W, grid, mask_rows=0, act="none", want_masked=False, status_out=None, max_order=4, keep=None,
+                    lanes=None):
+        """keep: optional bool / uint8 [H, W] map; act(W) is zeroed where it is 0 before the fit (ops_lsq.lsq).
+        lanes: fit the first ``lanes`` maps only (default all; ops_lsq.lsq)."""
         if self.order > max_order:
             raise NotImplementedError(
                 "Requested order {} for polynomial fit is not implemented".format(self.order))
         Wm = W.reshape(-1, self.nclasses, self.H, self.W)
         beta, masked = _ops.lsq(Wm, grid, self.order, self.y_const, mask_rows, act, self.reg_ls_value,
-                                self.use_cholesky, want_masked, status_out, keep)
+                                self.use_cholesky, want_masked, status_out, keep, lanes)
         return beta, masked
 
     def _split(self, beta):
-        b = beta.to(self.out_dtype).unsqueeze(-1)            # [B, L, d+1, 1]
-        beta0, beta1 = b[:, 0], b[:, 1]
+        b = beta.to(self.out_dtype).unsqueeze(-1)            # [B, L, d+1, 1]; fewer lanes after a prefix fit
+        K = b.shape[1]
+        beta0, beta1 = b[:, 0], b[:, 1] if K > 1 else None
         beta2 = beta3 = None
         if self.nclasses > 3:
-            beta2, beta3 = b[:, 2], b[:, 3]
+            beta2, beta3 = (b[:, 2] if K > 2 else None), (b[:, 3] if K > 3 else None)
         return beta0, beta1, beta2, beta3
 
     def forward(self, W, grid):
@@ -203,6 +206,8 @@ class Net(nn.Module):
     A singular / non-finite normal matrix raises RuntimeError (main.py:289-292 skips the
     batch).  Set ``self.defer_status_check = True`` to skip the per-step host sync; the
     OR-ed status word is then left in ``self.lsq_status`` (device int32) for the caller.
+    ``self.fit_lanes = K`` makes a training forward end to end fit lanes [0, K) only (beta_K .. beta3 are None, masked
+    has K maps, the other systems never reach the status word); eval forwards fit every lane.
     """
 
     def __init__(self, args):
@@ -294,6 +299,9 @@ class Net(nn.Module):
                 self.keep = self.keep.cuda()
         self.defer_status_check = False
         self.lsq_status = None
+        # a lane curriculum (engine.train_epoch, --lane_curriculum): a training forward end to end fits lanes
+        # [0, fit_lanes) only and returns None for the other betas; None fits every lane, and so does every eval forward
+        self.fit_lanes = None
 
     def forward(self, input, gt_line, end_to_end, early_return=False, gt=None):
         line, horizon = None, None
@@ -353,23 +361,24 @@ class Net(nn.Module):
                 horizon = self.horizon_estimation(shared_encoder)
             # activation (:295) + row mask (:301) [+ the trapezium keep map] + least squares (:314) in one launch;
             # `masked` is materialised only because the API returns it (:315)
+            lanes = self.fit_lanes if self.training else None
             if warp is not None:
                 beta, masked = self._lsq_warp(output, warp, self.zero_rows, self.activation.kind, True, st, status is None,
-                                              keep)
+                                              keep, lanes)
             else:
                 beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows,
                                                          act=self.activation.kind, want_masked=True,
-                                                         status_out=status, max_order=3, keep=keep)
+                                                         status_out=status, max_order=3, keep=keep, lanes=lanes)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)
         return beta0, beta1, beta2, beta3, masked, output, line, horizon, output_seg
 
-    def _lsq_warp(self, W, warp, mask_rows, act, want_masked, status, check, keep=None):
+    def _lsq_warp(self, W, warp, mask_rows, act, want_masked, status, check, keep=None, lanes=None):
         ls = self.ls_layer
         if ls.order > 3:
             raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(ls.order))
         Wm = W.reshape(-1, ls.nclasses, ls.H, ls.W)
         beta, masked = _ops.lsq_warp(Wm, warp, ls.order, mask_rows, act, ls.reg_ls_value, ls.use_cholesky, want_masked,
-                                     status, keep)
+                                     status, keep, lanes)
         if check:
             # the status word holds the warp's guard as well as the solve's: one host read, as torch.inverse's raise
             st = int(status.item())

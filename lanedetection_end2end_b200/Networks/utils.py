@@ -92,6 +92,7 @@ _FLAGS = [
     ("--seg_proxy", _B(False)),
     ("--weight_seg_proxy", dict(type=float, default=1.0)),
     ("--trapezium_mask", _B(False)),
+    ("--lane_curriculum", dict(type=int, default=0)),
     ("--gamma", dict(type=float, default=0.0)),
     ("--clas", _B(False)),
     ("--cudnn", _B(True)),
@@ -273,6 +274,33 @@ _INIT = {
     "kaiming": lambda w: init.kaiming_normal_(w, a=0, mode="fan_in", nonlinearity="relu"),
     "orthogonal": lambda w: init.orthogonal_(w, gain=1),
 }
+
+
+def expand_lanes(state_dict, model):
+    """Warm-start a 4-lane Net from a 2-lane checkpoint (the egolanes first, then all four): every tensor of
+    ``state_dict`` whose key and shape match ``model``'s is copied, and the lane channels of the decoder's output_conv
+    (its ``output_conv.weight`` / ``output_conv.bias``, whose shapes differ in the lane dimension only) go into the
+    model's first channels.  The other channels and every key the checkpoint lacks (the --clas heads of a model
+    trained without them, say) keep the model's values, e.g. define_init_weights'.  Returns the model keys it did not
+    fill, in the model's order."""
+    own = model.state_dict()
+    missing = []
+    with torch.no_grad():
+        for k, dst in own.items():
+            src = state_dict.get(k)
+            if src is None:
+                missing.append(k)
+                continue
+            if tuple(src.shape) == tuple(dst.shape):
+                dst.copy_(src)
+                continue
+            head = k.rsplit(".", 2)[-2:] in (["output_conv", "weight"], ["output_conv", "bias"])
+            diff = [d for d in range(dst.dim()) if src.dim() == dst.dim() and src.shape[d] != dst.shape[d]]
+            if not head or len(diff) != 1 or src.shape[diff[0]] > dst.shape[diff[0]]:
+                raise ValueError("expand_lanes: %s is %s in the checkpoint and %s in the model" % (
+                    k, tuple(src.shape), tuple(dst.shape)))
+            dst.narrow(diff[0], 0, src.shape[diff[0]]).copy_(src)
+    return missing
 
 
 def define_init_weights(model, init_w="normal", activation="relu"):

@@ -274,6 +274,20 @@ _NET_PROTOS = {
                                   _p, ctypes.c_size_t, _p]),
     "lf_lsq_bwd_per_image": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
     "lf_lsq_grid_grad_per_image": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p]),
+    # prefix fits of a lane curriculum: the entry point's arguments with Lmap after L
+    "lf_lsq_fwd_lanes": (_i, [_p, _i, _p, _p, _p] + [_i] * 8 + [ctypes.c_double, _i, _p, _p, _p, _p, _p, ctypes.c_size_t,
+                                                                 _p]),
+    "lf_lsq_fwd_keep_lanes": (_i, [_p, _i, _p, _p, _p, _p] + [_i] * 8 + [ctypes.c_double, _i, _p, _p, _p, _p, _p,
+                                                                         ctypes.c_size_t, _p]),
+    "lf_lsq_fwd_rowsums_lanes": (_i, [_p, _i, _p, _p] + [_i] * 8 + [ctypes.c_double, _i, _p, _p, _p, _p, _p, _p,
+                                                                    ctypes.c_size_t, _p]),
+    "lf_lsq_fwd_rowsums_keep_lanes": (_i, [_p, _i, _p, _p, _p] + [_i] * 8 + [ctypes.c_double, _i, _p, _p, _p, _p, _p, _p,
+                                                                             ctypes.c_size_t, _p]),
+    "lf_lsq_bwd_lanes": (_i, [_p, _i, _p, _p, _p] + [_i] * 8 + [_p, _p, _p, _p, _p]),
+    "lf_lsq_bwd_keep_lanes": (_i, [_p, _i, _p, _p, _p, _p] + [_i] * 8 + [_p, _p, _p, _p, _p]),
+    "lf_lsq_fwd_per_image_lanes": (_i, [_p, _i, _p, _p, _p] + [_i] * 8 + [ctypes.c_double, _i, _p, _p, _p, _p, _p, _p,
+                                                                          ctypes.c_size_t, _p]),
+    "lf_lsq_bwd_per_image_lanes": (_i, [_p, _i, _p, _p, _p] + [_i] * 8 + [_p, _p, _p, _p, _p]),
     "lf_backproj_loss_per_image_scratch": (ctypes.c_size_t, [_i, _i]),
     "lf_backproj_loss_per_image": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "lf_area_loss": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),

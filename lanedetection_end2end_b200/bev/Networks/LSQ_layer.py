@@ -6,7 +6,8 @@ Differences from the BP variant (all served by the same fused kernel, csrc/lsq.c
   * ``y = 1 - y'`` (:109), orders 0..2 only (:110-118), beta returned as float32 (:167);
   * ``Net.forward(input, end_to_end)`` -> (beta0, beta1, beta2, beta3, masked, M, output, line, horizon) (:326); with
     --clas the end-to-end forward runs the line-type head (line [B, 3, 4], its own tail) and the horizon head;
-  * --trapezium_mask: the end-to-end fit takes the BP Net's keep map (LSQ_layer.trapezium_keep).
+  * --trapezium_mask: the end-to-end fit takes the BP Net's keep map (LSQ_layer.trapezium_keep);
+  * ``fit_lanes``: a lane curriculum's prefix fit in training forwards, as in the BP Net.
 """
 from math import ceil
 
@@ -135,6 +136,8 @@ class Net(nn.Module):
                 self.keep = self.keep.cuda()
         self.defer_status_check = False
         self.lsq_status = None
+        # a lane curriculum, as in the back-projection Net: a training forward end to end fits lanes [0, fit_lanes) only
+        self.fit_lanes = None
 
     def forward(self, input, end_to_end):
         line, horizon = None, None
@@ -160,6 +163,7 @@ class Net(nn.Module):
             if self.keep is not None and self.keep.device != output.device:
                 self.keep = self.keep.to(output.device)
             beta, masked = self.ls_layer.forward_all(output, grid, mask_rows=self.zero_rows, act=self.activation.kind,
-                                                     want_masked=True, status_out=status, max_order=2, keep=self.keep)
+                                                     want_masked=True, status_out=status, max_order=2, keep=self.keep,
+                                                     lanes=self.fit_lanes if self.training else None)
         beta0, beta1, beta2, beta3 = self.ls_layer._split(beta)
         return beta0, beta1, beta2, beta3, masked, self.M, output, line, horizon

@@ -912,6 +912,67 @@ static int pick_nchunks(int B, int groups, int H, int mask_rows, int ctas_per_sm
     return best;
 }
 
+// ---------------------------------------------------------------------------------
+// Prefix fits (the *_lanes entry points, a lane curriculum): lanes [0, L) of maps with Lmap >= L channels, o and d_o
+// [B][Lmap][H][W].  The bodies index a map as (b * L + l) * H * W; moving o and d_o of image b by b * (Lmap - L) maps
+// turns that into (b * Lmap + l) * H * W, so the fitted lanes run the plain kernels' bodies unchanged and every plain
+// kernel keeps its code.  masked, beta, zinv, rowsums and the workspace stay compact, sized by L.  per_image: the
+// per-image tables of lsq_image_args as well.
+// ---------------------------------------------------------------------------------
+template <bool BF16>
+__device__ __forceinline__ LsqArgs lsq_lanes_args(const LsqArgs& a, int b, int Lmap, int per_image) {
+    LsqArgs ai = per_image ? lsq_image_args(a, b) : a;
+    const size_t shift = (size_t)b * (Lmap - a.L) * a.H * a.W * (BF16 ? 2 : 4);     // bytes
+    ai.o = reinterpret_cast<const char*>(a.o) + shift;
+    if (a.d_o) ai.d_o = reinterpret_cast<char*>(a.d_o) + shift;
+    return ai;
+}
+
+template <int ACT_T, bool BF16, int NL, bool ROWSUMS, bool KEEP>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_FWD_CTAS_PER_SM) lsq_fwd_rowsep_lanes_kernel(const LsqArgs a,
+                                                                                                float* rowsums,
+                                                                                                const uint8_t* keep,
+                                                                                                int Lmap, int per_image) {
+    lsq_fwd_rowsep_body<ACT_T, BF16, NL, ROWSUMS, KEEP>(lsq_lanes_args<BF16>(a, blockIdx.y, Lmap, per_image), rowsums,
+                                                        keep);
+}
+
+template <int ACT_T, bool BF16, bool KEEP>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_fwd_general_lanes_kernel(const LsqArgs a, const uint8_t* keep,
+                                                                             int Lmap) {
+    lsq_fwd_general_body<ACT_T, BF16, KEEP>(lsq_lanes_args<BF16>(a, blockIdx.y, Lmap, 0), keep);
+}
+
+// d_o of the unfitted lanes [L, Lmap) of image b is +0.0: the CTAs of lane group 0 store zeros over their chunk's rows,
+// after the fitted lanes' pass (so after the body's PDL wait), in the same launch.
+template <bool BF16>
+__device__ __forceinline__ void lsq_bwd_zero_unfitted(const LsqArgs& a, int b, int chunk, int Lmap) {
+    int m_begin, m_end, r_begin, r_end;
+    lsq_chunk_rows(a, chunk, m_begin, m_end, r_begin, r_end);
+    const int nm = m_end - m_begin, nrows = nm + (r_end - r_begin);
+    for (int l = a.L; l < Lmap; ++l)
+        for (int i = 0; i < nrows; ++i) {
+            const int r = i < nm ? m_begin + i : r_begin + (i - nm);
+            const size_t row = ((size_t)(b * Lmap + l) * a.H + r) * a.W;
+            for (int c = threadIdx.x; c < a.W; c += LSQ_THREADS) store_map1<BF16>(a.d_o, row + c, 0.f);
+        }
+}
+
+template <int ACT_T, bool BF16, int NL, bool KEEP>
+__global__ void __launch_bounds__(LSQ_THREADS, LSQ_BWD_CTAS_PER_SM) lsq_bwd_rowsep_lanes_kernel(const LsqArgs a,
+                                                                                                const uint8_t* keep,
+                                                                                                int Lmap, int per_image) {
+    lsq_bwd_rowsep_body<ACT_T, BF16, NL, KEEP>(lsq_lanes_args<BF16>(a, blockIdx.y, Lmap, per_image), keep);
+    if (blockIdx.z == 0) lsq_bwd_zero_unfitted<BF16>(a, blockIdx.y, blockIdx.x, Lmap);
+}
+
+template <int ACT_T, bool BF16, bool KEEP>
+__global__ void __launch_bounds__(LSQ_THREADS) lsq_bwd_general_lanes_kernel(const LsqArgs a, const uint8_t* keep,
+                                                                             int Lmap) {
+    lsq_bwd_general_body<ACT_T, BF16, KEEP>(lsq_lanes_args<BF16>(a, blockIdx.y, Lmap, 0), keep);
+    if (blockIdx.z == 0) lsq_bwd_zero_unfitted<BF16>(a, blockIdx.y, blockIdx.x, Lmap);
+}
+
 }  // namespace lf
 
 using namespace lf;
@@ -972,7 +1033,7 @@ extern "C" size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order) 
     (void)W;
     if (B <= 0 || L <= 0 || H <= 0 || order < 0 || order > LF_MAX_ORDER) return 0;
     if ((size_t)B * L * sizeof(int) > LSQ_TICKET_BYTES) return 0;
-    // worst case: rows_per_cta = 8 -> nchunks = ceil(H/8)
+    // worst case: 8 rows per chunk -> nchunks = ceil(H/8)
     const size_t nchunks = (size_t)(H + LSQ_WARPS - 1) / LSQ_WARPS;
     return LSQ_TICKET_BYTES + (size_t)B * L * nchunks * (3 * order + 2) * sizeof(double);
 }
@@ -1018,12 +1079,71 @@ extern "C" size_t lf_lsq_workspace_bytes(int B, int L, int H, int W, int order) 
         }                                                                     \
     } while (0)
 
+// The *_lanes kernels, used when Lmap > L (a prefix fit): rowsums / keep NULL select the instantiation as for the
+// per-image kernels, per_image the per-image tables.
+template <int ACT_T, bool BF16, int NL>
+static void launch_lanes_nl(int bwd, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums, const uint8_t* keep,
+                            int Lmap, int pi) {
+    if (bwd) {
+        if (keep)
+            lf_launch(lsq_bwd_rowsep_lanes_kernel<ACT_T, BF16, NL, true>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap, pi);
+        else
+            lf_launch(lsq_bwd_rowsep_lanes_kernel<ACT_T, BF16, NL, false>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap, pi);
+    } else if (rowsums) {
+        if (keep)
+            lf_launch(lsq_fwd_rowsep_lanes_kernel<ACT_T, BF16, NL, true, true>, grid, LSQ_THREADS, 0, stream, a, rowsums,
+                      keep, Lmap, pi);
+        else
+            lf_launch(lsq_fwd_rowsep_lanes_kernel<ACT_T, BF16, NL, true, false>, grid, LSQ_THREADS, 0, stream, a, rowsums,
+                      keep, Lmap, pi);
+    } else {
+        if (keep)
+            lf_launch(lsq_fwd_rowsep_lanes_kernel<ACT_T, BF16, NL, false, true>, grid, LSQ_THREADS, 0, stream, a, rowsums,
+                      keep, Lmap, pi);
+        else
+            lf_launch(lsq_fwd_rowsep_lanes_kernel<ACT_T, BF16, NL, false, false>, grid, LSQ_THREADS, 0, stream, a, rowsums,
+                      keep, Lmap, pi);
+    }
+}
+
+template <int ACT_T, bool BF16>
+static void launch_lanes_t(int rowsep, int nl, int bwd, dim3 grid, cudaStream_t stream, const LsqArgs& a, float* rowsums,
+                           const uint8_t* keep, int Lmap, int pi) {
+    if (!rowsep) {
+        if (bwd)
+            keep ? lf_launch(lsq_bwd_general_lanes_kernel<ACT_T, BF16, true>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap)
+                 : lf_launch(lsq_bwd_general_lanes_kernel<ACT_T, BF16, false>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap);
+        else
+            keep ? lf_launch(lsq_fwd_general_lanes_kernel<ACT_T, BF16, true>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap)
+                 : lf_launch(lsq_fwd_general_lanes_kernel<ACT_T, BF16, false>, grid, LSQ_THREADS, 0, stream, a, keep, Lmap);
+        return;
+    }
+    switch (nl) {
+        case 1: launch_lanes_nl<ACT_T, BF16, 1>(bwd, grid, stream, a, rowsums, keep, Lmap, pi); break;
+        case 2: launch_lanes_nl<ACT_T, BF16, 2>(bwd, grid, stream, a, rowsums, keep, Lmap, pi); break;
+        case 3: launch_lanes_nl<ACT_T, BF16, 3>(bwd, grid, stream, a, rowsums, keep, Lmap, pi); break;
+        default: launch_lanes_nl<ACT_T, BF16, 4>(bwd, grid, stream, a, rowsums, keep, Lmap, pi); break;
+    }
+}
+
+static int launch_lanes(const LsqPlan& p, int bwd, int o_dtype, dim3 grid, cudaStream_t stream, const LsqArgs& a,
+                        float* rowsums, const uint8_t* keep, int Lmap, int pi) {
+    if (a.act == LF_ACT_SQUARE)
+        o_dtype == LF_BF16 ? launch_lanes_t<LF_ACT_SQUARE, true>(p.rowsep, p.nl, bwd, grid, stream, a, rowsums, keep, Lmap, pi)
+                           : launch_lanes_t<LF_ACT_SQUARE, false>(p.rowsep, p.nl, bwd, grid, stream, a, rowsums, keep, Lmap, pi);
+    else
+        o_dtype == LF_BF16 ? launch_lanes_t<LSQ_ACT_RUNTIME, true>(p.rowsep, p.nl, bwd, grid, stream, a, rowsums, keep, Lmap, pi)
+                           : launch_lanes_t<LSQ_ACT_RUNTIME, false>(p.rowsep, p.nl, bwd, grid, stream, a, rowsums, keep, Lmap, pi);
+    return check_launch();
+}
+
 // lf_lsq_fwd and lf_lsq_fwd_keep (keep = NULL: the KEEP = false kernels, exactly as before the keep map existed)
 static int lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
-                   const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
-                   int solver, double* beta, double* zinv, float* masked, int* status, void* workspace,
+                   const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act,
+                   double reg_ls, int solver, double* beta, double* zinv, float* masked, int* status, void* workspace,
                    size_t workspace_bytes, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && status && workspace);
+    LF_REQUIRE(Lmap >= L && Lmap <= 65535);
     LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
     LsqPlan p{};
     const int rc = lsq_plan(0, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
@@ -1035,10 +1155,10 @@ static int lsq_fwd(const void* o, int o_dtype, const float* xtab, const float* y
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act; a.solver = solver;
     a.reg_ls = reg_ls; a.beta = beta; a.zinv = zinv; a.masked = masked; a.status = status;
     a.nchunks = p.nchunks;
-    a.rows_per_cta = 0;
     a.tickets = reinterpret_cast<int*>(workspace);
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
     dim3 grid(a.nchunks, B, p.groups);
+    if (Lmap > L) return launch_lanes(p, 0, o_dtype, grid, stream, a, nullptr, keep, Lmap, 0);
     if (p.rowsep) {
         if (keep)
             LSQ_DISPATCH_NL(lsq_fwd_rowsep_keep_kernel, p.nl, grid, a, keep);
@@ -1057,7 +1177,7 @@ extern "C" int lf_lsq_fwd(const void* o, int o_dtype, const float* xtab, const f
                           int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
                           double* beta, double* zinv, float* masked, int* status, void* workspace,
                           size_t workspace_bytes, lf_stream_t stream_) {
-    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
                    masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1066,7 +1186,7 @@ extern "C" int lf_lsq_fwd_keep(const void* o, int o_dtype, const float* xtab, co
                                double reg_ls, int solver, double* beta, double* zinv, float* masked, int* status,
                                void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
     LF_REQUIRE(keep);
-    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
                    masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1091,10 +1211,11 @@ static void launch_rowsums(int nl, dim3 grid, cudaStream_t stream, const LsqArgs
 // lf_lsq_fwd on the row-separable kernel that also stores the row sums: same arguments and plan, yrow required,
 // rowsums [B][L][H][3] float32 (rows >= mask_rows written).  keep as in lsq_fwd.
 static int lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
-                           int L, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                           int L, int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
                            double* beta, double* zinv, float* masked, int* status, float* rowsums, void* workspace,
                            size_t workspace_bytes, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && yrow && beta && zinv && status && rowsums && workspace);
+    LF_REQUIRE(Lmap >= L && Lmap <= 65535);
     LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
     LsqPlan p{};
     const int rc = lsq_plan(0, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
@@ -1109,6 +1230,7 @@ static int lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab, const 
     a.tickets = reinterpret_cast<int*>(workspace);
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
     dim3 grid(a.nchunks, B, p.groups);
+    if (Lmap > L) return launch_lanes(p, 0, o_dtype, grid, stream, a, rowsums, keep, Lmap, 0);
     if (act == LF_ACT_SQUARE)
         o_dtype == LF_BF16 ? launch_rowsums<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums, keep)
                            : launch_rowsums<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums, keep);
@@ -1122,7 +1244,7 @@ extern "C" int lf_lsq_fwd_rowsums(const void* o, int o_dtype, const float* xtab,
                                   int W, int order, int mask_rows, int act, double reg_ls, int solver, double* beta,
                                   double* zinv, float* masked, int* status, float* rowsums, void* workspace,
                                   size_t workspace_bytes, lf_stream_t stream_) {
-    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, nullptr, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, nullptr, B, L, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
                            masked, status, rowsums, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1132,7 +1254,7 @@ extern "C" int lf_lsq_fwd_rowsums_keep(const void* o, int o_dtype, const float* 
                                        int* status, float* rowsums, void* workspace, size_t workspace_bytes,
                                        lf_stream_t stream_) {
     LF_REQUIRE(keep);
-    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, keep, B, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, keep, B, L, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
                            masked, status, rowsums, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1149,9 +1271,10 @@ extern "C" int lf_lsq_grid_grad(const float* rowsums, const float* yrow, const d
 
 // lf_lsq_bwd and lf_lsq_bwd_keep (keep = NULL: the KEEP = false kernels)
 static int lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
-                   const uint8_t* keep, int B, int L, int H, int W, int order, int mask_rows, int act, const double* beta,
-                   const double* zinv, const double* gbeta, void* d_o, cudaStream_t stream) {
+                   const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows, int act,
+                   const double* beta, const double* zinv, const double* gbeta, void* d_o, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && (ytab || yrow) && beta && zinv && gbeta && d_o);
+    LF_REQUIRE(Lmap >= L && Lmap <= 65535);
     LsqPlan p{};
     const int rc = lsq_plan(1, o_dtype, yrow != nullptr, ytab != nullptr, B, L, H, W, order, mask_rows, act, &p);
     if (rc != LF_OK) return rc;
@@ -1161,8 +1284,8 @@ static int lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* y
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act;
     a.beta = const_cast<double*>(beta); a.zinv = const_cast<double*>(zinv); a.gbeta = gbeta; a.d_o = d_o;
     a.nchunks = p.nchunks;
-    a.rows_per_cta = 0;
     dim3 grid(a.nchunks, B, p.groups);
+    if (Lmap > L) return launch_lanes(p, 1, o_dtype, grid, stream, a, nullptr, keep, Lmap, 0);
     if (p.rowsep) {
         if (keep)
             LSQ_DISPATCH_NL(lsq_bwd_rowsep_keep_kernel, p.nl, grid, a, keep);
@@ -1180,7 +1303,7 @@ static int lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* y
 extern "C" int lf_lsq_bwd(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
                           int L, int H, int W, int order, int mask_rows, int act, const double* beta,
                           const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
-    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
                    reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1189,7 +1312,7 @@ extern "C" int lf_lsq_bwd_keep(const void* o, int o_dtype, const float* xtab, co
                                const double* beta, const double* zinv, const double* gbeta, void* d_o,
                                lf_stream_t stream_) {
     LF_REQUIRE(keep);
-    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
                    reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -1223,12 +1346,12 @@ static void launch_fwd_pi(int nl, dim3 grid, cudaStream_t stream, const LsqArgs&
     }
 }
 
-extern "C" int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
-                                    int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
-                                    int solver, double* beta, double* zinv, float* masked, int* status, float* rowsums,
-                                    void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+static int lsq_fwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
+                             int L, int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                             double* beta, double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                             size_t workspace_bytes, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && yrow && beta && zinv && status && workspace);
+    LF_REQUIRE(Lmap >= L && Lmap <= 65535);
     LF_REQUIRE(solver == LF_SOLVER_INVERSE || solver == LF_SOLVER_CHOLESKY);
     LsqPlan p{};
     const int rc = lsq_plan(0, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
@@ -1244,6 +1367,7 @@ extern "C" int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xta
     a.tickets = reinterpret_cast<int*>(workspace);
     a.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + LSQ_TICKET_BYTES);
     dim3 grid(a.nchunks, B, p.groups);
+    if (Lmap > L) return launch_lanes(p, 0, o_dtype, grid, stream, a, rowsums, keep, Lmap, 1);
     if (act == LF_ACT_SQUARE)
         o_dtype == LF_BF16 ? launch_fwd_pi<LF_ACT_SQUARE, true>(p.nl, grid, stream, a, rowsums, keep)
                            : launch_fwd_pi<LF_ACT_SQUARE, false>(p.nl, grid, stream, a, rowsums, keep);
@@ -1253,11 +1377,11 @@ extern "C" int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xta
     return check_launch();
 }
 
-extern "C" int lf_lsq_bwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
-                                    int B, int L, int H, int W, int order, int mask_rows, int act, const double* beta,
-                                    const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+static int lsq_bwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep, int B,
+                             int L, int Lmap, int H, int W, int order, int mask_rows, int act, const double* beta,
+                             const double* zinv, const double* gbeta, void* d_o, cudaStream_t stream) {
     LF_REQUIRE(o && xtab && yrow && beta && zinv && gbeta && d_o);
+    LF_REQUIRE(Lmap >= L && Lmap <= 65535);
     LsqPlan p{};
     const int rc = lsq_plan(1, o_dtype, 1, 0, B, L, H, W, order, mask_rows, act, &p);
     if (rc != LF_OK) return rc;
@@ -1268,13 +1392,103 @@ extern "C" int lf_lsq_bwd_per_image(const void* o, int o_dtype, const float* xta
     a.B = B; a.L = L; a.H = H; a.W = W; a.order = order; a.mask_rows = mask_rows; a.act = act;
     a.beta = const_cast<double*>(beta); a.zinv = const_cast<double*>(zinv); a.gbeta = gbeta; a.d_o = d_o;
     a.nchunks = p.nchunks;
-    a.rows_per_cta = 0;
     dim3 grid(a.nchunks, B, p.groups);
+    if (Lmap > L) return launch_lanes(p, 1, o_dtype, grid, stream, a, nullptr, keep, Lmap, 1);
     if (keep)
         LSQ_DISPATCH_NL(lsq_bwd_rowsep_pi_keep_kernel, p.nl, grid, a, keep);
     else
         LSQ_DISPATCH_NL(lsq_bwd_rowsep_pi_kernel, p.nl, grid, a, keep);
     return check_launch();
+}
+
+extern "C" int lf_lsq_fwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                                    int B, int L, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                                    int solver, double* beta, double* zinv, float* masked, int* status, float* rowsums,
+                                    void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd_per_image(o, o_dtype, xtab, yrow, keep, B, L, L, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                             masked, status, rowsums, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_bwd_per_image(const void* o, int o_dtype, const float* xtab, const float* yrow, const uint8_t* keep,
+                                    int B, int L, int H, int W, int order, int mask_rows, int act, const double* beta,
+                                    const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
+    return lsq_bwd_per_image(o, o_dtype, xtab, yrow, keep, B, L, L, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                             reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Prefix fits (a lane curriculum): the entry points above with the maps' channel count Lmap >= L after L.  Lanes [0, L)
+// of o [B][Lmap][H][W] are fitted exactly as the plain entry point fits o[:, :L]; masked is [B][L][H][W]; d_o is
+// [B][Lmap][H][W] with lanes [L, Lmap) zero (written by the backward's own launch).  Lmap = L runs the plain kernels.
+extern "C" int lf_lsq_fwd_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
+                                int L, int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls, int solver,
+                                double* beta, double* zinv, float* masked, int* status, void* workspace,
+                                size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, Lmap, H, W, order, mask_rows, act, reg_ls, solver, beta,
+                   zinv, masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                                     const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows,
+                                     int act, double reg_ls, int solver, double* beta, double* zinv, float* masked,
+                                     int* status, void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_fwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, Lmap, H, W, order, mask_rows, act, reg_ls, solver, beta, zinv,
+                   masked, status, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_rowsums_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow, int B, int L,
+                                        int Lmap, int H, int W, int order, int mask_rows, int act, double reg_ls,
+                                        int solver, double* beta, double* zinv, float* masked, int* status,
+                                        float* rowsums, void* workspace, size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, nullptr, B, L, Lmap, H, W, order, mask_rows, act, reg_ls, solver, beta,
+                           zinv, masked, status, rowsums, workspace, workspace_bytes,
+                           reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_rowsums_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow,
+                                             const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order,
+                                             int mask_rows, int act, double reg_ls, int solver, double* beta,
+                                             double* zinv, float* masked, int* status, float* rowsums, void* workspace,
+                                             size_t workspace_bytes, lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_fwd_rowsums(o, o_dtype, xtab, yrow, keep, B, L, Lmap, H, W, order, mask_rows, act, reg_ls, solver, beta,
+                           zinv, masked, status, rowsums, workspace, workspace_bytes,
+                           reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_bwd_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow, int B,
+                                int L, int Lmap, int H, int W, int order, int mask_rows, int act, const double* beta,
+                                const double* zinv, const double* gbeta, void* d_o, lf_stream_t stream_) {
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, nullptr, B, L, Lmap, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                   reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_bwd_keep_lanes(const void* o, int o_dtype, const float* xtab, const float* ytab, const float* yrow,
+                                     const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order, int mask_rows,
+                                     int act, const double* beta, const double* zinv, const double* gbeta, void* d_o,
+                                     lf_stream_t stream_) {
+    LF_REQUIRE(keep);
+    return lsq_bwd(o, o_dtype, xtab, ytab, yrow, keep, B, L, Lmap, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                   reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_fwd_per_image_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow,
+                                          const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order,
+                                          int mask_rows, int act, double reg_ls, int solver, double* beta, double* zinv,
+                                          float* masked, int* status, float* rowsums, void* workspace,
+                                          size_t workspace_bytes, lf_stream_t stream_) {
+    return lsq_fwd_per_image(o, o_dtype, xtab, yrow, keep, B, L, Lmap, H, W, order, mask_rows, act, reg_ls, solver, beta,
+                             zinv, masked, status, rowsums, workspace, workspace_bytes,
+                             reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int lf_lsq_bwd_per_image_lanes(const void* o, int o_dtype, const float* xtab, const float* yrow,
+                                          const uint8_t* keep, int B, int L, int Lmap, int H, int W, int order,
+                                          int mask_rows, int act, const double* beta, const double* zinv,
+                                          const double* gbeta, void* d_o, lf_stream_t stream_) {
+    return lsq_bwd_per_image(o, o_dtype, xtab, yrow, keep, B, L, Lmap, H, W, order, mask_rows, act, beta, zinv, gbeta, d_o,
+                             reinterpret_cast<cudaStream_t>(stream_));
 }
 
 // g_rowp [B][H][3] f64: image b's table gradient, summed over its lanes (rowsums, beta, zinv, gbeta as lf_lsq_grid_grad,

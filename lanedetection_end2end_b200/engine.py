@@ -445,9 +445,41 @@ def _valid_replays(loader, model, fields, casts, post, report, print_freq, gt_li
     status.print_skipped(labels)
 
 
+def check_lane_curriculum(args):
+    """--lane_curriculum E: ValueError unless E == 0 (off) or E > 0 with 4 lanes."""
+    e = getattr(args, "lane_curriculum", 0)
+    if e < 0:
+        raise ValueError("--lane_curriculum takes a number of epochs >= 0, got %d" % e)
+    if e > 0 and args.nclasses != 4:
+        raise ValueError("--lane_curriculum fits the egolanes first and then all four lanes: it needs --nclasses 4, got "
+                         "%d" % args.nclasses)
+
+
+def curriculum_lanes(args, epoch):
+    """The lanes an end-to-end training epoch fits under --lane_curriculum E: lanes 0 and 1 (the egolanes, in the loader's
+    lane order) before epoch E, None (every lane) from E on and whenever the flag is off."""
+    e = getattr(args, "lane_curriculum", 0)
+    return 2 if e > 0 and epoch < e else None
+
+
+class _FitLanes:
+    """``with _FitLanes(model, K):`` sets ``model.fit_lanes`` to K and restores the previous value on exit."""
+
+    def __init__(self, model, lanes):
+        self.model, self.lanes = model, lanes
+
+    def __enter__(self):
+        self.saved = getattr(self.model, "fit_lanes", None)
+        self.model.fit_lanes = self.lanes
+
+    def __exit__(self, *exc):
+        self.model.fit_lanes = self.saved
+
+
 def check_bp_args(args, criterion, model):
     """The settings train_epoch and inference.validate run: ValueError naming the first one they do not.  A criterion
     built with --learn_homography is bound to ``model``'s learned warp."""
+    check_lane_curriculum(args)
     if args.clas and not args.end_to_end:
         raise ValueError("--clas needs --end_to_end True (the heads run on the end-to-end branch only)")
     if not args.end_to_end and args.nclasses != 4:
@@ -496,7 +528,13 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     A model built with --seg_proxy (``model.seg_proxy``) trains its second decoder in the same step: the loss is
     Loss_crit.seg_proxy_loss, ``L_fit + weight_seg_proxy * criterion_seg(output_seg, gt)`` in float64, L_fit the loss
     above; losses.avg is that total.  The proxy term has a device meter of its own; pass a dict as ``seg_metrics`` to
-    receive its average under "ce"."""
+    receive its average under "ce".
+
+    --lane_curriculum E (4 lanes): an end-to-end epoch < E sets ``model.fit_lanes = 2`` for its replays (restored on
+    exit), so the fit, the status word that guards the update and the loss cover the egolanes only: the loss is
+    fused_backprojection_loss over lanes 0 and 1, the 2-lane model's, while the --clas heads keep their 4-lane losses.
+    From epoch E on every lane is fitted, as without the flag.  With weight_decay > 0 the optimizer still decays the
+    outer lanes' output_conv channels in those epochs, whose gradient is zero."""
     from .optim import FusedOptimizer
     from .Loss_crit import fused_backprojection_loss, seg_proxy_loss
     from .Networks import utils as nutils
@@ -515,13 +553,16 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
     meters = DeviceMeters(("loss", "rmse") + (("seg_proxy",) if proxy else ()), next(model.parameters()).device)
     static = {}
 
+    # --lane_curriculum: an end-to-end epoch before E fits (and takes the loss over) the egolanes only
+    K = (curriculum_lanes(args, epoch) if e2e else None) or L
+
     def loss_fn(out):
         if not e2e:
             with torch.no_grad():
                 static["rmse"], static["x_cal"] = lane_losses(criterion, out, static["lanes"], static["valid"], L)
             return criterion_seg(out[5], static["gt"])
-        loss, x_cal = fused_backprojection_loss(criterion, out[:L], static["lanes"], static["valid"])
-        static["x_cal"] = [x_cal[:, l] for l in range(L)] + [None] * (4 - L)
+        loss, x_cal = fused_backprojection_loss(criterion, out[:K], static["lanes"], static["valid"])
+        static["x_cal"] = [x_cal[:, l] for l in range(K)] + [None] * (4 - K)
         if args.clas:
             loss_horizon = criterion_horizon(out[7], static["gt_horizon"]).double()
             loss_line = criterion_line_class(out[6], static["gt_line"]).double()
@@ -552,13 +593,15 @@ def train_epoch(loader, model, optimizer, criterion, criterion_seg, criterion_li
             lanes = static["lanes"]
             nutils.save_weightmap('train', masked, *static["x_cal"], lanes[:, 0, :], lanes[:, 1, :], lanes[:, 2, :],
                                   lanes[:, 3, :], static["gt"], 0, i, static["input"], args.no_ortho, args.resize,
-                                  args.save_path, args.nclasses, args.no_mapping)
+                                  args.save_path, K, args.no_mapping)
 
     fields = lambda b: {"input": b[0], "gt": b[1].squeeze(1), "lanes": b[2], "gt_line": b[4], "gt_horizon": b[5],
                         "valid": b[6]}
     casts = {"input": torch.float32, "gt": torch.int64}
-    if _train_replays(loader, model, optimizer, static, fields, casts, post, report, args.print_freq, args.save_freq,
-                      gt_line=not e2e, loss_fn=loss_fn, end_to_end=e2e) is None:
+    with _FitLanes(model, K if K < L else None):
+        step = _train_replays(loader, model, optimizer, static, fields, casts, post, report, args.print_freq,
+                              args.save_freq, gt_line=not e2e, loss_fn=loss_fn, end_to_end=e2e)
+    if step is None:
         return 0, 0
     m = meters.read()
     if proxy and seg_metrics is not None:
@@ -587,6 +630,7 @@ def _train_skip_epoch(loader, model, optimizer, criterion_seg):
 def check_bev_args(args):
     """The settings train_epoch_bev and inference.validate_bev run: ValueError naming the first one they do not."""
     from .Loss_crit import AREA_WEIGHTS
+    check_lane_curriculum(args)
     if args.clas and (args.nclasses != 4 or not args.end_to_end):
         raise ValueError("--clas needs 4 lanes and --end_to_end True (BEV/main.py:39-40; the heads run on the end-to-end "
                          "branch only), got %d lanes with end_to_end %s" % (args.nclasses, bool(args.end_to_end)))
@@ -634,7 +678,8 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
     --end_to_end False, --pretrained, loss policies other than area, orders other than 2 and other lane counts raise
     ValueError (check_bev_args).  clip_grad_norm is accepted and does nothing, as in train_epoch; clipping is asked
     for on the optimizer (max_grad_norm), as there.  Dropout masks are drawn in the
-    graph; BatchNorm running statistics are those of the epoch's batches."""
+    graph; BatchNorm running statistics are those of the epoch's batches.  --lane_curriculum as in train_epoch: before
+    epoch E the fit and fused_area_loss (and the exact-area metric) cover lanes 0 and 1, the heads all four."""
     from .optim import FusedOptimizer
     from .Loss_crit import fused_area_loss
     from .Networks import utils as nutils
@@ -645,10 +690,11 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
     e2e, L, wf = bool(args.end_to_end), args.nclasses, args.weight_funct
     meters = DeviceMeters(("loss", "area", "exact"), next(model.parameters()).device)
     static = {}
+    K = (curriculum_lanes(args, epoch) if e2e else None) or L     # --lane_curriculum, as in train_epoch
 
     def loss_fn(out):
         if e2e:
-            loss, static["exact"] = fused_area_loss(out[:L], static["params"], wf, exact=True)
+            loss, static["exact"] = fused_area_loss(out[:K], static["params"], wf, exact=True)
             if args.clas:
                 loss = clas_loss(loss, out, static, criterion_line_class, criterion_horizon, args)
             return loss
@@ -680,8 +726,10 @@ def train_epoch_bev(loader, model, optimizer, criterion, criterion_seg, criterio
                                   args.resize, args.save_path)
 
     fields = lambda b: {"input": b[0], "gt": b[1], "params": b[2], "gt_line": b[4], "gt_horizon": b[5]}
-    if _train_replays(loader, model, optimizer, static, fields, {"input": torch.float32}, post, report, args.print_freq,
-                      args.save_freq, loss_fn=loss_fn, end_to_end=e2e) is None:
+    with _FitLanes(model, K if K < L else None):
+        step = _train_replays(loader, model, optimizer, static, fields, {"input": torch.float32}, post, report,
+                              args.print_freq, args.save_freq, loss_fn=loss_fn, end_to_end=e2e)
+    if step is None:
         return 0, 0, 0
     m = meters.read()
     return m["loss"][1], m["area"][1], m["exact"][1]

@@ -1,6 +1,7 @@
 """Host side of the fused weighted least-squares layer: grid tables, workspace
 and the ``torch.autograd.Function`` that calls ``lf_lsq_fwd`` / ``lf_lsq_bwd``
-(include/lanefit_b200.h), or their ``*_keep`` variants when a per-pixel keep map is given.  Torch is plumbing here (device memory, streams,
+(include/lanefit_b200.h), or their ``*_keep`` variants when a per-pixel keep map is given, and their ``*_lanes`` forms
+when only the first ``lanes`` maps are fitted (a lane curriculum).  Torch is plumbing here (device memory, streams,
 autograd graph); all arithmetic on the maps happens in csrc/lsq.cu.
 """
 import torch
@@ -92,18 +93,23 @@ def status_message(st):
 
 
 class LsqFunction(torch.autograd.Function):
-    """beta, masked = LSQ(o).  o: [B,L,H,W] f32/bf16 raw (or pre-activated) maps."""
+    """beta, masked = LSQ(o).  o: [B,Lmap,H,W] f32/bf16 raw (or pre-activated) maps, of which the first ``lanes`` (default
+    all) are fitted: beta [B, lanes, order+1], masked [B, lanes, H, W], and the gradient of the other maps is zero."""
 
     @staticmethod
-    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out, rowp=None, keep=None):
+    def forward(ctx, o, tables, order, mask_rows, act, reg_ls, solver, want_masked, status_out, rowp=None, keep=None,
+                lanes=None):
         # rowp: a learned warp's (alpha, gamma, y') per row (homography.WarpTables.rowp); the forward then also keeps the
         # row sums and the backward returns dL/drowp.  keep: uint8 [H, W] from keep_map, or None
         _capi.require_cuda(o)
         if order < 0 or order > _capi.MAX_ORDER:
             raise NotImplementedError("Requested order {} for polynomial fit is not implemented".format(order))
         o = o.contiguous()
-        B, L, H, W = o.shape
+        B, Lmap, H, W = o.shape
         assert (H, W) == (tables.H, tables.W)
+        L = Lmap if lanes is None else lanes
+        # a prefix fit: the *_lanes entry points take the maps' channel count after L
+        Ls, lsfx = ((L,), "") if L == Lmap else ((L, Lmap), "_lanes")
         n = order + 1
         h = _capi.lib()
         dev = o.device
@@ -124,24 +130,24 @@ class LsqFunction(torch.autograd.Function):
             if rowp is not None and ctx.needs_input_grad[9]:
                 rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
-                _capi.call("lf_lsq_fwd_per_image", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
-                           _capi.ptr(tables.yrow), _capi.ptr(keep), B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                _capi.call("lf_lsq_fwd_per_image" + lsfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.yrow), _capi.ptr(keep), B, *Ls, H, W, order, mask_rows, act, float(reg_ls), solver,
                            _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status), _capi.ptr(rowsums),
                            _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
                            nbytes=B * L * H * W * (esz + (4 if want_masked else 0)) + 4 * B * H * W)
         elif rowp is not None and ctx.needs_input_grad[9]:
             rowsums = torch.empty(B, L, H, 3, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
-                _capi.call("lf_lsq_fwd_rowsums" + sfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
-                           _capi.ptr(tables.yrow), *kp, B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                _capi.call("lf_lsq_fwd_rowsums" + sfx + lsfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.yrow), *kp, B, *Ls, H, W, order, mask_rows, act, float(reg_ls), solver,
                            _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status), _capi.ptr(rowsums),
                            _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
                            nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
         else:
             # the fixed warp, or a learned warp without a gradient (validation, test scoring): no row sums
             with torch.cuda.device(dev):
-                _capi.call("lf_lsq_fwd" + sfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
-                           _capi.ptr(tables.ytab), _capi.ptr(tables.yrow), *kp, B, L, H, W, order, mask_rows, act, float(reg_ls), solver,
+                _capi.call("lf_lsq_fwd" + sfx + lsfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(tables.xtab),
+                           _capi.ptr(tables.ytab), _capi.ptr(tables.yrow), *kp, B, *Ls, H, W, order, mask_rows, act, float(reg_ls), solver,
                            _capi.ptr(beta), _capi.ptr(zinv), _capi.ptr(masked), _capi.ptr(status),
                            _capi.ptr(ws), ws.numel(), _capi.stream_ptr(),
                            nbytes=B * L * H * W * (esz + (4 if want_masked else 0)))
@@ -153,7 +159,7 @@ class LsqFunction(torch.autograd.Function):
                 raise RuntimeError(status_message(st))
         ctx.save_for_backward(o, beta, zinv, rowsums, keep)
         ctx.tables = tables
-        ctx.cfg = (order, mask_rows, act)
+        ctx.cfg = (order, mask_rows, act, L)
         if masked is not None:
             ctx.mark_non_differentiable(masked)
             return beta, masked
@@ -162,60 +168,75 @@ class LsqFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gbeta, _gmasked):
         o, beta, zinv, rowsums, keep = ctx.saved_tensors
-        order, mask_rows, act = ctx.cfg
+        order, mask_rows, act, L = ctx.cfg
         t = ctx.tables
-        B, L, H, W = o.shape
+        B, Lmap, H, W = o.shape
+        Ls, lsfx = ((L,), "") if L == Lmap else ((L, Lmap), "_lanes")
         gbeta = gbeta.to(torch.float64).contiguous()
         d_o = torch.empty_like(o)
         if getattr(t, "per_image", False):
             with torch.cuda.device(o.device):
-                _capi.call("lf_lsq_bwd_per_image", _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(t.xtab), _capi.ptr(t.yrow),
-                           _capi.ptr(keep), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
+                _capi.call("lf_lsq_bwd_per_image" + lsfx, _capi.ptr(o), _capi.dtype_id(o), _capi.ptr(t.xtab),
+                           _capi.ptr(t.yrow), _capi.ptr(keep), B, *Ls, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
                            _capi.ptr(gbeta), _capi.ptr(d_o), _capi.stream_ptr(),
-                           nbytes=2 * B * L * H * W * o.element_size() + 4 * B * H * W)
+                           nbytes=B * (L + Lmap) * H * W * o.element_size() + 4 * B * H * W)
                 g_rowp = None
                 if rowsums is not None:
                     g_rowp = torch.empty(B, H, 3, dtype=torch.float64, device=o.device)
                     _capi.call("lf_lsq_grid_grad_per_image", _capi.ptr(rowsums), _capi.ptr(t.yrow), _capi.ptr(beta),
                                _capi.ptr(zinv), _capi.ptr(gbeta), B, L, H, order, mask_rows, _capi.ptr(g_rowp),
                                _capi.stream_ptr())
-            return d_o, None, None, None, None, None, None, None, None, g_rowp, None
+            return d_o, None, None, None, None, None, None, None, None, g_rowp, None, None
         with torch.cuda.device(o.device):
-            _capi.call("lf_lsq_bwd" + ("" if keep is None else "_keep"), _capi.ptr(o), _capi.dtype_id(o),
+            _capi.call("lf_lsq_bwd" + ("" if keep is None else "_keep") + lsfx, _capi.ptr(o), _capi.dtype_id(o),
                        _capi.ptr(t.xtab), _capi.ptr(t.ytab), _capi.ptr(t.yrow),
-                       *(() if keep is None else (_capi.ptr(keep),)), B, L, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
+                       *(() if keep is None else (_capi.ptr(keep),)), B, *Ls, H, W, order, mask_rows, act, _capi.ptr(beta), _capi.ptr(zinv),
                        _capi.ptr(gbeta), _capi.ptr(d_o), _capi.stream_ptr(),
-                       nbytes=2 * B * L * H * W * o.element_size())
+                       nbytes=B * (L + Lmap) * H * W * o.element_size())
         g_rowp = None
         if rowsums is not None:
             g_rowp = torch.empty(H, 3, dtype=torch.float64, device=o.device)
             _capi.call("lf_lsq_grid_grad", _capi.ptr(rowsums), _capi.ptr(t.yrow), _capi.ptr(beta), _capi.ptr(zinv),
                        _capi.ptr(gbeta), B, L, H, order, mask_rows, _capi.ptr(g_rowp), _capi.stream_ptr())
-        return d_o, None, None, None, None, None, None, None, None, g_rowp, None
+        return d_o, None, None, None, None, None, None, None, None, g_rowp, None, None
+
+
+def check_lanes(lanes, L):
+    """The number of lanes to fit of L maps: None means all; otherwise an int in [1, L] (ValueError else)."""
+    if lanes is None:
+        return None
+    if isinstance(lanes, bool) or not isinstance(lanes, int) or not 1 <= lanes <= L:
+        raise ValueError("lanes must be an int in [1, %d] (the maps' lane count) or None, got %r" % (L, lanes))
+    return lanes
 
 
 def lsq(o, grid, order, const=255.0, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False,
-        want_masked=False, status_out=None, keep=None):
+        want_masked=False, status_out=None, keep=None, lanes=None):
     """Functional entry: returns (beta [B,L,order+1] f64, masked or None).  keep: optional bool / uint8 [H, W] map
-    shared by every image and lane; act(o) is zeroed where it is 0 (masked holds the zeros, d_o is 0 there)."""
+    shared by every image and lane; act(o) is zeroed where it is 0 (masked holds the zeros, d_o is 0 there).
+    lanes: fit the first ``lanes`` maps only (default all): beta [B, lanes, order+1], masked [B, lanes, H, W], a zero
+    gradient for the other maps, and their systems never reach ``status_out``."""
     B, L, H, W = o.shape
+    lanes = check_lanes(lanes, L)
     tables = grid_tables(grid, H, W, const)
     if act not in _capi.ACT_IDS:
         raise NotImplementedError("Activation type: {} is not implemented".format(act))
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
     return LsqFunction.apply(o, tables, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked,
-                             status_out, None, keep_map(keep, H, W, o.device))
+                             status_out, None, keep_map(keep, H, W, o.device), lanes)
 
 
 def lsq_warp(o, warp, order, mask_rows=0, act="none", reg_ls=0.0, use_cholesky=False, want_masked=False, status_out=None,
-             keep=None):
+             keep=None, lanes=None):
     """``lsq`` on a learned warp's tables (homography.WarpTables): beta has a gradient with respect to ``warp.rowp``
     as well as ``o``; the row sums behind it cover the kept pixels only.  A per-image warp (``warp.per_image``, a
-    predicted homography) fits image b on its own tables and gives rowp [B, R, 3] its per-image gradient."""
+    predicted homography) fits image b on its own tables and gives rowp [B, R, 3] its per-image gradient.  lanes as in
+    ``lsq``."""
     if getattr(warp, "per_image", False) and warp.xtab.shape[0] != o.shape[0]:
         raise ValueError("per-image warp tables for %d images, maps for %d" % (warp.xtab.shape[0], o.shape[0]))
     if act not in _capi.ACT_IDS:
         raise NotImplementedError("Activation type: {} is not implemented".format(act))
+    lanes = check_lanes(lanes, o.shape[1])
     solver = _capi.SOLVER_CHOLESKY if use_cholesky else _capi.SOLVER_INVERSE
     return LsqFunction.apply(o, warp, order, mask_rows, _capi.ACT_IDS[act], reg_ls, solver, want_masked, status_out,
-                             warp.rowp, keep_map(keep, o.shape[2], o.shape[3], o.device))
+                             warp.rowp, keep_map(keep, o.shape[2], o.shape[3], o.device), lanes)
