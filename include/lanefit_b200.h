@@ -686,7 +686,9 @@ int lf_linear_bwd_weight(const float* dy, const float* relu_out, const float* x,
  * out [B][C][H][W] class planes (C = nl + 1) -> maps [B][nl][H][W], maps[b][k] = (argmax == k+1) ? k+1 : 0, rows < mask_rows
  * zeroed.  lf_ce2d_fwd / _bwd replace nn.CrossEntropyLoss(weight) on the planar logits (BP/Loss_crit.py:64-65,
  * BP/main.py:258,307): target [B][H][W] int64, weight [C] or NULL; partial = 2*lf_ce2d_blocks() doubles of scratch, sums = 2
- * doubles (weighted loss sum, weight sum) kept for the backward, loss = 1 double; dx = gout * dloss/dx (gout NULL = 1). */
+ * doubles (weighted loss sum, weight sum) kept for the backward, loss = 1 double; dx = gout * dloss/dx (gout NULL = 1).
+ * A target outside [0, C) adds to neither sum and its pixel's dx is +0.0, also when no pixel is counted (loss = 0/0 = NaN,
+ * as torch's cross_entropy with every target ignored). */
 int lf_seg_lane_maps(const float* out, int B, int C, int H, int W, int nl, int mask_rows, float* maps, lf_stream_t stream);
 /* lf_seg_lane_maps plus the gt_line substitution of BP/Networks/LSQ_layer.py:308-311 (`masked[gt_mask] = masked[0, 0]...`):
  * gt_line [B][nl] float on the device, or NULL (then the output is lf_seg_lane_maps'); where gt_line[b][k] != 0, maps[b][k] is

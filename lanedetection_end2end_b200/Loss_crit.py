@@ -89,7 +89,9 @@ def seg_proxy_loss(loss_fit, criterion_seg, output_seg, gt, weight):
     """The --seg_proxy joint loss: (loss_fit + weight * ce, ce) with ce = criterion_seg(output_seg, gt), the sum formed in
     float64 in that order, so an eager loop and a graph replay form the same bits.  ``loss_fit`` is the end-to-end loss
     (with --clas, ``loss * weight_fit + (line + horizon) * weight_class``).  Targets outside [0, L] add to neither the
-    loss nor the weight sum (lf_ce2d); the reference's nn.CrossEntropyLoss would device-assert on them."""
+    loss nor the weight sum (lf_ce2d), and their gradient is +0.0; the reference's nn.CrossEntropyLoss would
+    device-assert on them.  With no target in range the loss is NaN and the gradient zero, as torch's cross_entropy gives
+    when every target is its ignore_index."""
     ce = criterion_seg(output_seg, gt)
     return loss_fit.double() + weight * ce.double(), ce
 

@@ -5,7 +5,9 @@
 //    lf_seg_lane_maps_line adds the gt_line substitution of :308-311 in the same launch, so it needs no host read of gt_line.
 //  * lf_ce2d_*         -- the weighted pixel-wise nn.CrossEntropyLoss(weights) of BP/Loss_crit.py:64-65 on the planar
 //    [B, C, H, W] logits (BP/main.py:258,307): loss = sum_i w[t_i] (lse_i - x_{t_i}) / sum_i w[t_i], and its gradient
-//    w[t_i] (softmax_c - [c == t_i]) / sum w, recomputed from the logits (nothing saved but the two sums).
+//    w[t_i] (softmax_c - [c == t_i]) / sum w, recomputed from the logits (nothing saved but the two sums).  A pixel whose
+//    target is outside [0, C) adds to neither sum and gets a +0.0 gradient, also when no pixel is counted (sum w = 0,
+//    loss NaN): torch's cross_entropy with every target at ignore_index gives the same NaN loss and zero gradient.
 // Bound: HBM -- each kernel reads the C planes once (the gradient kernel also writes them); fp32 per pixel, fp64 across
 // pixels, deterministic two-stage sums.
 #include "lf_common.cuh"
@@ -90,11 +92,12 @@ __global__ void __launch_bounds__(SEG_THREADS) ce2d_kernel(const float* __restri
             num += (double)(w * ((m + logf(s)) - xt));
             den += (double)w;
         } else {
+            // an uncounted pixel writes +0.0 without touching gscale, which is inf or NaN when no pixel is counted
             const float inv = 1.f / s;
             float* di = dx + (size_t)b * C * HW + p;
 #pragma unroll
             for (int c = 0; c < SEG_MAXC; ++c)
-                if (c < C) di[(size_t)c * HW] = gscale * w * (expf(v[c] - m) * inv - ((counted && c == t) ? 1.f : 0.f));
+                if (c < C) di[(size_t)c * HW] = counted ? gscale * w * (expf(v[c] - m) * inv - (c == t ? 1.f : 0.f)) : 0.f;
         }
     }
     if (!GRAD) {
