@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import lsq_contract as lc
+import lsq_tables_contract as tc
 from conftest import GOLDEN
 from test_epoch_gpu import paths  # noqa: F401  (the synthetic TuSimple directory fixture)
 from test_lsq_contract_gpu import GUARD, SENT, SENT64, Workspace, _check, _guarded
@@ -219,15 +220,10 @@ def test_keep_entry_points_against_fp64(case):
         # the row-sum instantiation: beta in the same gate, the same masked, and (A_r, B_r, C_r) over the kept pixels
         b2, z2, m2, st2, rs = _fwd_keep(o_t, c, xt, ytt, yrt, keep_t, rowsums=True)
         assert st2 == 0 and lc.forward_excess(b2, z2, ref) <= 1.0 and torch.equal(m2, masked)
-        a64 = lc.act64(_zeroed(o_exact, keep, c["act"]), c["act"])[0]
-        w = a64 * a64
-        x = xtab.reshape(H, W).astype(np.float64)
-        cols = np.arange(W, dtype=np.float64)
         mr = c["mask_rows"]
-        for k, s in enumerate((w.sum(-1), (w * x).sum(-1), (w * cols).sum(-1))):
-            got = rs[..., mr:, k].double().numpy()
-            scale = (np.abs(w) * (np.abs(x) if k == 1 else cols if k == 2 else 1.0)).sum(-1)[..., mr:]
-            assert (np.abs(got - s[..., mr:]) <= 1e-5 * scale + 1e-30).all(), (c["name"], k)
+        ref_rs, bound_rs = tc.rowsums_reference(o_exact, xtab, H, W, mr, c["act"], c["dtype"], keep)
+        exc = lc.excess(rs[..., mr:, :].double().numpy(), ref_rs, bound_rs)
+        assert exc <= 1.0, "%s: row sums outside the gate (%.3g)" % (c["name"], exc)
     # backward: the contract's reference with d_o = 0 demanded exactly at the masked pixels
     beta_b, zinv_b, g = lc.nonsymmetric_backward_inputs(c["B"], c["L"], c["order"], float(np.abs(yrow).max()), 0)
     got = _bwd_keep(o_t, c, xt, ytt, yrt, keep_t, beta_b, zinv_b, g)
